@@ -119,6 +119,26 @@ struct j2p_frame_desc {
 int j2p_session_create(j2p_session **out, int device, const struct j2p_frame_desc *desc);
 void j2p_session_destroy(j2p_session *s);
 
+/* ---- batch sessions: many frames of one geometry, one launch chain per iteration ----------------
+ * `nframes` frames that all have the geometry and solver parameters of `desc` (plane sizes,
+ * sampling factors, weight, pweight, iterations); quantisation tables and coefficients are per
+ * frame.  Every iteration solves all frames with the launches one frame would take (4:4:4 and
+ * 4:2:0; other sampling factors launch the projection of those planes once per frame), and every
+ * frame's result is bit-identical to solving it alone in j2p_session_create's session on the same
+ * device.  A batch of one behaves exactly like j2p_session_create.
+ *
+ * The per-plane calls (j2p_session_upload, j2p_session_download, j2p_session_plane_ptr) address
+ * plane = frame * nchannel + channel; the whole-session calls (reset, iterate, profile,
+ * wait_iteration, sync, stream, launches) act on the whole batch.  A batch is re-armed once, by the
+ * first j2p_session_iterate(s, 0, n) or j2p_session_reset after its planes were uploaded, so new
+ * frames can be uploaded into a batch and solved again.  Objective logging and the strip calls are
+ * refused on a batch of more than one frame (J2P_ERR_ARG); so are nframes == 0 and out-of-range
+ * planes or frames. */
+int j2p_session_create_batch(j2p_session **out, int device, const struct j2p_frame_desc *desc,
+                             unsigned nframes);
+/* Frames of the session (1 for every session not made by j2p_session_create_batch). */
+unsigned j2p_session_frames(const j2p_session *s);
+
 /* ---- row strips of one frame across several GPUs (SURVEY.md §8e, BASELINE config 4) ------------
  * A strip session holds frame rows [row0, row0+rows) of the frame described by `desc` (which
  * always describes the WHOLE frame) plus two halo rows on every side that has a neighbour.
@@ -202,7 +222,8 @@ int j2p_session_profile(j2p_session *s, unsigned n, float *ms_gradient, float *m
  * (compute.c:449-452) at the pace of the device without draining the stream. */
 int j2p_session_wait_iteration(j2p_session *s, unsigned iter);
 
-/* HBM -> host: the current iterate of `channel`, H x W floats raster. */
+/* HBM -> host: the current iterate of `channel`, H x W floats raster (batch sessions:
+ * plane = frame * nchannel + channel). */
 int j2p_session_download(j2p_session *s, unsigned channel, float *out);
 
 /* HBM -> host, joint (3-plane) whole-frame sessions: the image as the reference hands it to libpng,
@@ -213,6 +234,9 @@ int j2p_session_download(j2p_session *s, unsigned channel, float *out);
  * 3 or 6 bytes per pixel cross PCIe instead of 12. */
 int j2p_session_download_scanlines(j2p_session *s, unsigned w, unsigned h, unsigned bits,
                                    unsigned char *out);
+/* The same for frame `frame` of a batch session (j2p_session_download_scanlines is frame 0). */
+int j2p_session_download_frame_scanlines(j2p_session *s, unsigned frame, unsigned w, unsigned h,
+                                         unsigned bits, unsigned char *out);
 
 /* Objective terms of the most recent iteration, as logged by the reference (compute.c:271-272):
  * out[0]=objective, out[1]=prob_dist, out[2]=tv, out[3]=tv2.  Only tracked when logging was
@@ -231,7 +255,8 @@ void j2p_host_prefault(void *p, size_t bytes);
 /* Raw handles for callers that schedule their own work around the session (bench timing with
  * CUDA events on the launching stream; torch interop).  The stream is a cudaStream_t. */
 void *j2p_session_stream(j2p_session *s);
-/* Device pointer of the current iterate of `channel` (H x W floats). */
+/* Device pointer of the current iterate of `channel` (H x W floats; batch sessions: plane =
+ * frame * nchannel + channel).  Null when out of range. */
 void *j2p_session_plane_ptr(j2p_session *s, unsigned channel);
 
 /* Launch counters: number of kernel launches issued by this session since creation. */

@@ -129,6 +129,12 @@ def declare_product(lib: C.CDLL) -> C.CDLL:
     lib.j2p_thread_device.argtypes = []
     lib.j2p_session_create.restype = C.c_int
     lib.j2p_session_create.argtypes = [C.POINTER(vp), C.c_int, C.POINTER(FrameDesc)]
+    lib.j2p_session_create_batch.restype = C.c_int
+    lib.j2p_session_create_batch.argtypes = [C.POINTER(vp), C.c_int, C.POINTER(FrameDesc), C.c_uint]
+    lib.j2p_session_frames.restype = C.c_uint
+    lib.j2p_session_frames.argtypes = [vp]
+    lib.j2p_session_download_frame_scanlines.restype = C.c_int
+    lib.j2p_session_download_frame_scanlines.argtypes = [vp, C.c_uint, C.c_uint, C.c_uint, C.c_uint, vp]
     lib.j2p_session_create_strip.restype = C.c_int
     lib.j2p_session_create_strip.argtypes = [C.POINTER(vp), C.c_int, C.POINTER(FrameDesc), C.c_uint, C.c_uint]
     lib.j2p_session_strip_info.restype = C.c_int
@@ -202,6 +208,7 @@ HEADER_SYMBOLS = [
     'j2p_session_iterate', 'j2p_session_profile', 'j2p_session_wait_iteration', 'j2p_session_download', 'j2p_session_set_logging',
     'j2p_session_objective', 'j2p_session_sync', 'j2p_session_stream', 'j2p_session_plane_ptr',
     'j2p_session_launches', 'j2p_version', 'j2p_host_prefault', 'j2p_set_thread_device', 'j2p_thread_device', 'j2p_session_download_scanlines',
+    'j2p_session_create_batch', 'j2p_session_frames', 'j2p_session_download_frame_scanlines',
 ]
 
 _product = None
@@ -218,3 +225,98 @@ def load_product() -> C.CDLL:
                 'There is no CPU fallback.')
         _product = declare_product(C.CDLL(PRODUCT_LIB, mode=C.RTLD_LOCAL))
     return _product
+
+
+def frame_desc(img: CoefImage, channels, weight, pweight, iterations) -> FrameDesc:
+    """j2p_frame_desc of planes `channels` of img; pweight: one value per entry of `channels`."""
+    d = FrameDesc()
+    d.nchannel = len(channels)
+    for k, ch in enumerate(channels):
+        p = img.planes[ch]
+        d.plane_w[k], d.plane_h[k], d.w_samp[k], d.h_samp[k] = p.w, p.h, p.w_samp, p.h_samp
+        d.pweight[k] = float(pweight[k])
+    d.weight = float(weight)
+    d.iterations = int(iterations)
+    return d
+
+
+class Session:
+    """A resident session over the C ABI: a batch of `nframes` frames of one geometry
+    (j2p_session_create_batch), or with batch=False an ordinary one-frame session
+    (j2p_session_create).  Raises RuntimeError with j2p_last_error() on any failure."""
+
+    def __init__(self, lib, desc: FrameDesc, nframes: int = 1, device: int = 0, batch: bool = True):
+        self.lib, self.desc, self.nframes = lib, desc, nframes
+        self.nc = int(desc.nchannel)
+        self.s = C.c_void_p()
+        rc = (lib.j2p_session_create_batch(C.byref(self.s), device, C.byref(desc), nframes) if batch
+              else lib.j2p_session_create(C.byref(self.s), device, C.byref(desc)))
+        self._check(rc)
+        self.W, self.H = int(lib.j2p_session_width(self.s)), int(lib.j2p_session_height(self.s))
+
+    def _check(self, rc):
+        if rc != 0:
+            raise RuntimeError(self.lib.j2p_last_error().decode())
+
+    def upload(self, frames, channels, fdata=None):
+        """Frame f of the session <- planes `channels` of frames[f]; fdata: per frame, a list of
+        plane_h x plane_w conventional decodes, or None for the device decode."""
+        for f, img in enumerate(frames):
+            for k, ch in enumerate(channels):
+                p = img.planes[ch]
+                data = np.ascontiguousarray(p.data, dtype=np.int16)
+                quant = np.ascontiguousarray(p.quant, dtype=np.uint16)
+                fd = None if fdata is None else np.ascontiguousarray(fdata[f][k], dtype=np.float32)
+                self._check(self.lib.j2p_session_upload(self.s, f * self.nc + k, data.ctypes.data, quant.ctypes.data,
+                                                        None if fd is None else fd.ctypes.data))
+
+    def iterate(self, first: int, n: int):
+        self._check(self.lib.j2p_session_iterate(self.s, first, n))
+
+    def download(self):
+        """[frame][channel] -> (H, W) float32 current iterates (synchronises the session)."""
+        out = []
+        for f in range(self.nframes):
+            planes = []
+            for k in range(self.nc):
+                a = np.empty((self.H, self.W), np.float32)
+                self._check(self.lib.j2p_session_download(self.s, f * self.nc + k, a.ctypes.data))
+                planes.append(a)
+            out.append(planes)
+        return out
+
+    def sync(self):
+        self._check(self.lib.j2p_session_sync(self.s))
+
+    @property
+    def launches(self) -> int:
+        return int(self.lib.j2p_session_launches(self.s))
+
+    def close(self):
+        if self.s:
+            self.lib.j2p_session_destroy(self.s)
+            self.s = C.c_void_p()
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+def solve_batch(frames, channels, weight, pweight, iterations, fdata=None, device=0, lib=None):
+    """Solve planes `channels` of every CoefImage in `frames` (one geometry) as ONE batch session,
+    `iterations` iterations; fdata: per frame the caller's conventional decodes, or None (device
+    decode).  Returns the result planes per frame: [frame][channel] -> (H, W) float32."""
+    lib = lib or load_product()
+    desc = frame_desc(frames[0], channels, weight, pweight, iterations)
+    with Session(lib, desc, len(frames), device) as s:
+        s.upload(frames, channels, fdata)
+        s.iterate(0, iterations)
+        return s.download()

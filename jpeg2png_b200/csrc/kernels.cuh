@@ -77,7 +77,42 @@ struct FrameDev {
     int log_on;
     int log_slot;         // which of the two prob_dist slots k_project accumulates into
     double *logsums;      // [0]=tv, [1]=tv2, [2+3*slot+c] = sum over plane c of (residual/q)^2
+    // Batch sessions (nframes > 1, several frames of one geometry; session.cu): the pointers above
+    // are frame 0's.  Frame f's x, xp, g, gp sit f * frame_stride elements after them, its
+    // coefficients f * data_stride elements after pl[c].data, its tables (q, qq, rqq) at
+    // tables[f][c][3][64] instead of q/qq/rqq, and its reduction state at partials + f * 5 * grad_ctas,
+    // sums + 4 f, norms + 16 f, counter + f.  The batched kernels take the frame from blockIdx.z.
+    int nframes;
+    unsigned long long frame_stride, data_stride;
+    const float *tables;  // device [nframes][nc][3][64]; null for single-frame sessions
+    const float *host_tables;  // the host copy of it (per-frame launches of the generic projection)
 };
+
+// Frame f's view of a batch for a kernel that handles one frame (a per-frame launch).
+inline FrameDev frame_view(const FrameDev &F, int f) {
+    FrameDev V = F;
+    V.nframes = 1;
+    V.tables = nullptr;
+    const unsigned long long fo = (unsigned long long)f * F.frame_stride;
+    for (int c = 0; c < F.nc; c++) {
+        V.pl[c].x += fo;
+        V.pl[c].xp += fo;
+        V.pl[c].g += fo;
+        V.pl[c].gp += fo;
+        V.pl[c].data += (unsigned long long)f * F.data_stride;
+        for (int k = 0; k < 64; k++) {
+            const float *t = F.host_tables + ((size_t)f * F.nc + c) * 192;
+            V.q[c][k] = t[k];
+            V.qq[c][k] = t[64 + k];
+            V.rqq[c][k] = t[128 + k];
+        }
+    }
+    V.partials += (size_t)f * 5 * F.grad_ctas;
+    V.sums += 4 * (size_t)f;
+    V.norms += 16 * (size_t)f;
+    V.counter += f;
+    return V;
+}
 
 // ---- the stand-alone halo kernel (kernels_strip.cu); pointers into OTHER ranks' memory are cudaIpc
 // mappings made by session.cu

@@ -497,7 +497,7 @@ static void launch_gradient_nc(const FrameDev &F, float factor, dim3 grid, int r
 }
 
 cudaError_t launch_gradient(const FrameDev &F, float factor, cudaStream_t s) {
-    if (!F.log_on && !g_grad_scalar) return launch_gradient_packed(F, factor, s);
+    if (!F.log_on && (!g_grad_scalar || F.nframes > 1)) return launch_gradient_packed(F, factor, s);   // a batch always takes the packed kernel
     int cx, bands, rows;
     grad_geometry(F.W, F.t1 - F.t0, F.grad_slots, &cx, &bands, &rows);
     const dim3 grid(cx, bands);

@@ -56,9 +56,14 @@ __device__ __forceinline__ f2 shr_from_right(f2 v, float from_right) { return pk
 #else
 #define J2P_GRAD_BOUNDS __launch_bounds__(GM_NT, J2P_GRAD_MIN_CTAS)
 #endif
-template <int NC, bool TGV, int GPM>
+// BATCH: a batch session (kernels.cuh, FrameDev::nframes); the frame is blockIdx.z and every frame
+// has the grid a single-frame session of its geometry gets.  Its base is formed once, in 64 bits;
+// the offsets inside a frame stay 32-bit.  !BATCH compiles to the single-frame kernel unchanged.
+template <int NC, bool TGV, int GPM, bool BATCH>
 __global__ void J2P_GRAD_BOUNDS k_gradient_packed(const __grid_constant__ FrameDev F, const float factor, const int band_rows) {
     const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    const unsigned frame = BATCH ? blockIdx.z : 0u;
+    const size_t fo = BATCH ? (size_t)frame * F.frame_stride : 0;     // elements from frame 0's planes to this frame's
     const int W = F.W, H = F.H;
     const int X0 = (blockIdx.x * GM_WARPS + wid) * GM_USE;   // first target column of this warp
     const int yb = F.t0 + blockIdx.y * band_rows;            // first target row of this CTA (local row index)
@@ -79,7 +84,7 @@ __global__ void J2P_GRAD_BOUNDS k_gradient_packed(const __grid_constant__ FrameD
     pdl_wait();
     pdl_launch_dependents();
     // strip sessions: the halo rows of x_k arrive from the neighbours' projection (strip_sync.cuh)
-    strip_wait_halo(F.sync, blockIdx.y == 0, blockIdx.y == gridDim.y - 1);
+    if (!BATCH) strip_wait_halo(F.sync, blockIdx.y == 0, blockIdx.y == gridDim.y - 1);
 
     double acc[NC];
     RowCarry<NC> A, B;
@@ -123,11 +128,11 @@ __global__ void J2P_GRAD_BOUNDS k_gradient_packed(const __grid_constant__ FrameD
     const unsigned PS = F.plane_stride;
     unsigned long long lp_x = 0, lp_xp = 0, lp_g = 0, lp_gp = 0, lp_gpc = 0;
     if (GPM != 0) {
-        asm volatile("mad.wide.s32 %0, %1, 4, %2;" : "=l"(lp_x) : "r"(pxc), "l"(F.pl[0].x));
-        asm volatile("mad.wide.s32 %0, %1, 4, %2;" : "=l"(lp_xp) : "r"(pxc), "l"(F.pl[0].xp));
-        asm volatile("mad.wide.s32 %0, %1, 4, %2;" : "=l"(lp_g) : "r"(pxc), "l"(F.pl[0].g));
-        asm volatile("mad.wide.s32 %0, %1, 4, %2;" : "=l"(lp_gp) : "r"(pxc), "l"(F.pl[0].gp));
-        if (GPM == 2) asm volatile("mad.wide.s32 %0, %1, 4, %2;" : "=l"(lp_gpc) : "r"(pxc >> 1), "l"(F.pl[0].gp));   // 2x2 planes: one sample per pixel pair
+        asm volatile("mad.wide.s32 %0, %1, 4, %2;" : "=l"(lp_x) : "r"(pxc), "l"(F.pl[0].x + fo));
+        asm volatile("mad.wide.s32 %0, %1, 4, %2;" : "=l"(lp_xp) : "r"(pxc), "l"(F.pl[0].xp + fo));
+        asm volatile("mad.wide.s32 %0, %1, 4, %2;" : "=l"(lp_g) : "r"(pxc), "l"(F.pl[0].g + fo));
+        asm volatile("mad.wide.s32 %0, %1, 4, %2;" : "=l"(lp_gp) : "r"(pxc), "l"(F.pl[0].gp + fo));
+        if (GPM == 2) asm volatile("mad.wide.s32 %0, %1, 4, %2;" : "=l"(lp_gpc) : "r"(pxc >> 1), "l"(F.pl[0].gp + fo));   // 2x2 planes: one sample per pixel pair
     }
     auto at = [](unsigned long long base, unsigned elem) {          // base + 4 * elem
         unsigned long long a;
@@ -153,8 +158,8 @@ __global__ void J2P_GRAD_BOUNDS k_gradient_packed(const __grid_constant__ FrameD
                 cp8(dst + (2 * c) * 256, at(lp_x, ro + c * PS));
                 cp8(dst + (2 * c + 1) * 256, at(lp_xp, ro + c * PS));
             } else {
-                cp8(dst + (2 * c) * 256, (unsigned long long)(F.pl[c].x + (ro + (unsigned)pxc)));
-                cp8(dst + (2 * c + 1) * 256, (unsigned long long)(F.pl[c].xp + (ro + (unsigned)pxc)));
+                cp8(dst + (2 * c) * 256, (unsigned long long)(F.pl[c].x + fo + (ro + (unsigned)pxc)));
+                cp8(dst + (2 * c + 1) * 256, (unsigned long long)(F.pl[c].xp + fo + (ro + (unsigned)pxc)));
             }
         }
         if (GPM == 1) {                     // every gp plane has the frame's geometry and every target row has its gp row
@@ -169,7 +174,7 @@ __global__ void J2P_GRAD_BOUNDS k_gradient_packed(const __grid_constant__ FrameD
 #pragma unroll
             for (int c = 0; c < NC; c++) {
                 const PlaneDev &P = F.pl[c];
-                const float *gr = P.gp + (size_t)min(r / (unsigned)P.sh, (unsigned)P.ch - 1u) * P.cw;
+                const float *gr = P.gp + fo + (size_t)min(r / (unsigned)P.sh, (unsigned)P.ch - 1u) * P.cw;
                 cp4(dst + (2 * NC + c) * 256, (unsigned long long)(gr + gpx[c][0]));
                 cp4(dst + (2 * NC + c) * 256 + 4, (unsigned long long)(gr + gpx[c][1]));
             }
@@ -376,7 +381,7 @@ __global__ void J2P_GRAD_BOUNDS k_gradient_packed(const __grid_constant__ FrameD
                     const float dgl = __shfl_up_sync(0xffffffffu, hi(N.dg[c]), 1);
                     o = addm2(N.ud[c], add2(o, shl_from_left(N.dg[c], dgl)), one);
                 }
-                float2 *dst = GPM != 0 ? reinterpret_cast<float2 *>(at(lp_g, ro + c * PS)) : reinterpret_cast<float2 *>(F.pl[c].g + (ro + (unsigned)pxc));
+                float2 *dst = GPM != 0 ? reinterpret_cast<float2 *>(at(lp_g, ro + c * PS)) : reinterpret_cast<float2 *>(F.pl[c].g + fo + (ro + (unsigned)pxc));
                 if (st) *dst = make_float2(lo(o), hi(o));
                 const f2 sq = mul2(o, o);
                 acc[c] = __dadd_rn(acc[c], (double)(st ? lo(sq) : 0.f));      // compute.c:203; + 0.0 leaves the sum as it is
@@ -419,6 +424,11 @@ __global__ void J2P_GRAD_BOUNDS k_gradient_packed(const __grid_constant__ FrameD
     __shared__ double fin[3];
     __shared__ unsigned ticket;
     const int tid = threadIdx.x;
+    // this frame's partials, ticket, sums and norms (a single frame: the session's own)
+    double *const partials = F.partials + (BATCH ? (size_t)frame * 5 * F.grad_ctas : 0);
+    unsigned *const counter = F.counter + frame;
+    double *const sums = F.sums + 4 * frame;
+    float *const norms = F.norms + 16 * frame;
 #pragma unroll
     for (int c = 0; c < NC; c++) {
         const double sum = warp_sum(acc[c]);
@@ -434,10 +444,10 @@ __global__ void J2P_GRAD_BOUNDS k_gradient_packed(const __grid_constant__ FrameD
         for (int c = 0; c < NC; c++) {
             double sum = 0.;
             for (int k = 0; k < GM_WARPS; k++) sum = __dadd_rn(sum, red[c][k]);
-            F.partials[(size_t)c * F.grad_ctas + cta] = sum;
+            partials[(size_t)c * F.grad_ctas + cta] = sum;
         }
         unsigned t;
-        asm volatile("atom.release.gpu.global.add.u32 %0, [%1], 1;" : "=r"(t) : "l"(F.counter) : "memory");
+        asm volatile("atom.release.gpu.global.add.u32 %0, [%1], 1;" : "=r"(t) : "l"(counter) : "memory");
         ticket = t;
     }
     __syncthreads();
@@ -446,7 +456,7 @@ __global__ void J2P_GRAD_BOUNDS k_gradient_packed(const __grid_constant__ FrameD
 #pragma unroll
         for (int c = 0; c < NC; c++) {
             double sum = 0.;
-            for (unsigned k = tid; k < ncta; k += GM_NT) sum = __dadd_rn(sum, __ldcg(&F.partials[(size_t)c * F.grad_ctas + k]));
+            for (unsigned k = tid; k < ncta; k += GM_NT) sum = __dadd_rn(sum, __ldcg(&partials[(size_t)c * F.grad_ctas + k]));
             sum = warp_sum(sum);
             if (lane == 0) red[c][wid] = sum;
         }
@@ -458,13 +468,13 @@ __global__ void J2P_GRAD_BOUNDS k_gradient_packed(const __grid_constant__ FrameD
             fin[tid] = sum;
             if (tid < NC) {
                 const float norm = fsqrt(__double2float_rn(sum));                               // compute.c:205
-                F.sums[tid] = sum;                                                              // strips driven by the host / NCCL combine these
-                F.norms[tid] = norm;
-                F.norms[4 + tid] = __frcp_rn(norm);                                             // shared reciprocal for k_project
+                sums[tid] = sum;                                                              // strips driven by the host / NCCL combine these
+                norms[tid] = norm;
+                norms[4 + tid] = __frcp_rn(norm);                                             // shared reciprocal for k_project
             }
         }
-        if (tid == 0) *F.counter = 0u;
-        if (F.sync.nranks > 1) {                                                                // strips over peer memory
+        if (tid == 0) *counter = 0u;
+        if (!BATCH && F.sync.nranks > 1) {                                                      // strips over peer memory
             __syncthreads();
             strip_post_sums(F.sync, fin, tid);
         }
@@ -491,11 +501,14 @@ static int sm_count() {
     }
     return n;
 }
+// A batch launches the batched instantiation with every frame on the grid a single-frame session of
+// that geometry gets: the band geometry comes from the SINGLE-FRAME instantiation's occupancy, so each
+// frame's sums of g^2 are folded in the same order as in its own session (DESIGN.md §7b).
 template <int NC, bool TGV, int GPM>
 static cudaError_t launch_instance(const FrameDev &F, float factor, cudaStream_t s) {
     static const int per_sm = [] {
         int n = 0;
-        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, k_gradient_packed<NC, TGV, GPM>, GM_NT, 0) != cudaSuccess) {
+        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, k_gradient_packed<NC, TGV, GPM, false>, GM_NT, 0) != cudaSuccess) {
             cudaGetLastError();
             n = 0;
         }
@@ -503,7 +516,8 @@ static cudaError_t launch_instance(const FrameDev &F, float factor, cudaStream_t
     }();
     int cx, bands, rows;
     grad_geometry(F.W, F.t1 - F.t0, sm_count() * per_sm, &cx, &bands, &rows);
-    return launch_chain(k_gradient_packed<NC, TGV, GPM>, dim3(cx, bands), dim3(GM_NT), 0, s, F, factor, rows);
+    if (F.nframes > 1) return launch_chain(k_gradient_packed<NC, TGV, GPM, true>, dim3(cx, bands, F.nframes), dim3(GM_NT), 0, s, F, factor, rows);
+    return launch_chain(k_gradient_packed<NC, TGV, GPM, false>, dim3(cx, bands), dim3(GM_NT), 0, s, F, factor, rows);
 }
 template <bool TGV, int GPM>
 static cudaError_t launch_packed_nc(const FrameDev &F, float factor, cudaStream_t s) {
@@ -516,7 +530,7 @@ static cudaError_t launch_packed_nc(const FrameDev &F, float factor, cudaStream_
 
 int packed_gradient_occupancy() {
     int per_sm = 0;
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_gradient_packed<3, true, 1>, GM_NT, 0) != cudaSuccess) {
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_gradient_packed<3, true, 1, false>, GM_NT, 0) != cudaSuccess) {
         cudaGetLastError();
         return 0;
     }

@@ -395,11 +395,18 @@ cudaError_t launch_project(const FrameDev &Fin, float factor, cudaStream_t s, in
             if (eb != cudaSuccess) return eb;
             c += count - 1;
         }
-        else if (P.sw == 2 && P.sh == 2) k_project<2, 2><<<grid, P_NT, 0, s>>>(F, G, factor);
-        else if (P.sw == 2 && P.sh == 1) k_project<2, 1><<<grid, P_NT, 0, s>>>(F, G, factor);
-        else if (P.sw == 1 && P.sh == 2) k_project<1, 2><<<grid, P_NT, 0, s>>>(F, G, factor);
-        else k_project<0, 0><<<grid, P_NT, 0, s>>>(F, G, factor);
-        if (*nlaunch == before) *nlaunch += 1;                       // one of the direct k_project<> launches above
+        else {
+            // k_project<> handles one frame: a batch launches it once per frame on that frame's view
+            for (int f = 0; f < F.nframes; f++) {
+                const FrameDev &V = F.nframes > 1 ? frame_view(F, f) : F;
+                if (P.sw == 2 && P.sh == 2) k_project<2, 2><<<grid, P_NT, 0, s>>>(V, G, factor);
+                else if (P.sw == 2 && P.sh == 1) k_project<2, 1><<<grid, P_NT, 0, s>>>(V, G, factor);
+                else if (P.sw == 1 && P.sh == 2) k_project<1, 2><<<grid, P_NT, 0, s>>>(V, G, factor);
+                else k_project<0, 0><<<grid, P_NT, 0, s>>>(V, G, factor);
+                *nlaunch += 1;
+            }
+        }
+        if (*nlaunch == before) *nlaunch += 1;                       // the logging k_project<1, 1> launch above
         const cudaError_t e = cudaGetLastError();
         if (e != cudaSuccess) return e;
     }

@@ -37,8 +37,9 @@ static_assert(PT_C4 == 1 << PT_SH, "tile width");
 #ifndef J2P_TILE_MIN_CTAS
 #define J2P_TILE_MIN_CTAS (256 / J2P_TILE_BLOCKS / 2)      // 32 warps per SM either way (64 registers)
 #endif
-// RES: the plane's coefficient grid is smaller than the frame (compute.c:338), e.g. 1080p luma
-template <bool RES>
+// RES: the plane's coefficient grid is smaller than the frame (compute.c:338), e.g. 1080p luma.
+// BATCH: a batch session (FrameDev::nframes); blockIdx.z = frame * count + k for planes c0 + k.
+template <bool RES, bool BATCH>
 __global__ void __launch_bounds__(PT_NT, J2P_TILE_MIN_CTAS) k_project_tile(const __grid_constant__ FrameDev F, const int c0, const float factor) {
     __shared__ __align__(16) float4 sx[8][PT_C4];                // x_k          -> later x_{k+1}
     __shared__ __align__(16) float4 sp[8][PT_C4];                // x_{k-1}      -> later gp
@@ -47,8 +48,11 @@ __global__ void __launch_bounds__(PT_NT, J2P_TILE_MIN_CTAS) k_project_tile(const
     __shared__ __align__(16) float sq[3][64];
     __shared__ float snorm[2];
     const int tid = threadIdx.x;
-    const int c = c0 + blockIdx.z;                               // planes of equal geometry share one launch
+    const int count = BATCH ? (int)gridDim.z / F.nframes : 1;
+    const int frame = BATCH ? (int)blockIdx.z / count : 0;
+    const int c = c0 + (int)blockIdx.z - frame * count;          // planes of equal geometry share one launch
     const PlaneDev &P = F.pl[c];
+    const size_t fo = BATCH ? (size_t)frame * F.frame_stride : 0;
     const int W = F.W;
     const int bw = P.cw >> 3;
     const int bx0 = blockIdx.x * PT_NB, by = strip_row_order(F.sync, blockIdx.y, gridDim.y);   // the grid covers real blocks only
@@ -66,8 +70,8 @@ __global__ void __launch_bounds__(PT_NT, J2P_TILE_MIN_CTAS) k_project_tile(const
         const int e = tid + PT_NT * i, row = e >> PT_SH, c4 = e & (PT_C4 - 1);
         if (c4 < valid_c4) {
             const size_t gi = row0 + (size_t)row * W + (size_t)c4 * 4;
-            cp_async16(&sx[row][c4 ^ row], P.x + gi);
-            cp_async16(&sp[row][c4 ^ row], P.xp + gi);
+            cp_async16(&sx[row][c4 ^ row], P.x + fo + gi);
+            cp_async16(&sp[row][c4 ^ row], P.xp + fo + gi);
         }
     }
     pdl_wait();                                                  // the gradient and its norm are complete and visible
@@ -75,19 +79,33 @@ __global__ void __launch_bounds__(PT_NT, J2P_TILE_MIN_CTAS) k_project_tile(const
 #pragma unroll
     for (int i = 0; i < 2; i++) {
         const int e = tid + PT_NT * i, row = e >> PT_SH, c4 = e & (PT_C4 - 1);
-        if (c4 < valid_c4) cp_async16(&sg[row][c4 ^ row], P.g + row0 + (size_t)row * W + (size_t)c4 * 4);
+        if (c4 < valid_c4) cp_async16(&sg[row][c4 ^ row], P.g + fo + row0 + (size_t)row * W + (size_t)c4 * 4);
     }
     cp_async_commit();
     const int b = tid >> 3, j = tid & 7;
     const bool real = b < nbx;
     int4 draw = make_int4(0, 0, 0, 0);
-    if (real) draw = __ldg(reinterpret_cast<const int4 *>(P.data + ((size_t)(by * bw + bx0 + b) * 64 + j * 8)));   // 512 B per warp, coalesced
+    if (real) draw = __ldg(reinterpret_cast<const int4 *>(P.data + (BATCH ? (size_t)frame * F.data_stride : 0) + ((size_t)(by * bw + bx0 + b) * 64 + j * 8)));   // 512 B per warp, coalesced
     if (tid < 64) {
-        sq[0][tid] = F.q[c][tid];
-        sq[1][tid] = F.qq[c][tid];
-        sq[2][tid] = F.rqq[c][tid];
+        if (BATCH) {                                             // this frame's tables (device copy)
+            const float *t = F.tables + ((size_t)frame * F.nc + c) * 192;
+            sq[0][tid] = t[tid];
+            sq[1][tid] = t[64 + tid];
+            sq[2][tid] = t[128 + tid];
+        } else {
+            sq[0][tid] = F.q[c][tid];
+            sq[1][tid] = F.qq[c][tid];
+            sq[2][tid] = F.rqq[c][tid];
+        }
     }
-    if (tid >= 64 && tid < 96) strip_norm(F, c, snorm, tid - 64);    // whole frame: what k_gradient left; strips: fold of every rank's sums
+    if (BATCH) {
+        if (tid == 64) {                                         // what k_gradient left for this frame
+            snorm[0] = F.norms[16 * frame + c];
+            snorm[1] = F.norms[16 * frame + 4 + c];
+        }
+    } else if (tid >= 64 && tid < 96) {
+        strip_norm(F, c, snorm, tid - 64);                       // whole frame: what k_gradient left; strips: fold of every rank's sums
+    }
     cp_async_wait<0>();
     __syncthreads();
 
@@ -198,12 +216,12 @@ __global__ void __launch_bounds__(PT_NT, J2P_TILE_MIN_CTAS) k_project_tile(const
     __syncthreads();
 
     // ---- coalesced copy-out: x_{k+1} over x_{k-1} (compute.c:387), gp for the next iteration ----
-    float *gp0 = P.gp + (size_t)(by * 8) * P.cw + (size_t)bx0 * 8;
+    float *gp0 = P.gp + fo + (size_t)(by * 8) * P.cw + (size_t)bx0 * 8;
 #pragma unroll
     for (int i = 0; i < 2; i++) {
         const int e = tid + PT_NT * i, row = e >> PT_SH, c4 = e & (PT_C4 - 1);
         if (c4 < valid_c4) {
-            *reinterpret_cast<float4 *>(P.xp + row0 + (size_t)row * W + (size_t)c4 * 4) = sx[row][c4 ^ row];
+            *reinterpret_cast<float4 *>(P.xp + fo + row0 + (size_t)row * W + (size_t)c4 * 4) = sx[row][c4 ^ row];
             if (use_prob) *reinterpret_cast<float4 *>(gp0 + (size_t)row * P.cw + (size_t)c4 * 4) = sp[row][c4 ^ row];
         }
     }
@@ -211,7 +229,7 @@ __global__ void __launch_bounds__(PT_NT, J2P_TILE_MIN_CTAS) k_project_tile(const
     // ---- strips over peer memory: the strip's first / last two rows also go straight into the
     // neighbours' halo rows (NVLink stores), and the last border CTA of the iteration raises their flag
     const StripSync &S = F.sync;
-    if (S.nranks > 1 && S.fused_halo) {
+    if (!BATCH && S.nranks > 1 && S.fused_halo) {
         const bool top = by == 0 && S.has_up, bottom = by == (int)gridDim.y - 1 && S.has_down;
         if (top || bottom) {
             for (int e = tid; e < 4 * PT_C4; e += PT_NT) {                // 2 rows x 64 pieces, top then bottom
@@ -230,13 +248,19 @@ __global__ void __launch_bounds__(PT_NT, J2P_TILE_MIN_CTAS) k_project_tile(const
 // Frame pixels of a 1x1 plane that no coefficient block covers (1080p: luma rows 1080..1087) are
 // only stepped: compute_projection never visits them (compute.c:349-350).  The region is the
 // bottom band (rows >= ch, full width) plus the right band (rows < ch, columns >= cw).
+// BATCH: the frame is blockIdx.z.
+template <bool BATCH>
 __global__ void k_step_uncovered(const __grid_constant__ FrameDev F, const int c, const float factor) {
     const PlaneDev &P = F.pl[c];
     const int W = F.W, H = F.H;
+    const int frame = BATCH ? (int)blockIdx.z : 0;
+    const size_t fo = BATCH ? (size_t)frame * F.frame_stride : 0;
+    const float *const xk = P.x + fo, *const gk = P.g + fo;
+    float *const xm = P.xp + fo;
     Stepper stepper;
     stepper.factor = factor;
     stepper.step = F.step;
-    stepper.norm = F.norms[c];
+    stepper.norm = F.norms[16 * frame + c];
     stepper.rn = 0.f;
     stepper.stepping = stepper.norm != 0.f;
     const unsigned bottom = (unsigned)(H - P.ch) * (unsigned)W, right_w = (unsigned)(W - P.cw);
@@ -252,7 +276,7 @@ __global__ void k_step_uncovered(const __grid_constant__ FrameDev F, const int c
             px = (unsigned)P.cw + k % right_w;
         }
         const size_t gi = (size_t)py * W + px;
-        P.xp[gi] = stepper(P.x[gi], P.xp[gi], P.g[gi]);
+        xm[gi] = stepper(xk[gi], xm[gi], gk[gi]);
     }
 }
 
@@ -260,8 +284,13 @@ static cudaError_t launch_step_uncovered(const FrameDev &F, int c, float factor,
     const PlaneDev &P = F.pl[c];
     const size_t n = (size_t)(F.H - P.ch) * F.W + (size_t)P.ch * (F.W - P.cw);
     int blocks = (int)((n + 255) / 256);
+    if (F.nframes > 1) {                                         // one launch for the plane in every frame
+        const int cap = (132 * 8 + F.nframes - 1) / F.nframes;
+        k_step_uncovered<true><<<dim3(blocks < cap ? blocks : cap, 1, F.nframes), 256, 0, s>>>(F, c, factor);
+        return cudaGetLastError();
+    }
     if (blocks > 132 * 8) blocks = 132 * 8;
-    k_step_uncovered<<<blocks, 256, 0, s>>>(F, c, factor);
+    k_step_uncovered<false><<<blocks, 256, 0, s>>>(F, c, factor);
     return cudaGetLastError();
 }
 
@@ -274,10 +303,13 @@ int project_tile_border_units(const PlaneDev &P) { return ((P.cw >> 3) + PT_NB -
 cudaError_t launch_project_tile(const FrameDev &F, int c, int count, float factor, cudaStream_t s, int *nlaunch, bool uncovered_only) {
     const PlaneDev &P = F.pl[c];
     const int bw = P.cw >> 3, bh = P.ch >> 3;
-    const dim3 grid((bw + PT_NB - 1) / PT_NB, bh, count);
+    const dim3 grid((bw + PT_NB - 1) / PT_NB, bh, count * F.nframes);
     cudaError_t e = cudaSuccess;
-    if (!uncovered_only) {
-        e = P.resample ? launch_chain(k_project_tile<true>, grid, dim3(PT_NT), 0, s, F, c, factor) : launch_chain(k_project_tile<false>, grid, dim3(PT_NT), 0, s, F, c, factor);
+    if (!uncovered_only && F.nframes > 1) {
+        e = P.resample ? launch_chain(k_project_tile<true, true>, grid, dim3(PT_NT), 0, s, F, c, factor) : launch_chain(k_project_tile<false, true>, grid, dim3(PT_NT), 0, s, F, c, factor);
+        *nlaunch += 1;
+    } else if (!uncovered_only) {
+        e = P.resample ? launch_chain(k_project_tile<true, false>, grid, dim3(PT_NT), 0, s, F, c, factor) : launch_chain(k_project_tile<false, false>, grid, dim3(PT_NT), 0, s, F, c, factor);
         *nlaunch += 1;
     }
     for (int k = c; k < c + count && e == cudaSuccess; k++)

@@ -32,6 +32,8 @@ constexpr size_t P22_SMEM = (size_t)3 * 16 * P22_C4 * sizeof(float4)      // x_k
                             + (size_t)P22_NB * TILE_STRIDE * sizeof(float) // transpose tiles
                             + 3 * 64 * sizeof(float) + 4 * sizeof(float);  // tables, norm
 
+// BATCH: a batch session (FrameDev::nframes); blockIdx.z = frame * count + k for planes c0 + k.
+template <bool BATCH>
 __global__ void __launch_bounds__(P22_NT, 3) k_project_tile22(const __grid_constant__ FrameDev F, const int c0, const float factor) {
     extern __shared__ __align__(16) unsigned char smem22[];
     float4 *sx = reinterpret_cast<float4 *>(smem22);                 // [16][P22_C4]  x_k  -> later x_{k+1}
@@ -43,8 +45,11 @@ __global__ void __launch_bounds__(P22_NT, 3) k_project_tile22(const __grid_const
     float *snorm = sq + 3 * 64;                                      // [2]
 
     const int tid = threadIdx.x;
-    const int c = c0 + blockIdx.z;                                   // planes of equal geometry share one launch
+    const int count = BATCH ? (int)gridDim.z / F.nframes : 1;
+    const int frame = BATCH ? (int)blockIdx.z / count : 0;
+    const int c = c0 + (int)blockIdx.z - frame * count;              // planes of equal geometry share one launch
     const PlaneDev &P = F.pl[c];
+    const size_t fo = BATCH ? (size_t)frame * F.frame_stride : 0;
     const int W = F.W;
     const int bw = P.cw >> 3;
     const int bx0 = blockIdx.x * P22_NB, by = strip_row_order(F.sync, blockIdx.y, gridDim.y);   // the grid covers real blocks only
@@ -62,8 +67,8 @@ __global__ void __launch_bounds__(P22_NT, 3) k_project_tile22(const __grid_const
         if (c4 < valid_c4) {
             const size_t gi = row0 + (size_t)row * W + (size_t)c4 * 4;
             const int pc = row * P22_C4 + (c4 ^ ((row >> 1) & 7));
-            cp_async16(&sx[pc], P.x + gi);
-            cp_async16(&sp[pc], P.xp + gi);
+            cp_async16(&sx[pc], P.x + fo + gi);
+            cp_async16(&sp[pc], P.xp + fo + gi);
         }
     }
     pdl_wait();                                                      // the gradient and its norm are complete and visible
@@ -71,19 +76,33 @@ __global__ void __launch_bounds__(P22_NT, 3) k_project_tile22(const __grid_const
 #pragma unroll
     for (int i = 0; i < 16 * P22_C4 / P22_NT; i++) {
         const int e = tid + P22_NT * i, row = e / P22_C4, c4 = e % P22_C4;
-        if (c4 < valid_c4) cp_async16(&sg[row * P22_C4 + (c4 ^ ((row >> 1) & 7))], P.g + row0 + (size_t)row * W + (size_t)c4 * 4);
+        if (c4 < valid_c4) cp_async16(&sg[row * P22_C4 + (c4 ^ ((row >> 1) & 7))], P.g + fo + row0 + (size_t)row * W + (size_t)c4 * 4);
     }
     cp_async_commit();
     const int b = tid >> 3, j = tid & 7;
     const bool real = b < nbx;
     int4 draw = make_int4(0, 0, 0, 0);
-    if (real) draw = __ldg(reinterpret_cast<const int4 *>(P.data + ((size_t)(by * bw + bx0 + b) * 64 + j * 8)));
+    if (real) draw = __ldg(reinterpret_cast<const int4 *>(P.data + (BATCH ? (size_t)frame * F.data_stride : 0) + ((size_t)(by * bw + bx0 + b) * 64 + j * 8)));
     if (tid < 64) {
-        sq[tid] = F.q[c][tid];
-        sq[64 + tid] = F.qq[c][tid];
-        sq[128 + tid] = F.rqq[c][tid];
+        if (BATCH) {                                                 // this frame's tables (device copy)
+            const float *t = F.tables + ((size_t)frame * F.nc + c) * 192;
+            sq[tid] = t[tid];
+            sq[64 + tid] = t[64 + tid];
+            sq[128 + tid] = t[128 + tid];
+        } else {
+            sq[tid] = F.q[c][tid];
+            sq[64 + tid] = F.qq[c][tid];
+            sq[128 + tid] = F.rqq[c][tid];
+        }
     }
-    if (tid >= 64 && tid < 96) strip_norm(F, c, snorm, tid - 64);    // whole frame: what k_gradient left; strips: fold of every rank's sums
+    if (BATCH) {
+        if (tid == 64) {                                             // what k_gradient left for this frame
+            snorm[0] = F.norms[16 * frame + c];
+            snorm[1] = F.norms[16 * frame + 4 + c];
+        }
+    } else if (tid >= 64 && tid < 96) {
+        strip_norm(F, c, snorm, tid - 64);                           // whole frame: what k_gradient left; strips: fold of every rank's sums
+    }
     cp_async_wait<0>();
     __syncthreads();
 
@@ -215,10 +234,10 @@ __global__ void __launch_bounds__(P22_NT, 3) k_project_tile22(const __grid_const
     for (int i = 0; i < 16 * P22_C4 / P22_NT; i++) {
         const int e = tid + P22_NT * i, row = e / P22_C4, c4 = e % P22_C4;
         if (c4 < valid_c4)
-            *reinterpret_cast<float4 *>(P.xp + row0 + (size_t)row * W + (size_t)c4 * 4) = sx[row * P22_C4 + (c4 ^ ((row >> 1) & 7))];
+            *reinterpret_cast<float4 *>(P.xp + fo + row0 + (size_t)row * W + (size_t)c4 * 4) = sx[row * P22_C4 + (c4 ^ ((row >> 1) & 7))];
     }
     if (use_prob) {
-        float *gp0 = P.gp + (size_t)(by * 8) * P.cw + (size_t)bx0 * 8;
+        float *gp0 = P.gp + fo + (size_t)(by * 8) * P.cw + (size_t)bx0 * 8;
 #pragma unroll
         for (int i = 0; i < 8 * P22_G4 / P22_NT; i++) {
             const int e = tid + P22_NT * i, row = e / P22_G4, c4 = e % P22_G4;
@@ -228,7 +247,7 @@ __global__ void __launch_bounds__(P22_NT, 3) k_project_tile22(const __grid_const
 
     // ---- strips over peer memory: border rows into the neighbours' halo rows (kernels_project_tile.cu)
     const StripSync &S = F.sync;
-    if (S.nranks > 1 && S.fused_halo) {
+    if (!BATCH && S.nranks > 1 && S.fused_halo) {
         const bool top = by == 0 && S.has_up, bottom = by == (int)gridDim.y - 1 && S.has_down;
         if (top || bottom) {
             for (int e = tid; e < 4 * P22_C4; e += P22_NT) {             // 2 rows x 64 pieces, top then bottom
@@ -244,14 +263,20 @@ __global__ void __launch_bounds__(P22_NT, 3) k_project_tile22(const __grid_const
     }
 }
 
-// frame pixels of a 2x2 plane beyond its coefficient grid (W > 2 cw or H > 2 ch): step only
+// frame pixels of a 2x2 plane beyond its coefficient grid (W > 2 cw or H > 2 ch): step only.
+// BATCH: the frame is blockIdx.z.
+template <bool BATCH>
 __global__ void k_step_uncovered22(const __grid_constant__ FrameDev F, const int c, const float factor) {
     const PlaneDev &P = F.pl[c];
     const int W = F.W, H = F.H, cwf = 2 * P.cw, chf = 2 * P.ch;
+    const int frame = BATCH ? (int)blockIdx.z : 0;
+    const size_t fo = BATCH ? (size_t)frame * F.frame_stride : 0;
+    const float *const xk = P.x + fo, *const gk = P.g + fo;
+    float *const xm = P.xp + fo;
     Stepper stepper;
     stepper.factor = factor;
     stepper.step = F.step;
-    stepper.norm = F.norms[c];
+    stepper.norm = F.norms[16 * frame + c];
     stepper.rn = 0.f;
     stepper.stepping = stepper.norm != 0.f;
     const unsigned bottom = (unsigned)(H - chf) * (unsigned)W, right_w = (unsigned)(W - cwf);
@@ -267,12 +292,13 @@ __global__ void k_step_uncovered22(const __grid_constant__ FrameDev F, const int
             px = (unsigned)cwf + k % right_w;
         }
         const size_t gi = (size_t)py * W + px;
-        P.xp[gi] = stepper(P.x[gi], P.xp[gi], P.g[gi]);
+        xm[gi] = stepper(xk[gi], xm[gi], gk[gi]);
     }
 }
 
 cudaError_t configure_project_tile22() {
-    return cudaFuncSetAttribute(k_project_tile22, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)P22_SMEM);
+    const cudaError_t e = cudaFuncSetAttribute(k_project_tile22<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)P22_SMEM);
+    return e != cudaSuccess ? e : cudaFuncSetAttribute(k_project_tile22<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)P22_SMEM);
 }
 
 // F: already restricted to the rows the session owns (launch_project).  Projects planes
@@ -280,16 +306,23 @@ cudaError_t configure_project_tile22() {
 cudaError_t launch_project_tile22(const FrameDev &F, int c, int count, float factor, cudaStream_t s, int *nlaunch) {
     const PlaneDev &P = F.pl[c];
     const int bw = P.cw >> 3, bh = P.ch >> 3;
-    const dim3 grid((bw + P22_NB - 1) / P22_NB, bh, count);
-    cudaError_t e = launch_chain(k_project_tile22, grid, dim3(P22_NT), P22_SMEM, s, F, c, factor);
+    const bool batch = F.nframes > 1;
+    const dim3 grid((bw + P22_NB - 1) / P22_NB, bh, count * F.nframes);
+    cudaError_t e = batch ? launch_chain(k_project_tile22<true>, grid, dim3(P22_NT), P22_SMEM, s, F, c, factor)
+                          : launch_chain(k_project_tile22<false>, grid, dim3(P22_NT), P22_SMEM, s, F, c, factor);
     *nlaunch += 1;
     for (int k = c; k < c + count && e == cudaSuccess; k++) {
         const PlaneDev &Q = F.pl[k];
         if (2 * Q.cw < F.W || 2 * Q.ch < F.H) {
             const size_t n = (size_t)(F.H - 2 * Q.ch) * F.W + (size_t)2 * Q.ch * (F.W - 2 * Q.cw);
             int blocks = (int)((n + 255) / 256);
-            if (blocks > 132 * 8) blocks = 132 * 8;
-            k_step_uncovered22<<<blocks, 256, 0, s>>>(F, k, factor);
+            if (batch) {                                             // one launch for the plane in every frame
+                const int cap = (132 * 8 + F.nframes - 1) / F.nframes;
+                k_step_uncovered22<true><<<dim3(blocks < cap ? blocks : cap, 1, F.nframes), 256, 0, s>>>(F, k, factor);
+            } else {
+                if (blocks > 132 * 8) blocks = 132 * 8;
+                k_step_uncovered22<false><<<blocks, 256, 0, s>>>(F, k, factor);
+            }
             e = cudaGetLastError();
             *nlaunch += 1;
         }

@@ -12,6 +12,12 @@
 //   data    ch*cw i16  quantised coefficients (read-only)
 //   fdata0  ch*cw fp32 conventional decode (kept so a session can be re-armed without host I/O)
 // plus per session: partials [3][grad_ctas] fp64, norms [3] fp32, one ticket counter.
+//
+// A batch session (j2p_session_create_batch) holds N frames of one geometry.  Frame f's x, xp, g,
+// gp are the slab of one frame repeated at a fixed frame stride; data and fdata0 likewise, each in
+// one block; partials [frame][5][grad_ctas], norms [frame][16], sums [frame][4], counters [frame];
+// the quantisation tables in device memory as [frame][nc][3][64].  An iteration is the launches of
+// a single-frame session, each covering every frame (kernels.cuh, FrameDev::nframes).
 #include <cuda_runtime.h>
 
 #include <math.h>
@@ -179,9 +185,15 @@ struct j2p_session {
     TileMaps maps;                    // TMA descriptors of the plane buffers (tma_maps.h)
     float *slab = nullptr;            // x, xp, g, gp of every plane (see create_impl)
     size_t slab_bytes = 0;
-    float *x[3] = {}, *xp[3] = {}, *g[3] = {}, *gp[3] = {}, *fdata0[3] = {};
+    float *x[3] = {}, *xp[3] = {}, *g[3] = {}, *gp[3] = {}, *fdata0[3] = {};   // frame 0's planes
     int16_t *data[3] = {};
-    bool uploaded[3] = {};
+    unsigned nframes = 1;             // frames of a batch session (1: an ordinary session)
+    size_t fdata_stride = 0;          // elements from one frame's fdata0 planes to the next frame's
+    std::vector<float> tables;        // host copy of the tables, [frame][nc][3][64]: q, q*q, RN(1/(q*q))
+    float *dev_tables = nullptr;      // batch sessions: the device copy the kernels read
+    bool tables_stale = false;        // tables changed since the last device copy
+    bool stale = false;               // batch sessions: planes uploaded since the last re-arm
+    std::vector<char> uploaded;       // per plane = frame * nchannel + channel
     bool strip = false;       // row strip of a larger frame (multi-GPU tiling)
     bool ipc_exported = false; // peers hold cudaIpc mappings of this session's plane buffers: never recycle them
     float pending_factor = 0.f;
@@ -271,7 +283,12 @@ extern "C" int j2p_thread_device(void) {
 extern "C" unsigned j2p_session_width(const j2p_session *s) { return s ? (unsigned)s->F.W : 0; }
 extern "C" unsigned j2p_session_height(const j2p_session *s) { return s ? (unsigned)s->F.Hg : 0; }
 extern "C" void *j2p_session_stream(j2p_session *s) { return s ? (void *)s->stream : nullptr; }
-extern "C" void *j2p_session_plane_ptr(j2p_session *s, unsigned c) { return (s && c < (unsigned)s->F.nc) ? s->F.pl[c].x : nullptr; }
+static float *plane_x(j2p_session *s, unsigned plane);
+extern "C" void *j2p_session_plane_ptr(j2p_session *s, unsigned plane) {
+    float *x = s ? plane_x(s, plane) : nullptr;
+    if (s && !x) fail(J2P_ERR_ARG, "plane %u out of range (%zu planes)", plane, s->uploaded.size());
+    return x;
+}
 extern "C" unsigned long long j2p_session_launches(const j2p_session *s) { return s ? s->launches : 0; }
 
 extern "C" void j2p_session_destroy(j2p_session *s) {
@@ -291,7 +308,7 @@ extern "C" void j2p_session_destroy(j2p_session *s) {
 }
 
 // row0/rows select a horizontal strip of the frame (frame rows); rows == 0 means the whole frame.
-static int create_impl(j2p_session *s, int device, const j2p_frame_desc *d, unsigned row0, unsigned rows) {
+static int create_impl(j2p_session *s, int device, const j2p_frame_desc *d, unsigned row0, unsigned rows, unsigned nframes) {
     const int ndev = j2p_device_count();
     if (ndev <= 0) return fail(J2P_ERR_NODEVICE, "no CUDA device available (the solver has no CPU fallback)");
     if (device < 0 || device >= ndev) return fail(J2P_ERR_ARG, "device %d out of range (0..%d)", device, ndev - 1);
@@ -363,12 +380,42 @@ static int create_impl(j2p_session *s, int device, const j2p_frame_desc *d, unsi
     // The gradient kernel addresses an array from one lane pointer plus c * PS (FrameDev::
     // plane_stride), and a strip session exports ONE cudaIpc handle.
     const size_t PS = (n + 63) & ~(size_t)63;                            // 256-byte aligned planes
-    const size_t slab_elems = PS * 4 * d->nchannel;
+    const size_t slab_elems = PS * 4 * d->nchannel;                      // one frame
     if (slab_elems > 0xffffffffull) return fail(J2P_ERR_ARG, "frame %ux%u too large for 32-bit element offsets", W, H);
-    CK(dev_alloc(s, &s->slab, slab_elems * sizeof(float)));
-    s->slab_bytes = slab_elems * sizeof(float);
+    CK(dev_alloc(s, &s->slab, slab_elems * sizeof(float) * nframes));
+    s->slab_bytes = slab_elems * sizeof(float) * nframes;
     F.slab = s->slab;
     F.plane_stride = (unsigned)PS;
+    s->nframes = nframes;
+    F.nframes = (int)nframes;
+    F.frame_stride = slab_elems;
+    // coefficients and the conventional decode: every plane of every frame in one block each, planes
+    // 256-byte aligned
+    size_t at_data[3], at_fd[3], data_elems = 0, fd_elems = 0;
+    for (unsigned c = 0; c < d->nchannel; c++) {
+        const unsigned cy0 = row0 / d->h_samp[c];
+        unsigned cy1 = (row0 + rows + d->h_samp[c] - 1) / d->h_samp[c];
+        if (cy1 > d->plane_h[c]) cy1 = d->plane_h[c];
+        const size_t nc = (size_t)d->plane_w[c] * (cy1 - cy0);
+        at_data[c] = data_elems;
+        at_fd[c] = fd_elems;
+        data_elems += (nc + 127) & ~(size_t)127;
+        fd_elems += (nc + 63) & ~(size_t)63;
+    }
+    F.data_stride = data_elems;
+    s->fdata_stride = fd_elems;
+    int16_t *data_blk = nullptr;
+    float *fd_blk = nullptr;
+    CK(dev_alloc(s, &data_blk, data_elems * sizeof(int16_t) * nframes));
+    CK(dev_alloc(s, &fd_blk, fd_elems * sizeof(float) * nframes));
+    s->tables.assign((size_t)nframes * d->nchannel * 192, 0.f);
+    s->uploaded.assign((size_t)nframes * d->nchannel, 0);
+    F.tables = nullptr;
+    F.host_tables = s->tables.data();
+    if (nframes > 1) {
+        CK(dev_alloc(s, &s->dev_tables, s->tables.size() * sizeof(float)));
+        F.tables = s->dev_tables;
+    }
     size_t at_x[3], at_xp[3], at_g[3], at_gp[3];
     for (unsigned c = 0; c < d->nchannel; c++) {
         at_x[c] = PS * (0 * d->nchannel + c);
@@ -388,18 +435,17 @@ static int create_impl(j2p_session *s, int device, const j2p_frame_desc *d, unsi
         P.use_prob = d->pweight[c] != 0.f;                              // compute.c:244
         P.p_alpha = d->pweight[c] * 2 * 255 * sqrtf(2);                 // compute.c:245
         P.cnt = (float)(d->w_samp[c] * d->h_samp[c]);                   // compute.c:359
-        const size_t nc = (size_t)P.cw * P.ch;
         s->x[c] = s->slab + at_x[c];
         s->xp[c] = s->slab + at_xp[c];
         s->g[c] = s->slab + at_g[c];
         s->gp[c] = s->slab + at_gp[c];
-        CK(dev_alloc(s, &s->fdata0[c], nc * sizeof(float)));
-        CK(dev_alloc(s, &s->data[c], nc * sizeof(int16_t)));
+        s->fdata0[c] = fd_blk + at_fd[c];
+        s->data[c] = data_blk + at_data[c];
         P.x = s->x[c]; P.xp = s->xp[c]; P.g = s->g[c]; P.gp = s->gp[c]; P.data = s->data[c];
     }
     // tensor maps for the TMA-fed projection: the two iterate buffers and the gradient of every plane
     // that has a tiled projection kernel; a driver without the entry point leaves the cp.async kernels
-    bool maps_ok = true;
+    bool maps_ok = nframes == 1;                                        // a batch always takes the cp.async kernels
     for (unsigned c = 0; c < d->nchannel && maps_ok; c++) {
         const bool p11 = d->w_samp[c] == 1 && d->h_samp[c] == 1, p22 = d->w_samp[c] == 2 && d->h_samp[c] == 2;
         if (!p11 && !p22) continue;
@@ -413,16 +459,16 @@ static int create_impl(j2p_session *s, int device, const j2p_frame_desc *d, unsi
     F.buf_sel = 0;
     F.grad_ctas = grad_cta_count(F.W, F.t1 - F.t0);
     F.grad_slots = g_cfg_slots[device];
-    CK(dev_alloc(s, &F.partials, sizeof(double) * 5 * (size_t)F.grad_ctas));
-    CK(dev_alloc(s, &F.norms, sizeof(float) * 16));     // [0..2] norms, [4..6] reciprocals, [8..10] strip sequence numbers
-    CK(dev_alloc(s, &F.sums, sizeof(double) * 4));
+    CK(dev_alloc(s, &F.partials, sizeof(double) * 5 * (size_t)F.grad_ctas * nframes));
+    CK(dev_alloc(s, &F.norms, sizeof(float) * 16 * nframes));     // per frame: [0..2] norms, [4..6] reciprocals, [8..10] strip sequence numbers
+    CK(dev_alloc(s, &F.sums, sizeof(double) * 4 * nframes));
     CK(dev_alloc(s, &F.logsums, sizeof(double) * 8));
     CK(cudaMemsetAsync(F.logsums, 0, sizeof(double) * 8, s->stream));
     F.log_on = 0;
     F.log_slot = 0;
-    CK(dev_alloc(s, &F.counter, sizeof(unsigned)));
-    CK(cudaMemsetAsync(F.counter, 0, sizeof(unsigned), s->stream));
-    CK(cudaMemsetAsync(F.norms, 0, sizeof(float) * 16, s->stream));
+    CK(dev_alloc(s, &F.counter, sizeof(unsigned) * nframes));
+    CK(cudaMemsetAsync(F.counter, 0, sizeof(unsigned) * nframes, s->stream));
+    CK(cudaMemsetAsync(F.norms, 0, sizeof(float) * 16 * nframes, s->stream));
     return J2P_OK;
 }
 
@@ -430,12 +476,12 @@ extern "C" int j2p_session_create(j2p_session **out, int device, const struct j2
     return j2p_session_create_strip(out, device, d, 0, 0);
 }
 
-extern "C" int j2p_session_create_strip(j2p_session **out, int device, const struct j2p_frame_desc *d, unsigned row0,
-                                        unsigned rows) {
+static int create_session(j2p_session **out, int device, const struct j2p_frame_desc *d, unsigned row0, unsigned rows,
+                          unsigned nframes) {
     if (!out || !d) return fail(J2P_ERR_ARG, "null argument");
     *out = nullptr;
     j2p_session *s = new j2p_session();
-    const int rc = create_impl(s, device, d, row0, rows);
+    const int rc = create_impl(s, device, d, row0, rows, nframes);
     if (rc != J2P_OK) {
         char keep[sizeof g_err];
         memcpy(keep, g_err, sizeof keep);
@@ -448,21 +494,53 @@ extern "C" int j2p_session_create_strip(j2p_session **out, int device, const str
     return J2P_OK;
 }
 
+extern "C" int j2p_session_create_strip(j2p_session **out, int device, const struct j2p_frame_desc *d, unsigned row0,
+                                        unsigned rows) {
+    return create_session(out, device, d, row0, rows, 1);
+}
+
+extern "C" int j2p_session_create_batch(j2p_session **out, int device, const struct j2p_frame_desc *d, unsigned nframes) {
+    if (out) *out = nullptr;
+    if (nframes == 0) return fail(J2P_ERR_ARG, "a batch needs at least one frame");
+    if (nframes > 65535) return fail(J2P_ERR_ARG, "a batch holds at most 65535 frames (%u requested)", nframes);
+    return create_session(out, device, d, 0, 0, nframes);
+}
+
+extern "C" unsigned j2p_session_frames(const j2p_session *s) { return s ? s->nframes : 0; }
+
+// strip entry points: refused on a batch of more than one frame
+static int refuse_batch(const j2p_session *s, const char *what) {
+    return fail(J2P_ERR_ARG, "%s is not available on a batch session (%u frames)", what, s->nframes);
+}
+
 static int reset_impl(j2p_session *s) {
     FrameDev &F = s->F;
+    for (size_t k = 0; k < s->uploaded.size(); k++)
+        if (!s->uploaded[k]) return fail(J2P_ERR_ARG, "plane %zu (frame %zu, channel %zu) has not been uploaded", k, k / F.nc, k % F.nc);
+    F.buf_sel = 0;
     for (int c = 0; c < F.nc; c++) {
-        if (!s->uploaded[c]) return fail(J2P_ERR_ARG, "plane %d has not been uploaded", c);
         PlaneDev &P = F.pl[c];
         P.x = s->x[c];
         P.xp = s->xp[c];
-        F.buf_sel = 0;
-        // owned rows only; a strip's halo rows are filled by the driver's first halo exchange
-        const size_t off = (size_t)F.t0 * F.W;
-        CK(launch_init_plane(s->fdata0[c], P.x + off, P.xp + off, F.W, F.t1 - F.t0, P.cw, P.ch, P.sw, P.sh, s->stream));
-        s->launches++;
-        // first step: cos == data*q exactly, so the DCT-distance gradient is exactly 0 (compute.c:283 vs :47)
-        CK(cudaMemsetAsync(P.gp, 0, (size_t)P.cw * P.ch * sizeof(float), s->stream));
     }
+    for (unsigned f = 0; f < s->nframes; f++) {
+        const size_t fo = (size_t)f * F.frame_stride;
+        for (int c = 0; c < F.nc; c++) {
+            PlaneDev &P = F.pl[c];
+            // owned rows only; a strip's halo rows are filled by the driver's first halo exchange
+            const size_t off = (size_t)F.t0 * F.W;
+            CK(launch_init_plane(s->fdata0[c] + f * s->fdata_stride, P.x + fo + off, P.xp + fo + off, F.W, F.t1 - F.t0, P.cw, P.ch, P.sw,
+                                 P.sh, s->stream));
+            s->launches++;
+            // first step: cos == data*q exactly, so the DCT-distance gradient is exactly 0 (compute.c:283 vs :47)
+            CK(cudaMemsetAsync(P.gp + fo, 0, (size_t)P.cw * P.ch * sizeof(float), s->stream));
+        }
+    }
+    if (s->dev_tables && s->tables_stale) {     // pageable source: the copy has read it when the call returns
+        CK(cudaMemcpyAsync(s->dev_tables, s->tables.data(), s->tables.size() * sizeof(float), cudaMemcpyHostToDevice, s->stream));
+        s->tables_stale = false;
+    }
+    s->stale = false;
     s->t = 1.f;
     s->next_iter = 0;
     for (int i = 0; i < kEventRing; i++) s->ev_iter[i] = -1;            // events of an earlier solve say nothing about this one
@@ -583,32 +661,50 @@ static int staged_d2h(j2p_session *s, void *dst, const void *src, size_t bytes) 
     return J2P_OK;
 }
 
-extern "C" int j2p_session_upload(j2p_session *s, unsigned c, const int16_t *data, const uint16_t *quant,
+// `plane` = frame * nchannel + channel (an ordinary session: the channel)
+extern "C" int j2p_session_upload(j2p_session *s, unsigned plane, const int16_t *data, const uint16_t *quant,
                                   const float *fdata) {
     if (!s || !data || !quant) return fail(J2P_ERR_ARG, "null argument");
-    if (c >= (unsigned)s->F.nc) return fail(J2P_ERR_ARG, "channel %u out of range", c);
+    if (plane >= s->uploaded.size()) return fail(J2P_ERR_ARG, "plane %u out of range (%zu planes)", plane, s->uploaded.size());
     CK(cudaSetDevice(s->device));
     FrameDev &F = s->F;
+    const unsigned f = plane / (unsigned)F.nc, c = plane % (unsigned)F.nc;
     PlaneDev &P = F.pl[c];
     const size_t nc = (size_t)P.cw * P.ch;
-    for (int j = 0; j < 64; j++) {
+    float *tab = s->tables.data() + (size_t)plane * 192;                // q, qq, rqq of this frame and plane
+    for (int j = 0; j < 64; j++)
         if (quant[j] == 0) return fail(J2P_ERR_ARG, "invalid quantization table (zero entry, jpeg.c:41-45)");
-        F.q[c][j] = (float)quant[j];
-        F.qq[c][j] = F.q[c][j] * F.q[c][j];                             // fp32 product (compute.c:49)
-        F.rqq[c][j] = (float)(1.0 / (double)F.qq[c][j]);                // RN(1/qq): fp64 quotient narrowed once is correctly rounded
+    for (int j = 0; j < 64; j++) {
+        tab[j] = (float)quant[j];
+        tab[64 + j] = tab[j] * tab[j];                                  // fp32 product (compute.c:49)
+        tab[128 + j] = (float)(1.0 / (double)tab[64 + j]);              // RN(1/qq): fp64 quotient narrowed once is correctly rounded
+        if (f == 0) {                                                   // what the single-frame kernels read
+            F.q[c][j] = tab[j];
+            F.qq[c][j] = tab[64 + j];
+            F.rqq[c][j] = tab[128 + j];
+        }
     }
-    int rcs = staged_h2d(s, s->data[c], data, nc * sizeof(int16_t));
+    s->tables_stale = true;
+    int16_t *ddst = s->data[c] + (size_t)f * F.data_stride;
+    float *fdst = s->fdata0[c] + (size_t)f * s->fdata_stride;
+    int rcs = staged_h2d(s, ddst, data, nc * sizeof(int16_t));
     if (rcs != J2P_OK) return rcs;
     if (fdata) {
-        rcs = staged_h2d(s, s->fdata0[c], fdata, nc * sizeof(float));
+        rcs = staged_h2d(s, fdst, fdata, nc * sizeof(float));
         if (rcs != J2P_OK) return rcs;
     } else {
-        CK(launch_decode(s->data[c], F.q[c], s->fdata0[c], P.cw, P.ch, s->stream));
+        CK(launch_decode(ddst, tab, fdst, P.cw, P.ch, s->stream));
         s->launches++;
     }
     // The host arrays have been read completely (they sit in the pinned ring or on the device);
     // the stream is NOT drained here, so the next plane's host copy overlaps this plane's DMA.
-    s->uploaded[c] = true;
+    s->uploaded[plane] = 1;
+    // A batch is re-armed once, by the first iterate (or reset) after its uploads: re-arming after
+    // every plane would cost nframes * nchannel resets per solve.
+    if (s->nframes > 1) {
+        s->stale = true;
+        return J2P_OK;
+    }
     bool all = true;
     for (int k = 0; k < F.nc; k++) all = all && s->uploaded[k];
     if (all) return reset_impl(s);
@@ -644,9 +740,9 @@ static int one_iteration(j2p_session *s, cudaEvent_t e0, cudaEvent_t e1, cudaEve
 }
 
 static int check_ready(j2p_session *s, unsigned first) {
-    for (int c = 0; c < s->F.nc; c++)
-        if (!s->uploaded[c]) return fail(J2P_ERR_ARG, "plane %d has not been uploaded", c);
-    if (first == 0 && s->next_iter != 0) {
+    for (size_t k = 0; k < s->uploaded.size(); k++)
+        if (!s->uploaded[k]) return fail(J2P_ERR_ARG, "plane %zu has not been uploaded", k);
+    if ((first == 0 && s->next_iter != 0) || s->stale) {
         const int rc = reset_impl(s);
         if (rc != J2P_OK) return rc;
     }
@@ -657,6 +753,7 @@ static int check_ready(j2p_session *s, unsigned first) {
 // ---- strip sessions: one iteration in two halves, the driver combines sums and exchanges halos ----
 extern "C" int j2p_session_gradient(j2p_session *s) {
     if (!s) return fail(J2P_ERR_ARG, "null session");
+    if (s->nframes > 1) return refuse_batch(s, "j2p_session_gradient");
     CK(cudaSetDevice(s->device));
     for (int c = 0; c < s->F.nc; c++)
         if (!s->uploaded[c]) return fail(J2P_ERR_ARG, "plane %d has not been uploaded", c);
@@ -669,10 +766,17 @@ extern "C" int j2p_session_gradient(j2p_session *s) {
     return J2P_OK;
 }
 
-extern "C" void *j2p_session_sums_ptr(j2p_session *s) { return s ? (void *)s->F.sums : nullptr; }
+extern "C" void *j2p_session_sums_ptr(j2p_session *s) {
+    if (s && s->nframes > 1) {
+        refuse_batch(s, "j2p_session_sums_ptr");
+        return nullptr;
+    }
+    return s ? (void *)s->F.sums : nullptr;
+}
 
 extern "C" int j2p_session_project(j2p_session *s, const double *sums_by_rank, unsigned nranks) {
     if (!s || !sums_by_rank || nranks == 0) return fail(J2P_ERR_ARG, "bad argument");
+    if (s->nframes > 1) return refuse_batch(s, "j2p_session_project");
     CK(cudaSetDevice(s->device));
     FrameDev &F = s->F;
     CK(launch_fold_sums(sums_by_rank, (int)nranks, F.nc, F.norms, s->stream));
@@ -686,6 +790,7 @@ extern "C" int j2p_session_project(j2p_session *s, const double *sums_by_rank, u
 
 extern "C" int j2p_session_halo(j2p_session *s, unsigned c, int side, void **send, void **recv, size_t *count) {
     if (!s || !send || !recv || !count) return fail(J2P_ERR_ARG, "null argument");
+    if (s->nframes > 1) return refuse_batch(s, "j2p_session_halo");
     if (c >= (unsigned)s->F.nc || (side != 0 && side != 1)) return fail(J2P_ERR_ARG, "bad channel or side");
     const FrameDev &F = s->F;
     float *x = F.pl[c].x;
@@ -704,6 +809,7 @@ extern "C" int j2p_session_halo(j2p_session *s, unsigned c, int side, void **sen
 
 extern "C" int j2p_session_copy_halo_to_prev(j2p_session *s) {
     if (!s) return fail(J2P_ERR_ARG, "null session");
+    if (s->nframes > 1) return refuse_batch(s, "j2p_session_copy_halo_to_prev");
     CK(cudaSetDevice(s->device));
     const FrameDev &F = s->F;
     const size_t W = (size_t)F.W;
@@ -718,6 +824,7 @@ extern "C" int j2p_session_copy_halo_to_prev(j2p_session *s) {
 
 extern "C" int j2p_session_strip_info(const j2p_session *s, unsigned *local_rows, unsigned *first_owned, unsigned *owned_rows) {
     if (!s) return fail(J2P_ERR_ARG, "null session");
+    if (s->nframes > 1) return refuse_batch(s, "j2p_session_strip_info");
     if (local_rows) *local_rows = (unsigned)s->F.H;
     if (first_owned) *first_owned = (unsigned)s->F.t0;
     if (owned_rows) *owned_rows = (unsigned)(s->F.t1 - s->F.t0);
@@ -786,20 +893,34 @@ extern "C" int j2p_session_wait_iteration(j2p_session *s, unsigned iter) {
     return J2P_OK;
 }
 
-extern "C" int j2p_session_download(j2p_session *s, unsigned c, float *out) {
+// current iterate of `plane` = frame * nchannel + channel, or null when out of range
+static float *plane_x(j2p_session *s, unsigned plane) {
+    if (plane >= s->uploaded.size()) return nullptr;
+    const unsigned f = plane / (unsigned)s->F.nc, c = plane % (unsigned)s->F.nc;
+    return s->F.pl[c].x + (size_t)f * s->F.frame_stride;
+}
+
+extern "C" int j2p_session_download(j2p_session *s, unsigned plane, float *out) {
     if (!s || !out) return fail(J2P_ERR_ARG, "null argument");
-    if (c >= (unsigned)s->F.nc) return fail(J2P_ERR_ARG, "channel %u out of range", c);
+    float *x = plane_x(s, plane);
+    if (!x) return fail(J2P_ERR_ARG, "plane %u out of range (%zu planes)", plane, s->uploaded.size());
     CK(cudaSetDevice(s->device));
     // the rows this session owns (the whole frame, or the strip without its halo rows)
     const size_t n = (size_t)s->F.W * (size_t)(s->F.t1 - s->F.t0);
-    return staged_d2h(s, out, s->F.pl[c].x + (size_t)s->F.t0 * s->F.W, n * sizeof(float));
+    return staged_d2h(s, out, x + (size_t)s->F.t0 * s->F.W, n * sizeof(float));
 }
 
 // The reference's post-processing of a joint result (jpeg2png.c:156-159 luma += 128; png.c:39-62
 // YCbCr -> RGB, clamp, scale, truncate, 8 bit or 16 bit big-endian) on the device, delivered as PNG
 // scanlines: h rows of 1 + w*3*bits/8 bytes, each starting with filter type 0.
 extern "C" int j2p_session_download_scanlines(j2p_session *s, unsigned w, unsigned h, unsigned bits, unsigned char *out) {
+    return j2p_session_download_frame_scanlines(s, 0, w, h, bits, out);
+}
+
+extern "C" int j2p_session_download_frame_scanlines(j2p_session *s, unsigned frame, unsigned w, unsigned h, unsigned bits,
+                                                    unsigned char *out) {
     if (!s || !out) return fail(J2P_ERR_ARG, "null argument");
+    if (frame >= s->nframes) return fail(J2P_ERR_ARG, "frame %u out of range (%u frames)", frame, s->nframes);
     if (s->F.nc != 3 || s->strip) return fail(J2P_ERR_ARG, "scanlines need a whole-frame session with three planes (joint mode)");
     if (bits != 8 && bits != 16) return fail(J2P_ERR_ARG, "bits must be 8 or 16");
     if (w == 0 || h == 0 || w > (unsigned)s->F.W || h > (unsigned)s->F.H) return fail(J2P_ERR_ARG, "image %ux%u does not fit the %dx%d frame", w, h, s->F.W, s->F.H);
@@ -807,7 +928,8 @@ extern "C" int j2p_session_download_scanlines(j2p_session *s, unsigned w, unsign
     const size_t bytes = (size_t)h * ((size_t)w * 3 * (bits / 8) + 1);
     uint8_t *dev = nullptr;
     CK(dev_alloc(s, &dev, bytes));                   // returns to the device cache with the session
-    CK(launch_scanlines(s->F.pl[0].x, s->F.pl[1].x, s->F.pl[2].x, s->F.W, (int)w, (int)h, (int)bits, dev, s->stream));
+    const size_t fo = (size_t)frame * s->F.frame_stride;
+    CK(launch_scanlines(s->F.pl[0].x + fo, s->F.pl[1].x + fo, s->F.pl[2].x + fo, s->F.W, (int)w, (int)h, (int)bits, dev, s->stream));
     s->launches++;
     return staged_d2h(s, out, dev, bytes);
 }
@@ -822,6 +944,7 @@ extern "C" int j2p_session_sync(j2p_session *s) {
 extern "C" int j2p_session_set_logging(j2p_session *s, int enabled) {
     if (!s) return fail(J2P_ERR_ARG, "null session");
     if (enabled && s->strip) return fail(J2P_ERR_ARG, "objective logging is not available on strip sessions");
+    if (enabled && s->nframes > 1) return refuse_batch(s, "objective logging");
     s->logging = enabled != 0;
     s->F.log_on = s->logging;
     return J2P_OK;
@@ -1202,6 +1325,7 @@ static void fill_sync(j2p_session *s, j2p_comm *c) {
 // solver kernels, the exchanges happen inside them.  J2P_STRIP_P2P=0, or peers whose memory cannot
 // be mapped, fall back to ncclAllGather + ncclSend/ncclRecv between the kernels.
 extern "C" int j2p_session_iterate_strip(j2p_session *s, j2p_comm *c, unsigned n) {
+    if (s && s->nframes > 1) return refuse_batch(s, "j2p_session_iterate_strip");
     if (!s || !c) return fail(J2P_ERR_ARG, "null argument");
     const NcclApi *api = nccl_api();
     if (!api) return fail(J2P_ERR_NODEVICE, "libnccl.so.2 could not be loaded");
