@@ -50,6 +50,33 @@ def test_cli_png_matches_reference_pipeline(codecs, tmp_path, w, h, q, ss, prog,
     assert (got == want).all(), f'{int((got != want).sum())} of {got.size} samples differ'
 
 
+@pytest.mark.parametrize('w,h,sampling', [
+    (95, 33, [(2, 1), (1, 1), (1, 1)]),          # 4:2:2
+    (40, 72, [(1, 2), (1, 1), (1, 1)]),          # 4:4:0
+    (48, 40, [(4, 1), (2, 1), (1, 1)]),          # mixed factors: chroma planes with w_samp 2 and 4
+    (36, 40, [(4, 1), (2, 1), (1, 2)]),          # mixed factors: Cb a (2,2) plane narrower than the frame
+])
+@pytest.mark.parametrize('sep', [False, True])
+def test_cli_png_matches_reference_pipeline_for_more_layouts(codecs, tmp_path, w, h, sampling, sep):  # noqa: F811
+    """Files with known coefficients (tests/jpeg_synth.py) in the layouts the Pillow-written files
+    above do not have, joint and -s, against the checker pipeline."""
+    from tests import jpeg_synth
+    subprocess.run(['make', '-C', CLI_DIR, 'jpeg2png'], check=True, capture_output=True)
+    planes, quants = jpeg_synth.random_planes(w, h, sampling, seed=w * 7 + h)
+    data = jpeg_synth.encode_baseline(w, h, sampling, planes, quants)
+    src = tmp_path / 'in.jpg'
+    src.write_bytes(data)
+    args = ['-s', '-i', '9,7,5', '-w', '0.3,0.0,0.2'] if sep else ['-i', '9', '-w', '0.3']
+    r = subprocess.run([os.path.join(CLI_DIR, 'jpeg2png'), '-q', *args, str(src)], capture_output=True, text=True)
+    assert r.returncode == 0, r.stderr
+    got = np.asarray(Image.open(tmp_path / 'in.png'))
+    img, err = read_jpeg(codecs, data)
+    assert img is not None, err
+    want = expected_rgb(img, not sep, [9, 7, 5] if sep else [9] * 3, [0.3, 0.0, 0.2] if sep else [0.3] * 3, [0.001] * 3)
+    assert got.shape == want.shape
+    assert (got == want).all(), f'{int((got != want).sum())} of {got.size} samples differ'
+
+
 def test_cli_refuses_to_overwrite_and_logs_csv(codecs, tmp_path):  # noqa: F811
     subprocess.run(['make', '-C', CLI_DIR, 'jpeg2png'], check=True, capture_output=True)
     src = tmp_path / 'pic.jpeg'

@@ -139,6 +139,25 @@ def test_reference_simd_equals_scalar():
     check_reference('simd_vs_c/simd', solve('oracle', case), lambda: solve('ref', case))
 
 
+@pytest.mark.skipif(not H.have_ref(), reason='needs both reference builds under oracle/_ref')
+def test_tables_above_32767_follow_the_scalar_reference():
+    """The one place the reference's two builds disagree: its SIMD step converts the quantisation
+    tables with _mm_cvtpi16_ps (compute_simd_step.c:17, :160), a signed 16-bit conversion, so a
+    16-bit table entry above 32767 turns negative there.  The scalar build reads struct coef's
+    uint16_t, and so do the oracle and the library (tests/test_gpu_kernel_matrix.py, 'u16')."""
+    img = synth.random_coefs([(48, 32), (24, 16), (24, 16)], [(1, 1), (2, 2), (2, 2)], 5)
+    rng = np.random.default_rng(5)
+    for p in img.planes:
+        p.quant[:] = rng.integers(1, 65536, size=64).astype(np.uint16)
+        p.quant[0] = 65535
+    f = H.decode_planes(img)
+    args = (img, [0, 1, 2], 0.3, [0.001] * 3, 4)
+    want = H.run_compute('ref_c', *args, [p.copy() for p in f])
+    H.assert_bit_identical(H.run_compute('oracle', *args, [p.copy() for p in f]), want, 'oracle vs scalar reference')
+    simd = H.run_compute('ref', *args, [p.copy() for p in f])
+    assert any((H.bits(a) != H.bits(b)).any() for a, b in zip(simd, want)), 'the SIMD reference now reads the tables unsigned'
+
+
 @pytest.mark.parametrize('w,h,q,ss,channels,weight,pw,iters', CONFIGS)
 def test_oracle_matches_reference(w, h, q, ss, channels, weight, pw, iters):
     case = config_case(w, h, q, ss, channels, weight, pw, iters)
