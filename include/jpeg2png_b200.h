@@ -238,6 +238,43 @@ int j2p_session_download_scanlines(j2p_session *s, unsigned w, unsigned h, unsig
 int j2p_session_download_frame_scanlines(j2p_session *s, unsigned frame, unsigned w, unsigned h,
                                          unsigned bits, unsigned char *out);
 
+/* ---- export of the RGB image into caller-owned device memory (tensors) -------------------------
+ * The colour conversion of j2p_session_download_scanlines, written into `dst` on the device for
+ * frames [frame0, frame0 + nframes) of a session, nothing staged through the host.  Per sample,
+ * x = the YCbCr -> RGB expression in double on (luma + 128 in fp32), narrowed to float and clamped
+ * to [0, 255] (jpeg2png.c:156-159, png.c:39-47); then
+ *   sample 8:  uint8  trunc(x)          = the 8-bit PNG sample
+ *   sample 16: uint16 trunc(x * 256)    = the 16-bit PNG sample (-1), in native byte order
+ *   sample 32: float  x
+ * HWC: h rows of w pixels of 3 samples (R, G, B); CHW: the R plane, then G, then B, h x w each.
+ * Frame f of the export starts at dst + f * frame_bytes.
+ *
+ * Streams: `stream` (a cudaStream_t) NULL means the session stream (separate variant: the luma
+ * session's); the legacy default stream is named by cudaStreamLegacy.  For every session stream other than the launch stream the export waits for the work
+ * queued there so far, and that stream waits for the export: the export reads the planes of the
+ * solve queued before it, and a later upload / reset / iterate of the session cannot overwrite them
+ * first.  Asynchronous: the host never blocks.
+ *
+ * J2P_ERR_ARG: null dst or o, nframes == 0 or frames out of range, w or h 0 or larger than a plane's
+ * frame, unknown sample or layout, frame_bytes smaller than one image, a joint export of a session
+ * whose nchannel != 3, a strip session; separate sessions that do not have nchannel == 1, have
+ * different frame counts, or live on different devices. */
+enum { J2P_LAYOUT_HWC = 0, J2P_LAYOUT_CHW = 1 };
+struct j2p_image_out {
+        unsigned w, h;        /* visible image (struct j2p_jpeg w,h); <= every plane's frame  */
+        unsigned sample;      /* 8: uint8, 16: uint16 (native endian), 32: float             */
+        unsigned layout;      /* J2P_LAYOUT_HWC (interleaved) or J2P_LAYOUT_CHW (planar)      */
+        size_t frame_bytes;   /* distance between consecutive frames in dst, >= one image     */
+};
+/* joint (nchannel == 3) whole-frame sessions, single or batch */
+int j2p_session_export(j2p_session *s, unsigned frame0, unsigned nframes,
+                       const struct j2p_image_out *o, void *dst, void *stream);
+/* separate mode (-s): three nchannel == 1 sessions (Y, Cb, Cr) on one device with equal frame
+ * counts; each plane is read with its own session's frame size */
+int j2p_session_export_separate(j2p_session *y, j2p_session *cb, j2p_session *cr, unsigned frame0,
+                                unsigned nframes, const struct j2p_image_out *o, void *dst,
+                                void *stream);
+
 /* Objective terms of the most recent iteration, as logged by the reference (compute.c:271-272):
  * out[0]=objective, out[1]=prob_dist, out[2]=tv, out[3]=tv2.  Only tracked when logging was
  * enabled with j2p_session_set_logging(s, 1) before iterating. */

@@ -47,6 +47,15 @@ class FrameDesc(C.Structure):
                 ('pweight', C.c_float * 3), ('iterations', C.c_uint)]
 
 
+LAYOUT_HWC, LAYOUT_CHW = 0, 1       # J2P_LAYOUT_HWC / J2P_LAYOUT_CHW
+
+
+class ImageOut(C.Structure):
+    """struct j2p_image_out — include/jpeg2png_b200.h."""
+    _fields_ = [('w', C.c_uint), ('h', C.c_uint), ('sample', C.c_uint), ('layout', C.c_uint),
+                ('frame_bytes', C.c_size_t)]
+
+
 def alloc_floats(n: int) -> int:
     """16-byte aligned malloc-family buffer (reference alloc_simd, utils.h:89-98)."""
     nbytes = (max(n, 1) * 4 + 15) & ~15
@@ -135,6 +144,10 @@ def declare_product(lib: C.CDLL) -> C.CDLL:
     lib.j2p_session_frames.argtypes = [vp]
     lib.j2p_session_download_frame_scanlines.restype = C.c_int
     lib.j2p_session_download_frame_scanlines.argtypes = [vp, C.c_uint, C.c_uint, C.c_uint, C.c_uint, vp]
+    lib.j2p_session_export.restype = C.c_int
+    lib.j2p_session_export.argtypes = [vp, C.c_uint, C.c_uint, C.POINTER(ImageOut), vp, vp]
+    lib.j2p_session_export_separate.restype = C.c_int
+    lib.j2p_session_export_separate.argtypes = [vp, vp, vp, C.c_uint, C.c_uint, C.POINTER(ImageOut), vp, vp]
     lib.j2p_session_create_strip.restype = C.c_int
     lib.j2p_session_create_strip.argtypes = [C.POINTER(vp), C.c_int, C.POINTER(FrameDesc), C.c_uint, C.c_uint]
     lib.j2p_session_strip_info.restype = C.c_int
@@ -209,6 +222,7 @@ HEADER_SYMBOLS = [
     'j2p_session_objective', 'j2p_session_sync', 'j2p_session_stream', 'j2p_session_plane_ptr',
     'j2p_session_launches', 'j2p_version', 'j2p_host_prefault', 'j2p_set_thread_device', 'j2p_thread_device', 'j2p_session_download_scanlines',
     'j2p_session_create_batch', 'j2p_session_frames', 'j2p_session_download_frame_scanlines',
+    'j2p_session_export', 'j2p_session_export_separate',
 ]
 
 _product = None

@@ -114,6 +114,22 @@ inline FrameDev frame_view(const FrameDev &F, int f) {
     return V;
 }
 
+// ---- the colour epilogue (kernels_epilogue.cu, k_scanlines): YCbCr planes of `nframes` frames ->
+// RGB in one of three output forms.  Each plane has its own base, row stride and frame stride, so
+// the three planes may come from one joint session or from three separate-mode sessions whose
+// frames differ in size.
+enum EpilogueMode { EP_SCANLINES = 0, EP_HWC = 1, EP_CHW = 2 };
+struct EpilogueArgs {
+    const float *plane[3];               // frame 0's Y, Cb, Cr (current iterates)
+    unsigned long long frame_stride[3];  // elements from one frame's plane to the next frame's
+    int ld[3];                           // row stride of each plane, elements
+    int w, h;                            // visible image, at most every plane's frame
+    int mode;                            // EpilogueMode
+    int sample;                          // bits per sample: 8 or 16 (scanlines), 8, 16 or 32 (HWC / CHW)
+    unsigned long long frame_bytes;      // output bytes from one frame to the next
+    uint8_t *out;
+};
+
 // ---- the stand-alone halo kernel (kernels_strip.cu); pointers into OTHER ranks' memory are cudaIpc
 // mappings made by session.cu
 struct HaloPeers {

@@ -50,7 +50,7 @@ cudaError_t launch_init_plane(const float *fdata, float *x, float *xp, int W, in
 bool project_tma_enabled();
 int project_tma_border_units(const PlaneDev &P);
 int project_tile_border_units(const PlaneDev &P);
-cudaError_t launch_scanlines(const float *Y, const float *Cb, const float *Cr, int W, int w, int h, int bits, uint8_t *out, cudaStream_t s);
+cudaError_t launch_scanlines(const EpilogueArgs &a, int nframes, cudaStream_t s);
 // kernels_strip.cu: the strip exchanges over peer memory (parameter blocks in kernels.cuh)
 cudaError_t launch_halo_exchange(const HaloPeers &P, unsigned seq, unsigned *ticket, int *err, int wait_for_arrival, cudaStream_t s);
 }  // namespace j2p
@@ -210,6 +210,7 @@ struct j2p_session {
     void *stage[kStageSlots] = {};            // pinned staging ring (lazily taken from the process-wide pool)
     cudaEvent_t stage_ev[kStageSlots] = {};
     unsigned stage_next = 0;
+    cudaEvent_t export_ev = nullptr;          // orders j2p_session_export on a caller stream with the session stream
 };
 
 // x_k <-> x_{k-1} after an iteration (reference SWAP at compute.c:438); all planes together, which
@@ -303,6 +304,7 @@ extern "C" void j2p_session_destroy(j2p_session *s) {
         if (s->stage_ev[k]) cudaEventDestroy(s->stage_ev[k]);
         if (s->stage[k]) g_pinned.put(s->stage[k]);
     }
+    if (s->export_ev) cudaEventDestroy(s->export_ev);
     if (s->stream) cudaStreamDestroy(s->stream);
     delete s;
 }
@@ -928,10 +930,93 @@ extern "C" int j2p_session_download_frame_scanlines(j2p_session *s, unsigned fra
     const size_t bytes = (size_t)h * ((size_t)w * 3 * (bits / 8) + 1);
     uint8_t *dev = nullptr;
     CK(dev_alloc(s, &dev, bytes));                   // returns to the device cache with the session
-    const size_t fo = (size_t)frame * s->F.frame_stride;
-    CK(launch_scanlines(s->F.pl[0].x + fo, s->F.pl[1].x + fo, s->F.pl[2].x + fo, s->F.W, (int)w, (int)h, (int)bits, dev, s->stream));
+    EpilogueArgs a{};
+    for (int c = 0; c < 3; c++) {
+        a.plane[c] = plane_x(s, frame * 3 + (unsigned)c);
+        a.frame_stride[c] = s->F.frame_stride;
+        a.ld[c] = s->F.W;
+    }
+    a.w = (int)w;
+    a.h = (int)h;
+    a.mode = EP_SCANLINES;
+    a.sample = (int)bits;
+    a.frame_bytes = bytes;
+    a.out = dev;
+    CK(launch_scanlines(a, 1, s->stream));
     s->launches++;
     return staged_d2h(s, out, dev, bytes);
+}
+
+// ---- export into caller device memory: the colour epilogue with a tensor layout, on the caller's
+// stream, ordered after the solve that produced the planes and before anything later queued on a
+// session stream can overwrite them.  `ss`: one joint session, or the Y, Cb, Cr separate sessions.
+static int export_impl(j2p_session *const *ss, int nsess, unsigned frame0, unsigned nframes, const struct j2p_image_out *o, void *dst,
+                       void *stream) {
+    if (!o || !dst) return fail(J2P_ERR_ARG, "null argument");
+    j2p_session *s0 = ss[0];
+    if (nframes == 0) return fail(J2P_ERR_ARG, "nframes must be at least 1");
+    if (frame0 >= s0->nframes || nframes > s0->nframes - frame0)
+        return fail(J2P_ERR_ARG, "frames %u..%u out of range (%u frames)", frame0, frame0 + nframes, s0->nframes);
+    if (o->sample != 8 && o->sample != 16 && o->sample != 32) return fail(J2P_ERR_ARG, "sample must be 8, 16 or 32 (got %u)", o->sample);
+    if (o->layout != J2P_LAYOUT_HWC && o->layout != J2P_LAYOUT_CHW) return fail(J2P_ERR_ARG, "unknown layout %u", o->layout);
+    if (o->w == 0 || o->h == 0) return fail(J2P_ERR_ARG, "image %ux%u is empty", o->w, o->h);
+    EpilogueArgs a{};
+    for (int c = 0; c < 3; c++) {
+        j2p_session *s = ss[nsess == 1 ? 0 : c];
+        const int W = s->F.W, H = s->F.Hg;
+        if (o->w > (unsigned)W || o->h > (unsigned)H) return fail(J2P_ERR_ARG, "image %ux%u does not fit the %dx%d frame of plane %d", o->w, o->h, W, H, c);
+        a.plane[c] = plane_x(s, nsess == 1 ? frame0 * 3 + (unsigned)c : frame0);
+        a.frame_stride[c] = s->F.frame_stride;
+        a.ld[c] = W;
+    }
+    const size_t image_bytes = (size_t)o->w * o->h * 3 * (o->sample / 8);
+    if (o->frame_bytes < image_bytes) return fail(J2P_ERR_ARG, "frame_bytes %zu is smaller than one image (%zu bytes)", o->frame_bytes, image_bytes);
+    a.w = (int)o->w;
+    a.h = (int)o->h;
+    a.mode = o->layout == J2P_LAYOUT_HWC ? EP_HWC : EP_CHW;
+    a.sample = (int)o->sample;
+    a.frame_bytes = o->frame_bytes;
+    a.out = (uint8_t *)dst;
+    CK(cudaSetDevice(s0->device));
+    const cudaStream_t st = stream ? (cudaStream_t)stream : s0->stream;
+    // every session stream other than the launch stream: the launch waits for its solve ...
+    for (int k = 0; k < nsess; k++) {
+        j2p_session *s = ss[k];
+        if (s->stream == st) continue;
+        if (!s->export_ev) CK(cudaEventCreateWithFlags(&s->export_ev, cudaEventDisableTiming));
+        CK(cudaEventRecord(s->export_ev, s->stream));
+        CK(cudaStreamWaitEvent(st, s->export_ev, 0));
+    }
+    CK(launch_scanlines(a, (int)nframes, st));
+    s0->launches++;
+    // ... and the session stream waits for the export before a later upload / reset / iterate
+    for (int k = 0; k < nsess; k++) {
+        j2p_session *s = ss[k];
+        if (s->stream == st) continue;
+        CK(cudaEventRecord(s->export_ev, st));
+        CK(cudaStreamWaitEvent(s->stream, s->export_ev, 0));
+    }
+    return J2P_OK;
+}
+
+extern "C" int j2p_session_export(j2p_session *s, unsigned frame0, unsigned nframes, const struct j2p_image_out *o, void *dst,
+                                  void *stream) {
+    if (!s) return fail(J2P_ERR_ARG, "null session");
+    if (s->F.nc != 3 || s->strip) return fail(J2P_ERR_ARG, "j2p_session_export needs a whole-frame session with three planes (joint mode)");
+    return export_impl(&s, 1, frame0, nframes, o, dst, stream);
+}
+
+extern "C" int j2p_session_export_separate(j2p_session *y, j2p_session *cb, j2p_session *cr, unsigned frame0, unsigned nframes,
+                                           const struct j2p_image_out *o, void *dst, void *stream) {
+    if (!y || !cb || !cr) return fail(J2P_ERR_ARG, "null session");
+    j2p_session *ss[3] = {y, cb, cr};
+    for (int c = 0; c < 3; c++) {
+        if (ss[c]->F.nc != 1 || ss[c]->strip)
+            return fail(J2P_ERR_ARG, "j2p_session_export_separate needs three whole-frame sessions with one plane each (plane %d has %d)", c, ss[c]->F.nc);
+        if (ss[c]->nframes != y->nframes) return fail(J2P_ERR_ARG, "the separate sessions hold different frame counts (%u, %u)", y->nframes, ss[c]->nframes);
+        if (ss[c]->device != y->device) return fail(J2P_ERR_ARG, "the separate sessions live on different devices (%d, %d)", y->device, ss[c]->device);
+    }
+    return export_impl(ss, 3, frame0, nframes, o, dst, stream);
 }
 
 extern "C" int j2p_session_sync(j2p_session *s) {
