@@ -204,6 +204,17 @@ unsigned j2p_session_height(const j2p_session *s);
 int j2p_session_upload(j2p_session *s, unsigned channel, const int16_t *data,
                        const uint16_t *quant, const float *fdata);
 
+/* j2p_session_upload(s, plane, ..., fdata = NULL) for coefficients that are already in device memory
+ * (for instance decoded there by libj2pentropy.so).  `data_dev`: int16 [blocks][64] on the session's
+ * device; `quant`: host uint16[64].  The session stream waits for the work queued on `stream` so far
+ * (a cudaStream_t; NULL: no wait, the data is ready for the session stream), then copies `data_dev`
+ * device to device and runs the conventional decode; the same re-arming rules as
+ * j2p_session_upload apply.  Returns once the work is queued: `data_dev` must stay valid until the
+ * session stream has copied it.  J2P_ERR_ARG: null pointers, plane out of range, a zero table entry,
+ * and memory that is not device memory on the session's device. */
+int j2p_session_upload_device(j2p_session *s, unsigned plane, const int16_t *data_dev,
+                              const uint16_t *quant, void *stream);
+
 /* Re-arm the iteration state from the already-resident coefficient planes and the resident copy
  * of the conventional decode (no host traffic) — lets a benchmark time the loop repeatedly. */
 int j2p_session_reset(j2p_session *s);

@@ -182,6 +182,8 @@ def declare_product(lib: C.CDLL) -> C.CDLL:
     lib.j2p_session_height.argtypes = [vp]
     lib.j2p_session_upload.restype = C.c_int
     lib.j2p_session_upload.argtypes = [vp, C.c_uint, vp, vp, vp]
+    lib.j2p_session_upload_device.restype = C.c_int
+    lib.j2p_session_upload_device.argtypes = [vp, C.c_uint, vp, vp, vp]
     lib.j2p_session_reset.restype = C.c_int
     lib.j2p_session_reset.argtypes = [vp]
     lib.j2p_session_iterate.restype = C.c_int
@@ -222,7 +224,7 @@ HEADER_SYMBOLS = [
     'j2p_session_objective', 'j2p_session_sync', 'j2p_session_stream', 'j2p_session_plane_ptr',
     'j2p_session_launches', 'j2p_version', 'j2p_host_prefault', 'j2p_set_thread_device', 'j2p_thread_device', 'j2p_session_download_scanlines',
     'j2p_session_create_batch', 'j2p_session_frames', 'j2p_session_download_frame_scanlines',
-    'j2p_session_export', 'j2p_session_export_separate',
+    'j2p_session_export', 'j2p_session_export_separate', 'j2p_session_upload_device',
 ]
 
 _product = None

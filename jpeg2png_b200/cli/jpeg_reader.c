@@ -46,6 +46,9 @@ struct dec {
         char *err;
         size_t errlen;
         int failed;
+        struct j2p_jpeg_layout *lay;   /* the layout pass (j2p_read_jpeg_layout), NULL for a full read */
+        unsigned scans_of[3];          /* layout pass: scans that name each component */
+        size_t data_cap, seg_cap;
 };
 
 static int fail(struct dec *d, const char *fmt, ...) {
@@ -227,6 +230,11 @@ static int restart(struct dec *d, struct comp **sc, int ns, unsigned *eobrun, in
         return 0;
 }
 
+/* after a scan's last MCU: leave d->p at the next marker that is not RSTn (extra RSTn and junk are skipped) */
+static void skip_to_marker(struct dec *d) {
+        while (d->p + 1 < d->end && !(d->p[0] == 0xFF && d->p[1] != 0x00 && !(d->p[1] >= 0xD0 && d->p[1] <= 0xD7) && d->p[1] != 0xFF)) d->p++;
+}
+
 static int decode_scan(struct dec *d, struct comp **sc, int ns, int ss, int se, int ah, int al) {
         d->acc = 0;
         d->nbits = 0;
@@ -261,8 +269,68 @@ static int decode_scan(struct dec *d, struct comp **sc, int ns, int ss, int se, 
                         }
                         since_restart++;
                 }
-        /* leave d->p at the next marker */
-        while (d->p + 1 < d->end && !(d->p[0] == 0xFF && d->p[1] != 0x00 && !(d->p[1] >= 0xD0 && d->p[1] <= 0xD7) && d->p[1] != 0xFF)) d->p++;
+        skip_to_marker(d);
+        return 0;
+}
+
+/* ---- layout pass: one sequential scan cut into segments ------------------------------------ */
+static int grow(void **p, size_t *cap, size_t need, size_t elem) {
+        if (need <= *cap) return 0;
+        size_t n = *cap ? *cap : 4096 / elem + 1;
+        while (n < need) n *= 2;
+        void *q = realloc(*p, n * elem);
+        if (!q) return -1;
+        *p = q;
+        *cap = n;
+        return 0;
+}
+static int layout_scan(struct dec *d, struct comp **sc, int ns) {
+        struct j2p_jpeg_layout *l = d->lay;
+        struct j2p_jpeg_scan *S = &l->scan[l->nscan++];
+        const int interleaved = ns > 1;
+        S->ncomp = (unsigned)ns;
+        for (int i = 0; i < ns; i++) {
+                S->comp[i] = (unsigned)(sc[i] - d->c);
+                S->bw[i] = interleaved ? (unsigned)sc[i]->h : 1;
+                S->bh[i] = interleaved ? (unsigned)sc[i]->v : 1;
+                memcpy(S->dc[i].bits, d->dc[sc[i]->td].bits, 17);
+                memcpy(S->dc[i].vals, d->dc[sc[i]->td].vals, 256);
+                memcpy(S->ac[i].bits, d->ac[sc[i]->ta].bits, 17);
+                memcpy(S->ac[i].vals, d->ac[sc[i]->ta].vals, 256);
+        }
+        if (interleaved) { S->mcux = d->mcux; S->mcuy = d->mcuy; }
+        else { S->mcux = sc[0]->wb; S->mcuy = sc[0]->hb; }
+        S->restart_interval = d->restart_interval;
+        const size_t total = (size_t)S->mcux * S->mcuy;
+        const size_t nseg = d->restart_interval ? (total + d->restart_interval - 1) / d->restart_interval : 1;
+        S->seg0 = l->nseg;
+        S->nseg = (unsigned)nseg;
+        unsigned eobrun = 0;
+        for (size_t k = 0; k < nseg; k++) {
+                if (k > 0 && restart(d, sc, ns, &eobrun, (int)(k - 1)) != 0) return -1;
+                if (grow((void **)&l->seg, &d->seg_cap, (size_t)l->nseg + 1, sizeof *l->seg) != 0) return fail(d, "could not allocate memory for coefs");
+                /* the bytes fill() would feed: up to the first FF not followed by 00, FF 00 -> FF */
+                if (grow((void **)&l->data, &d->data_cap, l->data_len + (size_t)(d->end - d->p), 1) != 0) return fail(d, "could not allocate memory for coefs");
+                struct j2p_jpeg_segment *g = &l->seg[l->nseg++];
+                g->off = l->data_len;
+                uint8_t *o = l->data + l->data_len;
+                const uint8_t *p = d->p;
+                while (p < d->end) {
+                        const uint8_t *q = memchr(p, 0xFF, (size_t)(d->end - p));
+                        const size_t run = (size_t)((q ? q : d->end) - p);
+                        memcpy(o, p, run);
+                        o += run;
+                        p += run;
+                        if (!q) break;
+                        if (p + 1 < d->end && p[1] == 0x00) { *o++ = 0xFF; p += 2; }
+                        else break;
+                }
+                g->len = (size_t)(o - (l->data + l->data_len));
+                l->data_len += g->len;
+                g->mcus = (unsigned)(d->restart_interval && k + 1 < nseg ? d->restart_interval : total - k * (d->restart_interval ? d->restart_interval : 0));
+                d->p = p;
+        }
+        skip_to_marker(d);
         return 0;
 }
 
@@ -328,20 +396,19 @@ static int parse_sof(struct dec *d, const uint8_t *s, unsigned len) {
                 c->hb = (ch + 7) / 8;
                 c->pwb = d->mcux * c->h;
                 c->phb = d->mcuy * c->v;
+                if (d->lay) continue;                                                                   /* the layout pass stores no blocks */
                 c->blk = calloc((size_t)c->pwb * c->phb * 64, sizeof(int16_t));
                 if (!c->blk) return fail(d, "could not allocate memory for coefs");                /* jpeg.c:69 */
         }
         return 0;
 }
 
-int j2p_read_jpeg_mem(const uint8_t *buf, size_t len, struct j2p_jpeg *out, char *err, size_t errlen) {
-        struct dec *d = calloc(1, sizeof *d);
-        if (!d) return -1;
-        d->p = buf; d->end = buf + len; d->err = err; d->errlen = errlen;
-        if (err && errlen) err[0] = 0;
-        memset(out, 0, sizeof *out);
+/* The marker loop shared by j2p_read_jpeg_mem and j2p_read_jpeg_layout: reads the headers and
+ * decodes every scan (full read) or cuts it into segments (layout pass).  Returns 1 when the layout
+ * pass stopped early on a file that is not device-decodable. */
+static int read_markers(struct dec *d, const uint8_t *buf, size_t len) {
         int have_sof = 0, done = 0;
-        if (len < 4 || buf[0] != 0xFF || buf[1] != 0xD8) { fail(d, "not a jpeg file (no SOI marker)"); goto out; }
+        if (len < 4 || buf[0] != 0xFF || buf[1] != 0xD8) { fail(d, "not a jpeg file (no SOI marker)"); return 0; }
         d->p += 2;
         while (!done && !d->failed) {
                 /* find next marker */
@@ -362,6 +429,7 @@ int j2p_read_jpeg_mem(const uint8_t *buf, size_t len, struct j2p_jpeg *out, char
                 else if (m == 0xC0 || m == 0xC1 || m == 0xC2) {
                         if (have_sof) { fail(d, "unsupported jpeg: multiple frames"); break; }
                         d->progressive = m == 0xC2;
+                        if (d->lay && d->progressive) return 1;
                         if (parse_sof(d, s, sl) == 0) have_sof = 1;
                 } else if (m == 0xC3 || (m >= 0xC5 && m <= 0xC7) || (m >= 0xC9 && m <= 0xCB) || (m >= 0xCD && m <= 0xCF)) {
                         fail(d, "unsupported jpeg: SOF%u (arithmetic, lossless or hierarchical coding)", m - 0xC0);
@@ -390,39 +458,98 @@ int j2p_read_jpeg_mem(const uint8_t *buf, size_t len, struct j2p_jpeg *out, char
                                     ((!d->progressive || ss > 0) && !d->ac[sc[i]->ta].present)) { fail(d, "corrupt jpeg: scan uses an undefined huffman table"); break; }
                         }
                         if (d->failed) break;
-                        decode_scan(d, sc, ns, ss, se, ah, al);
+                        if (d->lay) {
+                                for (int i = 0; i < ns; i++)
+                                        if (d->scans_of[sc[i] - d->c]++) return 1;      /* a component scanned twice */
+                                layout_scan(d, sc, ns);
+                        } else {
+                                decode_scan(d, sc, ns, ss, se, ah, al);
+                        }
                 }
                 /* everything else (APPn, COM, DNL, ...) is skipped */
         }
         if (!d->failed && !have_sof) fail(d, "corrupt jpeg: no frame header");
+        return 0;
+}
+
+/* the reference's checks of the frame (jpeg.c:40-64) and the planes' geometry and tables */
+static void check_planes(struct dec *d, struct coef *coefs) {
+        for (int i = 0; i < 3 && !d->failed; i++) {
+                struct comp *c = &d->c[i];
+                struct coef *o = &coefs[i];
+                if (!d->qt_present[c->tq]) { fail(d, "weird jpeg: no quant table pointer"); break; }          /* jpeg.c:40 */
+                for (int j = 0; j < 64; j++) {
+                        if (d->qt[c->tq][j] == 0) { fail(d, "invalid quantization table"); break; }            /* jpeg.c:43 */
+                        o->quant_table[j] = d->qt[c->tq][j];
+                }
+                if (d->failed) break;
+                o->w = c->wb * 8;
+                o->h = c->hb * 8;
+                o->w_samp = d->maxh / c->h;                                                                    /* jpeg.c:57-58 */
+                o->h_samp = d->maxv / c->v;
+                if (o->h / 8 != (d->H / o->h_samp + 7) / 8) { fail(d, "jpeg invalid coef h size"); break; }    /* jpeg.c:59-61 */
+                if (o->w / 8 != (d->W / o->w_samp + 7) / 8) { fail(d, "jpeg invalid coef w size"); break; }    /* jpeg.c:62-64 */
+        }
+}
+
+int j2p_read_jpeg_mem(const uint8_t *buf, size_t len, struct j2p_jpeg *out, char *err, size_t errlen) {
+        struct dec *d = calloc(1, sizeof *d);
+        if (!d) return -1;
+        d->p = buf; d->end = buf + len; d->err = err; d->errlen = errlen;
+        if (err && errlen) err[0] = 0;
+        memset(out, 0, sizeof *out);
+        read_markers(d, buf, len);
+        if (!d->failed) check_planes(d, out->coefs);
         if (!d->failed) {
                 out->w = d->W;
                 out->h = d->H;
-                for (int i = 0; i < 3 && !d->failed; i++) {
+                for (int i = 0; i < 3; i++) {
                         struct comp *c = &d->c[i];
                         struct coef *o = &out->coefs[i];
-                        if (!d->qt_present[c->tq]) { fail(d, "weird jpeg: no quant table pointer"); break; }          /* jpeg.c:40 */
-                        for (int j = 0; j < 64; j++) {
-                                if (d->qt[c->tq][j] == 0) { fail(d, "invalid quantization table"); break; }            /* jpeg.c:43 */
-                                o->quant_table[j] = d->qt[c->tq][j];
-                        }
-                        if (d->failed) break;
-                        o->w = c->wb * 8;
-                        o->h = c->hb * 8;
-                        o->w_samp = d->maxh / c->h;                                                                    /* jpeg.c:57-58 */
-                        o->h_samp = d->maxv / c->v;
-                        if (o->h / 8 != (d->H / o->h_samp + 7) / 8) { fail(d, "jpeg invalid coef h size"); break; }    /* jpeg.c:59-61 */
-                        if (o->w / 8 != (d->W / o->w_samp + 7) / 8) { fail(d, "jpeg invalid coef w size"); break; }    /* jpeg.c:62-64 */
                         o->data = malloc((size_t)o->w * o->h * sizeof(int16_t));
                         if (!o->data) { fail(d, "could not allocate memory for coefs"); break; }
                         for (unsigned by = 0; by < c->hb; by++)
                                 memcpy(o->data + (size_t)by * c->wb * 64, c->blk + (size_t)by * c->pwb * 64, (size_t)c->wb * 64 * sizeof(int16_t));
                 }
         }
-out:
         for (int i = 0; i < 3; i++) free(d->c[i].blk);
         const int rc = d->failed ? -1 : 0;
         if (rc != 0) for (int i = 0; i < 3; i++) { free(out->coefs[i].data); out->coefs[i].data = NULL; }
         free(d);
         return rc;
+}
+
+int j2p_read_jpeg_layout(const uint8_t *buf, size_t len, struct j2p_jpeg_layout *out, char *err, size_t errlen) {
+        struct dec *d = calloc(1, sizeof *d);
+        if (!d) return -1;
+        d->p = buf; d->end = buf + len; d->err = err; d->errlen = errlen;
+        if (err && errlen) err[0] = 0;
+        memset(out, 0, sizeof *out);
+        d->lay = out;
+        const int stopped = read_markers(d, buf, len);
+        int decodable = !stopped && !d->failed;
+        for (int i = 0; i < 3 && decodable; i++) decodable = d->scans_of[i] == 1;
+        if (decodable) {
+                check_planes(d, out->coefs);
+                out->w = d->W;
+                out->h = d->H;
+                for (int i = 0; i < 3; i++) { out->comp_h[i] = (unsigned)d->c[i].h; out->comp_v[i] = (unsigned)d->c[i].v; }
+        }
+        const int rc = d->failed ? -1 : 0;
+        out->device_decodable = rc == 0 && decodable;
+        if (!out->device_decodable) {
+                j2p_free_jpeg_layout(out);
+                out->nscan = 0;
+        }
+        free(d);
+        return rc;
+}
+
+void j2p_free_jpeg_layout(struct j2p_jpeg_layout *l) {
+        free(l->seg);
+        free(l->data);
+        l->seg = NULL;
+        l->data = NULL;
+        l->nseg = 0;
+        l->data_len = 0;
 }

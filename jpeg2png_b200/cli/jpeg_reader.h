@@ -31,4 +31,51 @@ struct j2p_jpeg {
  * The messages for the reference's own rejections are the reference's (jpeg.c:34,43,60,63). */
 int j2p_read_jpeg_mem(const uint8_t *buf, size_t len, struct j2p_jpeg *out, char *err, size_t errlen);
 
+/* ---- layout pass: the headers and the entropy-coded data of a file, without Huffman decoding ----
+ *
+ * j2p_read_jpeg_layout runs the marker loop and header checks of j2p_read_jpeg_mem (the same code)
+ * and, instead of decoding each scan, cuts its entropy-coded data into segments, one per restart
+ * interval, unstuffed (FF 00 -> FF), in one byte buffer.  A segment ends where the reader's bit
+ * reader stops feeding bits: at the first FF not followed by 00, or at the end of the file; bits
+ * past its end read as zero.  The restart markers between segments are checked by the reader's own
+ * restart rule, so "missing restart marker", "out of sequence" and "truncated" fail here as there.
+ *
+ * device_decodable: the file is sequential Huffman (SOF0/SOF1) and each of the three components is
+ * in exactly one scan.  Only then are coefs (geometry and tables, data NULL), scans and segments
+ * filled; for every other file the pass stops as soon as that is known (a progressive SOF, a
+ * component's second scan) and returns 0 with device_decodable = 0: such files are for
+ * j2p_read_jpeg_mem.  A non-zero return means j2p_read_jpeg_mem rejects the file too (it may name an
+ * earlier error, in the entropy-coded data). */
+struct j2p_jpeg_huff {
+        uint8_t bits[17];           /* bits[l]: codes of length l (bits[0] unused) */
+        uint8_t vals[256];
+};
+struct j2p_jpeg_scan {
+        unsigned ncomp;             /* components in scan order */
+        unsigned comp[3];           /* frame component (0..2) of each */
+        unsigned bw[3], bh[3];      /* blocks per MCU of each: (h, v) when interleaved, else (1, 1) */
+        unsigned mcux, mcuy;        /* MCU grid: the frame's MCUs when interleaved, else the component's real block grid */
+        unsigned restart_interval;  /* MCUs per segment, 0: one segment */
+        struct j2p_jpeg_huff dc[3], ac[3];  /* the tables in force at this SOS */
+        unsigned seg0, nseg;        /* its segments */
+};
+struct j2p_jpeg_segment {
+        size_t off, len;            /* unstuffed bytes in data */
+        unsigned mcus;              /* MCUs it codes */
+};
+struct j2p_jpeg_layout {
+        unsigned w, h;
+        struct coef coefs[3];       /* as struct j2p_jpeg, but data NULL */
+        unsigned comp_h[3], comp_v[3];   /* sampling factors of the frame header */
+        int device_decodable;
+        unsigned nscan;
+        struct j2p_jpeg_scan scan[3];
+        unsigned nseg;
+        struct j2p_jpeg_segment *seg;    /* malloc'd */
+        uint8_t *data;                   /* malloc'd */
+        size_t data_len;
+};
+int j2p_read_jpeg_layout(const uint8_t *buf, size_t len, struct j2p_jpeg_layout *out, char *err, size_t errlen);
+void j2p_free_jpeg_layout(struct j2p_jpeg_layout *l);
+
 #endif

@@ -211,6 +211,7 @@ struct j2p_session {
     cudaEvent_t stage_ev[kStageSlots] = {};
     unsigned stage_next = 0;
     cudaEvent_t export_ev = nullptr;          // orders j2p_session_export on a caller stream with the session stream
+    cudaEvent_t upload_ev = nullptr;          // orders j2p_session_upload_device after its producer stream
 };
 
 // x_k <-> x_{k-1} after an iteration (reference SWAP at compute.c:438); all planes together, which
@@ -305,6 +306,7 @@ extern "C" void j2p_session_destroy(j2p_session *s) {
         if (s->stage[k]) g_pinned.put(s->stage[k]);
     }
     if (s->export_ev) cudaEventDestroy(s->export_ev);
+    if (s->upload_ev) cudaEventDestroy(s->upload_ev);
     if (s->stream) cudaStreamDestroy(s->stream);
     delete s;
 }
@@ -663,16 +665,10 @@ static int staged_d2h(j2p_session *s, void *dst, const void *src, size_t bytes) 
     return J2P_OK;
 }
 
-// `plane` = frame * nchannel + channel (an ordinary session: the channel)
-extern "C" int j2p_session_upload(j2p_session *s, unsigned plane, const int16_t *data, const uint16_t *quant,
-                                  const float *fdata) {
-    if (!s || !data || !quant) return fail(J2P_ERR_ARG, "null argument");
-    if (plane >= s->uploaded.size()) return fail(J2P_ERR_ARG, "plane %u out of range (%zu planes)", plane, s->uploaded.size());
-    CK(cudaSetDevice(s->device));
+// the quantisation tables of `plane` (q, qq, rqq), shared by both uploads
+static int set_tables(j2p_session *s, unsigned plane, const uint16_t *quant, float **tab_out) {
     FrameDev &F = s->F;
     const unsigned f = plane / (unsigned)F.nc, c = plane % (unsigned)F.nc;
-    PlaneDev &P = F.pl[c];
-    const size_t nc = (size_t)P.cw * P.ch;
     float *tab = s->tables.data() + (size_t)plane * 192;                // q, qq, rqq of this frame and plane
     for (int j = 0; j < 64; j++)
         if (quant[j] == 0) return fail(J2P_ERR_ARG, "invalid quantization table (zero entry, jpeg.c:41-45)");
@@ -687,9 +683,41 @@ extern "C" int j2p_session_upload(j2p_session *s, unsigned plane, const int16_t 
         }
     }
     s->tables_stale = true;
+    *tab_out = tab;
+    return J2P_OK;
+}
+
+// after a plane's upload: re-arm a single-frame session once all its planes are in
+static int plane_uploaded(j2p_session *s, unsigned plane) {
+    s->uploaded[plane] = 1;
+    // A batch is re-armed once, by the first iterate (or reset) after its uploads: re-arming after
+    // every plane would cost nframes * nchannel resets per solve.
+    if (s->nframes > 1) {
+        s->stale = true;
+        return J2P_OK;
+    }
+    bool all = true;
+    for (int k = 0; k < s->F.nc; k++) all = all && s->uploaded[k];
+    if (all) return reset_impl(s);
+    return J2P_OK;
+}
+
+// `plane` = frame * nchannel + channel (an ordinary session: the channel)
+extern "C" int j2p_session_upload(j2p_session *s, unsigned plane, const int16_t *data, const uint16_t *quant,
+                                  const float *fdata) {
+    if (!s || !data || !quant) return fail(J2P_ERR_ARG, "null argument");
+    if (plane >= s->uploaded.size()) return fail(J2P_ERR_ARG, "plane %u out of range (%zu planes)", plane, s->uploaded.size());
+    CK(cudaSetDevice(s->device));
+    FrameDev &F = s->F;
+    const unsigned f = plane / (unsigned)F.nc, c = plane % (unsigned)F.nc;
+    PlaneDev &P = F.pl[c];
+    const size_t nc = (size_t)P.cw * P.ch;
+    float *tab;
+    int rcs = set_tables(s, plane, quant, &tab);
+    if (rcs != J2P_OK) return rcs;
     int16_t *ddst = s->data[c] + (size_t)f * F.data_stride;
     float *fdst = s->fdata0[c] + (size_t)f * s->fdata_stride;
-    int rcs = staged_h2d(s, ddst, data, nc * sizeof(int16_t));
+    rcs = staged_h2d(s, ddst, data, nc * sizeof(int16_t));
     if (rcs != J2P_OK) return rcs;
     if (fdata) {
         rcs = staged_h2d(s, fdst, fdata, nc * sizeof(float));
@@ -700,17 +728,43 @@ extern "C" int j2p_session_upload(j2p_session *s, unsigned plane, const int16_t 
     }
     // The host arrays have been read completely (they sit in the pinned ring or on the device);
     // the stream is NOT drained here, so the next plane's host copy overlaps this plane's DMA.
-    s->uploaded[plane] = 1;
-    // A batch is re-armed once, by the first iterate (or reset) after its uploads: re-arming after
-    // every plane would cost nframes * nchannel resets per solve.
-    if (s->nframes > 1) {
-        s->stale = true;
-        return J2P_OK;
+    return plane_uploaded(s, plane);
+}
+
+// coefficients already in device memory: the session stream waits for `stream`, copies them device
+// to device and runs the conventional decode, as j2p_session_upload(..., fdata = NULL) does
+extern "C" int j2p_session_upload_device(j2p_session *s, unsigned plane, const int16_t *data_dev, const uint16_t *quant,
+                                         void *stream) {
+    if (!s || !data_dev || !quant) return fail(J2P_ERR_ARG, "null argument");
+    if (plane >= s->uploaded.size()) return fail(J2P_ERR_ARG, "plane %u out of range (%zu planes)", plane, s->uploaded.size());
+    for (int j = 0; j < 64; j++)
+        if (quant[j] == 0) return fail(J2P_ERR_ARG, "invalid quantization table (zero entry, jpeg.c:41-45)");
+    CK(cudaSetDevice(s->device));
+    cudaPointerAttributes attr;
+    if (cudaPointerGetAttributes(&attr, data_dev) != cudaSuccess) {
+        cudaGetLastError();
+        return fail(J2P_ERR_ARG, "data_dev is not a CUDA pointer");
     }
-    bool all = true;
-    for (int k = 0; k < F.nc; k++) all = all && s->uploaded[k];
-    if (all) return reset_impl(s);
-    return J2P_OK;
+    if (attr.type != cudaMemoryTypeDevice || attr.device != s->device)
+        return fail(J2P_ERR_ARG, "data_dev is not device memory on device %d", s->device);
+    FrameDev &F = s->F;
+    const unsigned f = plane / (unsigned)F.nc, c = plane % (unsigned)F.nc;
+    PlaneDev &P = F.pl[c];
+    float *tab;
+    const int rc = set_tables(s, plane, quant, &tab);
+    if (rc != J2P_OK) return rc;
+    const cudaStream_t st = (cudaStream_t)stream;
+    if (st && st != s->stream) {
+        if (!s->upload_ev) CK(cudaEventCreateWithFlags(&s->upload_ev, cudaEventDisableTiming));
+        CK(cudaEventRecord(s->upload_ev, st));
+        CK(cudaStreamWaitEvent(s->stream, s->upload_ev, 0));
+    }
+    int16_t *ddst = s->data[c] + (size_t)f * F.data_stride;
+    float *fdst = s->fdata0[c] + (size_t)f * s->fdata_stride;
+    CK(cudaMemcpyAsync(ddst, data_dev, (size_t)P.cw * P.ch * sizeof(int16_t), cudaMemcpyDeviceToDevice, s->stream));
+    CK(launch_decode(ddst, tab, fdst, P.cw, P.ch, s->stream));
+    s->launches++;
+    return plane_uploaded(s, plane);
 }
 
 // one solver iteration on the session stream; optional events around each kernel

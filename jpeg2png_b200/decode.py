@@ -1,7 +1,9 @@
 """decode_jpeg: JPEG files in, RGB CUDA tensors out, through the solver.
 
-Every input is parsed on the host with the JPEG coefficient reader of the command line
-(libj2pcodecs.so, j2p_read_jpeg_mem) before any device work.  Inputs of one geometry are solved
+Every input's headers are read on the host with the JPEG reader of the command line
+(libj2pcodecs.so) before any device work: sequential files whose components are each in one scan
+go through its layout pass (j2p_read_jpeg_layout) and are Huffman-decoded on the device
+(libj2pentropy.so, DESIGN §7d); every other file is parsed by j2p_read_jpeg_mem.  Inputs of one geometry are solved
 together in batch sessions (j2p_session_create_batch), with the conventional decode on the device as
 the command line does it, and the colour conversion writes straight into one freshly allocated tensor
 per chunk (j2p_session_export) on the caller's current stream.  The returned tensors of a chunk are
@@ -36,7 +38,42 @@ class Jpeg(C.Structure):
     _fields_ = [('w', C.c_uint), ('h', C.c_uint), ('coefs', abi.Coef * 3)]
 
 
+class Huff(C.Structure):
+    """struct j2p_jpeg_huff — jpeg2png_b200/cli/jpeg_reader.h."""
+    _fields_ = [('bits', C.c_uint8 * 17), ('vals', C.c_uint8 * 256)]
+
+
+class Scan(C.Structure):
+    """struct j2p_jpeg_scan — jpeg2png_b200/cli/jpeg_reader.h."""
+    _fields_ = [('ncomp', C.c_uint), ('comp', C.c_uint * 3), ('bw', C.c_uint * 3), ('bh', C.c_uint * 3),
+                ('mcux', C.c_uint), ('mcuy', C.c_uint), ('restart_interval', C.c_uint),
+                ('dc', Huff * 3), ('ac', Huff * 3), ('seg0', C.c_uint), ('nseg', C.c_uint)]
+
+
+class Segment(C.Structure):
+    """struct j2p_jpeg_segment — jpeg2png_b200/cli/jpeg_reader.h."""
+    _fields_ = [('off', C.c_size_t), ('len', C.c_size_t), ('mcus', C.c_uint)]
+
+
+class Layout(C.Structure):
+    """struct j2p_jpeg_layout — jpeg2png_b200/cli/jpeg_reader.h."""
+    _fields_ = [('w', C.c_uint), ('h', C.c_uint), ('coefs', abi.Coef * 3), ('comp_h', C.c_uint * 3),
+                ('comp_v', C.c_uint * 3), ('device_decodable', C.c_int), ('nscan', C.c_uint), ('scan', Scan * 3),
+                ('nseg', C.c_uint), ('seg', C.POINTER(Segment)), ('data', C.POINTER(C.c_uint8)),
+                ('data_len', C.c_size_t)]
+
+
+class EntropyStats(C.Structure):
+    """struct j2p_entropy_stats — jpeg2png_b200/entropy/entropy.h."""
+    _fields_ = [('rounds', C.c_uint), ('round_trips', C.c_uint), ('launches', C.c_uint), ('subsequences', C.c_uint)]
+
+
+ENTROPY_LIB = os.path.join(abi._PKG_DIR, 'entropy', 'libj2pentropy.so')
+SUBSEQ_BITS = 1024                  # bits per subsequence of the device decoder (DESIGN §7d)
+ENT_FAILURES = {1: 'bad huffman code', 2: 'bad magnitude category', 3: 'coefficient index out of range'}
+
 _codecs = None
+_entropy = None
 
 
 def load_codecs() -> C.CDLL:
@@ -49,8 +86,87 @@ def load_codecs() -> C.CDLL:
         lib = C.CDLL(CODECS_LIB, mode=C.RTLD_LOCAL)
         lib.j2p_read_jpeg_mem.restype = C.c_int
         lib.j2p_read_jpeg_mem.argtypes = [C.c_char_p, C.c_size_t, C.POINTER(Jpeg), C.c_char_p, C.c_size_t]
+        lib.j2p_read_jpeg_layout.restype = C.c_int
+        lib.j2p_read_jpeg_layout.argtypes = [C.c_char_p, C.c_size_t, C.POINTER(Layout), C.c_char_p, C.c_size_t]
+        lib.j2p_free_jpeg_layout.restype = None
+        lib.j2p_free_jpeg_layout.argtypes = [C.POINTER(Layout)]
         _codecs = lib
     return _codecs
+
+
+def load_entropy() -> C.CDLL:
+    """libj2pentropy.so (the device entropy decoder) from the package tree."""
+    global _entropy
+    if _entropy is None:
+        if not os.path.exists(ENTROPY_LIB):
+            raise RuntimeError(f'{ENTROPY_LIB} is missing: the entropy decoder has not been built '
+                               '(run `python -c "import __graft_entry__ as g; g.build()"`)')
+        lib = C.CDLL(ENTROPY_LIB, mode=C.RTLD_LOCAL)
+        vp, lay = C.c_void_p, C.POINTER(C.POINTER(Layout))
+        lib.j2p_entropy_plan_size.restype = C.c_int
+        lib.j2p_entropy_plan_size.argtypes = [lay, C.c_uint, C.c_uint, C.POINTER(C.c_size_t), C.POINTER(C.c_size_t)]
+        lib.j2p_entropy_pack.restype = C.c_int
+        lib.j2p_entropy_pack.argtypes = [lay, C.c_uint, C.c_uint, C.POINTER(vp), vp, C.c_size_t]
+        lib.j2p_entropy_decode.restype = C.c_int
+        lib.j2p_entropy_decode.argtypes = [vp, vp, vp, vp, vp, C.POINTER(EntropyStats)]
+        lib.j2p_entropy_decode_host.restype = C.c_int
+        lib.j2p_entropy_decode_host.argtypes = [vp, vp, vp, C.POINTER(EntropyStats)]
+        lib.j2p_entropy_last_error.restype = C.c_char_p
+        lib.j2p_entropy_last_error.argtypes = []
+        _entropy = lib
+    return _entropy
+
+
+class FileLayout:
+    """A file's layout (j2p_read_jpeg_layout); frees the C buffers when collected."""
+
+    def __init__(self, data: bytes):
+        lib = load_codecs()
+        self.lay = Layout()
+        err = C.create_string_buffer(256)
+        if lib.j2p_read_jpeg_layout(data, len(data), C.byref(self.lay), err, 256) != 0:
+            raise ValueError(err.value.decode(errors='replace'))
+        self.device_decodable = bool(self.lay.device_decodable)
+        self.w, self.h = int(self.lay.w), int(self.lay.h)
+        self.compressed = int(self.lay.data_len)
+        self.planes = [Plane(int(c.w), int(c.h), int(c.w_samp), int(c.h_samp), None,
+                             np.array(list(c.quant_table), np.uint16)) for c in self.lay.coefs]
+
+    def key(self):
+        return Parsed.key(self)
+
+    def __del__(self):
+        try:
+            load_codecs().j2p_free_jpeg_layout(C.byref(self.lay))
+        except Exception:
+            pass
+
+
+def _layout_ptrs(layouts):
+    return (C.POINTER(Layout) * len(layouts))(*[C.pointer(x.lay) for x in layouts])
+
+
+def entropy_plan(layouts, outs, subseq_bits=SUBSEQ_BITS, pinned=False):
+    """Pack `layouts` (FileLayout) into a plan for libj2pentropy.so; outs[3 * i + c]: address of
+    file i's plane c.  Returns (plan buffer: a pinned uint8 tensor or a numpy array, its address,
+    plan bytes, work bytes)."""
+    lib = load_entropy()
+    ptrs = _layout_ptrs(layouts)
+    plan_bytes, work_bytes = C.c_size_t(), C.c_size_t()
+    if lib.j2p_entropy_plan_size(ptrs, len(layouts), subseq_bits, C.byref(plan_bytes), C.byref(work_bytes)) != 0:
+        raise RuntimeError(lib.j2p_entropy_last_error().decode())
+    if pinned:
+        buf = torch.empty(plan_bytes.value, dtype=torch.uint8, pin_memory=True)
+        addr = buf.data_ptr()
+    else:
+        buf = np.zeros(plan_bytes.value + 16, np.uint8)
+        addr = (buf.ctypes.data + 15) & ~15
+    if addr % 16:
+        raise RuntimeError('plan buffer is not 16-byte aligned')
+    o = (C.c_void_p * len(outs))(*outs)
+    if lib.j2p_entropy_pack(ptrs, len(layouts), subseq_bits, o, addr, plan_bytes.value) != 0:
+        raise RuntimeError(lib.j2p_entropy_last_error().decode())
+    return buf, addr, plan_bytes.value, work_bytes.value
 
 
 @dataclass
@@ -192,13 +308,53 @@ def _frame_desc(parsed: Parsed, channels, weight, pweights, iterations) -> abi.F
     return d
 
 
+class _DeviceCoefs:
+    """The coefficients of a chunk's device-decodable files, Huffman-decoded on the device by
+    libj2pentropy.so into one int16 tensor: the packed plan goes up in one pinned copy on `stream`,
+    the decoder runs there, and the constructor waits for the decode only.  status[i]: J2P_ENT_OK
+    or the failure kind of file i."""
+
+    def __init__(self, device, layouts, stream, subseq_bits=SUBSEQ_BITS):
+        dev = torch.device('cuda', device)
+        sizes = [p.w * p.h for lay in layouts for p in lay.planes]
+        offs = np.concatenate([[0], np.cumsum(sizes, dtype=np.int64)])
+        with torch.cuda.stream(stream):
+            self.coefs = torch.empty(max(int(offs[-1]), 1), dtype=torch.int16, device=dev)
+            base = self.coefs.data_ptr()
+            self.ptrs = [base + 2 * int(o) for o in offs[:-1]]           # planes are whole 128-byte blocks
+            self.plan, addr, plan_bytes, work_bytes = entropy_plan(layouts, self.ptrs, subseq_bits, pinned=True)
+            self.plan_dev = torch.empty(plan_bytes, dtype=torch.uint8, device=dev)
+            self.plan_dev.copy_(self.plan, non_blocking=True)
+            self.work = torch.empty(max(work_bytes, 16), dtype=torch.uint8, device=dev)
+            status = torch.empty(len(layouts), dtype=torch.int32, device=dev)
+            self.stats = EntropyStats()
+            lib = load_entropy()
+            if lib.j2p_entropy_decode(addr, self.plan_dev.data_ptr(), self.work.data_ptr(), status.data_ptr(),
+                                      stream.cuda_stream, C.byref(self.stats)) != 0:
+                raise RuntimeError(lib.j2p_entropy_last_error().decode())
+            stream.record_event().synchronize()
+            self.status = status.cpu().numpy()
+        self.plan = self.work = self.plan_dev = None
+
+    def plane(self, i, c):
+        return self.ptrs[3 * i + c]
+
+    def plane_tensor(self, i, c):
+        """A view of file i's plane c in the coefficient tensor (int16, blocks * 64)."""
+        start = (self.ptrs[3 * i + c] - self.coefs.data_ptr()) // 2
+        end = (self.ptrs[3 * i + c + 1] - self.coefs.data_ptr()) // 2 if 3 * i + c + 1 < len(self.ptrs) else self.coefs.numel()
+        return self.coefs[start:end]
+
+
 class _Chunk:
     """The batch session(s) of one chunk: created, uploaded, iterated and exported by the
-    constructor; close() waits for them and returns their blocks to the device cache."""
+    constructor; close() waits for them and returns their blocks to the device cache.
+    coefs: {item index: (_DeviceCoefs, its file index)} for items whose coefficients are on the
+    device (uploaded with j2p_session_upload_device after `coef_stream`)."""
 
-    def __init__(self, lib, device, items, flags, separate, dtype, layout):
+    def __init__(self, lib, device, items, flags, separate, dtype, layout, coefs=None, coef_stream=None):
         iters, weights, pweights = flags
-        self.lib, self.sessions = lib, []
+        self.lib, self.sessions, self.coefs = lib, [], coefs or {}
         first, n = items[0], len(items)
         if separate:
             work = [(_frame_desc(first, [c], weights[c], pweights, iters[c]), [c], iters[c]) for c in range(3)]
@@ -213,8 +369,13 @@ class _Chunk:
                 for f, parsed in enumerate(items):
                     for k, c in enumerate(channels):
                         p = parsed.planes[c]
-                        self._check(lib.j2p_session_upload(s, f * len(channels) + k, p.data.ctypes.data,
-                                                           p.quant.ctypes.data, None))     # conventional decode on the device
+                        if f in self.coefs:
+                            dc, i = self.coefs[f]
+                            self._check(lib.j2p_session_upload_device(s, f * len(channels) + k, dc.plane(i, c),
+                                                                      p.quant.ctypes.data, coef_stream.cuda_stream))
+                        else:
+                            self._check(lib.j2p_session_upload(s, f * len(channels) + k, p.data.ctypes.data,
+                                                               p.quant.ctypes.data, None))     # conventional decode on the device
                 self._check(lib.j2p_session_iterate(s, 0, it))
             w, h = first.w, first.h
             shape = (n, 3, h, w) if layout == abi.LAYOUT_CHW else (n, h, w, 3)
@@ -240,6 +401,41 @@ class _Chunk:
         for s in self.sessions:
             self.lib.j2p_session_destroy(s)
         self.sessions = []
+        self.coefs = {}             # the session streams are idle: the coefficient tensor can go
+
+
+# The front end (internal switch; tools/entropy_bench.py compares the two): with a device, files
+# that are device-decodable (j2p_read_jpeg_layout) are Huffman-decoded there and every other file is
+# parsed by j2p_read_jpeg_mem; True sends every file to j2p_read_jpeg_mem.
+_host_front_end = False
+
+
+def _where(i, path):
+    return f'input {i} ({path})' if path is not None else f'input {i}'
+
+
+def _front_end(data, device_ok):
+    """The host part of one input: a FileLayout for the device decoder, a Parsed from the host
+    reader, or the ValueError (always the host reader's message) or RuntimeError to raise."""
+    if not device_ok or _host_front_end:
+        try:
+            return parse_jpeg(data)
+        except ValueError as e:
+            return e
+    try:
+        lay = FileLayout(data)
+    except ValueError:
+        try:
+            parse_jpeg(data)
+        except ValueError as e:
+            return e
+        return RuntimeError('the layout pass rejected a file the host reader accepts')
+    if lay.device_decodable:
+        return lay
+    try:
+        return parse_jpeg(data)
+    except ValueError as e:
+        return e
 
 
 def decode_jpeg(inputs, *, iterations=50, weight=0.3, pweight=0.001, separate=False,
@@ -258,8 +454,14 @@ def decode_jpeg(inputs, *, iterations=50, weight=0.3, pweight=0.001, separate=Fa
     Inputs with the same geometry are solved together, max_frames per batch (default: as many as
     fit in a quarter of the free device memory).  The tensors of one batch are views of one
     allocation and share its storage.  The result is written on the current torch stream and can
-    be used there without synchronising.  Raises ValueError for bad arguments and unreadable
-    files (before any device work) and RuntimeError when no CUDA device is usable.
+    be used there without synchronising.
+
+    Sequential (baseline or extended) files whose three components are each coded in one scan are
+    Huffman-decoded on the device: only their compressed bytes are uploaded.  Every other file,
+    progressive ones included, is parsed on the host.  Raises ValueError for bad arguments and
+    unreadable files, with the host reader's message: header errors before any device work, errors
+    in a device-decoded file's entropy-coded data once its batch has been decoded, before that batch
+    is solved.  Raises RuntimeError when no CUDA device is usable.
     """
     flags = solver_flags(iterations, weight, pweight, separate)
     if dtype not in _SAMPLE:
@@ -277,27 +479,24 @@ def decode_jpeg(inputs, *, iterations=50, weight=0.3, pweight=0.001, separate=Fa
     if not read:
         return []
 
-    def parse(data):
-        try:
-            return parse_jpeg(data)
-        except ValueError as e:
-            return e
-
-    # the reader runs without the GIL (ctypes): a 1080p file takes about as long to parse on the host
-    # as to solve on the device, so many files are parsed in parallel
+    # Without a device the host reader reads every input (its errors first), as the solver needs a
+    # device anyway.  With one, the layout pass runs instead and only non-device-decodable files are
+    # parsed on the host.  Either runs without the GIL (ctypes), many files in parallel.
+    device_ok = torch.cuda.is_available()
     workers = min(len(read), os.cpu_count() or 1, 16)
     if workers > 1:
         with ThreadPoolExecutor(workers) as pool:
-            parsed = list(pool.map(parse, [data for data, _ in read]))
+            parsed = list(pool.map(lambda d: _front_end(d, device_ok), [data for data, _ in read]))
     else:
-        parsed = [parse(data) for data, _ in read]
+        parsed = [_front_end(data, device_ok) for data, _ in read]
     for i, (p, (_, path)) in enumerate(zip(parsed, read)):
         if isinstance(p, ValueError):
-            where = f'input {i} ({path})' if path is not None else f'input {i}'
-            raise ValueError(f'{where}: {p}')
+            raise ValueError(f'{_where(i, path)}: {p}')
+        if isinstance(p, RuntimeError):
+            raise RuntimeError(f'{_where(i, path)}: {p} (a decoder bug)')
 
     lib = abi.load_product()
-    if not torch.cuda.is_available() or lib.j2p_device_count() <= 0:
+    if not device_ok or lib.j2p_device_count() <= 0:
         raise RuntimeError('decode_jpeg needs a CUDA device: the solver has no CPU fallback')
     index = dev.index if dev.index is not None else torch.cuda.current_device()
     sample_bytes = _SAMPLE[dtype] // 8
@@ -310,8 +509,27 @@ def decode_jpeg(inputs, *, iterations=50, weight=0.3, pweight=0.001, separate=Fa
     previous = None
     try:
         with torch.cuda.device(index):
+            # the entropy decoder's own stream: waiting for a chunk's decode does not wait for the
+            # solve of the chunk before it
+            coef_stream = torch.cuda.Stream(index)
             for _, idx in chunks:
-                chunk = _Chunk(lib, index, [parsed[i] for i in idx], flags, separate, dtype, layout_id)
+                on_dev = [j for j, i in enumerate(idx) if isinstance(parsed[i], FileLayout)]
+                coefs = {}
+                if on_dev:
+                    dc = _DeviceCoefs(index, [parsed[idx[j]] for j in on_dev], coef_stream)
+                    for k, j in enumerate(on_dev):
+                        if dc.status[k] != 0:
+                            i = idx[j]
+                            where = _where(i, read[i][1])
+                            try:
+                                parse_jpeg(read[i][0])
+                            except ValueError as e:
+                                raise ValueError(f'{where}: {e}') from None
+                            raise RuntimeError(f'{where}: the device entropy decoder failed '
+                                               f'({ENT_FAILURES.get(int(dc.status[k]), int(dc.status[k]))}) on a file '
+                                               'the host reader accepts (a decoder bug)')
+                        coefs[j] = (dc, k)
+                chunk = _Chunk(lib, index, [parsed[i] for i in idx], flags, separate, dtype, layout_id, coefs, coef_stream)
                 for j, i in enumerate(idx):
                     results[i] = chunk.out[j]
                 if previous is not None:        # this chunk is queued: let the previous one finish
