@@ -57,14 +57,16 @@ class _DevMem:
 
 
 class ProductStrip:
-    """A strip session of libjpeg2png_b200.so (GPU)."""
+    """A strip session of libjpeg2png_b200.so (GPU).  The channel count is the frame's (1..3).
+    fdata: None to decode on the device, else the caller's conventional decode of the WHOLE frame
+    (one (h, w) float32 array per plane); the strip's coefficient rows are sliced from it."""
 
-    def __init__(self, lib, img, weight, pweight, iterations, row0, rows, device):
+    def __init__(self, lib, img, weight, pweight, iterations, row0, rows, device, fdata=None):
         import torch
         from . import abi
-        self.torch, self.lib, self.nc = torch, lib, 3
+        self.torch, self.lib, self.nc = torch, lib, len(img.planes)
         d = abi.FrameDesc()
-        d.nchannel = 3
+        d.nchannel = self.nc
         for c, p in enumerate(img.planes):
             d.plane_w[c], d.plane_h[c], d.w_samp[c], d.h_samp[c] = p.w, p.h, p.w_samp, p.h_samp
             d.pweight[c] = pweight[c]
@@ -79,7 +81,8 @@ class ProductStrip:
             bw = p.w // 8
             data = np.ascontiguousarray(p.data.reshape(-1, 64)[(cy0 // 8) * bw:(cy1 // 8) * bw].reshape(-1))
             quant = np.ascontiguousarray(p.quant)
-            if lib.j2p_session_upload(s, c, data.ctypes.data, quant.ctypes.data, None) != 0:   # decode on the device
+            fd = None if fdata is None else np.ascontiguousarray(fdata[c][cy0:cy1], dtype=np.float32)
+            if lib.j2p_session_upload(s, c, data.ctypes.data, quant.ctypes.data, None if fd is None else fd.ctypes.data) != 0:
                 raise RuntimeError(lib.j2p_last_error().decode())
         self.width = lib.j2p_session_width(s)
         owned = C.c_uint()

@@ -3,7 +3,9 @@
 Given a frame (its planes' coefficient grids and sampling factors, the TGV weight) and a mode
 (single session or a batch of N frames, objective logging, the J2P_GRAD_SCALAR / J2P_PROJ_TILE22 /
 J2P_PROJ_TMA switches), this says which kernel instantiations one solver iteration launches and
-how many launches that is.  It follows jpeg2png_b200/csrc:
+how many launches that is.  `Mode.strip` restates a row-strip session (j2p_session_create_strip):
+the same frame can launch a different gradient instantiation, group its 1x1 planes differently and
+need stepped-only launches in one strip and not in another.  It follows jpeg2png_b200/csrc:
 
   launch_gradient / launch_gradient_packed   kernels_gradient.cu, kernels_gradient_packed.cu
   launch_project                             kernels_project.cu
@@ -50,6 +52,7 @@ class Mode:
     tile22: bool = True          # J2P_PROJ_TILE22 (0 turns it off)
     tma: bool = False            # J2P_PROJ_TMA=1
     device_decode: bool = False  # uploads without the caller's conventional decode (k_decode)
+    strip: tuple | None = None   # (row0, rows): a strip session of frame rows [row0, row0 + rows)
 
 
 def frame_size(planes):
@@ -57,15 +60,32 @@ def frame_size(planes):
     return max(p.cw * p.sw for p in planes), max(p.ch * p.sh for p in planes)
 
 
+def strip_rows(p: PlaneGeom, row0: int, rows: int) -> int:
+    """Coefficient rows of plane p a strip of frame rows [row0, row0 + rows) holds
+    (session.cu create_impl; strips.plane_rows_of_strip)."""
+    return min(-(-(row0 + rows) // p.sh), p.ch) - row0 // p.sh
+
+
+def local(planes, mode: Mode):
+    """(planes as the session holds them, W, rows the solver kernels target).  A strip session holds
+    the coefficient rows of its strip and targets its owned rows; a whole frame is its own strip."""
+    W, H = frame_size(planes)
+    if mode.strip is None:
+        return tuple(planes), W, H
+    row0, rows = mode.strip
+    return tuple(PlaneGeom(p.cw, strip_rows(p, row0, rows), p.sw, p.sh) for p in planes), W, rows
+
+
 def _b(v: bool) -> str:
     return 'true' if v else 'false'
 
 
 def gradient_kernel(planes, weight, mode: Mode) -> str:
-    """launch_gradient: the packed kernel unless logging or J2P_GRAD_SCALAR (single sessions only)."""
+    """launch_gradient: the packed kernel unless logging or J2P_GRAD_SCALAR (single sessions only).
+    In a strip the predicates see the strip's coefficient rows and its owned rows."""
     nc = len(planes)
     tgv = weight != 0.0
-    W, H = frame_size(planes)
+    planes, W, H = local(planes, mode)
     if not mode.log and (not mode.grad_scalar or mode.nframes > 1):
         full = all(p.sw == 1 and p.sh == 1 and p.cw == W and p.ch >= H for p in planes)
         c420 = (nc == 3 and planes[0].sw == 1 and planes[0].sh == 1 and planes[0].cw == W and
@@ -79,15 +99,19 @@ def gradient_kernel(planes, weight, mode: Mode) -> str:
 
 
 def projection_kernels(planes, mode: Mode):
-    """launch_project: the launches of one projection, in order (a list of kernel names)."""
-    W, H = frame_size(planes)
+    """launch_project: the launches of one projection, in order (a list of kernel names).  In a
+    strip, grouping and the stepped-only launches go by the strip's coefficient rows and owned rows;
+    `resample` stays the whole frame's."""
+    _, Wf, Hf = local(planes, Mode())
+    whole = planes
+    planes, W, H = local(planes, mode)
     batch = mode.nframes > 1
     tma = mode.tma and not batch        # a batch has no tensor maps (session.cu)
     out = []
     c = 0
     while c < len(planes):
         P = planes[c]
-        resample = not (P.cw == W and P.ch == H)
+        resample = not (whole[c].cw == Wf and whole[c].ch == Hf)
         if mode.log and (P.sw, P.sh) == (1, 1):
             out.append('k_project<1, 1>')              # one launch per plane, no grouping
             c += 1
@@ -125,8 +149,10 @@ def projection_kernels(planes, mode: Mode):
 
 
 def iteration(planes, weight, mode: Mode = Mode()):
-    """(kernel names launched by one iteration in order, number of launches)."""
-    ks = [gradient_kernel(planes, weight, mode)] + projection_kernels(planes, mode)
+    """(kernel names launched by one iteration in order, number of launches).  A strip iteration
+    folds the ranks' sums (k_fold_sums, j2p_session_project) between the two halves."""
+    fold = ['k_fold_sums'] if mode.strip is not None else []
+    ks = [gradient_kernel(planes, weight, mode)] + fold + projection_kernels(planes, mode)
     return ks, len(ks)
 
 

@@ -57,6 +57,30 @@ def test_strips_match_single_process(case, world, tmp_path):
     H.assert_bit_identical(got, want, f'{case} x{world} strips')
 
 
+@pytest.mark.parametrize('world', [2, 3, 8])
+@pytest.mark.parametrize('case', ['c420', 'c444'])
+def test_lockstep_driver_matches_single_process(case, world):
+    """The one-process lock-step driver of tests/test_gpu_strips_one_device.py, with oracle strips
+    only: N strips driven by it must give the whole-frame oracle's bits, so on the GPU a difference
+    is the product's and not the driver's."""
+    from tests.strip_backend import LockStep, OracleStrip
+    w, h, q, ss, weight, pw, iters = CASES[case]
+    img = synth.synth_coefs(w, h, q, ss, seed=4242)
+    fdata = H.decode_planes(img)
+    plan = strips.plan_strips(img.frame_h, 8 * max(p.h_samp for p in img.planes), world)
+    drv = LockStep([OracleStrip(img, weight, pw, iters, row0, rows, fdata) for row0, rows in plan])
+    try:
+        drv.start()
+        for _ in range(iters):
+            drv.project(drv.gradient())
+        got = drv.download()
+    finally:
+        for s in drv.strips:
+            s.close()
+    want = H.run_compute('oracle', img, [0, 1, 2], weight, pw, iters, [p.copy() for p in fdata])
+    H.assert_bit_identical(got, want, f'{case} x{world} lock-step strips')
+
+
 def test_plan_strips_alignment():
     for frame_h, mcu, world in [(4320, 16, 8), (1088, 16, 8), (2160, 8, 4), (64, 16, 4), (1088, 16, 3)]:
         plan = strips.plan_strips(frame_h, mcu, world)
