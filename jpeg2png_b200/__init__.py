@@ -1,8 +1,9 @@
 """jpeg2png_b200: the jpeg2png solver on H100.  `decode_jpeg` (jpeg2png_b200.decode) turns JPEG files
-into CUDA tensors, `encode_png` (jpeg2png_b200.encode) turns such tensors into PNG files on the
-device; torch is imported only when one of them is first used."""
+into CUDA tensors, `encode_png` (jpeg2png_b200.encode) and `encode_jpeg` (jpeg2png_b200.jpeg_encode)
+turn such tensors into PNG or JPEG files on the device; torch is imported only when one of them is
+first used."""
 
-__all__ = ['decode_jpeg', 'encode_png']
+__all__ = ['decode_jpeg', 'encode_png', 'encode_jpeg']
 
 
 def __getattr__(name):
@@ -12,4 +13,7 @@ def __getattr__(name):
     if name == 'encode_png':
         from .encode import encode_png
         return encode_png
+    if name == 'encode_jpeg':
+        from .jpeg_encode import encode_jpeg
+        return encode_jpeg
     raise AttributeError(f'module {__name__!r} has no attribute {name!r}')

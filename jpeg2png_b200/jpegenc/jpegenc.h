@@ -1,0 +1,81 @@
+/* jpegenc.h — libj2pjpegenc.so: RGB images in device memory to baseline JPEG files, encoded on the
+ * device.
+ *
+ * Each image is 8-bit RGB addressed with element strides for row, column and channel, so HWC, CHW
+ * and strided views are read in place.  The file is the one libjpeg's compressor writes with its
+ * defaults, as Pillow's JPEG writer drives it (quality q, subsampling s, no other options): SOI;
+ * APP0 JFIF 1.01, no units, density 1 x 1; DQT of table 0 (luma) and of table 1 (chroma), 8-bit,
+ * IJG quality scaling with the baseline clamp; SOF0 with components 1, 2, 3 sampled 1x1, 2x1 or 2x2
+ * for luma and 1x1 for chroma; DHT of the Annex K tables DC0, AC0, DC1, AC1; SOS of one interleaved
+ * scan; the entropy-coded data; EOI.  jpegenc_core.h states each step.
+ *
+ * One call: j2p_jpegenc_plan gives the size of the device work area for a list of images;
+ * j2p_jpegenc_encode queues the whole encode on a stream (after what is already queued there), reads
+ * back the n + 1 file offsets and, when given a host buffer, copies the files into it.  The launches
+ * of one call do not depend on the number or the sizes of the images.  j2p_jpegenc_encode_host runs
+ * the same steps serially on host memory and writes the same bytes.
+ *
+ * The work area is sized from a worst-case bound, so one call needs one read-back.  The bound of a
+ * block follows from the Annex K tables.  Luma: a DC difference costs at most 9 + 11 bits (category
+ * 11), and each of the 63 AC coefficients at most 16 + 10 (run 0, category 10, a 16-bit code); a
+ * run of zeros costs less per coefficient (ZRL is 11 bits for 16 zeros, EOB 4 bits, and a run r
+ * before a coefficient at most 16 + 10 bits for r + 1 of them).  So 20 + 63 x 26 = 1658 bits.
+ * Chroma: 11 + 11 for the DC and at most 22 per AC coefficient (its run 0, category 10 code is 12
+ * bits), 22 + 63 x 22 = 1408.  J2P_JPEGENC_BLOCK_BITS is the larger, and stuffing at most doubles
+ * the bytes.  For 64 images of 1920 x 1080 the work area is about 2.4 GB at 4:2:0, 4.7 GB at 4:4:4.
+ */
+#ifndef J2P_JPEGENC_H
+#define J2P_JPEGENC_H
+
+#include <stddef.h>
+#include <stdint.h>
+
+#ifdef __cplusplus
+extern "C" {
+#endif
+
+#define J2P_JPEGENC_BLOCK_BITS 1658u
+
+enum j2p_jpegenc_sampling { J2P_JPEGENC_444 = 0, J2P_JPEGENC_422 = 1, J2P_JPEGENC_420 = 2 };
+
+struct j2p_jpegenc_image {
+        const void *data;               /* first sample (R of the top-left pixel), uint8 */
+        uint32_t width, height;         /* 1 .. 65535 */
+        int64_t row_stride, col_stride, chan_stride;      /* in samples */
+};
+
+struct j2p_jpegenc_params {
+        int quality;                    /* 1 .. 100 */
+        int sampling;                   /* enum j2p_jpegenc_sampling */
+};
+
+struct j2p_jpegenc_stats {
+        unsigned launches;              /* kernel launches of the call */
+        uint64_t blocks;                /* 8 x 8 blocks coded, dummy blocks included, all images */
+};
+
+/* Work area for the n images: work_bytes in all, the files at out_offset in it.  Refuses null
+ * pointers, n == 0, a width or height of 0 or above 65535 (SOF's 16-bit fields), a quality outside
+ * 1 .. 100 and an unknown sampling.  Returns 0, or -1 (j2p_jpegenc_last_error). */
+int j2p_jpegenc_plan(const struct j2p_jpegenc_image *images, unsigned n, const struct j2p_jpegenc_params *params, size_t *work_bytes,
+                     size_t *out_offset);
+
+/* Encodes on `stream` (a cudaStream_t; NULL: the legacy default stream) into `work` (device memory
+ * of work_bytes on the images' device).  Writes offsets[0..n]: file i is bytes [offsets[i],
+ * offsets[i+1]) of the output, which starts at work + out_offset.  If dst is not NULL the files are
+ * copied there (dst_cap bytes at least offsets[n]).  Returns when the offsets (and dst) are on the
+ * host.  Also refuses image data or work memory that is not device memory of one device. */
+int j2p_jpegenc_encode(const struct j2p_jpegenc_image *images, unsigned n, const struct j2p_jpegenc_params *params, void *work,
+                       size_t work_bytes, void *stream, uint64_t *offsets, void *dst, size_t dst_cap, struct j2p_jpegenc_stats *stats);
+
+/* The same steps run serially on host memory (images and work in host memory). */
+int j2p_jpegenc_encode_host(const struct j2p_jpegenc_image *images, unsigned n, const struct j2p_jpegenc_params *params, void *work,
+                            size_t work_bytes, uint64_t *offsets);
+
+const char *j2p_jpegenc_last_error(void);
+
+#ifdef __cplusplus
+}
+#endif
+
+#endif

@@ -1,0 +1,181 @@
+"""encode_jpeg against Pillow on the host: prints one JSON line.
+
+usage: python tools/jpegenc_bench.py [--device D] [--files N] [--reps R] [--calls C]
+
+Workloads:
+  (a) N x 1920x1080 Q75 4:2:0 files (tools/decode_bench.py's), decoded by decode_jpeg at 100
+      iterations to uint8 CHW tensors, then encoded at q95 4:4:4, q90 4:2:0 and q75 4:2:0;
+  (b) N x 256x256 Q10 4:2:0 files, decoded at 50 iterations, encoded at q75 4:2:0;
+  (c) one 7680x4320 image (synth.cartoon_image), encoded at q90 4:2:0    (N = 64 by default).
+For each, reported are:
+  encoder       CUDA events around one whole j2p_jpegenc_encode call on all images (the host's
+                plan, the plan upload, the clearing of the bit stream, the seven kernels and the
+                read-back of the offsets), mean of C calls;
+  kernels       device time of each kernel per call (torch.profiler, C more calls);
+  encode_jpeg   wall clock of encode_jpeg(list of tensors) until the files are bytes;
+  host          wall clock of: tensors made contiguous HWC on the device and copied into one
+                shared-memory buffer on the host, then Pillow's JPEG writer, one file per task, in
+                as many worker processes as the process may use CPUs (png_bench.host_threads).
+                Processes, not threads: Pillow holds the GIL while it encodes, so a thread pool runs
+                the files one after another.  The workers are started before the timing.  With,
+                apart, the copies alone and Pillow on the first image alone in this process;
+  total bytes against encode_png's files for the same tensors, and whether every file equals the
+  host arm's byte for byte.
+Wall-clock figures are the best of R after one warm-up.  Also the card's name and power limit
+(read-only nvidia-smi query in the same run).  Writes nothing.
+"""
+import argparse
+import ctypes as C
+import io
+import json
+import os
+import sys
+import multiprocessing as mp
+from concurrent.futures import ProcessPoolExecutor
+from multiprocessing import shared_memory
+
+import numpy as np
+import torch
+from PIL import Image
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+from batch_bench import gpu_card  # noqa: E402
+from decode_bench import jpeg_files  # noqa: E402
+from png_bench import best_of, host_threads  # noqa: E402
+from jpeg2png_b200 import abi, decode_jpeg, encode_jpeg, encode_png, synth  # noqa: E402
+from jpeg2png_b200 import jpeg_encode as J  # noqa: E402
+
+KERNELS = ('k_je_blocks', 'k_je_sizes', 'k_je_scan', 'k_je_emit', 'k_je_ffcount', 'k_je_offsets', 'k_je_stuff')
+
+
+def encoder_ms(tensors, quality, subsampling, calls):
+    """CUDA events around one whole j2p_jpegenc_encode call, mean of `calls`; and each kernel's
+    device time per call from torch.profiler over `calls` more calls."""
+    lib = J.load_jpegenc()
+    p = J.params(quality, subsampling)
+    d = J._descs(tensors, 'CHW', lambda x: x.data_ptr(), lambda x: x.stride())
+    n, o = C.c_size_t(), C.c_size_t()
+    J._check(lib.j2p_jpegenc_plan(d, len(tensors), C.byref(p), C.byref(n), C.byref(o)))
+    work = torch.empty(n.value, dtype=torch.uint8, device=tensors[0].device)
+    offs = (C.c_uint64 * (len(tensors) + 1))()
+    stream = torch.cuda.current_stream()
+
+    def call():
+        J._check(lib.j2p_jpegenc_encode(d, len(tensors), C.byref(p), work.data_ptr(), n.value, stream.cuda_stream, offs, None, 0, None))
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    call()
+    times = []
+    for _ in range(calls):
+        e0.record()
+        call()
+        e1.record()
+        e1.synchronize()
+        times.append(e0.elapsed_time(e1))
+    with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
+        for _ in range(calls):
+            call()
+        torch.cuda.synchronize()
+    kernels = {}
+    for ev in prof.key_averages():
+        name = next((k for k in KERNELS if k in ev.key), None)
+        if name:
+            us = getattr(ev, 'device_time_total', None) or getattr(ev, 'cuda_time_total', 0)
+            kernels[name] = kernels.get(name, 0.0) + us / 1e3 / calls
+    return {'ms_per_call': float(np.mean(times)), 'work_bytes': n.value, 'kernel_ms_per_call': kernels}
+
+
+def pillow(hwc, quality, subsampling):
+    buf = io.BytesIO()
+    Image.fromarray(hwc, 'RGB').save(buf, 'JPEG', quality=quality, subsampling=subsampling)
+    return buf.getvalue()
+
+
+_shm = {}
+
+
+def _pillow_shared(name, size, offset, h, w, quality, subsampling):
+    """In a worker process: Pillow on image (h, w, 3) at `offset` of the shared buffer `name`."""
+    if name not in _shm:
+        _shm[name] = shared_memory.SharedMemory(name=name)
+    hwc = np.ndarray((h, w, 3), np.uint8, buffer=_shm[name].buf[:size], offset=offset)
+    return pillow(hwc, quality, subsampling)
+
+
+def host_arm(tensors, quality, subsampling, reps, procs):
+    """Best-of-`reps` seconds and files of the host arm (copies, then Pillow in `procs` worker
+    processes), and apart the copies alone and Pillow on the first image in this process."""
+    shapes = [(t.shape[1], t.shape[2]) for t in tensors]
+    offs = np.cumsum([0] + [h * w * 3 for h, w in shapes]).tolist()
+    shm = shared_memory.SharedMemory(create=True, size=offs[-1])
+    try:
+        buf = torch.from_numpy(np.ndarray((offs[-1],), np.uint8, buffer=shm.buf))
+        views = [buf[offs[k]:offs[k + 1]].view(h, w, 3) for k, (h, w) in enumerate(shapes)]
+
+        def copies():
+            for v, t in zip(views, tensors):
+                v.copy_(t.permute(1, 2, 0).contiguous())
+        with ProcessPoolExecutor(procs, mp_context=mp.get_context('spawn')) as pool:
+            list(pool.map(_pillow_shared, [shm.name] * procs, [offs[-1]] * procs, [0] * procs, [1] * procs, [1] * procs,
+                          [quality] * procs, [subsampling] * procs))        # start and attach every worker
+
+            def arm():
+                copies()
+                return list(pool.map(_pillow_shared, [shm.name] * len(shapes), [offs[-1]] * len(shapes), offs[:-1],
+                                     [h for h, _ in shapes], [w for _, w in shapes], [quality] * len(shapes),
+                                     [subsampling] * len(shapes)))
+            t_host, host_files = best_of(arm, reps)
+        t_copy, _ = best_of(copies, reps)
+        t_one, _ = best_of(lambda: pillow(views[0].numpy(), quality, subsampling), reps)
+        del buf, views
+    finally:
+        shm.close()
+        shm.unlink()
+    return t_host, host_files, t_copy, t_one
+
+
+def run(tensors, label, quality, subsampling, reps, calls, threads, png_bytes):
+    out = {'workload': label, 'images': len(tensors), 'quality': quality, 'subsampling': subsampling}
+    out['encoder'] = encoder_ms(tensors, quality, subsampling, calls)
+    t_gpu, files = best_of(lambda: encode_jpeg(tensors, quality=quality, subsampling=subsampling), reps)
+
+    t_host, host_files, t_copy, t_one = host_arm(tensors, quality, subsampling, reps, threads)
+    total = sum(map(len, files))
+    out['encode_jpeg'] = {'wall_ms': t_gpu * 1e3, 'ms_per_image': t_gpu / len(tensors) * 1e3, 'total_bytes': total}
+    out['host_pillow'] = {'wall_ms': t_host * 1e3, 'ms_per_image': t_host / len(tensors) * 1e3, 'processes': threads,
+                          'copies_alone_ms': t_copy * 1e3, 'one_image_one_thread_ms': t_one * 1e3}
+    out['speedup_vs_host'] = t_host / t_gpu
+    out['bytes_vs_encode_png'] = total / png_bytes
+    out['identical_to_host'] = files == host_files
+    return out
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument('--device', type=int, default=0)
+    ap.add_argument('--files', type=int, default=64)
+    ap.add_argument('--reps', type=int, default=3)
+    ap.add_argument('--calls', type=int, default=20)
+    args = ap.parse_args()
+    if abi.load_product().j2p_device_count() <= 0 or not torch.cuda.is_available():
+        raise SystemExit('jpegenc_bench.py: no CUDA device')
+    torch.cuda.set_device(args.device)
+    threads, n = host_threads(), args.files
+    line = {'card': gpu_card(args.device),
+            'timing': f'wall clock, one warm-up, best of {args.reps}; encoder: CUDA events, mean of {args.calls} calls',
+            'workloads': []}
+    big = decode_jpeg(jpeg_files(1920, 1080, 75, n), iterations=100, dtype=torch.uint8)
+    small = decode_jpeg(jpeg_files(256, 256, 10, n), iterations=50, dtype=torch.uint8)
+    img8k = torch.from_numpy(synth.cartoon_image(7680, 4320, 9).round().astype(np.uint8).transpose(2, 0, 1).copy()).cuda()
+    torch.cuda.synchronize()
+    for tensors, label, cases in ((big, f'{n} x 1920x1080 Q75 4:2:0, -i 100', ((95, '4:4:4'), (90, '4:2:0'), (75, '4:2:0'))),
+                                  (small, f'{n} x 256x256 Q10 4:2:0, -i 50', ((75, '4:2:0'),)),
+                                  ([img8k], '1 x 7680x4320 cartoon', ((90, '4:2:0'),))):
+        png_bytes = sum(map(len, encode_png(tensors)))
+        for q, s in cases:
+            line['workloads'].append(run(tensors, label, q, s, args.reps, args.calls, threads, png_bytes))
+    print(json.dumps(line), flush=True)
+
+
+if __name__ == '__main__':
+    main()
