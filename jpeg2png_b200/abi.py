@@ -121,6 +121,21 @@ class CoefArray:
 _PKG_DIR = os.path.dirname(os.path.abspath(__file__))
 PRODUCT_LIB = os.path.join(_PKG_DIR, 'csrc', 'libjpeg2png_b200.so')
 
+_libraries = {}
+
+
+def load_library(path: str, what: str, declare) -> C.CDLL:
+    """The library at path (one of the package tree's helper libraries, `what` naming it in the
+    error when it has not been built), loaded once and passed to declare(lib) to set its argtypes."""
+    if path not in _libraries:
+        if not os.path.exists(path):
+            raise RuntimeError(f'{path} is missing: the {what} has not been built '
+                               '(run `python -c "import __graft_entry__ as g; g.build()"`)')
+        lib = C.CDLL(path, mode=C.RTLD_LOCAL)
+        declare(lib)
+        _libraries[path] = lib
+    return _libraries[path]
+
 
 def declare_product(lib: C.CDLL) -> C.CDLL:
     """Attach argtypes/restypes for every symbol include/jpeg2png_b200.h declares."""

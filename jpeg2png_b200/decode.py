@@ -72,49 +72,37 @@ ENTROPY_LIB = os.path.join(abi._PKG_DIR, 'entropy', 'libj2pentropy.so')
 SUBSEQ_BITS = 1024                  # bits per subsequence of the device decoder (DESIGN §7d)
 ENT_FAILURES = {1: 'bad huffman code', 2: 'bad magnitude category', 3: 'coefficient index out of range'}
 
-_codecs = None
-_entropy = None
+def _declare_codecs(lib):
+    lib.j2p_read_jpeg_mem.restype = C.c_int
+    lib.j2p_read_jpeg_mem.argtypes = [C.c_char_p, C.c_size_t, C.POINTER(Jpeg), C.c_char_p, C.c_size_t]
+    lib.j2p_read_jpeg_layout.restype = C.c_int
+    lib.j2p_read_jpeg_layout.argtypes = [C.c_char_p, C.c_size_t, C.POINTER(Layout), C.c_char_p, C.c_size_t]
+    lib.j2p_free_jpeg_layout.restype = None
+    lib.j2p_free_jpeg_layout.argtypes = [C.POINTER(Layout)]
 
 
 def load_codecs() -> C.CDLL:
     """libj2pcodecs.so (the command line's JPEG reader) from the package tree."""
-    global _codecs
-    if _codecs is None:
-        if not os.path.exists(CODECS_LIB):
-            raise RuntimeError(f'{CODECS_LIB} is missing: the command line has not been built '
-                               '(run `python -c "import __graft_entry__ as g; g.build()"`)')
-        lib = C.CDLL(CODECS_LIB, mode=C.RTLD_LOCAL)
-        lib.j2p_read_jpeg_mem.restype = C.c_int
-        lib.j2p_read_jpeg_mem.argtypes = [C.c_char_p, C.c_size_t, C.POINTER(Jpeg), C.c_char_p, C.c_size_t]
-        lib.j2p_read_jpeg_layout.restype = C.c_int
-        lib.j2p_read_jpeg_layout.argtypes = [C.c_char_p, C.c_size_t, C.POINTER(Layout), C.c_char_p, C.c_size_t]
-        lib.j2p_free_jpeg_layout.restype = None
-        lib.j2p_free_jpeg_layout.argtypes = [C.POINTER(Layout)]
-        _codecs = lib
-    return _codecs
+    return abi.load_library(CODECS_LIB, 'command line', _declare_codecs)
+
+
+def _declare_entropy(lib):
+    vp, lay = C.c_void_p, C.POINTER(C.POINTER(Layout))
+    lib.j2p_entropy_plan_size.restype = C.c_int
+    lib.j2p_entropy_plan_size.argtypes = [lay, C.c_uint, C.c_uint, C.POINTER(C.c_size_t), C.POINTER(C.c_size_t)]
+    lib.j2p_entropy_pack.restype = C.c_int
+    lib.j2p_entropy_pack.argtypes = [lay, C.c_uint, C.c_uint, C.POINTER(vp), vp, C.c_size_t]
+    lib.j2p_entropy_decode.restype = C.c_int
+    lib.j2p_entropy_decode.argtypes = [vp, vp, vp, vp, vp, C.POINTER(EntropyStats)]
+    lib.j2p_entropy_decode_host.restype = C.c_int
+    lib.j2p_entropy_decode_host.argtypes = [vp, vp, vp, C.POINTER(EntropyStats)]
+    lib.j2p_entropy_last_error.restype = C.c_char_p
+    lib.j2p_entropy_last_error.argtypes = []
 
 
 def load_entropy() -> C.CDLL:
     """libj2pentropy.so (the device entropy decoder) from the package tree."""
-    global _entropy
-    if _entropy is None:
-        if not os.path.exists(ENTROPY_LIB):
-            raise RuntimeError(f'{ENTROPY_LIB} is missing: the entropy decoder has not been built '
-                               '(run `python -c "import __graft_entry__ as g; g.build()"`)')
-        lib = C.CDLL(ENTROPY_LIB, mode=C.RTLD_LOCAL)
-        vp, lay = C.c_void_p, C.POINTER(C.POINTER(Layout))
-        lib.j2p_entropy_plan_size.restype = C.c_int
-        lib.j2p_entropy_plan_size.argtypes = [lay, C.c_uint, C.c_uint, C.POINTER(C.c_size_t), C.POINTER(C.c_size_t)]
-        lib.j2p_entropy_pack.restype = C.c_int
-        lib.j2p_entropy_pack.argtypes = [lay, C.c_uint, C.c_uint, C.POINTER(vp), vp, C.c_size_t]
-        lib.j2p_entropy_decode.restype = C.c_int
-        lib.j2p_entropy_decode.argtypes = [vp, vp, vp, vp, vp, C.POINTER(EntropyStats)]
-        lib.j2p_entropy_decode_host.restype = C.c_int
-        lib.j2p_entropy_decode_host.argtypes = [vp, vp, vp, C.POINTER(EntropyStats)]
-        lib.j2p_entropy_last_error.restype = C.c_char_p
-        lib.j2p_entropy_last_error.argtypes = []
-        _entropy = lib
-    return _entropy
+    return abi.load_library(ENTROPY_LIB, 'entropy decoder', _declare_entropy)
 
 
 class FileLayout:

@@ -1,35 +1,15 @@
 // entropy.cu — libj2pentropy.so: packing of JPEG layouts, the device decoder (sync rounds, exclusive
 // scans, final pass, DC pass) and the serial host driver of the same phases.  See entropy.h and
 // entropy_core.h.
-#include <cuda_runtime.h>
-
-#include <stdarg.h>
-#include <stdio.h>
 #include <string.h>
 
 #include "../cli/jpeg_reader.h"
+#include "../common/codec_host.h"
 #include "entropy_core.h"
-
-static thread_local char g_err[256];
-
-static int fail(const char *fmt, ...) {
-    va_list ap;
-    va_start(ap, fmt);
-    vsnprintf(g_err, sizeof g_err, fmt, ap);
-    va_end(ap);
-    return -1;
-}
 
 extern "C" const char *j2p_entropy_last_error(void) { return g_err; }
 
-#define CK(x)                                                                                   \
-    do {                                                                                        \
-        const cudaError_t e_ = (x);                                                             \
-        if (e_ != cudaSuccess) return fail("%s: %s", #x, cudaGetErrorString(e_));               \
-    } while (0)
-
 static const uint32_t kMagic = 0x4a32454eu;     // "J2EN"
-static size_t align16(size_t n) { return (n + 15) & ~(size_t)15; }
 
 // ---- plan --------------------------------------------------------------------------------------
 struct Counts {

@@ -25,12 +25,7 @@
 #include <stdint.h>
 #include <string.h>
 
-#ifdef __CUDACC__
-#define J2P_HD __host__ __device__ __forceinline__
-#else
-#define J2P_HD static inline
-#endif
-
+#include "../common/codec_host.h"       /* J2P_HD */
 #include "entropy.h"
 
 #define J2P_ENT_MAX_BPM 48      /* blocks per MCU: three components of up to 4x4 (the reader allows 4) */

@@ -13,13 +13,14 @@ The module is not called encode_jpeg.py: importing it would make the package att
 from __future__ import annotations
 
 import ctypes as C
+import dataclasses
 import os
 
 import numpy as np
 import torch
 
 from . import abi
-from .encode import _axes
+from . import batch_encode as B
 
 JPEGENC_LIB = os.path.join(abi._PKG_DIR, 'jpegenc', 'libj2pjpegenc.so')
 SAMPLINGS = {'4:4:4': 0, '4:2:2': 1, '4:2:0': 2}
@@ -42,34 +43,22 @@ class Stats(C.Structure):
     _fields_ = [('launches', C.c_uint), ('blocks', C.c_uint64)]
 
 
-_lib = None
+def _declare(lib):
+    vp, sz = C.c_void_p, C.c_size_t
+    imgs, par = C.POINTER(Image), C.POINTER(Params)
+    lib.j2p_jpegenc_plan.restype = C.c_int
+    lib.j2p_jpegenc_plan.argtypes = [imgs, C.c_uint, par, C.POINTER(sz), C.POINTER(sz)]
+    lib.j2p_jpegenc_encode.restype = C.c_int
+    lib.j2p_jpegenc_encode.argtypes = [imgs, C.c_uint, par, vp, sz, vp, C.POINTER(C.c_uint64), vp, sz, C.POINTER(Stats)]
+    lib.j2p_jpegenc_encode_host.restype = C.c_int
+    lib.j2p_jpegenc_encode_host.argtypes = [imgs, C.c_uint, par, vp, sz, C.POINTER(C.c_uint64)]
+    lib.j2p_jpegenc_last_error.restype = C.c_char_p
+    lib.j2p_jpegenc_last_error.argtypes = []
 
 
 def load_jpegenc() -> C.CDLL:
     """libj2pjpegenc.so (the device JPEG encoder) from the package tree."""
-    global _lib
-    if _lib is None:
-        if not os.path.exists(JPEGENC_LIB):
-            raise RuntimeError(f'{JPEGENC_LIB} is missing: the JPEG encoder has not been built '
-                               '(run `python -c "import __graft_entry__ as g; g.build()"`)')
-        lib = C.CDLL(JPEGENC_LIB, mode=C.RTLD_LOCAL)
-        vp, sz = C.c_void_p, C.c_size_t
-        imgs, par = C.POINTER(Image), C.POINTER(Params)
-        lib.j2p_jpegenc_plan.restype = C.c_int
-        lib.j2p_jpegenc_plan.argtypes = [imgs, C.c_uint, par, C.POINTER(sz), C.POINTER(sz)]
-        lib.j2p_jpegenc_encode.restype = C.c_int
-        lib.j2p_jpegenc_encode.argtypes = [imgs, C.c_uint, par, vp, sz, vp, C.POINTER(C.c_uint64), vp, sz, C.POINTER(Stats)]
-        lib.j2p_jpegenc_encode_host.restype = C.c_int
-        lib.j2p_jpegenc_encode_host.argtypes = [imgs, C.c_uint, par, vp, sz, C.POINTER(C.c_uint64)]
-        lib.j2p_jpegenc_last_error.restype = C.c_char_p
-        lib.j2p_jpegenc_last_error.argtypes = []
-        _lib = lib
-    return _lib
-
-
-def _check(rc, error=RuntimeError):
-    if rc != 0:
-        raise error(load_jpegenc().j2p_jpegenc_last_error().decode())
+    return abi.load_library(JPEGENC_LIB, 'JPEG encoder', _declare)
 
 
 def params(quality, subsampling) -> Params:
@@ -81,60 +70,38 @@ def params(quality, subsampling) -> Params:
     return Params(int(quality), SAMPLINGS[subsampling])
 
 
+def _check_size(shape, h, w):
+    if not (1 <= h <= MAX_SIDE and 1 <= w <= MAX_SIDE):
+        raise ValueError(f'a JPEG image is 1..{MAX_SIDE} pixels high and wide; got shape {tuple(shape)}')
+
+
+CODEC = B.Codec('jpegenc', lambda: load_jpegenc(), Image, _check_size)
+
+
+def codec(p: Params) -> B.Codec:
+    """libj2pjpegenc.so for the shared driver, with the call parameters p."""
+    return dataclasses.replace(CODEC, params=(C.byref(p),))
+
+
 def _descs(items, layout, ptr, strides):
-    out = (Image * len(items))()
-    for d, x in zip(out, items):
-        h, w, ra, ca, ka = _axes(x.shape, layout)
-        if not (1 <= h <= MAX_SIDE and 1 <= w <= MAX_SIDE):
-            raise ValueError(f'a JPEG image is 1..{MAX_SIDE} pixels high and wide; got shape {tuple(x.shape)}')
-        st = strides(x)
-        d.data, d.width, d.height = ptr(x), w, h
-        d.row_stride, d.col_stride, d.chan_stride = st[ra], st[ca], st[ka]
-    return out
+    """The image structs of items; ptr(x) and strides(x) give x's address and strides in elements."""
+    return B.descs(CODEC, items, layout, ptr, strides)
+
+
+def _work_bytes(descs, p):
+    """The work area of one call on descs with the call parameters p."""
+    return codec(p).plan(descs)[0]
 
 
 def encode_host(images, quality=75, subsampling='4:2:0', layout='HWC'):
     """The serial host driver (j2p_jpegenc_encode_host) on numpy uint8 arrays: a list of JPEG files
     as bytes, the same bytes the device writes."""
-    if layout not in ('CHW', 'HWC'):
-        raise ValueError(f"layout must be 'CHW' or 'HWC', not {layout!r}")
+    B.check_layout(layout)
     p = params(quality, subsampling)
     for x in images:
         if x.dtype != np.uint8:
             raise ValueError(f'samples are uint8, not {x.dtype}')
-    lib = load_jpegenc()
-    d = _descs(images, layout, lambda x: x.ctypes.data, lambda x: [s // x.itemsize for s in x.strides])
-    work_bytes, out_off = C.c_size_t(), C.c_size_t()
-    _check(lib.j2p_jpegenc_plan(d, len(images), C.byref(p), C.byref(work_bytes), C.byref(out_off)), ValueError)
-    work = np.zeros(work_bytes.value, np.uint8)
-    offs = (C.c_uint64 * (len(images) + 1))()
-    _check(lib.j2p_jpegenc_encode_host(d, len(images), C.byref(p), work.ctypes.data, work_bytes.value, offs))
-    base = out_off.value
-    return [work[base + offs[i]:base + offs[i + 1]].tobytes() for i in range(len(images))]
-
-
-def _work_bytes(descs, p):
-    n = C.c_size_t()
-    _check(load_jpegenc().j2p_jpegenc_plan(descs, len(descs), C.byref(p), C.byref(n), None), ValueError)
-    return n.value
-
-
-def _chunks(descs, p, free_bytes):
-    """Split the images, in order, so that each chunk's work area fits in a quarter of the free
-    device memory (encode_png's rule); one chunk when everything fits."""
-    budget = free_bytes // 4
-    if _work_bytes(descs, p) <= budget:
-        return [list(range(len(descs)))]
-    chunks, cur, used = [], [], 0
-    for i in range(len(descs)):
-        need = _work_bytes((Image * 1)(descs[i]), p)
-        if cur and used + need > budget:
-            chunks.append(cur)
-            cur, used = [], 0
-        cur.append(i)
-        used += need
-    chunks.append(cur)
-    return chunks
+    return B.encode_host(codec(p), images, layout)
 
 
 def encode_jpeg(images, *, quality=75, subsampling='4:2:0', layout='CHW'):
@@ -153,47 +120,5 @@ def encode_jpeg(images, *, quality=75, subsampling='4:2:0', layout='CHW'):
     size, and for a tensor that is not on a CUDA device, and RuntimeError when no CUDA device is
     usable.
     """
-    if layout not in ('CHW', 'HWC'):
-        raise ValueError(f"layout must be 'CHW' or 'HWC', not {layout!r}")
-    p = params(quality, subsampling)
-    single = not isinstance(images, (list, tuple))
-    items = [images] if single else list(images)
-    for x in items:
-        if not isinstance(x, torch.Tensor):
-            raise ValueError(f'encode_jpeg takes torch tensors, not {type(x).__name__}')
-        if x.dtype != torch.uint8:
-            raise ValueError(f'encode_jpeg takes torch.uint8 tensors, not {x.dtype}')
-        h, w, *_ = _axes(x.shape, layout)
-        if not (1 <= h <= MAX_SIDE and 1 <= w <= MAX_SIDE):
-            raise ValueError(f'a JPEG image is 1..{MAX_SIDE} pixels high and wide; got shape {tuple(x.shape)}')
-        if x.device.type != 'cuda':
-            raise ValueError(f'encode_jpeg encodes CUDA tensors; this one is on {x.device}')
-    if not torch.cuda.is_available() or torch.cuda.device_count() <= 0:
-        raise RuntimeError('encode_jpeg needs a CUDA device: the encoder has no CPU fallback')
-    if not items:
-        return []
-    device = items[0].device
-    if any(x.device != device for x in items):
-        raise ValueError('all images of one call must be on the same device')
-    lib = load_jpegenc()
-    descs = _descs(items, layout, lambda x: x.data_ptr(), lambda x: x.stride())
-    results = [None] * len(items)
-    with torch.cuda.device(device):
-        stream = torch.cuda.current_stream(device)
-        free = torch.cuda.mem_get_info(device)[0]
-        for idx in _chunks(descs, p, free):
-            d = (Image * len(idx))(*[descs[i] for i in idx])
-            work_bytes, out_off = C.c_size_t(), C.c_size_t()
-            _check(lib.j2p_jpegenc_plan(d, len(idx), C.byref(p), C.byref(work_bytes), C.byref(out_off)), ValueError)
-            work = torch.empty(work_bytes.value, dtype=torch.uint8, device=device)
-            offs = (C.c_uint64 * (len(idx) + 1))()
-            _check(lib.j2p_jpegenc_encode(d, len(idx), C.byref(p), work.data_ptr(), work_bytes.value, stream.cuda_stream, offs,
-                                          None, 0, None))
-            total = offs[len(idx)]
-            host = torch.empty(total, dtype=torch.uint8, pin_memory=True)
-            host.copy_(work[out_off.value:out_off.value + total])        # synchronous: the files are on the host
-            view = host.numpy()
-            for k, i in enumerate(idx):
-                results[i] = view[offs[k]:offs[k + 1]].tobytes()
-            del work
-    return results[0] if single else results
+    B.check_layout(layout)
+    return B.encode_tensors('encode_jpeg', codec(params(quality, subsampling)), images, layout, (torch.uint8,))

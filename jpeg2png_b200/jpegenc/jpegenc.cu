@@ -4,32 +4,12 @@
 #include <cub/block/block_reduce.cuh>
 #include <cub/block/block_scan.cuh>
 
-#include <stdarg.h>
-#include <stdio.h>
-#include <stdlib.h>
 #include <string.h>
 
+#include "../common/codec_host.h"
 #include "jpegenc_core.h"
 
-static thread_local char g_err[256];
-
-static int fail(const char *fmt, ...) {
-    va_list ap;
-    va_start(ap, fmt);
-    vsnprintf(g_err, sizeof g_err, fmt, ap);
-    va_end(ap);
-    return -1;
-}
-
 extern "C" const char *j2p_jpegenc_last_error(void) { return g_err; }
-
-#define CK(x)                                                                                   \
-    do {                                                                                        \
-        const cudaError_t e_ = (x);                                                             \
-        if (e_ != cudaSuccess) return fail("%s: %s", #x, cudaGetErrorString(e_));               \
-    } while (0)
-
-static size_t align16(size_t n) { return (n + 15) & ~(size_t)15; }
 
 // ---- tables ------------------------------------------------------------------------------------
 static const uint8_t kNatural[64] = {0,  1,  8,  16, 9,  2,  3,  10, 17, 24, 32, 25, 18, 11, 4,  5,  12, 19, 26, 33, 40, 48,
@@ -587,88 +567,38 @@ __global__ void __launch_bounds__(kChunkThreads) k_je_stuff(const struct j2p_je_
     }
 }
 
-static int device_of(const void *ptr, const char *what, int *dev) {
-    cudaPointerAttributes a;
-    const cudaError_t e = cudaPointerGetAttributes(&a, ptr);
-    if (e != cudaSuccess) {
-        cudaGetLastError();
-        return fail("%s: %s", what, cudaGetErrorString(e));
-    }
-    if (a.type != cudaMemoryTypeDevice) return fail("%s is not device memory", what);
-    *dev = a.device;
-    return 0;
-}
-
-struct DeviceGuard {
-    int prev = -1;
-    ~DeviceGuard() {
-        if (prev >= 0) cudaSetDevice(prev);
-    }
-};
-
 extern "C" int j2p_jpegenc_encode(const struct j2p_jpegenc_image *images, unsigned n, const struct j2p_jpegenc_params *params, void *work,
                                   size_t work_bytes, void *stream, uint64_t *offsets, void *dst, size_t dst_cap, struct j2p_jpegenc_stats *stats) {
     Layout L;
     if (make_plan(images, n, params, &L, nullptr) != 0) return -1;
-    if (!work || !offsets) return fail("null argument");
-    if (work_bytes < L.total) return fail("work area of %zu bytes is smaller than the plan's %zu", work_bytes, L.total);
-    int dev = -1, d = -1;
-    if (device_of(work, "the work area", &dev) != 0) return -1;
-    for (unsigned i = 0; i < n; i++) {
-        char what[48];
-        snprintf(what, sizeof what, "image %u's data", i);
-        if (device_of(images[i].data, what, &d) != 0) return -1;
-        if (d != dev) return fail("image %u is on device %d, the work area on device %d", i, d, dev);
-    }
-    DeviceGuard guard;
-    CK(cudaGetDevice(&guard.prev));
-    CK(cudaSetDevice(dev));
-    const cudaStream_t st = (cudaStream_t)stream;
-    uint8_t *plan = (uint8_t *)malloc(L.off_tsum);
-    if (!plan) return fail("out of host memory");
-    if (fill_plan(images, n, params, L, plan) != 0) { free(plan); return -1; }
-    uint8_t *w = (uint8_t *)work;
-    const cudaError_t ec = cudaMemcpyAsync(w, plan, L.off_tsum, cudaMemcpyHostToDevice, st);
-    if (ec != cudaSuccess) { free(plan); return fail("plan upload: %s", cudaGetErrorString(ec)); }
-    struct j2p_je_img *imgs = (struct j2p_je_img *)(w + L.off_imgs);
-    const struct j2p_je_tables *t = (const struct j2p_je_tables *)(w + L.off_tab);
-    uint32_t *tsum = (uint32_t *)(w + L.off_tsum), *intra = (uint32_t *)(w + L.off_intra), *ffc = (uint32_t *)(w + L.off_ffc);
-    uint64_t *toff = (uint64_t *)(w + L.off_toff), *ffpre = (uint64_t *)(w + L.off_ffpre), *offs = (uint64_t *)(w + L.off_offs);
-    int16_t *coef = (int16_t *)(w + L.off_coef);
-    uint32_t *raw = (uint32_t *)(w + L.off_raw);
-    const cudaError_t em = cudaMemsetAsync(raw, 0, L.words * sizeof(uint32_t), st);
-    if (em != cudaSuccess) { free(plan); return fail("clearing the entropy words: %s", cudaGetErrorString(em)); }
-    const uint64_t bgrid = (L.nblk * 8 + kBlockThreads - 1) / kBlockThreads;
-    unsigned launches = 0;              // kernels queued without a launch error
-    auto counted = [&]() { launches += cudaPeekAtLastError() == cudaSuccess; };
-    k_je_blocks<<<(unsigned)bgrid, kBlockThreads, 0, st>>>(imgs, n, t, L.nblk, coef);
-    counted();
-    k_je_sizes<<<L.ntiles, kTileThreads, 0, st>>>(imgs, n, t, coef, intra, tsum);
-    counted();
-    k_je_scan<<<n, kScanThreads, 0, st>>>(imgs, tsum, toff, raw);
-    counted();
-    k_je_emit<<<L.ntiles, kTileThreads, 0, st>>>(imgs, n, t, coef, intra, toff, raw);
-    counted();
-    k_je_ffcount<<<L.nchunks, kChunkThreads, 0, st>>>(imgs, n, raw, ffc);
-    counted();
-    k_je_offsets<<<1, kScanThreads, 0, st>>>(imgs, n, ffc, L.nchunks, ffpre, offs);
-    counted();
-    k_je_stuff<<<L.nchunks, kChunkThreads, 0, st>>>(imgs, n, t, raw, ffpre, w + L.off_out);
-    counted();
-    const cudaError_t el = cudaGetLastError();
-    if (el != cudaSuccess) { free(plan); return fail("launch: %s", cudaGetErrorString(el)); }
-    const cudaError_t eo = cudaMemcpyAsync(offsets, offs, (n + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, st);
-    const cudaError_t es = eo == cudaSuccess ? cudaStreamSynchronize(st) : eo;
-    free(plan);                         // the upload has been read by now
-    if (es != cudaSuccess) return fail("encode: %s", cudaGetErrorString(es));
-    if (dst) {
-        if (dst_cap < offsets[n]) return fail("destination of %zu bytes is smaller than the files (%llu)", dst_cap, (unsigned long long)offsets[n]);
-        CK(cudaMemcpyAsync(dst, w + L.off_out, offsets[n], cudaMemcpyDeviceToHost, st));
-        CK(cudaStreamSynchronize(st));
-    }
-    if (stats) {
-        stats->launches = launches;
-        stats->blocks = L.nblk;
-    }
+    const auto fill = [&](uint8_t *plan) { return fill_plan(images, n, params, L, plan); };
+    const auto launch = [&](uint8_t *w, cudaStream_t st, const uint8_t *, auto counted) {
+        struct j2p_je_img *imgs = (struct j2p_je_img *)(w + L.off_imgs);
+        const struct j2p_je_tables *t = (const struct j2p_je_tables *)(w + L.off_tab);
+        uint32_t *tsum = (uint32_t *)(w + L.off_tsum), *intra = (uint32_t *)(w + L.off_intra), *ffc = (uint32_t *)(w + L.off_ffc);
+        uint64_t *toff = (uint64_t *)(w + L.off_toff), *ffpre = (uint64_t *)(w + L.off_ffpre), *offs = (uint64_t *)(w + L.off_offs);
+        int16_t *coef = (int16_t *)(w + L.off_coef);
+        uint32_t *raw = (uint32_t *)(w + L.off_raw);
+        const cudaError_t em = cudaMemsetAsync(raw, 0, L.words * sizeof(uint32_t), st);
+        if (em != cudaSuccess) return fail("clearing the entropy words: %s", cudaGetErrorString(em));
+        const uint64_t bgrid = (L.nblk * 8 + kBlockThreads - 1) / kBlockThreads;
+        k_je_blocks<<<(unsigned)bgrid, kBlockThreads, 0, st>>>(imgs, n, t, L.nblk, coef);
+        counted();
+        k_je_sizes<<<L.ntiles, kTileThreads, 0, st>>>(imgs, n, t, coef, intra, tsum);
+        counted();
+        k_je_scan<<<n, kScanThreads, 0, st>>>(imgs, tsum, toff, raw);
+        counted();
+        k_je_emit<<<L.ntiles, kTileThreads, 0, st>>>(imgs, n, t, coef, intra, toff, raw);
+        counted();
+        k_je_ffcount<<<L.nchunks, kChunkThreads, 0, st>>>(imgs, n, raw, ffc);
+        counted();
+        k_je_offsets<<<1, kScanThreads, 0, st>>>(imgs, n, ffc, L.nchunks, ffpre, offs);
+        counted();
+        k_je_stuff<<<L.nchunks, kChunkThreads, 0, st>>>(imgs, n, t, raw, ffpre, w + L.off_out);
+        counted();
+        return 0;
+    };
+    if (encode_call(images, n, L, L.off_tsum, work, work_bytes, stream, offsets, dst, dst_cap, stats, fill, launch) != 0) return -1;
+    if (stats) stats->blocks = L.nblk;
     return 0;
 }

@@ -22,13 +22,8 @@
 
 #include <stdint.h>
 
+#include "../common/codec_host.h"       // J2P_HD
 #include "jpegenc.h"
-
-#ifdef __CUDACC__
-#define J2P_HD __host__ __device__ __forceinline__
-#else
-#define J2P_HD static inline
-#endif
 
 #define J2P_JE_WORDS_PER_BLOCK 52u      // 32-bit words of J2P_JPEGENC_BLOCK_BITS, rounded up
 static_assert(J2P_JE_WORDS_PER_BLOCK * 32 >= J2P_JPEGENC_BLOCK_BITS && (J2P_JE_WORDS_PER_BLOCK - 1) * 32 < J2P_JPEGENC_BLOCK_BITS,

@@ -1,33 +1,12 @@
 // png.cu — libj2ppng.so: the plan of a call, the device encoder (filter, pieces, assembly, copy)
 // and the serial host driver of the same steps.  See png.h and png_core.h.
-#include <cuda_runtime.h>
-
-#include <stdarg.h>
-#include <stdio.h>
-#include <stdlib.h>
 #include <string.h>
 
+#include "../common/codec_host.h"
 #include "png_core.h"
-
-static thread_local char g_err[256];
-
-static int fail(const char *fmt, ...) {
-    va_list ap;
-    va_start(ap, fmt);
-    vsnprintf(g_err, sizeof g_err, fmt, ap);
-    va_end(ap);
-    return -1;
-}
 
 extern "C" const char *j2p_png_last_error(void) { return g_err; }
 
-#define CK(x)                                                                                   \
-    do {                                                                                        \
-        const cudaError_t e_ = (x);                                                             \
-        if (e_ != cudaSuccess) return fail("%s: %s", #x, cudaGetErrorString(e_));               \
-    } while (0)
-
-static size_t align16(size_t n) { return (n + 15) & ~(size_t)15; }
 static const uint32_t kSlot = J2P_PNG_SLOT;     // output slot of a piece
 
 struct PieceResult {
@@ -544,75 +523,31 @@ __global__ void __launch_bounds__(kCopyThreads) k_png_copy(const struct j2p_png_
     for (uint32_t j = threadIdx.x; j < r.len; j += kCopyThreads) dst[j] = src[j];
 }
 
-static int device_of(const void *ptr, const char *what, int *dev) {
-    cudaPointerAttributes a;
-    const cudaError_t e = cudaPointerGetAttributes(&a, ptr);
-    if (e != cudaSuccess) {
-        cudaGetLastError();
-        return fail("%s: %s", what, cudaGetErrorString(e));
-    }
-    if (a.type != cudaMemoryTypeDevice) return fail("%s is not device memory", what);
-    *dev = a.device;
-    return 0;
-}
-
-struct DeviceGuard {
-    int prev = -1;
-    ~DeviceGuard() {
-        if (prev >= 0) cudaSetDevice(prev);
-    }
-};
-
 extern "C" int j2p_png_encode(const struct j2p_png_image *images, unsigned n, void *work, size_t work_bytes, void *stream, uint64_t *offsets,
                               void *dst, size_t dst_cap, struct j2p_png_stats *stats) {
     Layout L;
     if (make_plan(images, n, &L, nullptr) != 0) return -1;
-    if (!work || !offsets) return fail("null argument");
-    if (work_bytes < L.total) return fail("work area of %zu bytes is smaller than the plan's %zu", work_bytes, L.total);
-    int dev = -1, d = -1;
-    if (device_of(work, "the work area", &dev) != 0) return -1;
-    for (unsigned i = 0; i < n; i++) {
-        char what[48];
-        snprintf(what, sizeof what, "image %u's data", i);
-        if (device_of(images[i].data, what, &d) != 0) return -1;
-        if (d != dev) return fail("image %u is on device %d, the work area on device %d", i, d, dev);
-    }
-    DeviceGuard guard;
-    CK(cudaGetDevice(&guard.prev));
-    CK(cudaSetDevice(dev));
-    const cudaStream_t st = (cudaStream_t)stream;
-    uint8_t *plan = (uint8_t *)malloc(L.off_filt);
-    if (!plan) return fail("out of host memory");
-    if (fill_plan(images, n, L, plan) != 0) { free(plan); return -1; }
-    uint8_t *w = (uint8_t *)work;
-    const cudaError_t ec = cudaMemcpyAsync(w, plan, L.off_filt, cudaMemcpyHostToDevice, st);
-    if (ec != cudaSuccess) { free(plan); return fail("plan upload: %s", cudaGetErrorString(ec)); }
-    struct j2p_png_img *imgs = (struct j2p_png_img *)(w + L.off_imgs);
-    const uint32_t *pmap = (const uint32_t *)(w + L.off_pmap), *tab = (const uint32_t *)(w + L.off_tab), *x2k = (const uint32_t *)(w + L.off_x2k);
-    PieceResult *res = (PieceResult *)(w + L.off_res);
-    uint64_t *offs = (uint64_t *)(w + L.off_offs);
-    static const size_t smem = sizeof(PieceShared);
-    const cudaError_t ea = cudaFuncSetAttribute(k_png_piece, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (ea != cudaSuccess) { free(plan); return fail("k_png_piece shared memory: %s", cudaGetErrorString(ea)); }
-    const uint64_t fgrid = (L.rows * 32 + kFilterThreads - 1) / kFilterThreads;
-    k_png_filter<<<(unsigned)fgrid, kFilterThreads, 0, st>>>(imgs, n, L.rows, w + L.off_filt);
-    k_png_piece<<<L.npieces, kPieceThreads, smem, st>>>(imgs, pmap, tab, x2k, w + L.off_filt, w + L.off_slots, res);
-    k_png_assemble<<<1, kAsmThreads, 0, st>>>(imgs, n, res, tab, idat_crc0((const uint32_t *)(plan + L.off_tab)), offs, w + L.off_out);
-    k_png_copy<<<L.npieces, kCopyThreads, 0, st>>>(imgs, pmap, w + L.off_slots, res, w + L.off_out);
-    const cudaError_t el = cudaGetLastError();
-    if (el != cudaSuccess) { free(plan); return fail("launch: %s", cudaGetErrorString(el)); }
-    const cudaError_t eo = cudaMemcpyAsync(offsets, offs, (n + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, st);
-    const cudaError_t es = eo == cudaSuccess ? cudaStreamSynchronize(st) : eo;
-    free(plan);                         // the upload has been read by now
-    if (es != cudaSuccess) return fail("encode: %s", cudaGetErrorString(es));
-    if (dst) {
-        if (dst_cap < offsets[n]) return fail("destination of %zu bytes is smaller than the files (%llu)", dst_cap, (unsigned long long)offsets[n]);
-        CK(cudaMemcpyAsync(dst, w + L.off_out, offsets[n], cudaMemcpyDeviceToHost, st));
-        CK(cudaStreamSynchronize(st));
-    }
-    if (stats) {
-        stats->launches = 4;
-        stats->pieces = L.npieces;
-    }
+    const auto fill = [&](uint8_t *plan) { return fill_plan(images, n, L, plan); };
+    const auto launch = [&](uint8_t *w, cudaStream_t st, const uint8_t *plan, auto counted) {
+        struct j2p_png_img *imgs = (struct j2p_png_img *)(w + L.off_imgs);
+        const uint32_t *pmap = (const uint32_t *)(w + L.off_pmap), *tab = (const uint32_t *)(w + L.off_tab), *x2k = (const uint32_t *)(w + L.off_x2k);
+        PieceResult *res = (PieceResult *)(w + L.off_res);
+        static const size_t smem = sizeof(PieceShared);
+        const cudaError_t ea = cudaFuncSetAttribute(k_png_piece, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        if (ea != cudaSuccess) return fail("k_png_piece shared memory: %s", cudaGetErrorString(ea));
+        const uint64_t fgrid = (L.rows * 32 + kFilterThreads - 1) / kFilterThreads;
+        k_png_filter<<<(unsigned)fgrid, kFilterThreads, 0, st>>>(imgs, n, L.rows, w + L.off_filt);
+        counted();
+        k_png_piece<<<L.npieces, kPieceThreads, smem, st>>>(imgs, pmap, tab, x2k, w + L.off_filt, w + L.off_slots, res);
+        counted();
+        k_png_assemble<<<1, kAsmThreads, 0, st>>>(imgs, n, res, tab, idat_crc0((const uint32_t *)(plan + L.off_tab)), (uint64_t *)(w + L.off_offs),
+                                                  w + L.off_out);
+        counted();
+        k_png_copy<<<L.npieces, kCopyThreads, 0, st>>>(imgs, pmap, w + L.off_slots, res, w + L.off_out);
+        counted();
+        return 0;
+    };
+    if (encode_call(images, n, L, L.off_filt, work, work_bytes, stream, offsets, dst, dst_cap, stats, fill, launch) != 0) return -1;
+    if (stats) stats->pieces = L.npieces;
     return 0;
 }

@@ -20,13 +20,8 @@
 
 #include <stdint.h>
 
+#include "../common/codec_host.h"       /* J2P_HD */
 #include "png.h"
-
-#ifdef __CUDACC__
-#define J2P_HD __host__ __device__ __forceinline__
-#else
-#define J2P_HD static inline
-#endif
 
 #define J2P_PNG_PIECE 65536u              /* bytes of filtered stream per piece */
 #define J2P_PNG_BLOCK_SYMS 16383u         /* symbols per deflate block (zlib's default) */

@@ -11,6 +11,7 @@ import torch
 
 from jpeg2png_b200 import decode_jpeg, encode_jpeg
 from jpeg2png_b200 import jpeg_encode as J
+from tests import codec_checks as CK
 from tests import jpegenc_cases as JC
 from tests.test_gpu_decode import FILES, _case
 
@@ -98,22 +99,7 @@ def test_producer_on_a_side_stream_needs_no_sync():
 def test_forced_split_gives_the_same_bytes(monkeypatch):
     names = [n for n in CORPUS if n.startswith(('97x61', '200x300', '31x33'))]
     ts = [_cuda(CORPUS[n][2]) for n in names]
-    whole = encode_jpeg(ts, quality=70, layout='HWC')
-    one = J._work_bytes(J._descs(ts[:1], 'HWC', lambda x: x.data_ptr(), lambda x: x.stride()), J.params(70, '4:2:0'))
-    calls = []
-    lib = J.load_jpegenc()
-
-    class Counting:                                    # the library, counting the images of each encode call
-        def __getattr__(self, k):
-            return getattr(lib, k)
-
-        def j2p_jpegenc_encode(self, d, n, *a):
-            calls.append(n)
-            return lib.j2p_jpegenc_encode(d, n, *a)
-    monkeypatch.setattr(torch.cuda, 'mem_get_info', lambda *a: (8 * one, 80 << 30))
-    monkeypatch.setattr(J, 'load_jpegenc', lambda: Counting())
-    assert encode_jpeg(ts, quality=70, layout='HWC') == whole
-    assert len(calls) > 1 and sum(calls) == len(ts)
+    CK.check_forced_split(monkeypatch, J.codec(J.params(70, '4:2:0')), ts, lambda: encode_jpeg(ts, quality=70, layout='HWC'))
 
 
 def test_refusals():
@@ -154,30 +140,6 @@ def test_refusals():
 def test_launch_count_does_not_depend_on_the_images():
     """The kernels that run on the device, counted by the profiler: each of the seven once per
     call, for one tiny image and for a mixed list alike, and as many as the call reports."""
-    lib = J.load_jpegenc()
-    p = J.Params(75, 2)
     names = ('k_je_blocks', 'k_je_sizes', 'k_je_scan', 'k_je_emit', 'k_je_ffcount', 'k_je_offsets', 'k_je_stuff')
-    for shapes in ([(1, 1)], [(300, 200)] * 5 + [(1, 1), (2000, 3000)]):
-        ts = [torch.zeros(h, w, 3, dtype=torch.uint8, device='cuda') for h, w in shapes]
-        d = (J.Image * len(ts))()
-        for di, t in zip(d, ts):
-            di.data, di.width, di.height = t.data_ptr(), t.shape[1], t.shape[0]
-            di.row_stride, di.col_stride, di.chan_stride = t.stride()
-        n, o = C.c_size_t(), C.c_size_t()
-        assert lib.j2p_jpegenc_plan(d, len(ts), C.byref(p), C.byref(n), C.byref(o)) == 0
-        work = torch.empty(n.value, dtype=torch.uint8, device='cuda')
-        offs = (C.c_uint64 * (len(ts) + 1))()
-        st = J.Stats()
-        torch.cuda.synchronize()
-        with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
-            assert lib.j2p_jpegenc_encode(d, len(ts), C.byref(p), work.data_ptr(), n.value, torch.cuda.current_stream().cuda_stream,
-                                          offs, None, 0, C.byref(st)) == 0
-            torch.cuda.synchronize()
-        ran = {k: 0 for k in names}
-        for ev in prof.key_averages():
-            k = next((k for k in names if k in ev.key), None)
-            if k:
-                ran[k] += ev.count
-        assert ran == {k: 1 for k in names}, ran
-        assert st.launches == sum(ran.values())
-        assert st.blocks == sum(-(-h // 16) * -(-w // 16) * 6 for h, w in shapes)      # 4:2:0 MCUs, six blocks each
+    for shapes, st in CK.check_launch_count('jpeg', names):
+        assert st['blocks'] == sum(-(-h // 16) * -(-w // 16) * 6 for h, w in shapes)      # 4:2:0 MCUs, six blocks each

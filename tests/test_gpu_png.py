@@ -1,7 +1,7 @@
 """encode_png and libj2ppng.so on the GPU: the device writes the host driver's bytes on every CPU
 case (one mixed call and one call per image), an 8K 16-bit image, JPEG files through
-decode_jpeg + encode_png against the checker pipeline, a producer on a side stream, and the
-refusals."""
+decode_jpeg + encode_png against the checker pipeline, a producer on a side stream, a forced
+split, the refusals and launch counts."""
 import ctypes as C
 import zlib
 
@@ -11,6 +11,7 @@ import torch
 
 from jpeg2png_b200 import decode_jpeg, encode_png
 from jpeg2png_b200 import encode as E
+from tests import codec_checks as CK
 from tests import png_cases as P
 from tests.test_codecs import codecs, read_jpeg  # noqa: F401  (codecs is a fixture)
 from tests.test_gpu_cli import expected_rgb
@@ -107,6 +108,11 @@ def test_producer_on_a_side_stream_needs_no_sync():
     assert got == want
 
 
+def test_forced_split_gives_the_same_bytes(monkeypatch):
+    ts = [_cuda(P._smooth(120 + 40 * k, 200, np.uint16 if k % 2 else np.uint8, seed=k)) for k in range(6)]
+    CK.check_forced_split(monkeypatch, E.CODEC, ts, lambda: encode_png(ts, layout='HWC'))
+
+
 def test_refusals():
     with pytest.raises(ValueError, match='CUDA tensors'):
         encode_png(torch.zeros(3, 8, 8, dtype=torch.uint8))
@@ -140,17 +146,7 @@ def test_refusals():
 
 
 def test_launch_count_does_not_depend_on_the_images():
-    lib = E.load_png()
-    for shapes in ([(1, 1)], [(300, 200)] * 5 + [(1, 1), (2000, 3000)]):
-        ts = [torch.zeros(h, w, 3, dtype=torch.uint8, device='cuda') for h, w in shapes]
-        d = (E.Image * len(ts))()
-        for di, t in zip(d, ts):
-            di.data, di.width, di.height, di.sample_bytes = t.data_ptr(), t.shape[1], t.shape[0], 1
-            di.row_stride, di.col_stride, di.chan_stride = t.stride()
-        n, o = C.c_size_t(), C.c_size_t()
-        assert lib.j2p_png_plan(d, len(ts), C.byref(n), C.byref(o)) == 0
-        work = torch.empty(n.value, dtype=torch.uint8, device='cuda')
-        offs = (C.c_uint64 * (len(ts) + 1))()
-        st = E.Stats()
-        assert lib.j2p_png_encode(d, len(ts), work.data_ptr(), n.value, None, offs, None, 0, C.byref(st)) == 0
-        assert st.launches == 4
+    """The kernels that run on the device, counted by the profiler: each of the four once per call,
+    for one tiny image and for a mixed list alike, and as many as the call reports."""
+    for _, st in CK.check_launch_count('png', ('k_png_filter', 'k_png_piece', 'k_png_assemble', 'k_png_copy')):
+        assert st['launches'] == 4

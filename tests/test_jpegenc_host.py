@@ -3,21 +3,15 @@ steps as the kernels of libj2pjpegenc.so): Pillow's bytes for every size, conten
 sampling of the corpus, the files back through the project's decoders, the refusals, and the
 library's kernel inventory."""
 import ctypes as C
-import os
-import re
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
 
 from jpeg2png_b200 import decode as D
 from jpeg2png_b200 import jpeg_encode as J
+from tests import codec_checks as CK
 from tests import entropy_cases as EC
 from tests import jpegenc_cases as JC
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-LIB = os.path.join(ROOT, 'jpeg2png_b200', 'jpegenc', 'libj2pjpegenc.so')
 
 # kernel -> the GPU test that reaches it (every call of j2p_jpegenc_encode launches all seven)
 KERNELS = {
@@ -201,22 +195,5 @@ def test_encode_jpeg_without_a_device_raises_runtime_error():
         encode_jpeg([])
 
 
-def _kernels():
-    cuobjdump = shutil.which('cuobjdump') or '/usr/local/cuda/bin/cuobjdump'
-    if not os.path.exists(cuobjdump) or not os.path.exists(LIB):
-        pytest.skip('CUDA toolkit or the built library is missing')
-    out = subprocess.run([cuobjdump, '-res-usage', LIB], check=True, capture_output=True, text=True).stdout
-    found = re.findall(r'Function (\w+):\s*\n\s*REG:(\d+) STACK:(\d+) SHARED:\d+ LOCAL:(\d+)', out)
-    assert found, 'no kernels found in the library?'
-
-    def name(m):                    # _Z<length><name><parameters>
-        n = re.match(r'_Z(\d+)', m)
-        return m[n.end():n.end() + int(n.group(1))] if n else m
-    return {name(m): (int(r), int(s), int(l)) for m, r, s, l in found}
-
-
 def test_kernel_inventory_is_covered_and_does_not_spill():
-    ks = _kernels()
-    assert sorted(ks) == sorted(KERNELS), f'kernels without a GPU test in KERNELS, or stale entries: {sorted(ks)}'
-    for k, (reg, stack, local) in ks.items():
-        assert stack == 0 and local == 0, f'{k} uses {stack} bytes of stack and {local} of local memory'
+    CK.check_kernel_inventory('jpegenc/libj2pjpegenc.so', KERNELS)

@@ -5,19 +5,16 @@ refusals, and the library's kernel inventory."""
 import ctypes as C
 import io
 import os
-import re
-import shutil
-import subprocess
 import zlib
 
 import numpy as np
 import pytest
 
 from jpeg2png_b200 import encode as E
+from tests import codec_checks as CK
 from tests import png_cases as P
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-LIB = os.path.join(ROOT, 'jpeg2png_b200', 'png', 'libj2ppng.so')
 
 # kernel -> the GPU test that reaches it (every call of j2p_png_encode launches all four)
 KERNELS = {
@@ -233,22 +230,5 @@ def test_encode_png_without_a_device_raises_runtime_error():
         encode_png([])
 
 
-def _kernels():
-    cuobjdump = shutil.which('cuobjdump') or '/usr/local/cuda/bin/cuobjdump'
-    if not os.path.exists(cuobjdump) or not os.path.exists(LIB):
-        pytest.skip('CUDA toolkit or the built library is missing')
-    out = subprocess.run([cuobjdump, '-res-usage', LIB], check=True, capture_output=True, text=True).stdout
-    found = re.findall(r'Function (\w+):\s*\n\s*REG:(\d+) STACK:(\d+) SHARED:\d+ LOCAL:(\d+)', out)
-    assert found, 'no kernels found in the library?'
-
-    def name(m):                    # _Z<length><name><parameters>
-        n = re.match(r'_Z(\d+)', m)
-        return m[n.end():n.end() + int(n.group(1))] if n else m
-    return {name(m): (int(r), int(s), int(l)) for m, r, s, l in found}
-
-
 def test_kernel_inventory_is_covered_and_does_not_spill():
-    ks = _kernels()
-    assert sorted(ks) == sorted(KERNELS), f'kernels without a GPU test in KERNELS, or stale entries: {sorted(ks)}'
-    for k, (reg, stack, local) in ks.items():
-        assert stack == 0 and local == 0, f'{k} uses {stack} bytes of stack and {local} of local memory'
+    CK.check_kernel_inventory('png/libj2ppng.so', KERNELS)

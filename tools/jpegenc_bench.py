@@ -25,7 +25,6 @@ Wall-clock figures are the best of R after one warm-up.  Also the card's name an
 (read-only nvidia-smi query in the same run).  Writes nothing.
 """
 import argparse
-import ctypes as C
 import io
 import json
 import os
@@ -42,47 +41,18 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 from batch_bench import gpu_card  # noqa: E402
 from decode_bench import jpeg_files  # noqa: E402
-from png_bench import best_of, host_threads  # noqa: E402
+from png_bench import best_of, encoder_call, encoder_ms, host_threads  # noqa: E402
 from jpeg2png_b200 import abi, decode_jpeg, encode_jpeg, encode_png, synth  # noqa: E402
 from jpeg2png_b200 import jpeg_encode as J  # noqa: E402
 
 KERNELS = ('k_je_blocks', 'k_je_sizes', 'k_je_scan', 'k_je_emit', 'k_je_ffcount', 'k_je_offsets', 'k_je_stuff')
 
 
-def encoder_ms(tensors, quality, subsampling, calls):
-    """CUDA events around one whole j2p_jpegenc_encode call, mean of `calls`; and each kernel's
-    device time per call from torch.profiler over `calls` more calls."""
-    lib = J.load_jpegenc()
-    p = J.params(quality, subsampling)
-    d = J._descs(tensors, 'CHW', lambda x: x.data_ptr(), lambda x: x.stride())
-    n, o = C.c_size_t(), C.c_size_t()
-    J._check(lib.j2p_jpegenc_plan(d, len(tensors), C.byref(p), C.byref(n), C.byref(o)))
-    work = torch.empty(n.value, dtype=torch.uint8, device=tensors[0].device)
-    offs = (C.c_uint64 * (len(tensors) + 1))()
-    stream = torch.cuda.current_stream()
-
-    def call():
-        J._check(lib.j2p_jpegenc_encode(d, len(tensors), C.byref(p), work.data_ptr(), n.value, stream.cuda_stream, offs, None, 0, None))
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    call()
-    times = []
-    for _ in range(calls):
-        e0.record()
-        call()
-        e1.record()
-        e1.synchronize()
-        times.append(e0.elapsed_time(e1))
-    with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
-        for _ in range(calls):
-            call()
-        torch.cuda.synchronize()
-    kernels = {}
-    for ev in prof.key_averages():
-        name = next((k for k in KERNELS if k in ev.key), None)
-        if name:
-            us = getattr(ev, 'device_time_total', None) or getattr(ev, 'cuda_time_total', 0)
-            kernels[name] = kernels.get(name, 0.0) + us / 1e3 / calls
-    return {'ms_per_call': float(np.mean(times)), 'work_bytes': n.value, 'kernel_ms_per_call': kernels}
+def jpeg_encoder_ms(tensors, quality, subsampling, calls):
+    """encoder_ms of one j2p_jpegenc_encode call on all images, and the size of its work area."""
+    call, work_bytes = encoder_call(J.codec(J.params(quality, subsampling)), tensors)
+    out = encoder_ms(call, KERNELS, calls)
+    return {'ms_per_call': out['ms_per_call'], 'work_bytes': work_bytes, 'kernel_ms_per_call': out['kernel_ms_per_call']}
 
 
 def pillow(hwc, quality, subsampling):
@@ -136,7 +106,7 @@ def host_arm(tensors, quality, subsampling, reps, procs):
 
 def run(tensors, label, quality, subsampling, reps, calls, threads, png_bytes):
     out = {'workload': label, 'images': len(tensors), 'quality': quality, 'subsampling': subsampling}
-    out['encoder'] = encoder_ms(tensors, quality, subsampling, calls)
+    out['encoder'] = jpeg_encoder_ms(tensors, quality, subsampling, calls)
     t_gpu, files = best_of(lambda: encode_jpeg(tensors, quality=quality, subsampling=subsampling), reps)
 
     t_host, host_files, t_copy, t_one = host_arm(tensors, quality, subsampling, reps, threads)

@@ -45,12 +45,14 @@ sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 from batch_bench import gpu_card  # noqa: E402
 from decode_bench import jpeg_files  # noqa: E402
 from jpeg2png_b200 import abi, decode_jpeg, encode_png  # noqa: E402
+from jpeg2png_b200 import batch_encode as B  # noqa: E402
 from jpeg2png_b200 import encode as E  # noqa: E402
 from jpeg2png_b200.pngcheck import holds_pixels  # noqa: E402
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CLI = os.path.join(ROOT, 'jpeg2png_b200', 'cli', 'jpeg2png')
 CODECS = os.path.join(ROOT, 'jpeg2png_b200', 'cli', 'libj2pcodecs.so')
+KERNELS = ('k_png_filter', 'k_png_piece', 'k_png_assemble', 'k_png_copy')
 
 
 def host_threads():
@@ -113,24 +115,21 @@ def best_of(fn, reps):
     return best, result
 
 
-def _descs(tensors):
-    return E._descs(tensors, 'CHW', lambda x: E._DTYPES[x.dtype], lambda x: x.data_ptr(), lambda x: x.stride())
-
-
-def encoder_ms(tensors, calls):
-    """CUDA events around one whole j2p_png_encode call on all images (host plan, plan upload,
-    kernels, offset read-back), mean of `calls`; and each kernel's device time per call from
-    torch.profiler over `calls` more calls."""
-    lib = E.load_png()
-    d = _descs(tensors)
-    n, o = C.c_size_t(), C.c_size_t()
-    E._check(lib.j2p_png_plan(d, len(tensors), C.byref(n), C.byref(o)))
-    work = torch.empty(n.value, dtype=torch.uint8, device=tensors[0].device)
+def encoder_call(codec, tensors):
+    """One whole device encode call of codec's library on all tensors (CHW), with its work area
+    allocated once; and the work area's size."""
+    d = B.descs(codec, tensors, 'CHW')
+    n, _ = codec.plan(d)
+    work = torch.empty(n, dtype=torch.uint8, device=tensors[0].device)
     offs = (C.c_uint64 * (len(tensors) + 1))()
     stream = torch.cuda.current_stream()
+    return lambda: codec.call('encode', d, work.data_ptr(), n, stream.cuda_stream, offs, None, 0, None), n
 
-    def call():
-        E._check(lib.j2p_png_encode(d, len(tensors), work.data_ptr(), n.value, stream.cuda_stream, offs, None, 0, None))
+
+def encoder_ms(call, kernel_names, calls):
+    """CUDA events around call() (host plan, plan upload, kernels, offset read-back), mean of
+    `calls`; and the device time per call of each kernel in kernel_names from torch.profiler over
+    `calls` more calls."""
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     call()
     times = []
@@ -146,20 +145,26 @@ def encoder_ms(tensors, calls):
         torch.cuda.synchronize()
     kernels = {}
     for ev in prof.key_averages():
-        name = next((k for k in ('k_png_filter', 'k_png_piece', 'k_png_assemble', 'k_png_copy') if k in ev.key), None)
+        name = next((k for k in kernel_names if k in ev.key), None)
         if name:
             us = getattr(ev, 'device_time_total', None) or getattr(ev, 'cuda_time_total', 0)
             kernels[name] = kernels.get(name, 0.0) + us / 1e3 / calls
+    return {'ms_per_call': float(np.mean(times)), 'kernel_ms_per_call': kernels}
+
+
+def png_encoder_ms(tensors, calls):
+    """encoder_ms of one j2p_png_encode call on all images, and GB/s of filtered bytes."""
+    out = encoder_ms(encoder_call(E.CODEC, tensors)[0], KERNELS, calls)
     filtered = sum(t.shape[1] * (1 + t.shape[2] * 3 * t.element_size()) for t in tensors)
-    ms = float(np.mean(times))
-    return {'ms_per_call': ms, 'filtered_bytes': filtered, 'GB_per_s': filtered / ms / 1e6, 'kernel_ms_per_call': kernels}
+    return {'ms_per_call': out['ms_per_call'], 'filtered_bytes': filtered, 'GB_per_s': filtered / out['ms_per_call'] / 1e6,
+            'kernel_ms_per_call': out['kernel_ms_per_call']}
 
 
 def run_workload(files, label, iterations, dtype, reps, calls, writer, threads, e2e):
     tensors = decode_jpeg(files, iterations=iterations, dtype=dtype)
     torch.cuda.synchronize()
     out = {'workload': label, 'files': len(files), 'dtype': str(dtype).replace('torch.', '')}
-    out['encoder'] = encoder_ms(tensors, calls)
+    out['encoder'] = png_encoder_ms(tensors, calls)
 
     t_gpu, pngs = best_of(lambda: encode_png(tensors), reps)
 
@@ -224,7 +229,7 @@ def main():
     yy = torch.arange(4320, device='cuda', dtype=torch.int32)[:, None]
     xx = torch.arange(7680, device='cuda', dtype=torch.int32)[None, :]
     img8k = (torch.stack([yy * 7 + xx * 3, yy * 13 + xx, xx * 5 + yy]) % 65536).to(torch.uint16)
-    line['one_8k_uint16_image'] = encoder_ms([img8k], args.calls)
+    line['one_8k_uint16_image'] = png_encoder_ms([img8k], args.calls)
     print(json.dumps(line), flush=True)
 
 
