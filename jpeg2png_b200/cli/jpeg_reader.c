@@ -48,7 +48,8 @@ struct dec {
         int failed;
         struct j2p_jpeg_layout *lay;   /* the layout pass (j2p_read_jpeg_layout), NULL for a full read */
         unsigned scans_of[3];          /* layout pass: scans that name each component */
-        size_t data_cap, seg_cap;
+        struct j2p_jpeg_prog_layout *play;   /* the progressive layout pass (j2p_read_jpeg_prog_layout) */
+        size_t data_cap, seg_cap, scan_cap;
 };
 
 static int fail(struct dec *d, const char *fmt, ...) {
@@ -284,9 +285,10 @@ static int grow(void **p, size_t *cap, size_t need, size_t elem) {
         *cap = n;
         return 0;
 }
-static int layout_scan(struct dec *d, struct comp **sc, int ns) {
-        struct j2p_jpeg_layout *l = d->lay;
-        struct j2p_jpeg_scan *S = &l->scan[l->nscan++];
+/* S: the scan's descriptor; the segments are appended to *seg (seg_n) and their bytes to *data
+ * (data_len), which both layout passes own */
+static int layout_scan(struct dec *d, struct comp **sc, int ns, struct j2p_jpeg_scan *S, struct j2p_jpeg_segment **seg, unsigned *seg_n,
+                       uint8_t **data, size_t *data_len) {
         const int interleaved = ns > 1;
         S->ncomp = (unsigned)ns;
         for (int i = 0; i < ns; i++) {
@@ -303,17 +305,17 @@ static int layout_scan(struct dec *d, struct comp **sc, int ns) {
         S->restart_interval = d->restart_interval;
         const size_t total = (size_t)S->mcux * S->mcuy;
         const size_t nseg = d->restart_interval ? (total + d->restart_interval - 1) / d->restart_interval : 1;
-        S->seg0 = l->nseg;
+        S->seg0 = *seg_n;
         S->nseg = (unsigned)nseg;
         unsigned eobrun = 0;
         for (size_t k = 0; k < nseg; k++) {
                 if (k > 0 && restart(d, sc, ns, &eobrun, (int)(k - 1)) != 0) return -1;
-                if (grow((void **)&l->seg, &d->seg_cap, (size_t)l->nseg + 1, sizeof *l->seg) != 0) return fail(d, "could not allocate memory for coefs");
+                if (grow((void **)seg, &d->seg_cap, (size_t)*seg_n + 1, sizeof **seg) != 0) return fail(d, "could not allocate memory for coefs");
                 /* the bytes fill() would feed: up to the first FF not followed by 00, FF 00 -> FF */
-                if (grow((void **)&l->data, &d->data_cap, l->data_len + (size_t)(d->end - d->p), 1) != 0) return fail(d, "could not allocate memory for coefs");
-                struct j2p_jpeg_segment *g = &l->seg[l->nseg++];
-                g->off = l->data_len;
-                uint8_t *o = l->data + l->data_len;
+                if (grow((void **)data, &d->data_cap, *data_len + (size_t)(d->end - d->p), 1) != 0) return fail(d, "could not allocate memory for coefs");
+                struct j2p_jpeg_segment *g = &(*seg)[(*seg_n)++];
+                g->off = *data_len;
+                uint8_t *o = *data + *data_len;
                 const uint8_t *p = d->p;
                 while (p < d->end) {
                         const uint8_t *q = memchr(p, 0xFF, (size_t)(d->end - p));
@@ -325,8 +327,8 @@ static int layout_scan(struct dec *d, struct comp **sc, int ns) {
                         if (p + 1 < d->end && p[1] == 0x00) { *o++ = 0xFF; p += 2; }
                         else break;
                 }
-                g->len = (size_t)(o - (l->data + l->data_len));
-                l->data_len += g->len;
+                g->len = (size_t)(o - (*data + *data_len));
+                *data_len += g->len;
                 g->mcus = (unsigned)(d->restart_interval && k + 1 < nseg ? d->restart_interval : total - k * (d->restart_interval ? d->restart_interval : 0));
                 d->p = p;
         }
@@ -396,7 +398,7 @@ static int parse_sof(struct dec *d, const uint8_t *s, unsigned len) {
                 c->hb = (ch + 7) / 8;
                 c->pwb = d->mcux * c->h;
                 c->phb = d->mcuy * c->v;
-                if (d->lay) continue;                                                                   /* the layout pass stores no blocks */
+                if (d->lay || d->play) continue;                                                        /* the layout passes store no blocks */
                 c->blk = calloc((size_t)c->pwb * c->phb * 64, sizeof(int16_t));
                 if (!c->blk) return fail(d, "could not allocate memory for coefs");                /* jpeg.c:69 */
         }
@@ -430,6 +432,7 @@ static int read_markers(struct dec *d, const uint8_t *buf, size_t len) {
                         if (have_sof) { fail(d, "unsupported jpeg: multiple frames"); break; }
                         d->progressive = m == 0xC2;
                         if (d->lay && d->progressive) return 1;
+                        if (d->play && !d->progressive) return 1;
                         if (parse_sof(d, s, sl) == 0) have_sof = 1;
                 } else if (m == 0xC3 || (m >= 0xC5 && m <= 0xC7) || (m >= 0xC9 && m <= 0xCB) || (m >= 0xCD && m <= 0xCF)) {
                         fail(d, "unsupported jpeg: SOF%u (arithmetic, lossless or hierarchical coding)", m - 0xC0);
@@ -461,7 +464,21 @@ static int read_markers(struct dec *d, const uint8_t *buf, size_t len) {
                         if (d->lay) {
                                 for (int i = 0; i < ns; i++)
                                         if (d->scans_of[sc[i] - d->c]++) return 1;      /* a component scanned twice */
-                                layout_scan(d, sc, ns);
+                                struct j2p_jpeg_layout *l = d->lay;
+                                layout_scan(d, sc, ns, &l->scan[l->nscan++], &l->seg, &l->nseg, &l->data, &l->data_len);
+                        } else if (d->play) {
+                                struct j2p_jpeg_prog_layout *l = d->play;
+                                if (grow((void **)&l->scan, &d->scan_cap, (size_t)l->nscan + 1, sizeof *l->scan) != 0) {
+                                        fail(d, "could not allocate memory for coefs");
+                                        break;
+                                }
+                                struct j2p_jpeg_prog_scan *S = &l->scan[l->nscan++];
+                                memset(S, 0, sizeof *S);
+                                S->ss = (unsigned)ss;
+                                S->se = (unsigned)se;
+                                S->ah = (unsigned)ah;
+                                S->al = (unsigned)al;
+                                layout_scan(d, sc, ns, &S->s, &l->seg, &l->nseg, &l->data, &l->data_len);
                         } else {
                                 decode_scan(d, sc, ns, ss, se, ah, al);
                         }
@@ -543,6 +560,40 @@ int j2p_read_jpeg_layout(const uint8_t *buf, size_t len, struct j2p_jpeg_layout 
         }
         free(d);
         return rc;
+}
+
+int j2p_read_jpeg_prog_layout(const uint8_t *buf, size_t len, struct j2p_jpeg_prog_layout *out, char *err, size_t errlen) {
+        struct dec *d = calloc(1, sizeof *d);
+        if (!d) return -1;
+        d->p = buf; d->end = buf + len; d->err = err; d->errlen = errlen;
+        if (err && errlen) err[0] = 0;
+        memset(out, 0, sizeof *out);
+        d->play = out;
+        const int stopped = read_markers(d, buf, len);
+        const int decodable = !stopped && !d->failed;
+        if (decodable) {
+                check_planes(d, out->coefs);
+                out->w = d->W;
+                out->h = d->H;
+                for (int i = 0; i < 3; i++) { out->comp_h[i] = (unsigned)d->c[i].h; out->comp_v[i] = (unsigned)d->c[i].v; }
+        }
+        const int rc = d->failed ? -1 : 0;
+        out->progressive_decodable = rc == 0 && decodable;
+        if (!out->progressive_decodable) j2p_free_jpeg_prog_layout(out);
+        free(d);
+        return rc;
+}
+
+void j2p_free_jpeg_prog_layout(struct j2p_jpeg_prog_layout *l) {
+        free(l->scan);
+        free(l->seg);
+        free(l->data);
+        l->scan = NULL;
+        l->seg = NULL;
+        l->data = NULL;
+        l->nscan = 0;
+        l->nseg = 0;
+        l->data_len = 0;
 }
 
 void j2p_free_jpeg_layout(struct j2p_jpeg_layout *l) {

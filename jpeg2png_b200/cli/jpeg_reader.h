@@ -78,4 +78,32 @@ struct j2p_jpeg_layout {
 int j2p_read_jpeg_layout(const uint8_t *buf, size_t len, struct j2p_jpeg_layout *out, char *err, size_t errlen);
 void j2p_free_jpeg_layout(struct j2p_jpeg_layout *l);
 
+/* ---- progressive layout pass: every scan of a progressive file, cut as above ----
+ *
+ * j2p_read_jpeg_prog_layout runs the same marker loop and header checks and cuts every scan of a
+ * progressive (SOF2) file into segments as j2p_read_jpeg_layout does, recording each scan's
+ * spectral selection and successive approximation with the tables and restart interval in force at
+ * its SOS.  A component may be in any number of scans, or none.  progressive_decodable: the file is
+ * progressive and the reader accepts it up to the scan headers (coefs, scans and segments filled);
+ * for every other file the pass stops as soon as that is known (a sequential SOF) and returns 0 with
+ * progressive_decodable = 0.  A non-zero return means j2p_read_jpeg_mem rejects the file too. */
+struct j2p_jpeg_prog_scan {
+        struct j2p_jpeg_scan s;     /* components, MCU grid, tables, restart interval, segments */
+        unsigned ss, se, ah, al;    /* spectral selection and successive approximation (G.1.1.1) */
+};
+struct j2p_jpeg_prog_layout {
+        unsigned w, h;
+        struct coef coefs[3];       /* as struct j2p_jpeg, but data NULL */
+        unsigned comp_h[3], comp_v[3];
+        int progressive_decodable;
+        unsigned nscan;
+        struct j2p_jpeg_prog_scan *scan;     /* malloc'd, in file order */
+        unsigned nseg;
+        struct j2p_jpeg_segment *seg;        /* malloc'd */
+        uint8_t *data;                       /* malloc'd */
+        size_t data_len;
+};
+int j2p_read_jpeg_prog_layout(const uint8_t *buf, size_t len, struct j2p_jpeg_prog_layout *out, char *err, size_t errlen);
+void j2p_free_jpeg_prog_layout(struct j2p_jpeg_prog_layout *l);
+
 #endif

@@ -63,11 +63,31 @@ class Layout(C.Structure):
                 ('data_len', C.c_size_t)]
 
 
+class ProgScan(C.Structure):
+    """struct j2p_jpeg_prog_scan — jpeg2png_b200/cli/jpeg_reader.h."""
+    _fields_ = [('s', Scan), ('ss', C.c_uint), ('se', C.c_uint), ('ah', C.c_uint), ('al', C.c_uint)]
+
+
+class ProgLayout(C.Structure):
+    """struct j2p_jpeg_prog_layout — jpeg2png_b200/cli/jpeg_reader.h."""
+    _fields_ = [('w', C.c_uint), ('h', C.c_uint), ('coefs', abi.Coef * 3), ('comp_h', C.c_uint * 3),
+                ('comp_v', C.c_uint * 3), ('progressive_decodable', C.c_int), ('nscan', C.c_uint),
+                ('scan', C.POINTER(ProgScan)), ('nseg', C.c_uint), ('seg', C.POINTER(Segment)),
+                ('data', C.POINTER(C.c_uint8)), ('data_len', C.c_size_t)]
+
+
 class EntropyStats(C.Structure):
     """struct j2p_entropy_stats — jpeg2png_b200/entropy/entropy.h."""
     _fields_ = [('rounds', C.c_uint), ('round_trips', C.c_uint), ('launches', C.c_uint), ('subsequences', C.c_uint)]
 
 
+class ProgressiveStats(C.Structure):
+    """struct j2p_progressive_stats — jpeg2png_b200/progressive/progressive.h."""
+    _fields_ = [('rounds', C.c_uint), ('round_trips', C.c_uint), ('launches', C.c_uint), ('steps', C.c_uint),
+                ('subsequences', C.c_uint), ('refine_segments', C.c_uint), ('step_launches', C.c_uint)]
+
+
+PROGRESSIVE_LIB = os.path.join(abi._PKG_DIR, 'progressive', 'libj2pprogressive.so')
 ENTROPY_LIB = os.path.join(abi._PKG_DIR, 'entropy', 'libj2pentropy.so')
 SUBSEQ_BITS = 1024                  # bits per subsequence of the device decoder (DESIGN §7d)
 ENT_FAILURES = {1: 'bad huffman code', 2: 'bad magnitude category', 3: 'coefficient index out of range'}
@@ -79,6 +99,10 @@ def _declare_codecs(lib):
     lib.j2p_read_jpeg_layout.argtypes = [C.c_char_p, C.c_size_t, C.POINTER(Layout), C.c_char_p, C.c_size_t]
     lib.j2p_free_jpeg_layout.restype = None
     lib.j2p_free_jpeg_layout.argtypes = [C.POINTER(Layout)]
+    lib.j2p_read_jpeg_prog_layout.restype = C.c_int
+    lib.j2p_read_jpeg_prog_layout.argtypes = [C.c_char_p, C.c_size_t, C.POINTER(ProgLayout), C.c_char_p, C.c_size_t]
+    lib.j2p_free_jpeg_prog_layout.restype = None
+    lib.j2p_free_jpeg_prog_layout.argtypes = [C.POINTER(ProgLayout)]
 
 
 def load_codecs() -> C.CDLL:
@@ -105,6 +129,25 @@ def load_entropy() -> C.CDLL:
     return abi.load_library(ENTROPY_LIB, 'entropy decoder', _declare_entropy)
 
 
+def _declare_progressive(lib):
+    vp, lay = C.c_void_p, C.POINTER(C.POINTER(ProgLayout))
+    lib.j2p_progressive_plan_size.restype = C.c_int
+    lib.j2p_progressive_plan_size.argtypes = [lay, C.c_uint, C.c_uint, C.POINTER(C.c_size_t), C.POINTER(C.c_size_t)]
+    lib.j2p_progressive_pack.restype = C.c_int
+    lib.j2p_progressive_pack.argtypes = [lay, C.c_uint, C.c_uint, C.POINTER(vp), vp, C.c_size_t]
+    lib.j2p_progressive_decode.restype = C.c_int
+    lib.j2p_progressive_decode.argtypes = [vp, vp, vp, vp, vp, C.POINTER(ProgressiveStats)]
+    lib.j2p_progressive_decode_host.restype = C.c_int
+    lib.j2p_progressive_decode_host.argtypes = [vp, vp, vp, C.POINTER(ProgressiveStats)]
+    lib.j2p_progressive_last_error.restype = C.c_char_p
+    lib.j2p_progressive_last_error.argtypes = []
+
+
+def load_progressive() -> C.CDLL:
+    """libj2pprogressive.so (the progressive device entropy decoder) from the package tree."""
+    return abi.load_library(PROGRESSIVE_LIB, 'progressive decoder', _declare_progressive)
+
+
 class FileLayout:
     """A file's layout (j2p_read_jpeg_layout); frees the C buffers when collected."""
 
@@ -126,6 +169,31 @@ class FileLayout:
     def __del__(self):
         try:
             load_codecs().j2p_free_jpeg_layout(C.byref(self.lay))
+        except Exception:
+            pass
+
+
+class ProgFileLayout:
+    """A progressive file's layout (j2p_read_jpeg_prog_layout); frees the C buffers when collected."""
+
+    def __init__(self, data: bytes):
+        lib = load_codecs()
+        self.lay = ProgLayout()
+        err = C.create_string_buffer(256)
+        if lib.j2p_read_jpeg_prog_layout(data, len(data), C.byref(self.lay), err, 256) != 0:
+            raise ValueError(err.value.decode(errors='replace'))
+        self.progressive_decodable = bool(self.lay.progressive_decodable)
+        self.w, self.h = int(self.lay.w), int(self.lay.h)
+        self.compressed = int(self.lay.data_len)
+        self.planes = [Plane(int(c.w), int(c.h), int(c.w_samp), int(c.h_samp), None,
+                             np.array(list(c.quant_table), np.uint16)) for c in self.lay.coefs]
+
+    def key(self):
+        return Parsed.key(self)
+
+    def __del__(self):
+        try:
+            load_codecs().j2p_free_jpeg_prog_layout(C.byref(self.lay))
         except Exception:
             pass
 
@@ -154,6 +222,25 @@ def entropy_plan(layouts, outs, subseq_bits=SUBSEQ_BITS, pinned=False):
     o = (C.c_void_p * len(outs))(*outs)
     if lib.j2p_entropy_pack(ptrs, len(layouts), subseq_bits, o, addr, plan_bytes.value) != 0:
         raise RuntimeError(lib.j2p_entropy_last_error().decode())
+    return buf, addr, plan_bytes.value, work_bytes.value
+
+
+def progressive_plan(layouts, outs, subseq_bits=SUBSEQ_BITS, pinned=False):
+    """entropy_plan for ProgFileLayouts and libj2pprogressive.so."""
+    lib = load_progressive()
+    ptrs = (C.POINTER(ProgLayout) * len(layouts))(*[C.pointer(x.lay) for x in layouts])
+    plan_bytes, work_bytes = C.c_size_t(), C.c_size_t()
+    if lib.j2p_progressive_plan_size(ptrs, len(layouts), subseq_bits, C.byref(plan_bytes), C.byref(work_bytes)) != 0:
+        raise RuntimeError(lib.j2p_progressive_last_error().decode())
+    if pinned:
+        buf = torch.empty(plan_bytes.value, dtype=torch.uint8, pin_memory=True)
+        addr = buf.data_ptr()
+    else:
+        buf = np.zeros(plan_bytes.value + 16, np.uint8)
+        addr = (buf.ctypes.data + 15) & ~15
+    o = (C.c_void_p * len(outs))(*outs)
+    if lib.j2p_progressive_pack(ptrs, len(layouts), subseq_bits, o, addr, plan_bytes.value) != 0:
+        raise RuntimeError(lib.j2p_progressive_last_error().decode())
     return buf, addr, plan_bytes.value, work_bytes.value
 
 
@@ -303,6 +390,9 @@ class _DeviceCoefs:
     or the failure kind of file i."""
 
     def __init__(self, device, layouts, stream, subseq_bits=SUBSEQ_BITS):
+        self._decode(device, layouts, stream, subseq_bits, entropy_plan, load_entropy(), 'entropy', EntropyStats())
+
+    def _decode(self, device, layouts, stream, subseq_bits, make_plan, lib, name, stats):
         dev = torch.device('cuda', device)
         sizes = [p.w * p.h for lay in layouts for p in lay.planes]
         offs = np.concatenate([[0], np.cumsum(sizes, dtype=np.int64)])
@@ -310,16 +400,15 @@ class _DeviceCoefs:
             self.coefs = torch.empty(max(int(offs[-1]), 1), dtype=torch.int16, device=dev)
             base = self.coefs.data_ptr()
             self.ptrs = [base + 2 * int(o) for o in offs[:-1]]           # planes are whole 128-byte blocks
-            self.plan, addr, plan_bytes, work_bytes = entropy_plan(layouts, self.ptrs, subseq_bits, pinned=True)
+            self.plan, addr, plan_bytes, work_bytes = make_plan(layouts, self.ptrs, subseq_bits, pinned=True)
             self.plan_dev = torch.empty(plan_bytes, dtype=torch.uint8, device=dev)
             self.plan_dev.copy_(self.plan, non_blocking=True)
             self.work = torch.empty(max(work_bytes, 16), dtype=torch.uint8, device=dev)
             status = torch.empty(len(layouts), dtype=torch.int32, device=dev)
-            self.stats = EntropyStats()
-            lib = load_entropy()
-            if lib.j2p_entropy_decode(addr, self.plan_dev.data_ptr(), self.work.data_ptr(), status.data_ptr(),
-                                      stream.cuda_stream, C.byref(self.stats)) != 0:
-                raise RuntimeError(lib.j2p_entropy_last_error().decode())
+            self.stats = stats
+            if getattr(lib, f'j2p_{name}_decode')(addr, self.plan_dev.data_ptr(), self.work.data_ptr(), status.data_ptr(),
+                                                  stream.cuda_stream, C.byref(self.stats)) != 0:
+                raise RuntimeError(getattr(lib, f'j2p_{name}_last_error')().decode())
             stream.record_event().synchronize()
             self.status = status.cpu().numpy()
         self.plan = self.work = self.plan_dev = None
@@ -332,6 +421,14 @@ class _DeviceCoefs:
         start = (self.ptrs[3 * i + c] - self.coefs.data_ptr()) // 2
         end = (self.ptrs[3 * i + c + 1] - self.coefs.data_ptr()) // 2 if 3 * i + c + 1 < len(self.ptrs) else self.coefs.numel()
         return self.coefs[start:end]
+
+
+class _ProgCoefs(_DeviceCoefs):
+    """_DeviceCoefs for progressive files (ProgFileLayout), decoded by libj2pprogressive.so."""
+
+    def __init__(self, device, layouts, stream, subseq_bits=SUBSEQ_BITS):
+        self._decode(device, layouts, stream, subseq_bits, progressive_plan, load_progressive(), 'progressive',
+                     ProgressiveStats())
 
 
 class _Chunk:
@@ -402,9 +499,10 @@ def _where(i, path):
     return f'input {i} ({path})' if path is not None else f'input {i}'
 
 
-def _front_end(data, device_ok):
-    """The host part of one input: a FileLayout for the device decoder, a Parsed from the host
-    reader, or the ValueError (always the host reader's message) or RuntimeError to raise."""
+def _front_end(data, device_ok, progressive=False):
+    """The host part of one input: a FileLayout for the device decoder, a ProgFileLayout for the
+    progressive device decoder (progressive=True), a Parsed from the host reader, or the ValueError
+    (always the host reader's message) or RuntimeError to raise."""
     if not device_ok or _host_front_end:
         try:
             return parse_jpeg(data)
@@ -420,6 +518,17 @@ def _front_end(data, device_ok):
         return RuntimeError('the layout pass rejected a file the host reader accepts')
     if lay.device_decodable:
         return lay
+    if progressive:
+        try:
+            prog = ProgFileLayout(data)
+        except ValueError:
+            try:
+                parse_jpeg(data)
+            except ValueError as e:
+                return e
+            return RuntimeError('the progressive layout pass rejected a file the host reader accepts')
+        if prog.progressive_decodable:
+            return prog
     try:
         return parse_jpeg(data)
     except ValueError as e:
@@ -427,7 +536,7 @@ def _front_end(data, device_ok):
 
 
 def decode_jpeg(inputs, *, iterations=50, weight=0.3, pweight=0.001, separate=False,
-                dtype=torch.uint8, layout='CHW', device=None, max_frames=None):
+                dtype=torch.uint8, layout='CHW', device=None, max_frames=None, progressive_on_device=False):
     """Decode JPEG files into RGB tensors on a CUDA device, deblocked by the solver.
 
     inputs: bytes-like, a path (str / os.PathLike), or a list or tuple of them.  A single input
@@ -445,8 +554,9 @@ def decode_jpeg(inputs, *, iterations=50, weight=0.3, pweight=0.001, separate=Fa
     be used there without synchronising.
 
     Sequential (baseline or extended) files whose three components are each coded in one scan are
-    Huffman-decoded on the device: only their compressed bytes are uploaded.  Every other file,
-    progressive ones included, is parsed on the host.  Raises ValueError for bad arguments and
+    Huffman-decoded on the device: only their compressed bytes are uploaded.  progressive_on_device:
+    progressive files are Huffman-decoded on the device too (libj2pprogressive.so, DESIGN §7g);
+    by default they are parsed on the host, as is every other file.  Raises ValueError for bad arguments and
     unreadable files, with the host reader's message: header errors before any device work, errors
     in a device-decoded file's entropy-coded data once its batch has been decoded, before that batch
     is solved.  Raises RuntimeError when no CUDA device is usable.
@@ -474,9 +584,9 @@ def decode_jpeg(inputs, *, iterations=50, weight=0.3, pweight=0.001, separate=Fa
     workers = min(len(read), os.cpu_count() or 1, 16)
     if workers > 1:
         with ThreadPoolExecutor(workers) as pool:
-            parsed = list(pool.map(lambda d: _front_end(d, device_ok), [data for data, _ in read]))
+            parsed = list(pool.map(lambda d: _front_end(d, device_ok, progressive_on_device), [data for data, _ in read]))
     else:
-        parsed = [_front_end(data, device_ok) for data, _ in read]
+        parsed = [_front_end(data, device_ok, progressive_on_device) for data, _ in read]
     for i, (p, (_, path)) in enumerate(zip(parsed, read)):
         if isinstance(p, ValueError):
             raise ValueError(f'{_where(i, path)}: {p}')
@@ -501,10 +611,12 @@ def decode_jpeg(inputs, *, iterations=50, weight=0.3, pweight=0.001, separate=Fa
             # solve of the chunk before it
             coef_stream = torch.cuda.Stream(index)
             for _, idx in chunks:
-                on_dev = [j for j, i in enumerate(idx) if isinstance(parsed[i], FileLayout)]
                 coefs = {}
-                if on_dev:
-                    dc = _DeviceCoefs(index, [parsed[idx[j]] for j in on_dev], coef_stream)
+                for kind, decoder in ((FileLayout, _DeviceCoefs), (ProgFileLayout, _ProgCoefs)):
+                    on_dev = [j for j, i in enumerate(idx) if isinstance(parsed[i], kind)]
+                    if not on_dev:
+                        continue
+                    dc = decoder(index, [parsed[idx[j]] for j in on_dev], coef_stream)
                     for k, j in enumerate(on_dev):
                         if dc.status[k] != 0:
                             i = idx[j]

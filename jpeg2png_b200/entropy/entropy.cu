@@ -116,29 +116,6 @@ extern "C" int j2p_entropy_plan_size(const struct j2p_jpeg_layout *const *layout
     return 0;
 }
 
-// build_huff of jpeg_reader.c, plus the 9-bit first level
-static void build_table(const struct j2p_jpeg_huff *src, j2p_ent_table *t) {
-    memset(t, 0, sizeof *t);
-    int code = 0, k = 0;
-    for (int l = 1; l <= 16; l++) {
-        t->valptr[l] = k;
-        t->mincode[l] = code;
-        code += src->bits[l];
-        k += src->bits[l];
-        t->maxcode[l] = src->bits[l] ? code - 1 : -1;
-        code <<= 1;
-    }
-    memcpy(t->vals, src->vals, 256);
-    for (int p = 0; p < 512; p++)
-        for (int l = 1; l <= 9; l++) {
-            const int c = p >> (9 - l);
-            if (t->maxcode[l] >= 0 && c <= t->maxcode[l] && c >= t->mincode[l]) {
-                t->lut[p] = (uint16_t)((l << 8) | t->vals[t->valptr[l] + c - t->mincode[l]]);
-                break;
-            }
-        }
-}
-
 extern "C" int j2p_entropy_pack(const struct j2p_jpeg_layout *const *L, unsigned n, unsigned S, int16_t *const *out, void *dst,
                                 size_t plan_bytes) {
     Counts c;
@@ -180,8 +157,8 @@ extern "C" int j2p_entropy_pack(const struct j2p_jpeg_layout *const *L, unsigned
                 sc->bh[s] = ls->bh[s];
                 sc->dctab[s] = 6 * iscan + 2 * s;
                 sc->actab[s] = 6 * iscan + 2 * s + 1;
-                build_table(&ls->dc[s], &tabs[sc->dctab[s]]);
-                build_table(&ls->ac[s], &tabs[sc->actab[s]]);
+                j2p_ent_build_table(&ls->dc[s], &tabs[sc->dctab[s]]);
+                j2p_ent_build_table(&ls->ac[s], &tabs[sc->actab[s]]);
                 for (unsigned y = 0; y < ls->bh[s]; y++)
                     for (unsigned x = 0; x < ls->bw[s]; x++, bpm++) {
                         sc->slot[bpm] = (uint8_t)s;

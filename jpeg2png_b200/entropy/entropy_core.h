@@ -25,6 +25,7 @@
 #include <stdint.h>
 #include <string.h>
 
+#include "../cli/jpeg_reader.h"         /* struct j2p_jpeg_huff */
 #include "../common/codec_host.h"       /* J2P_HD */
 #include "entropy.h"
 
@@ -77,6 +78,29 @@ struct j2p_ent_view {
         uint32_t *changed;
         uint32_t *status;           /* per file */
 };
+
+/* build_huff of jpeg_reader.c, plus the 9-bit first level (host) */
+static inline void j2p_ent_build_table(const struct j2p_jpeg_huff *src, struct j2p_ent_table *t) {
+        memset(t, 0, sizeof *t);
+        int code = 0, k = 0;
+        for (int l = 1; l <= 16; l++) {
+                t->valptr[l] = k;
+                t->mincode[l] = code;
+                code += src->bits[l];
+                k += src->bits[l];
+                t->maxcode[l] = src->bits[l] ? code - 1 : -1;
+                code <<= 1;
+        }
+        memcpy(t->vals, src->vals, 256);
+        for (int p = 0; p < 512; p++)
+                for (int l = 1; l <= 9; l++) {
+                        const int c = p >> (9 - l);
+                        if (t->maxcode[l] >= 0 && c <= t->maxcode[l] && c >= t->mincode[l]) {
+                                t->lut[p] = (uint16_t)((l << 8) | t->vals[t->valptr[l] + c - t->mincode[l]]);
+                                break;
+                        }
+                }
+}
 
 #ifdef __CUDA_ARCH__
 __constant__ uint8_t j2p_ent_zz[64] =
