@@ -1,4 +1,4 @@
-# The build of one codec library (entropy, png, jpegenc): one .cu into one sm_90a shared object,
+# The build of one codec library (entropy, png, jpegenc, jpegopt, progressive): one .cu into one sm_90a shared object,
 # kept out of libjpeg2png_b200.so, whose kernels are the solver's.  The including Makefile sets LIB,
 # SRC, DEPS (its headers) and, where the library needs them, EXTRA_NVFLAGS.
 

@@ -3,9 +3,11 @@
 The encoder is libj2pjpegenc.so (jpeg2png_b200/jpegenc, DESIGN §7f).  It writes the file that
 Pillow writes for the same pixels with `quality` and `subsampling` and no other options (libjpeg's
 compressor defaults: JFIF header, IJG quality tables, slow-integer DCT, the Annex K Huffman tables,
-one interleaved scan).  Colour conversion, downsampling, DCT, quantisation, Huffman coding and byte
-stuffing all run on the device; only the finished files cross PCIe.  `encode_host` runs the same
-steps serially on numpy arrays and gives the same bytes.
+one interleaved scan).  With `optimize=True` the encoder is libj2pjpegopt.so (jpeg2png_b200/jpegopt),
+which writes Pillow's `optimize=True` file: the same coefficients, coded with Huffman tables built
+per image from its own symbol counts.  Colour conversion, downsampling, DCT, quantisation, the
+tables, Huffman coding and byte stuffing all run on the device; only the finished files cross PCIe.
+`encode_host` runs the same steps serially on numpy arrays and gives the same bytes.
 
 The module is not called encode_jpeg.py: importing it would make the package attribute
 `encode_jpeg` the module instead of the function.
@@ -23,6 +25,7 @@ from . import abi
 from . import batch_encode as B
 
 JPEGENC_LIB = os.path.join(abi._PKG_DIR, 'jpegenc', 'libj2pjpegenc.so')
+JPEGOPT_LIB = os.path.join(abi._PKG_DIR, 'jpegopt', 'libj2pjpegopt.so')
 SAMPLINGS = {'4:4:4': 0, '4:2:2': 1, '4:2:0': 2}
 MAX_SIDE = 65535                    # SOF's 16-bit height and width
 
@@ -43,22 +46,35 @@ class Stats(C.Structure):
     _fields_ = [('launches', C.c_uint), ('blocks', C.c_uint64)]
 
 
-def _declare(lib):
+def _declare(lib, name='jpegenc'):
     vp, sz = C.c_void_p, C.c_size_t
     imgs, par = C.POINTER(Image), C.POINTER(Params)
-    lib.j2p_jpegenc_plan.restype = C.c_int
-    lib.j2p_jpegenc_plan.argtypes = [imgs, C.c_uint, par, C.POINTER(sz), C.POINTER(sz)]
-    lib.j2p_jpegenc_encode.restype = C.c_int
-    lib.j2p_jpegenc_encode.argtypes = [imgs, C.c_uint, par, vp, sz, vp, C.POINTER(C.c_uint64), vp, sz, C.POINTER(Stats)]
-    lib.j2p_jpegenc_encode_host.restype = C.c_int
-    lib.j2p_jpegenc_encode_host.argtypes = [imgs, C.c_uint, par, vp, sz, C.POINTER(C.c_uint64)]
-    lib.j2p_jpegenc_last_error.restype = C.c_char_p
-    lib.j2p_jpegenc_last_error.argtypes = []
+    fn = lambda f: getattr(lib, f'j2p_{name}_{f}')  # noqa: E731
+    fn('plan').restype = C.c_int
+    fn('plan').argtypes = [imgs, C.c_uint, par, C.POINTER(sz), C.POINTER(sz)]
+    fn('encode').restype = C.c_int
+    fn('encode').argtypes = [imgs, C.c_uint, par, vp, sz, vp, C.POINTER(C.c_uint64), vp, sz, C.POINTER(Stats)]
+    fn('encode_host').restype = C.c_int
+    fn('encode_host').argtypes = [imgs, C.c_uint, par, vp, sz, C.POINTER(C.c_uint64)]
+    fn('last_error').restype = C.c_char_p
+    fn('last_error').argtypes = []
+
+
+def _declare_opt(lib):
+    _declare(lib, 'jpegopt')
+    u8 = C.POINTER(C.c_uint8)
+    lib.j2p_jpegopt_build_table.restype = C.c_int
+    lib.j2p_jpegopt_build_table.argtypes = [C.POINTER(C.c_uint64), u8, u8, C.POINTER(C.c_uint)]
 
 
 def load_jpegenc() -> C.CDLL:
     """libj2pjpegenc.so (the device JPEG encoder) from the package tree."""
     return abi.load_library(JPEGENC_LIB, 'JPEG encoder', _declare)
+
+
+def load_jpegopt() -> C.CDLL:
+    """libj2pjpegopt.so (the device JPEG encoder with optimized Huffman tables) from the package tree."""
+    return abi.load_library(JPEGOPT_LIB, 'optimizing JPEG encoder', _declare_opt)
 
 
 def params(quality, subsampling) -> Params:
@@ -76,11 +92,29 @@ def _check_size(shape, h, w):
 
 
 CODEC = B.Codec('jpegenc', lambda: load_jpegenc(), Image, _check_size)
+CODEC_OPT = B.Codec('jpegopt', lambda: load_jpegopt(), Image, _check_size)
 
 
-def codec(p: Params) -> B.Codec:
-    """libj2pjpegenc.so for the shared driver, with the call parameters p."""
-    return dataclasses.replace(CODEC, params=(C.byref(p),))
+def codec(p: Params, optimize=False) -> B.Codec:
+    """libj2pjpegenc.so, or libj2pjpegopt.so when optimize, for the shared driver, with the call
+    parameters p."""
+    return dataclasses.replace(CODEC_OPT if optimize else CODEC, params=(C.byref(p),))
+
+
+def check_optimize(optimize):
+    if not isinstance(optimize, bool):
+        raise ValueError(f'optimize must be True or False, not {optimize!r}')
+
+
+def build_table(counts):
+    """The optimized table of 256 symbol counts (j2p_jpegopt_build_table): (bits[16], vals), the
+    DHT's code counts per length 1..16 and its symbols in order."""
+    c = (C.c_uint64 * 256)(*[int(v) for v in counts])
+    bits, vals, nv = (C.c_uint8 * 16)(), (C.c_uint8 * 256)(), C.c_uint()
+    lib = load_jpegopt()
+    if lib.j2p_jpegopt_build_table(c, bits, vals, C.byref(nv)) != 0:
+        raise ValueError(lib.j2p_jpegopt_last_error().decode())
+    return list(bits), list(vals)[:nv.value]
 
 
 def _descs(items, layout, ptr, strides):
@@ -93,32 +127,39 @@ def _work_bytes(descs, p):
     return codec(p).plan(descs)[0]
 
 
-def encode_host(images, quality=75, subsampling='4:2:0', layout='HWC'):
-    """The serial host driver (j2p_jpegenc_encode_host) on numpy uint8 arrays: a list of JPEG files
-    as bytes, the same bytes the device writes."""
+def encode_host(images, quality=75, subsampling='4:2:0', layout='HWC', optimize=False):
+    """The serial host driver (j2p_jpegenc_encode_host, or j2p_jpegopt_encode_host when optimize)
+    on numpy uint8 arrays: a list of JPEG files as bytes, the same bytes the device writes."""
     B.check_layout(layout)
     p = params(quality, subsampling)
+    check_optimize(optimize)
     for x in images:
         if x.dtype != np.uint8:
             raise ValueError(f'samples are uint8, not {x.dtype}')
-    return B.encode_host(codec(p), images, layout)
+    return B.encode_host(codec(p, optimize), images, layout)
 
 
-def encode_jpeg(images, *, quality=75, subsampling='4:2:0', layout='CHW'):
+def encode_jpeg(images, *, quality=75, subsampling='4:2:0', layout='CHW', optimize=False):
     """Encode RGB CUDA tensors as baseline JPEG files on the device.
 
     images: one tensor or a list or tuple of them, torch.uint8, shaped (3, h, w) for layout='CHW'
     or (h, w, 3) for 'HWC', with any strides, 1..65535 pixels high and wide.  quality: an integer
     in 1..100; subsampling: '4:4:4', '4:2:2' or '4:2:0'.  Returns the JPEG file as bytes, or a list
     of bytes in input order: byte for byte the file Pillow writes for the same pixels with
-    `save(f, 'JPEG', quality=quality, subsampling=subsampling)`.
+    `save(f, 'JPEG', quality=quality, subsampling=subsampling, optimize=optimize)`.
+
+    optimize: False writes the Annex K Huffman tables; True builds each image's tables from its own
+    symbol counts, on the device, as libjpeg does for `optimize=True`: the same coefficients, files
+    typically 6-9% smaller, at the cost of two more kernels per call.
 
     The work is queued on torch's current stream, after what is already there, so a tensor just
     written on that stream needs no synchronisation.  Images of any mix of sizes go into one call;
     a list is split into several only when the work area would not fit in a quarter of the free
-    device memory.  Raises ValueError for a wrong dtype, shape, layout, quality, subsampling or
-    size, and for a tensor that is not on a CUDA device, and RuntimeError when no CUDA device is
-    usable.
+    device memory.  Raises ValueError for a wrong dtype, shape, layout, quality, subsampling,
+    optimize (not a bool) or size, and for a tensor that is not on a CUDA device, and RuntimeError
+    when no CUDA device is usable.
     """
     B.check_layout(layout)
-    return B.encode_tensors('encode_jpeg', codec(params(quality, subsampling)), images, layout, (torch.uint8,))
+    p = params(quality, subsampling)
+    check_optimize(optimize)
+    return B.encode_tensors('encode_jpeg', codec(p, optimize), images, layout, (torch.uint8,))

@@ -49,12 +49,17 @@ struct j2p_je_img {
         uint64_t file_off, file_len;
 };
 
+// derived Huffman codes of the four tables: DC0, AC0, DC1, AC1 (jpeg_make_c_derived_tbl)
+struct j2p_je_huff {
+        uint16_t code[4][256];
+        uint8_t size[4][256];
+};
+
 // per call: quantisation reciprocals (natural order), derived Huffman codes, the header template
 struct j2p_je_tables {
         uint16_t recip[2][64], corr[2][64];
         uint8_t shift[2][64];           // total right shift of the product
-        uint16_t code[4][256];          // DC0, AC0, DC1, AC1
-        uint8_t size[4][256];
+        struct j2p_je_huff huff;        // the Annex K tables
         uint8_t zz[64];                 // zig-zag position of each natural index
         uint32_t hs, vs;                // luma sampling factors (chroma 1 x 1)
         uint8_t head[J2P_JE_HEAD];
@@ -217,37 +222,47 @@ J2P_HD int j2p_je_nbits(int v) {
         return (int)n;
 }
 
-// Walks the symbols of a block (zig-zag coefficients c, DC prediction pred): put(code, size) for
-// each Huffman code and each run of extra bits, in order.
+// Walks the symbols of a block (zig-zag coefficients c, DC prediction pred): sym(table, symbol)
+// for each Huffman-coded symbol (table 0 DC0, 1 AC0, 2 DC1, 3 AC1; the DC category, run << 4 |
+// size, ZRL 0xF0 or EOB 0x00) and extra(bits, n) for each run of extra bits, in order.
 #ifdef __CUDACC__
-#pragma nv_exec_check_disable           // put / orw are host lambdas in the host driver, device ones in the kernels
+#pragma nv_exec_check_disable           // sym / extra are host lambdas in the host driver, device ones in the kernels
 #endif
-template <typename Put>
-J2P_HD void j2p_je_walk(const int16_t *c, int pred, const struct j2p_je_tables *t, uint32_t comp, Put &&put) {
+template <typename Sym, typename Extra>
+J2P_HD void j2p_je_symbols(const int16_t *c, int pred, uint32_t comp, Sym &&sym, Extra &&extra) {
         const int dc = comp ? 2 : 0, ac = dc + 1;
         int diff = c[0] - pred, nb = j2p_je_nbits(diff);
-        put(t->code[dc][nb], t->size[dc][nb]);
-        if (nb) put((uint32_t)(diff < 0 ? diff - 1 : diff) & ((1u << nb) - 1), nb);
+        sym(dc, nb);
+        if (nb) extra((uint32_t)(diff < 0 ? diff - 1 : diff) & ((1u << nb) - 1), nb);
         int run = 0;
         for (int k = 1; k < 64; k++) {
                 const int v = c[k];
                 if (v == 0) { run++; continue; }
                 while (run > 15) {
-                        put(t->code[ac][0xf0], t->size[ac][0xf0]);
+                        sym(ac, 0xf0);
                         run -= 16;
                 }
                 nb = j2p_je_nbits(v);
-                const int s = (run << 4) + nb;
-                put(t->code[ac][s], t->size[ac][s]);
-                put((uint32_t)(v < 0 ? v - 1 : v) & ((1u << nb) - 1), nb);
+                sym(ac, (run << 4) + nb);
+                extra((uint32_t)(v < 0 ? v - 1 : v) & ((1u << nb) - 1), nb);
                 run = 0;
         }
-        if (run > 0) put(t->code[ac][0], t->size[ac][0]);
+        if (run > 0) sym(ac, 0);
 }
 
-J2P_HD uint32_t j2p_je_block_bits(const int16_t *c, int pred, const struct j2p_je_tables *t, uint32_t comp) {
+// The block's symbols through the tables h: put(code, size) for each Huffman code and each run of
+// extra bits, in order.
+#ifdef __CUDACC__
+#pragma nv_exec_check_disable           // put / orw are host lambdas in the host driver, device ones in the kernels
+#endif
+template <typename Put>
+J2P_HD void j2p_je_walk(const int16_t *c, int pred, const struct j2p_je_huff *h, uint32_t comp, Put &&put) {
+        j2p_je_symbols(c, pred, comp, [&](int tbl, int s) { put(h->code[tbl][s], h->size[tbl][s]); }, put);
+}
+
+J2P_HD uint32_t j2p_je_block_bits(const int16_t *c, int pred, const struct j2p_je_huff *h, uint32_t comp) {
         uint32_t n = 0;
-        j2p_je_walk(c, pred, t, comp, [&](uint32_t, int s) { n += (uint32_t)s; });
+        j2p_je_walk(c, pred, h, comp, [&](uint32_t, int s) { n += (uint32_t)s; });
         return n;
 }
 
@@ -278,9 +293,9 @@ struct j2p_je_writer {
 #pragma nv_exec_check_disable
 #endif
 template <typename Or>
-J2P_HD void j2p_je_emit(const int16_t *c, int pred, const struct j2p_je_tables *t, uint32_t comp, uint64_t pos, Or orw) {
+J2P_HD void j2p_je_emit(const int16_t *c, int pred, const struct j2p_je_huff *h, uint32_t comp, uint64_t pos, Or orw) {
         j2p_je_writer<Or> w = {orw, 0, (uint32_t)(pos & 31), pos >> 5};
-        j2p_je_walk(c, pred, t, comp, w);
+        j2p_je_walk(c, pred, h, comp, w);
         if (w.fill) w.orw(w.word, (uint32_t)(w.acc >> 32));
 }
 

@@ -1,0 +1,384 @@
+// jpegenc_plan.h — the host side shared by libj2pjpegenc.so and libj2pjpegopt.so: the quantisation
+// tables and their reciprocals, the Annex K Huffman tables and the header template, the plan of a
+// call (the layout of its work area), the steps that both the kernels and the host driver call per
+// block, and the serial host driver.  The two libraries differ only in where an image's Huffman
+// tables and header come from: the call's Annex K ones, or the image's own optimized ones
+// (jpegopt_core.h), and in the work-area bound of a block that follows.
+#ifndef J2P_JPEGENC_PLAN_H
+#define J2P_JPEGENC_PLAN_H
+
+#include <string.h>
+
+#include "../common/codec_host.h"
+#include "jpegenc_core.h"
+
+// ---- tables ------------------------------------------------------------------------------------
+static const uint8_t kNatural[64] = {0,  1,  8,  16, 9,  2,  3,  10, 17, 24, 32, 25, 18, 11, 4,  5,  12, 19, 26, 33, 40, 48,
+                                     41, 34, 27, 20, 13, 6,  7,  14, 21, 28, 35, 42, 49, 56, 57, 50, 43, 36, 29, 22, 15, 23,
+                                     30, 37, 44, 51, 58, 59, 52, 45, 38, 31, 39, 46, 53, 60, 61, 54, 47, 55, 62, 63};
+
+// ITU-T T.81 Annex K.1, natural order
+static const uint8_t kBaseQuant[2][64] = {
+    {16, 11, 10, 16, 24,  40,  51,  61,  12, 12, 14, 19, 26,  58,  60,  55,  14, 13, 16, 24, 40,  57,  69,  56,
+     14, 17, 22, 29, 51,  87,  80,  62,  18, 22, 37, 56, 68,  109, 103, 77,  24, 35, 55, 64, 81,  104, 113, 92,
+     49, 64, 78, 87, 103, 121, 120, 101, 72, 92, 95, 98, 112, 100, 103, 99},
+    {17, 18, 24, 47, 99, 99, 99, 99, 18, 21, 26, 66, 99, 99, 99, 99, 24, 26, 56, 99, 99, 99, 99, 99, 47, 66, 99, 99,
+     99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99,
+     99, 99, 99, 99, 99, 99, 99, 99}};
+
+// ITU-T T.81 Annex K.3: code counts per length 1..16, then the symbols; DC0, AC0, DC1, AC1
+static const uint8_t kDcBits[2][16] = {{0, 1, 5, 1, 1, 1, 1, 1, 1, 0, 0, 0, 0, 0, 0, 0}, {0, 3, 1, 1, 1, 1, 1, 1, 1, 1, 1, 0, 0, 0, 0, 0}};
+static const uint8_t kDcVals[12] = {0, 1, 2, 3, 4, 5, 6, 7, 8, 9, 10, 11};
+static const uint8_t kAcBits[2][16] = {{0, 2, 1, 3, 3, 2, 4, 3, 5, 5, 4, 4, 0, 0, 1, 0x7d}, {0, 2, 1, 2, 4, 4, 3, 4, 7, 5, 4, 4, 0, 1, 2, 0x77}};
+static const uint8_t kAcVals[2][162] = {
+    {0x01, 0x02, 0x03, 0x00, 0x04, 0x11, 0x05, 0x12, 0x21, 0x31, 0x41, 0x06, 0x13, 0x51, 0x61, 0x07, 0x22, 0x71, 0x14, 0x32, 0x81,
+     0x91, 0xa1, 0x08, 0x23, 0x42, 0xb1, 0xc1, 0x15, 0x52, 0xd1, 0xf0, 0x24, 0x33, 0x62, 0x72, 0x82, 0x09, 0x0a, 0x16, 0x17, 0x18,
+     0x19, 0x1a, 0x25, 0x26, 0x27, 0x28, 0x29, 0x2a, 0x34, 0x35, 0x36, 0x37, 0x38, 0x39, 0x3a, 0x43, 0x44, 0x45, 0x46, 0x47, 0x48,
+     0x49, 0x4a, 0x53, 0x54, 0x55, 0x56, 0x57, 0x58, 0x59, 0x5a, 0x63, 0x64, 0x65, 0x66, 0x67, 0x68, 0x69, 0x6a, 0x73, 0x74, 0x75,
+     0x76, 0x77, 0x78, 0x79, 0x7a, 0x83, 0x84, 0x85, 0x86, 0x87, 0x88, 0x89, 0x8a, 0x92, 0x93, 0x94, 0x95, 0x96, 0x97, 0x98, 0x99,
+     0x9a, 0xa2, 0xa3, 0xa4, 0xa5, 0xa6, 0xa7, 0xa8, 0xa9, 0xaa, 0xb2, 0xb3, 0xb4, 0xb5, 0xb6, 0xb7, 0xb8, 0xb9, 0xba, 0xc2, 0xc3,
+     0xc4, 0xc5, 0xc6, 0xc7, 0xc8, 0xc9, 0xca, 0xd2, 0xd3, 0xd4, 0xd5, 0xd6, 0xd7, 0xd8, 0xd9, 0xda, 0xe1, 0xe2, 0xe3, 0xe4, 0xe5,
+     0xe6, 0xe7, 0xe8, 0xe9, 0xea, 0xf1, 0xf2, 0xf3, 0xf4, 0xf5, 0xf6, 0xf7, 0xf8, 0xf9, 0xfa},
+    {0x00, 0x01, 0x02, 0x03, 0x11, 0x04, 0x05, 0x21, 0x31, 0x06, 0x12, 0x41, 0x51, 0x07, 0x61, 0x71, 0x13, 0x22, 0x32, 0x81, 0x08,
+     0x14, 0x42, 0x91, 0xa1, 0xb1, 0xc1, 0x09, 0x23, 0x33, 0x52, 0xf0, 0x15, 0x62, 0x72, 0xd1, 0x0a, 0x16, 0x24, 0x34, 0xe1, 0x25,
+     0xf1, 0x17, 0x18, 0x19, 0x1a, 0x26, 0x27, 0x28, 0x29, 0x2a, 0x35, 0x36, 0x37, 0x38, 0x39, 0x3a, 0x43, 0x44, 0x45, 0x46, 0x47,
+     0x48, 0x49, 0x4a, 0x53, 0x54, 0x55, 0x56, 0x57, 0x58, 0x59, 0x5a, 0x63, 0x64, 0x65, 0x66, 0x67, 0x68, 0x69, 0x6a, 0x73, 0x74,
+     0x75, 0x76, 0x77, 0x78, 0x79, 0x7a, 0x82, 0x83, 0x84, 0x85, 0x86, 0x87, 0x88, 0x89, 0x8a, 0x92, 0x93, 0x94, 0x95, 0x96, 0x97,
+     0x98, 0x99, 0x9a, 0xa2, 0xa3, 0xa4, 0xa5, 0xa6, 0xa7, 0xa8, 0xa9, 0xaa, 0xb2, 0xb3, 0xb4, 0xb5, 0xb6, 0xb7, 0xb8, 0xb9, 0xba,
+     0xc2, 0xc3, 0xc4, 0xc5, 0xc6, 0xc7, 0xc8, 0xc9, 0xca, 0xd2, 0xd3, 0xd4, 0xd5, 0xd6, 0xd7, 0xd8, 0xd9, 0xda, 0xe2, 0xe3, 0xe4,
+     0xe5, 0xe6, 0xe7, 0xe8, 0xe9, 0xea, 0xf2, 0xf3, 0xf4, 0xf5, 0xf6, 0xf7, 0xf8, 0xf9, 0xfa}};
+
+// IJG quality scaling (jpeg_quality_scaling, jpeg_add_quant_table with force_baseline)
+static void quant_table(int quality, int tbl, uint16_t *q) {
+    const long s = quality < 50 ? 5000 / quality : 200 - 2 * quality;
+    for (int i = 0; i < 64; i++) {
+        long v = (kBaseQuant[tbl][i] * s + 50) / 100;
+        q[i] = (uint16_t)(v < 1 ? 1 : v > 255 ? 255 : v);
+    }
+}
+
+// libjpeg-turbo's reciprocal of a divisor d >= 2 (compute_reciprocal, 16-bit DCT elements):
+// (|x| + corr) * recip >> shift is x / d rounded half away from zero for every |x| < 2^15
+static void reciprocal(uint32_t d, uint16_t *recip, uint16_t *corr, uint8_t *shift) {
+    int b = 31 - __builtin_clz(d);
+    int r = 16 + b;
+    uint64_t fq = (1ull << r) / d, fr = (1ull << r) % d;
+    uint32_t c = d / 2;
+    if (fr == 0) {
+        fq >>= 1;
+        r--;
+    } else if (fr <= d / 2) {
+        c++;
+    } else {
+        fq++;
+    }
+    *recip = (uint16_t)fq;
+    *corr = (uint16_t)c;
+    *shift = (uint8_t)r;
+}
+
+// jpeg_make_c_derived_tbl: canonical codes from the counts per length (Annex C)
+J2P_HD void j2p_je_derive(const uint8_t *bits, const uint8_t *vals, uint16_t *code, uint8_t *size) {
+    uint32_t c = 0, p = 0;
+    for (int len = 1; len <= 16; len++) {
+        for (int k = 0; k < bits[len - 1]; k++, p++) {
+            code[vals[p]] = (uint16_t)c++;
+            size[vals[p]] = (uint8_t)len;
+        }
+        c <<= 1;
+    }
+}
+
+static uint8_t *put16(uint8_t *o, uint32_t v) {
+    o[0] = (uint8_t)(v >> 8);
+    o[1] = (uint8_t)v;
+    return o + 2;
+}
+
+static uint8_t *put_dht(uint8_t *o, int index, const uint8_t *bits, const uint8_t *vals) {
+    uint32_t n = 0;
+    for (int k = 0; k < 16; k++) n += bits[k];
+    o = put16(o, 0xffc4);
+    o = put16(o, 2 + 1 + 16 + n);
+    *o++ = (uint8_t)index;
+    memcpy(o, bits, 16);
+    memcpy(o + 16, vals, n);
+    return o + 16 + n;
+}
+
+static void make_tables(const struct j2p_jpegenc_params *p, struct j2p_je_tables *t) {
+    memset(t, 0, sizeof *t);
+    t->hs = p->sampling == J2P_JPEGENC_444 ? 1 : 2;
+    t->vs = p->sampling == J2P_JPEGENC_420 ? 2 : 1;
+    uint16_t q[2][64];
+    for (int tbl = 0; tbl < 2; tbl++) {
+        quant_table(p->quality, tbl, q[tbl]);
+        for (int i = 0; i < 64; i++) reciprocal((uint32_t)q[tbl][i] << 3, &t->recip[tbl][i], &t->corr[tbl][i], &t->shift[tbl][i]);
+    }
+    for (int k = 0; k < 64; k++) t->zz[kNatural[k]] = (uint8_t)k;
+    j2p_je_derive(kDcBits[0], kDcVals, t->huff.code[0], t->huff.size[0]);
+    j2p_je_derive(kAcBits[0], kAcVals[0], t->huff.code[1], t->huff.size[1]);
+    j2p_je_derive(kDcBits[1], kDcVals, t->huff.code[2], t->huff.size[2]);
+    j2p_je_derive(kAcBits[1], kAcVals[1], t->huff.code[3], t->huff.size[3]);
+
+    uint8_t *o = t->head;
+    o = put16(o, 0xffd8);
+    static const uint8_t app0[18] = {0xff, 0xe0, 0, 16, 'J', 'F', 'I', 'F', 0, 1, 1, 0, 0, 1, 0, 1, 0, 0};
+    memcpy(o, app0, 18);
+    o += 18;
+    for (int tbl = 0; tbl < 2; tbl++) {
+        o = put16(o, 0xffdb);
+        o = put16(o, 67);
+        *o++ = (uint8_t)tbl;
+        for (int k = 0; k < 64; k++) *o++ = (uint8_t)q[tbl][kNatural[k]];
+    }
+    o = put16(o, 0xffc0);               // the size is patched per image (j2p_je_head_byte)
+    o = put16(o, 17);
+    *o++ = 8;
+    o = put16(o, 0);
+    o = put16(o, 0);
+    *o++ = 3;
+    const uint8_t comps[9] = {1, (uint8_t)(t->hs << 4 | t->vs), 0, 2, 0x11, 1, 3, 0x11, 1};
+    memcpy(o, comps, 9);
+    o += 9;
+    o = put_dht(o, 0x00, kDcBits[0], kDcVals);
+    o = put_dht(o, 0x10, kAcBits[0], kAcVals[0]);
+    o = put_dht(o, 0x01, kDcBits[1], kDcVals);
+    o = put_dht(o, 0x11, kAcBits[1], kAcVals[1]);
+    static const uint8_t sos[14] = {0xff, 0xda, 0, 12, 3, 1, 0x00, 2, 0x11, 3, 0x11, 0, 63, 0};
+    memcpy(o, sos, 14);
+}
+
+// ---- plan --------------------------------------------------------------------------------------
+// work: [images][tables] [tile sums][tile offsets][block offsets in the tile][coefficients]
+//       [0xFF counts per chunk][their exclusive scan][offsets]
+//       (own codes only: [derived tables][headers][header lengths][symbol counts])
+//       [entropy words][files]
+// The symbol counts sit just before the entropy words, so that one memset clears both.
+struct Layout {
+    uint32_t n, ntiles, nchunks;
+    uint64_t nblk, words;
+    size_t off_imgs, off_tab, off_tsum, off_toff, off_intra, off_coef, off_ffc, off_ffpre, off_offs, off_raw, off_out, total;
+    size_t off_huff, off_head, off_hlen, off_hist;      // per image; empty without own codes
+};
+
+#define J2P_JE_SYMBOLS 256u             // symbol counts per table and image (4 tables)
+
+// wpb: entropy words per block of the worst case; own: room for per-image tables and headers
+static int make_plan(const struct j2p_jpegenc_image *im, unsigned n, const struct j2p_jpegenc_params *p, uint32_t wpb, bool own, Layout *L,
+                     struct j2p_je_img *imgs) {
+    if (!im) return fail("null argument: images");
+    if (!p) return fail("null argument: params");
+    if (n == 0) return fail("no images");
+    if (p->quality < 1 || p->quality > 100) return fail("quality must be 1 .. 100 (got %d)", p->quality);
+    if (p->sampling != J2P_JPEGENC_444 && p->sampling != J2P_JPEGENC_422 && p->sampling != J2P_JPEGENC_420)
+        return fail("unknown sampling %d (0: 4:4:4, 1: 4:2:2, 2: 4:2:0)", p->sampling);
+    const uint32_t hs = p->sampling == J2P_JPEGENC_444 ? 1 : 2, vs = p->sampling == J2P_JPEGENC_420 ? 2 : 1, bpm = hs * vs + 2;
+    uint64_t nblk = 0, words = 0, tiles = 0, chunks = 0, out = 0;
+    for (unsigned i = 0; i < n; i++) {
+        const struct j2p_jpegenc_image *x = &im[i];
+        if (!x->data) return fail("image %u: null data pointer", i);
+        if (x->width == 0 || x->height == 0 || x->width > 65535 || x->height > 65535)
+            return fail("image %u: width and height must be 1 .. 65535 (got %u x %u)", i, x->width, x->height);
+        const uint32_t mcux = (x->width + 8 * hs - 1) / (8 * hs), mcuy = (x->height + 8 * vs - 1) / (8 * vs);
+        const uint64_t nb = (uint64_t)mcux * mcuy * bpm;
+        const uint64_t nt = (nb + J2P_JE_TILE - 1) / J2P_JE_TILE;
+        const uint64_t raw_bytes = nb * (wpb * 4);
+        const uint64_t nc = (raw_bytes + J2P_JE_CHUNK - 1) / J2P_JE_CHUNK;
+        if (imgs) {
+            struct j2p_je_img *g = &imgs[i];
+            memset(g, 0, sizeof *g);
+            g->src = (const uint8_t *)x->data;
+            g->s_row = x->row_stride;
+            g->s_col = x->col_stride;
+            g->s_chan = x->chan_stride;
+            g->w = x->width;
+            g->h = x->height;
+            g->mcux = mcux;
+            g->mcuy = mcuy;
+            g->blk0 = nblk;
+            g->nblk = nb;
+            g->tile0 = (uint32_t)tiles;
+            g->ntiles = (uint32_t)nt;
+            g->chunk0 = (uint32_t)chunks;
+            g->nchunks = (uint32_t)nc;
+            g->raw_off = words;
+            g->out_cap = J2P_JE_HEAD + 2 * raw_bytes + 2;
+        }
+        nblk += nb;
+        tiles += nt;
+        chunks += nc;
+        words += (nb * wpb + 3) / 4 * 4 + 4;   // raw_off stays a multiple of 4 words: chunk_bytes reads uint4
+        out += J2P_JE_HEAD + 2 * raw_bytes + 2;
+    }
+    if (tiles >= 0x7fffffffu || chunks >= 0x7fffffffu) return fail("too many blocks for one call (%llu)", (unsigned long long)nblk);
+    const size_t m = own ? n : 0;
+    L->n = n;
+    L->nblk = nblk;
+    L->ntiles = (uint32_t)tiles;
+    L->nchunks = (uint32_t)chunks;
+    L->words = words;
+    size_t o = 0;
+    L->off_imgs = o;  o = align16(o + n * sizeof(struct j2p_je_img));
+    L->off_tab = o;   o = align16(o + sizeof(struct j2p_je_tables));
+    L->off_tsum = o;  o = align16(o + tiles * sizeof(uint32_t));
+    L->off_toff = o;  o = align16(o + tiles * sizeof(uint64_t));
+    L->off_intra = o; o = align16(o + nblk * sizeof(uint32_t));
+    L->off_coef = o;  o = align16(o + nblk * 64 * sizeof(int16_t));
+    L->off_ffc = o;   o = align16(o + chunks * sizeof(uint32_t));
+    L->off_ffpre = o; o = align16(o + (chunks + 1) * sizeof(uint64_t));
+    L->off_offs = o;  o = align16(o + (n + 1) * sizeof(uint64_t));
+    L->off_huff = o;  o = align16(o + m * sizeof(struct j2p_je_huff));
+    L->off_head = o;  o = align16(o + m * J2P_JE_HEAD);
+    L->off_hlen = o;  o = align16(o + m * sizeof(uint32_t));
+    L->off_hist = o;  o = align16(o + m * 4 * J2P_JE_SYMBOLS * sizeof(uint64_t));
+    L->off_raw = o;   o = align16(o + words * sizeof(uint32_t));
+    L->off_out = o;   o = align16(o + out);
+    L->total = o;
+    return 0;
+}
+
+// the plan region (images, tables) in host memory
+static int fill_plan(const struct j2p_jpegenc_image *im, unsigned n, const struct j2p_jpegenc_params *p, uint32_t wpb, bool own, const Layout &L,
+                     uint8_t *w) {
+    Layout tmp;
+    if (make_plan(im, n, p, wpb, own, &tmp, (struct j2p_je_img *)(w + L.off_imgs)) != 0) return -1;
+    make_tables(p, (struct j2p_je_tables *)(w + L.off_tab));
+    return 0;
+}
+
+// ---- steps shared by the kernels and the host driver ----------------------------------------------
+J2P_HD uint32_t comp_of(const struct j2p_je_tables *t, uint64_t b) {
+    const uint32_t k = (uint32_t)(b % j2p_je_bpm(t)), nl = t->hs * t->vs;
+    return k < nl ? 0 : 1 + (k - nl);
+}
+
+// column x of a block whose rows are through pass 1 (rows[y * stride + x]): pass 2, quantise, and
+// store in zig-zag order; a dummy keeps only its DC
+J2P_HD void finish_column(const struct j2p_je_tables *t, const struct j2p_je_where *w, const int *rows, int stride, int x, int16_t *coef) {
+    int d[8];
+#ifdef __CUDA_ARCH__
+#pragma unroll
+#endif
+    for (int y = 0; y < 8; y++) d[y] = rows[y * stride + x];
+    j2p_je_fdct_1d<2>(d);
+    const int tbl = w->comp ? 1 : 0;
+#ifdef __CUDA_ARCH__
+#pragma unroll
+#endif
+    for (int y = 0; y < 8; y++) {
+        const int i = y * 8 + x;
+        const int v = w->dummy && i ? 0 : j2p_je_quant(t, tbl, i, d[y]);
+        coef[t->zz[i]] = (int16_t)v;
+    }
+}
+
+J2P_HD int pred_of(const struct j2p_je_tables *t, const int16_t *coef, uint64_t blk0, uint64_t b) {
+    const uint64_t pb = j2p_je_prev(t, b);
+    return pb == ~(uint64_t)0 ? 0 : coef[(blk0 + pb) * 64];
+}
+
+J2P_HD uint64_t raw_bytes(const struct j2p_je_img *im) { return (im->bits + 7) / 8; }
+
+// ---- host driver -------------------------------------------------------------------------------
+// encode_jpeg's default codes: the call's Annex K tables and header template for every image
+struct FixedCodes {
+    const struct j2p_je_tables *t;
+    const struct j2p_je_huff *huff(uint32_t) const { return &t->huff; }
+    uint32_t head_len(uint32_t) const { return J2P_JE_HEAD; }
+    uint8_t head_byte(uint32_t, const struct j2p_je_img *im, uint32_t k) const { return j2p_je_head_byte(t, im, k); }
+};
+
+// The steps of the kernels run serially on host memory.  codes(L, w, imgs, t, coef) runs between
+// the blocks and the sizes and returns where each image's Huffman tables and header come from: an
+// object with huff(i), head_len(i) and head_byte(i, im, k), such as FixedCodes.
+template <class Codes>
+static int encode_host_steps(const struct j2p_jpegenc_image *images, unsigned n, const struct j2p_jpegenc_params *params, uint32_t wpb, bool own,
+                             void *work, size_t work_bytes, uint64_t *offsets, Codes codes) {
+    Layout L;
+    if (make_plan(images, n, params, wpb, own, &L, nullptr) != 0) return -1;
+    if (!work || !offsets) return fail("null argument");
+    if (work_bytes < L.total) return fail("work area of %zu bytes is smaller than the plan's %zu", work_bytes, L.total);
+    uint8_t *w = (uint8_t *)work;
+    if (fill_plan(images, n, params, wpb, own, L, w) != 0) return -1;
+    struct j2p_je_img *imgs = (struct j2p_je_img *)(w + L.off_imgs);
+    const struct j2p_je_tables *t = (const struct j2p_je_tables *)(w + L.off_tab);
+    uint32_t *tsum = (uint32_t *)(w + L.off_tsum), *intra = (uint32_t *)(w + L.off_intra), *ffc = (uint32_t *)(w + L.off_ffc);
+    uint64_t *toff = (uint64_t *)(w + L.off_toff), *ffpre = (uint64_t *)(w + L.off_ffpre);
+    int16_t *coef = (int16_t *)(w + L.off_coef);
+    uint32_t *raw = (uint32_t *)(w + L.off_raw);
+    uint8_t *out = w + L.off_out;
+    memset(w + L.off_hist, 0, L.off_raw - L.off_hist + L.words * sizeof(uint32_t));
+    for (unsigned i = 0; i < n; i++) {
+        const struct j2p_je_img *im = &imgs[i];
+        for (uint64_t b = 0; b < im->nblk; b++) {                       // blocks
+            const struct j2p_je_where wh = j2p_je_locate(im, t, b);
+            int rows[64];
+            for (int y = 0; y < 8; y++) j2p_je_block_row(im, t, &wh, y, rows + 8 * y);
+            for (int x = 0; x < 8; x++) finish_column(t, &wh, rows, 8, x, coef + (im->blk0 + b) * 64);
+        }
+    }
+    const auto c = codes(L, w, (const struct j2p_je_img *)imgs, t, (const int16_t *)coef);
+    for (unsigned i = 0; i < n; i++) {                                  // sizes and scans
+        struct j2p_je_img *im = &imgs[i];
+        uint64_t bits = 0;
+        for (uint32_t k = 0; k < im->ntiles; k++) {
+            uint32_t s = 0;
+            for (uint64_t b = (uint64_t)k * J2P_JE_TILE; b < im->nblk && b < (uint64_t)(k + 1) * J2P_JE_TILE; b++) {
+                intra[im->blk0 + b] = s;
+                s += j2p_je_block_bits(coef + (im->blk0 + b) * 64, pred_of(t, coef, im->blk0, b), c.huff(i), comp_of(t, b));
+            }
+            tsum[im->tile0 + k] = s;
+            toff[im->tile0 + k] = bits;
+            bits += s;
+        }
+        im->bits = bits;
+        uint64_t pw;
+        const uint32_t mask = j2p_je_pad(bits, &pw);
+        raw[im->raw_off + pw] |= mask;
+    }
+    for (unsigned i = 0; i < n; i++) {                                  // emit
+        const struct j2p_je_img *im = &imgs[i];
+        for (uint64_t b = 0; b < im->nblk; b++) {
+            const uint64_t pos = toff[im->tile0 + b / J2P_JE_TILE] + intra[im->blk0 + b];
+            j2p_je_emit(coef + (im->blk0 + b) * 64, pred_of(t, coef, im->blk0, b), c.huff(i), comp_of(t, b), pos,
+                        [&](uint64_t k, uint32_t v) { raw[im->raw_off + k] |= v; });
+        }
+    }
+    uint64_t ff = 0, off = 0;                                           // 0xFF counts, file offsets
+    for (unsigned i = 0; i < n; i++) {
+        struct j2p_je_img *im = &imgs[i];
+        const uint32_t *rw = raw + im->raw_off;
+        const uint64_t nbytes = raw_bytes(im);
+        for (uint32_t k = 0; k < im->nchunks; k++) {
+            uint32_t cnt = 0;
+            for (uint64_t j = (uint64_t)k * J2P_JE_CHUNK; j < nbytes && j < (uint64_t)(k + 1) * J2P_JE_CHUNK; j++) cnt += j2p_je_byte(rw, j) == 0xff;
+            ffc[im->chunk0 + k] = cnt;
+            ffpre[im->chunk0 + k] = ff;
+            ff += cnt;
+        }
+        const uint64_t ffi = ff - ffpre[im->chunk0];
+        im->file_len = c.head_len(i) + nbytes + ffi + 2;
+        im->file_off = off;
+        offsets[i] = off;
+        off += im->file_len;
+    }
+    ffpre[L.nchunks] = ff;
+    offsets[n] = off;
+    for (unsigned i = 0; i < n; i++) {                                  // files
+        const struct j2p_je_img *im = &imgs[i];
+        uint8_t *o = out + im->file_off;
+        for (uint32_t k = 0; k < c.head_len(i); k++) *o++ = c.head_byte(i, im, k);
+        const uint32_t *rw = raw + im->raw_off;
+        for (uint64_t j = 0; j < raw_bytes(im); j++) {
+            const uint8_t v = j2p_je_byte(rw, j);
+            *o++ = v;
+            if (v == 0xff) *o++ = 0;
+        }
+        *o++ = 0xff;
+        *o++ = 0xd9;
+    }
+    return 0;
+}
+
+#endif  // J2P_JPEGENC_PLAN_H

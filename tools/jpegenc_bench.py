@@ -21,6 +21,9 @@ For each, reported are:
                 apart, the copies alone and Pillow on the first image alone in this process;
   total bytes against encode_png's files for the same tensors, and whether every file equals the
   host arm's byte for byte.
+Under "optimize_workloads", the same figures for encode_jpeg(..., optimize=True) (libj2pjpegopt.so,
+nine kernels) against Pillow with optimize=True, on (a) at q90 4:2:0 and q95 4:4:4, (b) at q75
+4:2:0 and (c), with the total bytes over the default files' bytes for the same tensors.
 Wall-clock figures are the best of R after one warm-up.  Also the card's name and power limit
 (read-only nvidia-smi query in the same run).  Writes nothing.
 """
@@ -35,7 +38,7 @@ from multiprocessing import shared_memory
 
 import numpy as np
 import torch
-from PIL import Image
+from PIL import Image, ImageFile
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
@@ -46,33 +49,38 @@ from jpeg2png_b200 import abi, decode_jpeg, encode_jpeg, encode_png, synth  # no
 from jpeg2png_b200 import jpeg_encode as J  # noqa: E402
 
 KERNELS = ('k_je_blocks', 'k_je_sizes', 'k_je_scan', 'k_je_emit', 'k_je_ffcount', 'k_je_offsets', 'k_je_stuff')
+KERNELS_OPT = ('k_jo_blocks', 'k_jo_hist', 'k_jo_tables', 'k_jo_sizes', 'k_jo_scan', 'k_jo_emit', 'k_jo_ffcount', 'k_jo_offsets',
+               'k_jo_stuff')
 
 
-def jpeg_encoder_ms(tensors, quality, subsampling, calls):
-    """encoder_ms of one j2p_jpegenc_encode call on all images, and the size of its work area."""
-    call, work_bytes = encoder_call(J.codec(J.params(quality, subsampling)), tensors)
-    out = encoder_ms(call, KERNELS, calls)
+def jpeg_encoder_ms(tensors, quality, subsampling, calls, optimize=False):
+    """encoder_ms of one j2p_jpegenc_encode (or j2p_jpegopt_encode) call on all images, and the size
+    of its work area."""
+    call, work_bytes = encoder_call(J.codec(J.params(quality, subsampling), optimize), tensors)
+    out = encoder_ms(call, KERNELS_OPT if optimize else KERNELS, calls)
     return {'ms_per_call': out['ms_per_call'], 'work_bytes': work_bytes, 'kernel_ms_per_call': out['kernel_ms_per_call']}
 
 
-def pillow(hwc, quality, subsampling):
+def pillow(hwc, quality, subsampling, optimize=False):
     buf = io.BytesIO()
-    Image.fromarray(hwc, 'RGB').save(buf, 'JPEG', quality=quality, subsampling=subsampling)
+    if optimize:        # libjpeg cannot suspend in an optimized file's second pass: room for the whole file
+        ImageFile.MAXBLOCK = max(ImageFile.MAXBLOCK, 4 * hwc.shape[0] * hwc.shape[1] * 3 + 65536)
+    Image.fromarray(hwc, 'RGB').save(buf, 'JPEG', quality=quality, subsampling=subsampling, optimize=optimize)
     return buf.getvalue()
 
 
 _shm = {}
 
 
-def _pillow_shared(name, size, offset, h, w, quality, subsampling):
+def _pillow_shared(name, size, offset, h, w, quality, subsampling, optimize=False):
     """In a worker process: Pillow on image (h, w, 3) at `offset` of the shared buffer `name`."""
     if name not in _shm:
         _shm[name] = shared_memory.SharedMemory(name=name)
     hwc = np.ndarray((h, w, 3), np.uint8, buffer=_shm[name].buf[:size], offset=offset)
-    return pillow(hwc, quality, subsampling)
+    return pillow(hwc, quality, subsampling, optimize)
 
 
-def host_arm(tensors, quality, subsampling, reps, procs):
+def host_arm(tensors, quality, subsampling, reps, procs, optimize=False):
     """Best-of-`reps` seconds and files of the host arm (copies, then Pillow in `procs` worker
     processes), and apart the copies alone and Pillow on the first image in this process."""
     shapes = [(t.shape[1], t.shape[2]) for t in tensors]
@@ -93,10 +101,10 @@ def host_arm(tensors, quality, subsampling, reps, procs):
                 copies()
                 return list(pool.map(_pillow_shared, [shm.name] * len(shapes), [offs[-1]] * len(shapes), offs[:-1],
                                      [h for h, _ in shapes], [w for _, w in shapes], [quality] * len(shapes),
-                                     [subsampling] * len(shapes)))
+                                     [subsampling] * len(shapes), [optimize] * len(shapes)))
             t_host, host_files = best_of(arm, reps)
         t_copy, _ = best_of(copies, reps)
-        t_one, _ = best_of(lambda: pillow(views[0].numpy(), quality, subsampling), reps)
+        t_one, _ = best_of(lambda: pillow(views[0].numpy(), quality, subsampling, optimize), reps)
         del buf, views
     finally:
         shm.close()
@@ -116,6 +124,24 @@ def run(tensors, label, quality, subsampling, reps, calls, threads, png_bytes):
                           'copies_alone_ms': t_copy * 1e3, 'one_image_one_thread_ms': t_one * 1e3}
     out['speedup_vs_host'] = t_host / t_gpu
     out['bytes_vs_encode_png'] = total / png_bytes
+    out['identical_to_host'] = files == host_files
+    return out
+
+
+def run_optimized(tensors, label, quality, subsampling, reps, calls, threads):
+    """run's figures for optimize=True, with the bytes over the default files' bytes."""
+    out = {'workload': label, 'images': len(tensors), 'quality': quality, 'subsampling': subsampling, 'optimize': True}
+    out['encoder'] = jpeg_encoder_ms(tensors, quality, subsampling, calls, optimize=True)
+    out['encoder_default_ms_per_call'] = jpeg_encoder_ms(tensors, quality, subsampling, calls)['ms_per_call']
+    t_gpu, files = best_of(lambda: encode_jpeg(tensors, quality=quality, subsampling=subsampling, optimize=True), reps)
+    default_bytes = sum(map(len, encode_jpeg(tensors, quality=quality, subsampling=subsampling)))
+    t_host, host_files, t_copy, t_one = host_arm(tensors, quality, subsampling, reps, threads, optimize=True)
+    total = sum(map(len, files))
+    out['encode_jpeg'] = {'wall_ms': t_gpu * 1e3, 'ms_per_image': t_gpu / len(tensors) * 1e3, 'total_bytes': total}
+    out['host_pillow'] = {'wall_ms': t_host * 1e3, 'ms_per_image': t_host / len(tensors) * 1e3, 'processes': threads,
+                          'copies_alone_ms': t_copy * 1e3, 'one_image_one_thread_ms': t_one * 1e3}
+    out['speedup_vs_host'] = t_host / t_gpu
+    out['bytes_vs_default'] = total / default_bytes
     out['identical_to_host'] = files == host_files
     return out
 
@@ -144,6 +170,12 @@ def main():
         png_bytes = sum(map(len, encode_png(tensors)))
         for q, s in cases:
             line['workloads'].append(run(tensors, label, q, s, args.reps, args.calls, threads, png_bytes))
+    line['optimize_workloads'] = []
+    for tensors, label, cases in ((big, f'{n} x 1920x1080 Q75 4:2:0, -i 100', ((90, '4:2:0'), (95, '4:4:4'))),
+                                  (small, f'{n} x 256x256 Q10 4:2:0, -i 50', ((75, '4:2:0'),)),
+                                  ([img8k], '1 x 7680x4320 cartoon', ((90, '4:2:0'),))):
+        for q, s in cases:
+            line['optimize_workloads'].append(run_optimized(tensors, label, q, s, args.reps, args.calls, threads))
     print(json.dumps(line), flush=True)
 
 
