@@ -1,7 +1,8 @@
 """jpeg2png_b200: the jpeg2png solver on H100.  `decode_jpeg` (jpeg2png_b200.decode) turns JPEG files
 into CUDA tensors, `encode_png` (jpeg2png_b200.encode) and `encode_jpeg` (jpeg2png_b200.jpeg_encode)
 turn such tensors into PNG or JPEG files on the device (`encode_jpeg(..., optimize=True)` with
-per-image optimized Huffman tables, as Pillow's `optimize=True`); torch is imported only when one of
+per-image optimized Huffman tables, as Pillow's `optimize=True`, and `encode_jpeg(...,
+progressive=True)` with Pillow's progressive files); torch is imported only when one of
 them is first used."""
 
 __all__ = ['decode_jpeg', 'encode_png', 'encode_jpeg']

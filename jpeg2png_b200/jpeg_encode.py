@@ -5,7 +5,9 @@ Pillow writes for the same pixels with `quality` and `subsampling` and no other 
 compressor defaults: JFIF header, IJG quality tables, slow-integer DCT, the Annex K Huffman tables,
 one interleaved scan).  With `optimize=True` the encoder is libj2pjpegopt.so (jpeg2png_b200/jpegopt),
 which writes Pillow's `optimize=True` file: the same coefficients, coded with Huffman tables built
-per image from its own symbol counts.  Colour conversion, downsampling, DCT, quantisation, the
+per image from its own symbol counts.  With `progressive=True` the encoder is libj2pjpegprog.so
+(jpeg2png_b200/jpegprog), which writes Pillow's `progressive=True` file: the same coefficients in
+libjpeg's ten-scan progression, each scan with tables built from its own symbol counts.  Colour conversion, downsampling, DCT, quantisation, the
 tables, Huffman coding and byte stuffing all run on the device; only the finished files cross PCIe.
 `encode_host` runs the same steps serially on numpy arrays and gives the same bytes.
 
@@ -26,6 +28,7 @@ from . import batch_encode as B
 
 JPEGENC_LIB = os.path.join(abi._PKG_DIR, 'jpegenc', 'libj2pjpegenc.so')
 JPEGOPT_LIB = os.path.join(abi._PKG_DIR, 'jpegopt', 'libj2pjpegopt.so')
+JPEGPROG_LIB = os.path.join(abi._PKG_DIR, 'jpegprog', 'libj2pjpegprog.so')
 SAMPLINGS = {'4:4:4': 0, '4:2:2': 1, '4:2:0': 2}
 MAX_SIDE = 65535                    # SOF's 16-bit height and width
 
@@ -67,6 +70,10 @@ def _declare_opt(lib):
     lib.j2p_jpegopt_build_table.argtypes = [C.POINTER(C.c_uint64), u8, u8, C.POINTER(C.c_uint)]
 
 
+def _declare_prog(lib):
+    _declare(lib, 'jpegprog')
+
+
 def load_jpegenc() -> C.CDLL:
     """libj2pjpegenc.so (the device JPEG encoder) from the package tree."""
     return abi.load_library(JPEGENC_LIB, 'JPEG encoder', _declare)
@@ -75,6 +82,11 @@ def load_jpegenc() -> C.CDLL:
 def load_jpegopt() -> C.CDLL:
     """libj2pjpegopt.so (the device JPEG encoder with optimized Huffman tables) from the package tree."""
     return abi.load_library(JPEGOPT_LIB, 'optimizing JPEG encoder', _declare_opt)
+
+
+def load_jpegprog() -> C.CDLL:
+    """libj2pjpegprog.so (the device encoder of progressive JPEG files) from the package tree."""
+    return abi.load_library(JPEGPROG_LIB, 'progressive JPEG encoder', _declare_prog)
 
 
 def params(quality, subsampling) -> Params:
@@ -93,17 +105,24 @@ def _check_size(shape, h, w):
 
 CODEC = B.Codec('jpegenc', lambda: load_jpegenc(), Image, _check_size)
 CODEC_OPT = B.Codec('jpegopt', lambda: load_jpegopt(), Image, _check_size)
+CODEC_PROG = B.Codec('jpegprog', lambda: load_jpegprog(), Image, _check_size)
 
 
-def codec(p: Params, optimize=False) -> B.Codec:
-    """libj2pjpegenc.so, or libj2pjpegopt.so when optimize, for the shared driver, with the call
-    parameters p."""
-    return dataclasses.replace(CODEC_OPT if optimize else CODEC, params=(C.byref(p),))
+def codec(p: Params, optimize=False, progressive=False) -> B.Codec:
+    """libj2pjpegenc.so, or libj2pjpegopt.so when optimize, or libj2pjpegprog.so when progressive
+    (whatever optimize), for the shared driver, with the call parameters p."""
+    c = CODEC_PROG if progressive else CODEC_OPT if optimize else CODEC
+    return dataclasses.replace(c, params=(C.byref(p),))
 
 
 def check_optimize(optimize):
     if not isinstance(optimize, bool):
         raise ValueError(f'optimize must be True or False, not {optimize!r}')
+
+
+def check_progressive(progressive):
+    if not isinstance(progressive, bool):
+        raise ValueError(f'progressive must be True or False, not {progressive!r}')
 
 
 def build_table(counts):
@@ -127,39 +146,48 @@ def _work_bytes(descs, p):
     return codec(p).plan(descs)[0]
 
 
-def encode_host(images, quality=75, subsampling='4:2:0', layout='HWC', optimize=False):
-    """The serial host driver (j2p_jpegenc_encode_host, or j2p_jpegopt_encode_host when optimize)
-    on numpy uint8 arrays: a list of JPEG files as bytes, the same bytes the device writes."""
+def encode_host(images, quality=75, subsampling='4:2:0', layout='HWC', optimize=False, progressive=False):
+    """The serial host driver (j2p_jpegenc_encode_host, or j2p_jpegopt_encode_host when optimize,
+    or j2p_jpegprog_encode_host when progressive) on numpy uint8 arrays: a list of JPEG files as
+    bytes, the same bytes the device writes."""
     B.check_layout(layout)
     p = params(quality, subsampling)
     check_optimize(optimize)
+    check_progressive(progressive)
     for x in images:
         if x.dtype != np.uint8:
             raise ValueError(f'samples are uint8, not {x.dtype}')
-    return B.encode_host(codec(p, optimize), images, layout)
+    return B.encode_host(codec(p, optimize, progressive), images, layout)
 
 
-def encode_jpeg(images, *, quality=75, subsampling='4:2:0', layout='CHW', optimize=False):
-    """Encode RGB CUDA tensors as baseline JPEG files on the device.
+def encode_jpeg(images, *, quality=75, subsampling='4:2:0', layout='CHW', optimize=False, progressive=False):
+    """Encode RGB CUDA tensors as baseline or progressive JPEG files on the device.
 
     images: one tensor or a list or tuple of them, torch.uint8, shaped (3, h, w) for layout='CHW'
     or (h, w, 3) for 'HWC', with any strides, 1..65535 pixels high and wide.  quality: an integer
     in 1..100; subsampling: '4:4:4', '4:2:2' or '4:2:0'.  Returns the JPEG file as bytes, or a list
     of bytes in input order: byte for byte the file Pillow writes for the same pixels with
-    `save(f, 'JPEG', quality=quality, subsampling=subsampling, optimize=optimize)`.
+    `save(f, 'JPEG', quality=quality, subsampling=subsampling, optimize=optimize,
+    progressive=progressive)`.
 
     optimize: False writes the Annex K Huffman tables; True builds each image's tables from its own
     symbol counts, on the device, as libjpeg does for `optimize=True`: the same coefficients, files
     typically 6-9% smaller, at the cost of two more kernels per call.
 
+    progressive: True writes libjpeg's progressive file (SOF2, its ten-scan script for YCbCr, each
+    scan with Huffman tables built from its own symbol counts, as libjpeg always does for a
+    progressive file): the same coefficients, shown coarse to fine as the file arrives.  optimize
+    changes no byte of a progressive file, as with Pillow.
+
     The work is queued on torch's current stream, after what is already there, so a tensor just
     written on that stream needs no synchronisation.  Images of any mix of sizes go into one call;
     a list is split into several only when the work area would not fit in a quarter of the free
     device memory.  Raises ValueError for a wrong dtype, shape, layout, quality, subsampling,
-    optimize (not a bool) or size, and for a tensor that is not on a CUDA device, and RuntimeError
+    optimize or progressive (not a bool) or size, and for a tensor that is not on a CUDA device, and RuntimeError
     when no CUDA device is usable.
     """
     B.check_layout(layout)
     p = params(quality, subsampling)
     check_optimize(optimize)
-    return B.encode_tensors('encode_jpeg', codec(p, optimize), images, layout, (torch.uint8,))
+    check_progressive(progressive)
+    return B.encode_tensors('encode_jpeg', codec(p, optimize, progressive), images, layout, (torch.uint8,))

@@ -1,5 +1,6 @@
 // jpegenc_kernels.cuh — the bodies of the encoder's kernels as __device__ functions, shared by
-// libj2pjpegenc.so (whose __global__ kernels are thin wrappers around them) and libj2pjpegopt.so.
+// libj2pjpegenc.so (whose __global__ kernels are thin wrappers around them), libj2pjpegopt.so and
+// libj2pjpegprog.so (which runs the blocks, scan and ffcount bodies on its per-scan streams).
 // Where an image's Huffman tables and header come from is a parameter:
 //   huff(i)                the derived tables of image i (called by every thread of the CTA, before
 //                          any of them returns, so that it may stage them in shared memory); the

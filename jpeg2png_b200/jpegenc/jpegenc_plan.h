@@ -1,9 +1,10 @@
-// jpegenc_plan.h — the host side shared by libj2pjpegenc.so and libj2pjpegopt.so: the quantisation
+// jpegenc_plan.h — the host side shared by libj2pjpegenc.so, libj2pjpegopt.so and libj2pjpegprog.so: the quantisation
 // tables and their reciprocals, the Annex K Huffman tables and the header template, the plan of a
 // call (the layout of its work area), the steps that both the kernels and the host driver call per
-// block, and the serial host driver.  The two libraries differ only in where an image's Huffman
-// tables and header come from: the call's Annex K ones, or the image's own optimized ones
-// (jpegopt_core.h), and in the work-area bound of a block that follows.
+// block, and the serial host driver.  The first two libraries differ only in where an image's
+// Huffman tables and header come from: the call's Annex K ones, or the image's own optimized ones
+// (jpegopt_core.h), and in the work-area bound of a block that follows.  The progressive encoder
+// (../jpegprog) takes the plan's checks, the tables and the blocks step, and lays out its own scans.
 #ifndef J2P_JPEGENC_PLAN_H
 #define J2P_JPEGENC_PLAN_H
 
@@ -281,6 +282,16 @@ J2P_HD int pred_of(const struct j2p_je_tables *t, const int16_t *coef, uint64_t 
 J2P_HD uint64_t raw_bytes(const struct j2p_je_img *im) { return (im->bits + 7) / 8; }
 
 // ---- host driver -------------------------------------------------------------------------------
+// the blocks step of the kernels on one image, serially: its coefficients at coef + im->blk0 * 64
+static void host_blocks(const struct j2p_je_img *im, const struct j2p_je_tables *t, int16_t *coef) {
+    for (uint64_t b = 0; b < im->nblk; b++) {
+        const struct j2p_je_where wh = j2p_je_locate(im, t, b);
+        int rows[64];
+        for (int y = 0; y < 8; y++) j2p_je_block_row(im, t, &wh, y, rows + 8 * y);
+        for (int x = 0; x < 8; x++) finish_column(t, &wh, rows, 8, x, coef + (im->blk0 + b) * 64);
+    }
+}
+
 // encode_jpeg's default codes: the call's Annex K tables and header template for every image
 struct FixedCodes {
     const struct j2p_je_tables *t;
@@ -309,15 +320,7 @@ static int encode_host_steps(const struct j2p_jpegenc_image *images, unsigned n,
     uint32_t *raw = (uint32_t *)(w + L.off_raw);
     uint8_t *out = w + L.off_out;
     memset(w + L.off_hist, 0, L.off_raw - L.off_hist + L.words * sizeof(uint32_t));
-    for (unsigned i = 0; i < n; i++) {
-        const struct j2p_je_img *im = &imgs[i];
-        for (uint64_t b = 0; b < im->nblk; b++) {                       // blocks
-            const struct j2p_je_where wh = j2p_je_locate(im, t, b);
-            int rows[64];
-            for (int y = 0; y < 8; y++) j2p_je_block_row(im, t, &wh, y, rows + 8 * y);
-            for (int x = 0; x < 8; x++) finish_column(t, &wh, rows, 8, x, coef + (im->blk0 + b) * 64);
-        }
-    }
+    for (unsigned i = 0; i < n; i++) host_blocks(&imgs[i], t, coef);   // blocks
     const auto c = codes(L, w, (const struct j2p_je_img *)imgs, t, (const int16_t *)coef);
     for (unsigned i = 0; i < n; i++) {                                  // sizes and scans
         struct j2p_je_img *im = &imgs[i];

@@ -69,25 +69,6 @@ extern "C" int j2p_jpegopt_encode_host(const struct j2p_jpegenc_image *images, u
 // ---- device ------------------------------------------------------------------------------------
 static const int kTableThreads = 128;       // one warp per table of an image
 
-// a warp as the lanes of a table build
-struct WarpLanes {
-    uint32_t lane, n;
-    __device__ void sync() const { __syncwarp(); }
-    __device__ int least(uint64_t f, int c) const {
-#pragma unroll
-        for (int o = 16; o; o >>= 1) {
-            const uint64_t f2 = __shfl_xor_sync(0xffffffffu, f, o);
-            const int c2 = __shfl_xor_sync(0xffffffffu, c, o);
-            if (c2 >= 0 && (c < 0 || f2 < f || (f2 == f && c2 > c))) {
-                f = f2;
-                c = c2;
-            }
-        }
-        return c;
-    }
-    __device__ uint32_t ballot(bool p) const { return __ballot_sync(0xffffffffu, p); }
-};
-
 // image i's derived tables into shared memory, by every thread of the CTA
 __device__ __forceinline__ const struct j2p_je_huff *stage(struct j2p_je_huff *sh, const struct j2p_je_huff *huffs, uint32_t i) {
     const uint4 *src = (const uint4 *)(huffs + i);

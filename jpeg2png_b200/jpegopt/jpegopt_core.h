@@ -55,6 +55,27 @@ struct j2p_jo_serial {
         J2P_HD uint32_t ballot(bool p) const { return p ? 1u : 0u; }
 };
 
+#ifdef __CUDACC__
+// a warp as the lanes of a table build
+struct WarpLanes {
+    uint32_t lane, n;
+    __device__ void sync() const { __syncwarp(); }
+    __device__ int least(uint64_t f, int c) const {
+#pragma unroll
+        for (int o = 16; o; o >>= 1) {
+            const uint64_t f2 = __shfl_xor_sync(0xffffffffu, f, o);
+            const int c2 = __shfl_xor_sync(0xffffffffu, c, o);
+            if (c2 >= 0 && (c < 0 || f2 < f || (f2 == f && c2 > c))) {
+                f = f2;
+                c = c2;
+            }
+        }
+        return c;
+    }
+    __device__ uint32_t ballot(bool p) const { return __ballot_sync(0xffffffffu, p); }
+};
+#endif
+
 J2P_HD uint32_t j2p_jo_popc(uint32_t m) {
 #ifdef __CUDA_ARCH__
         return __popc(m);

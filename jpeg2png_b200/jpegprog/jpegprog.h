@@ -1,0 +1,53 @@
+/* jpegprog.h — libj2pjpegprog.so: RGB images in device memory to progressive JPEG files, encoded on
+ * the device.
+ *
+ * The file is the one libjpeg's compressor writes with jpeg_simple_progression, as Pillow's JPEG
+ * writer drives it with `progressive=True` (and quality q, subsampling s; `optimize` changes no
+ * byte): SOI, JFIF APP0, the two DQTs and SOF2 of libj2pjpegenc.so's file (jpegenc.h), then ten
+ * scans, each after the DHTs of the tables it uses, then EOI.  The coefficients are the baseline
+ * file's; each scan's tables are built from that scan's own symbol counts (jpegopt_core.h).  The
+ * scan script and the coding rules are in jpegprog_core.h.
+ *
+ * The images, parameters and statistics are jpegenc.h's structs, and the calls mirror its calls.
+ * Every (image, scan) pair is its own bit stream.  One call queues a memset and
+ * J2P_JPEGPROG_LAUNCHES kernels, whatever the number and sizes of the images: blocks (and each AC
+ * scan's block summaries), runs (the EOB-run state each block of an AC scan receives), hist (symbol
+ * counts per image and table), tables (ten per image, and each stream's DHT and SOS header), sizes,
+ * scan, emit, ffcount, offsets, stuff.  j2p_jpegprog_encode_host runs the same steps serially on
+ * host memory and writes the same bytes.
+ *
+ * Work-area bound: a block of the AC first scan over 63 coefficients costs at most 63 x (16 + 10)
+ * bits and one EOB-run emission of 16 + 14, J2P_JPEGPROG_BLOCK_BITS = 1668; every other scan's bound
+ * is smaller (jpegprog_core.h), and each stream gets its own.
+ */
+#ifndef J2P_JPEGPROG_H
+#define J2P_JPEGPROG_H
+
+#include "../jpegenc/jpegenc.h"
+
+#ifdef __cplusplus
+extern "C" {
+#endif
+
+#define J2P_JPEGPROG_BLOCK_BITS 1668u
+#define J2P_JPEGPROG_LAUNCHES 10u
+
+/* As j2p_jpegenc_plan, for the progressive files. */
+int j2p_jpegprog_plan(const struct j2p_jpegenc_image *images, unsigned n, const struct j2p_jpegenc_params *params, size_t *work_bytes,
+                      size_t *out_offset);
+
+/* As j2p_jpegenc_encode, for the progressive files (stats->launches is J2P_JPEGPROG_LAUNCHES). */
+int j2p_jpegprog_encode(const struct j2p_jpegenc_image *images, unsigned n, const struct j2p_jpegenc_params *params, void *work,
+                        size_t work_bytes, void *stream, uint64_t *offsets, void *dst, size_t dst_cap, struct j2p_jpegenc_stats *stats);
+
+/* The same steps run serially on host memory (images and work in host memory). */
+int j2p_jpegprog_encode_host(const struct j2p_jpegenc_image *images, unsigned n, const struct j2p_jpegenc_params *params, void *work,
+                             size_t work_bytes, uint64_t *offsets);
+
+const char *j2p_jpegprog_last_error(void);
+
+#ifdef __cplusplus
+}
+#endif
+
+#endif

@@ -24,6 +24,10 @@ For each, reported are:
 Under "optimize_workloads", the same figures for encode_jpeg(..., optimize=True) (libj2pjpegopt.so,
 nine kernels) against Pillow with optimize=True, on (a) at q90 4:2:0 and q95 4:4:4, (b) at q75
 4:2:0 and (c), with the total bytes over the default files' bytes for the same tensors.
+Under "progressive_workloads", the same figures for encode_jpeg(..., progressive=True)
+(libj2pjpegprog.so, ten kernels) against Pillow with progressive=True, on (a) at q90 4:2:0 and q95
+4:4:4, (b) at q75 4:2:0, (c), and one flat 7680x4320 image at q90 4:2:0 (every AC scan one EOB-run
+segment, walked by one thread of k_jp_runs).  --progressive-only measures only these.
 Wall-clock figures are the best of R after one warm-up.  Also the card's name and power limit
 (read-only nvidia-smi query in the same run).  Writes nothing.
 """
@@ -51,36 +55,38 @@ from jpeg2png_b200 import jpeg_encode as J  # noqa: E402
 KERNELS = ('k_je_blocks', 'k_je_sizes', 'k_je_scan', 'k_je_emit', 'k_je_ffcount', 'k_je_offsets', 'k_je_stuff')
 KERNELS_OPT = ('k_jo_blocks', 'k_jo_hist', 'k_jo_tables', 'k_jo_sizes', 'k_jo_scan', 'k_jo_emit', 'k_jo_ffcount', 'k_jo_offsets',
                'k_jo_stuff')
+KERNELS_PROG = ('k_jp_blocks', 'k_jp_runs', 'k_jp_hist', 'k_jp_tables', 'k_jp_sizes', 'k_jp_scan', 'k_jp_emit', 'k_jp_ffcount',
+                'k_jp_offsets', 'k_jp_stuff')
 
 
-def jpeg_encoder_ms(tensors, quality, subsampling, calls, optimize=False):
-    """encoder_ms of one j2p_jpegenc_encode (or j2p_jpegopt_encode) call on all images, and the size
-    of its work area."""
-    call, work_bytes = encoder_call(J.codec(J.params(quality, subsampling), optimize), tensors)
-    out = encoder_ms(call, KERNELS_OPT if optimize else KERNELS, calls)
+def jpeg_encoder_ms(tensors, quality, subsampling, calls, optimize=False, progressive=False):
+    """encoder_ms of one j2p_jpegenc_encode (or j2p_jpegopt_encode, j2p_jpegprog_encode) call on all
+    images, and the size of its work area."""
+    call, work_bytes = encoder_call(J.codec(J.params(quality, subsampling), optimize, progressive), tensors)
+    out = encoder_ms(call, KERNELS_PROG if progressive else KERNELS_OPT if optimize else KERNELS, calls)
     return {'ms_per_call': out['ms_per_call'], 'work_bytes': work_bytes, 'kernel_ms_per_call': out['kernel_ms_per_call']}
 
 
-def pillow(hwc, quality, subsampling, optimize=False):
+def pillow(hwc, quality, subsampling, optimize=False, progressive=False):
     buf = io.BytesIO()
-    if optimize:        # libjpeg cannot suspend in an optimized file's second pass: room for the whole file
+    if optimize or progressive:     # libjpeg cannot suspend in a multi-pass file's last pass: room for the whole file
         ImageFile.MAXBLOCK = max(ImageFile.MAXBLOCK, 4 * hwc.shape[0] * hwc.shape[1] * 3 + 65536)
-    Image.fromarray(hwc, 'RGB').save(buf, 'JPEG', quality=quality, subsampling=subsampling, optimize=optimize)
+    Image.fromarray(hwc, 'RGB').save(buf, 'JPEG', quality=quality, subsampling=subsampling, optimize=optimize, progressive=progressive)
     return buf.getvalue()
 
 
 _shm = {}
 
 
-def _pillow_shared(name, size, offset, h, w, quality, subsampling, optimize=False):
+def _pillow_shared(name, size, offset, h, w, quality, subsampling, optimize=False, progressive=False):
     """In a worker process: Pillow on image (h, w, 3) at `offset` of the shared buffer `name`."""
     if name not in _shm:
         _shm[name] = shared_memory.SharedMemory(name=name)
     hwc = np.ndarray((h, w, 3), np.uint8, buffer=_shm[name].buf[:size], offset=offset)
-    return pillow(hwc, quality, subsampling, optimize)
+    return pillow(hwc, quality, subsampling, optimize, progressive)
 
 
-def host_arm(tensors, quality, subsampling, reps, procs, optimize=False):
+def host_arm(tensors, quality, subsampling, reps, procs, optimize=False, progressive=False):
     """Best-of-`reps` seconds and files of the host arm (copies, then Pillow in `procs` worker
     processes), and apart the copies alone and Pillow on the first image in this process."""
     shapes = [(t.shape[1], t.shape[2]) for t in tensors]
@@ -101,10 +107,10 @@ def host_arm(tensors, quality, subsampling, reps, procs, optimize=False):
                 copies()
                 return list(pool.map(_pillow_shared, [shm.name] * len(shapes), [offs[-1]] * len(shapes), offs[:-1],
                                      [h for h, _ in shapes], [w for _, w in shapes], [quality] * len(shapes),
-                                     [subsampling] * len(shapes), [optimize] * len(shapes)))
+                                     [subsampling] * len(shapes), [optimize] * len(shapes), [progressive] * len(shapes)))
             t_host, host_files = best_of(arm, reps)
         t_copy, _ = best_of(copies, reps)
-        t_one, _ = best_of(lambda: pillow(views[0].numpy(), quality, subsampling, optimize), reps)
+        t_one, _ = best_of(lambda: pillow(views[0].numpy(), quality, subsampling, optimize, progressive), reps)
         del buf, views
     finally:
         shm.close()
@@ -146,12 +152,31 @@ def run_optimized(tensors, label, quality, subsampling, reps, calls, threads):
     return out
 
 
+def run_progressive(tensors, label, quality, subsampling, reps, calls, threads):
+    """run's figures for progressive=True, with the bytes over the default files' bytes."""
+    out = {'workload': label, 'images': len(tensors), 'quality': quality, 'subsampling': subsampling, 'progressive': True}
+    out['encoder'] = jpeg_encoder_ms(tensors, quality, subsampling, calls, progressive=True)
+    out['encoder_default_ms_per_call'] = jpeg_encoder_ms(tensors, quality, subsampling, calls)['ms_per_call']
+    t_gpu, files = best_of(lambda: encode_jpeg(tensors, quality=quality, subsampling=subsampling, progressive=True), reps)
+    default_bytes = sum(map(len, encode_jpeg(tensors, quality=quality, subsampling=subsampling)))
+    t_host, host_files, t_copy, t_one = host_arm(tensors, quality, subsampling, reps, threads, progressive=True)
+    total = sum(map(len, files))
+    out['encode_jpeg'] = {'wall_ms': t_gpu * 1e3, 'ms_per_image': t_gpu / len(tensors) * 1e3, 'total_bytes': total}
+    out['host_pillow'] = {'wall_ms': t_host * 1e3, 'ms_per_image': t_host / len(tensors) * 1e3, 'processes': threads,
+                          'copies_alone_ms': t_copy * 1e3, 'one_image_one_thread_ms': t_one * 1e3}
+    out['speedup_vs_host'] = t_host / t_gpu
+    out['bytes_vs_default'] = total / default_bytes
+    out['identical_to_host'] = files == host_files
+    return out
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--device', type=int, default=0)
     ap.add_argument('--files', type=int, default=64)
     ap.add_argument('--reps', type=int, default=3)
     ap.add_argument('--calls', type=int, default=20)
+    ap.add_argument('--progressive-only', action='store_true')
     args = ap.parse_args()
     if abi.load_product().j2p_device_count() <= 0 or not torch.cuda.is_available():
         raise SystemExit('jpegenc_bench.py: no CUDA device')
@@ -163,7 +188,18 @@ def main():
     big = decode_jpeg(jpeg_files(1920, 1080, 75, n), iterations=100, dtype=torch.uint8)
     small = decode_jpeg(jpeg_files(256, 256, 10, n), iterations=50, dtype=torch.uint8)
     img8k = torch.from_numpy(synth.cartoon_image(7680, 4320, 9).round().astype(np.uint8).transpose(2, 0, 1).copy()).cuda()
+    flat8k = torch.full((3, 4320, 7680), 77, dtype=torch.uint8, device='cuda')
     torch.cuda.synchronize()
+    line['progressive_workloads'] = []
+    for tensors, label, cases in ((big, f'{n} x 1920x1080 Q75 4:2:0, -i 100', ((90, '4:2:0'), (95, '4:4:4'))),
+                                  (small, f'{n} x 256x256 Q10 4:2:0, -i 50', ((75, '4:2:0'),)),
+                                  ([img8k], '1 x 7680x4320 cartoon', ((90, '4:2:0'),)),
+                                  ([flat8k], '1 x 7680x4320 flat', ((90, '4:2:0'),))):
+        for q, s in cases:
+            line['progressive_workloads'].append(run_progressive(tensors, label, q, s, args.reps, args.calls, threads))
+    if args.progressive_only:
+        print(json.dumps(line), flush=True)
+        return
     for tensors, label, cases in ((big, f'{n} x 1920x1080 Q75 4:2:0, -i 100', ((95, '4:4:4'), (90, '4:2:0'), (75, '4:2:0'))),
                                   (small, f'{n} x 256x256 Q10 4:2:0, -i 50', ((75, '4:2:0'),)),
                                   ([img8k], '1 x 7680x4320 cartoon', ((90, '4:2:0'),))):
