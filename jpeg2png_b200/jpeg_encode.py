@@ -7,8 +7,11 @@ one interleaved scan).  With `optimize=True` the encoder is libj2pjpegopt.so (jp
 which writes Pillow's `optimize=True` file: the same coefficients, coded with Huffman tables built
 per image from its own symbol counts.  With `progressive=True` the encoder is libj2pjpegprog.so
 (jpeg2png_b200/jpegprog), which writes Pillow's `progressive=True` file: the same coefficients in
-libjpeg's ten-scan progression, each scan with tables built from its own symbol counts.  Colour conversion, downsampling, DCT, quantisation, the
-tables, Huffman coding and byte stuffing all run on the device; only the finished files cross PCIe.
+libjpeg's ten-scan progression, each scan with tables built from its own symbol counts.
+`restart_marker_blocks` and `restart_marker_rows` add restart intervals to any of the three files,
+as Pillow's keywords of the same names do (DESIGN §7i).  Colour conversion, downsampling, DCT,
+quantisation, the tables, Huffman coding and byte stuffing all run on the device; only the finished
+files cross PCIe.
 `encode_host` runs the same steps serially on numpy arrays and gives the same bytes.
 
 The module is not called encode_jpeg.py: importing it would make the package attribute
@@ -41,7 +44,7 @@ class Image(C.Structure):
 
 class Params(C.Structure):
     """struct j2p_jpegenc_params — jpeg2png_b200/jpegenc/jpegenc.h."""
-    _fields_ = [('quality', C.c_int), ('sampling', C.c_int)]
+    _fields_ = [('quality', C.c_int), ('sampling', C.c_int), ('restart_marker_blocks', C.c_int), ('restart_marker_rows', C.c_int)]
 
 
 class Stats(C.Structure):
@@ -89,13 +92,28 @@ def load_jpegprog() -> C.CDLL:
     return abi.load_library(JPEGPROG_LIB, 'progressive JPEG encoder', _declare_prog)
 
 
-def params(quality, subsampling) -> Params:
-    """Checked call parameters: quality an integer in 1..100, subsampling '4:4:4', '4:2:2' or '4:2:0'."""
+MAX_RESTART = 65535                 # DRI's 16-bit interval
+
+
+def _check_restart(name, v):
+    """A restart keyword: an integer (not a bool) in 0..65535.  Pillow turns -1 into DRI 65535 and
+    writes a value above 65535 as its DRI mod 65536 while counting the full value between markers,
+    a corrupt file; both are refused here."""
+    if isinstance(v, bool) or not isinstance(v, (int, np.integer)) or not 0 <= v <= MAX_RESTART:
+        raise ValueError(f'{name} must be an integer in 0..{MAX_RESTART}, not {v!r}')
+    return int(v)
+
+
+def params(quality, subsampling, restart_marker_blocks=0, restart_marker_rows=0) -> Params:
+    """Checked call parameters: quality an integer in 1..100, subsampling '4:4:4', '4:2:2' or '4:2:0',
+    the restart keywords integers in 0..65535."""
     if isinstance(quality, bool) or not isinstance(quality, (int, np.integer)) or not 1 <= quality <= 100:
         raise ValueError(f'quality must be an integer in 1..100, not {quality!r}')
     if subsampling not in SAMPLINGS:
         raise ValueError(f"subsampling must be '4:4:4', '4:2:2' or '4:2:0', not {subsampling!r}")
-    return Params(int(quality), SAMPLINGS[subsampling])
+    blocks = _check_restart('restart_marker_blocks', restart_marker_blocks)
+    rows = _check_restart('restart_marker_rows', restart_marker_rows)
+    return Params(int(quality), SAMPLINGS[subsampling], blocks, rows)
 
 
 def _check_size(shape, h, w):
@@ -146,12 +164,13 @@ def _work_bytes(descs, p):
     return codec(p).plan(descs)[0]
 
 
-def encode_host(images, quality=75, subsampling='4:2:0', layout='HWC', optimize=False, progressive=False):
+def encode_host(images, quality=75, subsampling='4:2:0', layout='HWC', optimize=False, progressive=False, restart_marker_blocks=0,
+                restart_marker_rows=0):
     """The serial host driver (j2p_jpegenc_encode_host, or j2p_jpegopt_encode_host when optimize,
     or j2p_jpegprog_encode_host when progressive) on numpy uint8 arrays: a list of JPEG files as
     bytes, the same bytes the device writes."""
     B.check_layout(layout)
-    p = params(quality, subsampling)
+    p = params(quality, subsampling, restart_marker_blocks, restart_marker_rows)
     check_optimize(optimize)
     check_progressive(progressive)
     for x in images:
@@ -160,7 +179,8 @@ def encode_host(images, quality=75, subsampling='4:2:0', layout='HWC', optimize=
     return B.encode_host(codec(p, optimize, progressive), images, layout)
 
 
-def encode_jpeg(images, *, quality=75, subsampling='4:2:0', layout='CHW', optimize=False, progressive=False):
+def encode_jpeg(images, *, quality=75, subsampling='4:2:0', layout='CHW', optimize=False, progressive=False, restart_marker_blocks=0,
+                restart_marker_rows=0):
     """Encode RGB CUDA tensors as baseline or progressive JPEG files on the device.
 
     images: one tensor or a list or tuple of them, torch.uint8, shaped (3, h, w) for layout='CHW'
@@ -168,7 +188,8 @@ def encode_jpeg(images, *, quality=75, subsampling='4:2:0', layout='CHW', optimi
     in 1..100; subsampling: '4:4:4', '4:2:2' or '4:2:0'.  Returns the JPEG file as bytes, or a list
     of bytes in input order: byte for byte the file Pillow writes for the same pixels with
     `save(f, 'JPEG', quality=quality, subsampling=subsampling, optimize=optimize,
-    progressive=progressive)`.
+    progressive=progressive, restart_marker_blocks=restart_marker_blocks,
+    restart_marker_rows=restart_marker_rows)`.
 
     optimize: False writes the Annex K Huffman tables; True builds each image's tables from its own
     symbol counts, on the device, as libjpeg does for `optimize=True`: the same coefficients, files
@@ -179,15 +200,26 @@ def encode_jpeg(images, *, quality=75, subsampling='4:2:0', layout='CHW', optimi
     progressive file): the same coefficients, shown coarse to fine as the file arrives.  optimize
     changes no byte of a progressive file, as with Pillow.
 
+    restart_marker_blocks, restart_marker_rows: integers in 0..65535 (0, the default: no restart
+    markers).  With blocks = b every scan gets a restart interval of b MCUs; with rows = r, which
+    overrides b as in libjpeg, a scan gets r times its MCUs per row, capped at 65535 MCUs (in a
+    progressive file the AC scans of one component count that component's blocks per row, so the
+    interval can change between scans).  Each interval ends padded to a byte and is followed by an
+    RST marker, and restarts its DC prediction and EOB run, so a decoder can start at any
+    interval and a damaged file loses one interval.  Every interval is its own bit stream on the
+    device, so very short intervals (one MCU) cost work area and time.  Unlike Pillow, negative
+    values and values above 65535 are refused (Pillow writes -1 as 65535, and a value above
+    65535 as a corrupt file).
+
     The work is queued on torch's current stream, after what is already there, so a tensor just
     written on that stream needs no synchronisation.  Images of any mix of sizes go into one call;
     a list is split into several only when the work area would not fit in a quarter of the free
     device memory.  Raises ValueError for a wrong dtype, shape, layout, quality, subsampling,
-    optimize or progressive (not a bool) or size, and for a tensor that is not on a CUDA device, and RuntimeError
-    when no CUDA device is usable.
+    optimize or progressive (not a bool), restart keyword or size, and for a tensor that is not on
+    a CUDA device, and RuntimeError when no CUDA device is usable.
     """
     B.check_layout(layout)
-    p = params(quality, subsampling)
+    p = params(quality, subsampling, restart_marker_blocks, restart_marker_rows)
     check_optimize(optimize)
     check_progressive(progressive)
     return B.encode_tensors('encode_jpeg', codec(p, optimize, progressive), images, layout, (torch.uint8,))

@@ -19,7 +19,8 @@ extern "C" int j2p_jpegenc_plan(const struct j2p_jpegenc_image *images, unsigned
 extern "C" int j2p_jpegenc_encode_host(const struct j2p_jpegenc_image *images, unsigned n, const struct j2p_jpegenc_params *params, void *work,
                                        size_t work_bytes, uint64_t *offsets) {
     return encode_host_steps(images, n, params, J2P_JE_WORDS_PER_BLOCK, false, work, work_bytes, offsets,
-                             [](const Layout &, uint8_t *, const struct j2p_je_img *, const struct j2p_je_tables *t, const int16_t *) {
+                             [](const Layout &, uint8_t *, const struct j2p_je_img *, const struct j2p_je_img *, const struct j2p_je_tables *t,
+                                const int16_t *) {
                                  return FixedCodes{t};
                              });
 }
@@ -31,39 +32,48 @@ __global__ void __launch_bounds__(kBlockThreads) k_je_blocks(const struct j2p_je
     blocks_body(imgs, n, t, nblk, coef);
 }
 
-__global__ void __launch_bounds__(kTileThreads) k_je_sizes(const struct j2p_je_img *__restrict__ imgs, uint32_t n,
-                                                          const struct j2p_je_tables *__restrict__ t, const int16_t *__restrict__ coef,
-                                                          uint32_t *__restrict__ intra, uint32_t *__restrict__ tsum) {
-    sizes_body(imgs, n, t, coef, intra, tsum, [&](uint32_t) { return &t->huff; });
+__global__ void __launch_bounds__(kTileThreads) k_je_sizes(const struct j2p_je_img *__restrict__ strs, uint32_t ns, bool plain, const struct j2p_je_tables *__restrict__ t,
+                                                          const int16_t *__restrict__ coef, uint32_t *__restrict__ intra,
+                                                          uint32_t *__restrict__ tsum) {
+    const StreamMap<1> sm = {strs, ns, plain};
+    sizes_body(sm, t, coef, intra, tsum, [&](uint32_t) { return &t->huff; });
 }
 
-__global__ void __launch_bounds__(kScanThreads) k_je_scan(struct j2p_je_img *__restrict__ imgs, const uint32_t *__restrict__ tsum,
+__global__ void __launch_bounds__(kScanThreads) k_je_scan(struct j2p_je_img *__restrict__ strs, const uint32_t *__restrict__ tsum,
                                                          uint64_t *__restrict__ toff, uint32_t *__restrict__ raw) {
-    scan_body(imgs, tsum, toff, raw);
+    scan_body(strs, tsum, toff, raw);
 }
 
-__global__ void __launch_bounds__(kTileThreads) k_je_emit(const struct j2p_je_img *__restrict__ imgs, uint32_t n,
+__global__ void __launch_bounds__(kTileThreads) k_je_emit(const struct j2p_je_img *__restrict__ strs, uint32_t ns,
                                                          const struct j2p_je_tables *__restrict__ t, const int16_t *__restrict__ coef,
                                                          const uint32_t *__restrict__ intra, const uint64_t *__restrict__ toff,
                                                          uint32_t *__restrict__ raw) {
-    emit_body(imgs, n, t, coef, intra, toff, raw, &t->huff);
+    emit_body(strs, ns, t, coef, intra, toff, raw, &t->huff);
 }
 
-__global__ void __launch_bounds__(kChunkThreads) k_je_ffcount(const struct j2p_je_img *__restrict__ imgs, uint32_t n,
+__global__ void __launch_bounds__(kChunkThreads) k_je_ffcount(const struct j2p_je_img *__restrict__ strs, uint32_t ns,
                                                              const uint32_t *__restrict__ raw, uint32_t *__restrict__ ffc) {
-    ffcount_body(imgs, n, raw, ffc);
+    ffcount_body(strs, ns, raw, ffc);
 }
 
-__global__ void __launch_bounds__(kScanThreads) k_je_offsets(struct j2p_je_img *__restrict__ imgs, uint32_t n, const uint32_t *__restrict__ ffc,
-                                                            uint32_t nchunks, uint64_t *__restrict__ ffpre, uint64_t *__restrict__ offsets) {
-    offsets_body(imgs, n, ffc, nchunks, ffpre, offsets, [](uint32_t) { return J2P_JE_HEAD; });
+// the scan header's length: the template, with DRI when the image has restart intervals
+__device__ __forceinline__ uint32_t fixed_head_len(const StreamMap<1> &sm, uint32_t s) {
+    return sm.plain ? J2P_JE_HEAD : J2P_JE_HEAD + (sm.strs[s].ri ? J2P_JE_DRI : 0);
 }
 
-__global__ void __launch_bounds__(kChunkThreads) k_je_stuff(const struct j2p_je_img *__restrict__ imgs, uint32_t n,
-                                                           const struct j2p_je_tables *__restrict__ t, const uint32_t *__restrict__ raw,
-                                                           const uint64_t *__restrict__ ffpre, uint8_t *__restrict__ out) {
-    stuff_body(imgs, n, raw, ffpre, out, [](uint32_t) { return J2P_JE_HEAD; },
-               [&](uint32_t, const struct j2p_je_img *im, uint32_t k) { return j2p_je_head_byte(t, im, k); });
+__global__ void __launch_bounds__(kScanThreads) k_je_offsets(struct j2p_je_img *__restrict__ strs, uint32_t ns, bool plain, uint32_t n,
+                                                            const uint32_t *__restrict__ ffc, uint32_t nchunks, uint64_t *__restrict__ ffpre,
+                                                            uint64_t *__restrict__ offsets) {
+    const StreamMap<1> sm = {strs, ns, plain};
+    offsets_body(strs, sm, n, ffc, nchunks, ffpre, offsets, [&](uint32_t s) { return fixed_head_len(sm, s); });
+}
+
+__global__ void __launch_bounds__(kChunkThreads) k_je_stuff(const struct j2p_je_img *__restrict__ strs, uint32_t ns, bool plain, const struct j2p_je_tables *__restrict__ t,
+                                                           const uint32_t *__restrict__ raw, const uint64_t *__restrict__ ffpre,
+                                                           uint8_t *__restrict__ out) {
+    const StreamMap<1> sm = {strs, ns, plain};
+    stuff_body(sm, raw, ffpre, out, [&](uint32_t s) { return fixed_head_len(sm, s); },
+               [&](uint32_t s, uint32_t k) { return sm.plain ? j2p_je_head_byte(t, &sm.strs[s], k) : j2p_je_scan_head_byte(t, &sm.strs[s], k); });
 }
 
 extern "C" int j2p_jpegenc_encode(const struct j2p_jpegenc_image *images, unsigned n, const struct j2p_jpegenc_params *params, void *work,
@@ -72,7 +82,7 @@ extern "C" int j2p_jpegenc_encode(const struct j2p_jpegenc_image *images, unsign
     if (make_plan(images, n, params, J2P_JE_WORDS_PER_BLOCK, false, &L, nullptr) != 0) return -1;
     const auto fill = [&](uint8_t *plan) { return fill_plan(images, n, params, J2P_JE_WORDS_PER_BLOCK, false, L, plan); };
     const auto launch = [&](uint8_t *w, cudaStream_t st, const uint8_t *, auto counted) {
-        struct j2p_je_img *imgs = (struct j2p_je_img *)(w + L.off_imgs);
+        struct j2p_je_img *imgs = (struct j2p_je_img *)(w + L.off_imgs), *strs = (struct j2p_je_img *)(w + L.off_strs);
         const struct j2p_je_tables *t = (const struct j2p_je_tables *)(w + L.off_tab);
         uint32_t *tsum = (uint32_t *)(w + L.off_tsum), *intra = (uint32_t *)(w + L.off_intra), *ffc = (uint32_t *)(w + L.off_ffc);
         uint64_t *toff = (uint64_t *)(w + L.off_toff), *ffpre = (uint64_t *)(w + L.off_ffpre), *offs = (uint64_t *)(w + L.off_offs);
@@ -83,17 +93,17 @@ extern "C" int j2p_jpegenc_encode(const struct j2p_jpegenc_image *images, unsign
         const uint64_t bgrid = (L.nblk * 8 + kBlockThreads - 1) / kBlockThreads;
         k_je_blocks<<<(unsigned)bgrid, kBlockThreads, 0, st>>>(imgs, n, t, L.nblk, coef);
         counted();
-        k_je_sizes<<<L.ntiles, kTileThreads, 0, st>>>(imgs, n, t, coef, intra, tsum);
+        k_je_sizes<<<L.ntiles, kTileThreads, 0, st>>>(strs, L.ns, L.plain, t, coef, intra, tsum);
         counted();
-        k_je_scan<<<n, kScanThreads, 0, st>>>(imgs, tsum, toff, raw);
+        k_je_scan<<<L.ns, kScanThreads, 0, st>>>(strs, tsum, toff, raw);
         counted();
-        k_je_emit<<<L.ntiles, kTileThreads, 0, st>>>(imgs, n, t, coef, intra, toff, raw);
+        k_je_emit<<<L.ntiles, kTileThreads, 0, st>>>(strs, L.ns, t, coef, intra, toff, raw);
         counted();
-        k_je_ffcount<<<L.nchunks, kChunkThreads, 0, st>>>(imgs, n, raw, ffc);
+        k_je_ffcount<<<L.nchunks, kChunkThreads, 0, st>>>(strs, L.ns, raw, ffc);
         counted();
-        k_je_offsets<<<1, kScanThreads, 0, st>>>(imgs, n, ffc, L.nchunks, ffpre, offs);
+        k_je_offsets<<<1, kScanThreads, 0, st>>>(strs, L.ns, L.plain, n, ffc, L.nchunks, ffpre, offs);
         counted();
-        k_je_stuff<<<L.nchunks, kChunkThreads, 0, st>>>(imgs, n, t, raw, ffpre, w + L.off_out);
+        k_je_stuff<<<L.nchunks, kChunkThreads, 0, st>>>(strs, L.ns, L.plain, t, raw, ffpre, w + L.off_out);
         counted();
         return 0;
     };

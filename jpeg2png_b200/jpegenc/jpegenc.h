@@ -23,6 +23,16 @@
  * Chroma: 11 + 11 for the DC and at most 22 per AC coefficient (its run 0, category 10 code is 12
  * bits), 22 + 63 x 22 = 1408.  J2P_JPEGENC_BLOCK_BITS is the larger, and stuffing at most doubles
  * the bytes.  For 64 images of 1920 x 1080 the work area is about 2.4 GB at 4:2:0, 4.7 GB at 4:4:4.
+ *
+ * Restart markers (restart_marker_blocks, restart_marker_rows; Pillow's keywords of the same names):
+ * the scan is cut into intervals of Ri MCUs, Ri = restart_marker_blocks, or restart_marker_rows x
+ * the MCUs per row capped at 65535 when that is set.  The header gets DRI (FF DD 00 04 Ri) between
+ * the DHTs and the SOS.  Each interval is its own bit stream: it starts with DC predictions of 0,
+ * is padded with 1-bits to a byte, and every interval but the first is preceded by RST0 + (its
+ * number - 1) mod 8.  So an interval adds at most 7 pad bits and 2 unstuffed marker bytes to the
+ * bound above, and each costs a stream descriptor, a 256-block tile, an 8 KiB stuffing chunk and
+ * 16 bytes of rounding words of work area (jpegenc_plan.h).  Values above 65535 are refused, where
+ * libjpeg would write DRI mod 65536 and count the full value (a corrupt file).
  */
 #ifndef J2P_JPEGENC_H
 #define J2P_JPEGENC_H
@@ -47,6 +57,9 @@ struct j2p_jpegenc_image {
 struct j2p_jpegenc_params {
         int quality;                    /* 1 .. 100 */
         int sampling;                   /* enum j2p_jpegenc_sampling */
+        int restart_marker_blocks;      /* 0 .. 65535: a restart interval of this many MCUs in every scan; 0 none */
+        int restart_marker_rows;        /* 0 .. 65535: one of this many MCU rows per scan (capped at 65535
+                                           MCUs); overrides restart_marker_blocks; 0 none */
 };
 
 struct j2p_jpegenc_stats {
@@ -56,7 +69,8 @@ struct j2p_jpegenc_stats {
 
 /* Work area for the n images: work_bytes in all, the files at out_offset in it.  Refuses null
  * pointers, n == 0, a width or height of 0 or above 65535 (SOF's 16-bit fields), a quality outside
- * 1 .. 100 and an unknown sampling.  Returns 0, or -1 (j2p_jpegenc_last_error). */
+ * 1 .. 100, an unknown sampling and a restart field outside 0 .. 65535.  Returns 0, or -1
+ * (j2p_jpegenc_last_error). */
 int j2p_jpegenc_plan(const struct j2p_jpegenc_image *images, unsigned n, const struct j2p_jpegenc_params *params, size_t *work_bytes,
                      size_t *out_offset);
 

@@ -28,12 +28,18 @@
 #define J2P_JE_WORDS_PER_BLOCK 52u      // 32-bit words of J2P_JPEGENC_BLOCK_BITS, rounded up
 static_assert(J2P_JE_WORDS_PER_BLOCK * 32 >= J2P_JPEGENC_BLOCK_BITS && (J2P_JE_WORDS_PER_BLOCK - 1) * 32 < J2P_JPEGENC_BLOCK_BITS,
               "J2P_JE_WORDS_PER_BLOCK is J2P_JPEGENC_BLOCK_BITS in words");
+// A stream (an image, or one restart interval of it) of nb blocks gets nb x J2P_JE_WORDS_PER_BLOCK
+// words, whole bytes, so the 1-bits that pad its coded bits to a byte stay inside them; its RST is
+// its 2-byte header, outside them.
+static_assert(J2P_JE_WORDS_PER_BLOCK * 32 % 8 == 0, "the padding of a stream's last byte fits its words");
 #define J2P_JE_TILE 256u                // blocks per tile of the size and emit kernels (never across images)
 #define J2P_JE_CHUNK 8192u              // entropy bytes per chunk of the stuffing kernels
 #define J2P_JE_HEAD 623u                // SOI .. SOS: 2 + 18 + 2 x 69 + 19 + 2 x 33 + 2 x 183 + 14
 #define J2P_JE_SOF_AT 158u              // offset of SOF0 in the header (its height follows at + 5)
 
-// per image of a call (host plan, read by the kernels)
+// per image of a call, or per bit stream (host plan, read by the kernels).  A stream is an image's
+// scan, or one restart interval of it; it carries its image's fields, and blk0, nblk, the tiles,
+// chunks, words and output of its own blocks.
 struct j2p_je_img {
         const uint8_t *src;
         int64_t s_row, s_col, s_chan;   // element strides
@@ -43,11 +49,17 @@ struct j2p_je_img {
         uint32_t tile0, ntiles;
         uint32_t chunk0, nchunks;       // stuffing chunks of the worst case
         uint64_t raw_off;               // first word of the image's entropy bits
-        uint64_t out_cap;               // worst-case file bytes
+        uint32_t img;                   // the image (its index in the call)
+        uint32_t part;                  // the restart interval in the scan, 0 the first
+        uint16_t ri;                    // the scan's restart interval in MCUs, 0 without restarts
+        uint8_t scan;                   // the scan of the file (progressive; 0 otherwise)
+        uint8_t pad_;
         // written by the encoder
         uint64_t bits;                  // entropy-coded bits before padding
         uint64_t file_off, file_len;
 };
+// one 128-byte line per descriptor: the kernels' binary searches over them touch one line a step
+static_assert(sizeof(struct j2p_je_img) == 128, "a stream descriptor is one 128-byte line");
 
 // derived Huffman codes of the four tables: DC0, AC0, DC1, AC1 (jpeg_make_c_derived_tbl)
 struct j2p_je_huff {

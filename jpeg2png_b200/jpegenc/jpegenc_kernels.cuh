@@ -1,12 +1,14 @@
 // jpegenc_kernels.cuh — the bodies of the encoder's kernels as __device__ functions, shared by
 // libj2pjpegenc.so (whose __global__ kernels are thin wrappers around them), libj2pjpegopt.so and
-// libj2pjpegprog.so (which runs the blocks, scan and ffcount bodies on its per-scan streams).
-// Where an image's Huffman tables and header come from is a parameter:
+// libj2pjpegprog.so.  The blocks body runs on images; the others run on bit streams (an image's
+// scan, or one restart interval of it; jpegenc_plan.h), each described by a j2p_je_img that names
+// its image.  Where an image's Huffman tables and a stream's header come from is a parameter:
 //   huff(i)                the derived tables of image i (called by every thread of the CTA, before
 //                          any of them returns, so that it may stage them in shared memory); the
 //                          emit body takes the tables themselves, staged by its caller;
-//   head_len(i)            the header's length;
-//   head_byte(i, im, k)    its byte k.
+//   head_len(s)            the length of the scan header that stream s starts with when it is its
+//                          scan's first interval (the others start with RST);
+//   head_byte(s, k)        its byte k.
 #ifndef J2P_JPEGENC_KERNELS_CUH
 #define J2P_JPEGENC_KERNELS_CUH
 
@@ -82,16 +84,35 @@ __device__ __forceinline__ void blocks_body(const struct j2p_je_img *__restrict_
     if (on) finish_column(t, &wh, rows[grp], 9, (int)lane, coef + g * 64);
 }
 
+// Where the kernels find a stream's image, scan and interval.  Without restart intervals (plain)
+// every image has PER streams (1, or a progressive file's ten scans), so stream s is scan s % PER of
+// image s / PER and the only interval of its scan: the kernels use that arithmetic, as they did
+// before restarts existed, and read none of the descriptor's stream fields for it.  With restart
+// intervals they read the descriptor.
+template <uint32_t PER>
+struct StreamMap {
+    const struct j2p_je_img *strs;
+    uint32_t ns;
+    bool plain;
+    __device__ __forceinline__ uint32_t img(uint32_t s) const { return plain ? s / PER : strs[s].img; }
+    __device__ __forceinline__ uint32_t scan(uint32_t s) const { return plain ? s % PER : strs[s].scan; }
+    // the (image, scan) of stream s as one index, img x PER + scan
+    __device__ __forceinline__ uint32_t scan_index(uint32_t s) const { return plain ? s : strs[s].img * PER + strs[s].scan; }
+    // whether stream s starts with RST rather than its scan's header
+    __device__ __forceinline__ bool rst(uint32_t s) const { return !plain && strs[s].part; }
+    __device__ __forceinline__ bool first_of_file(uint32_t s) const { return plain ? s % PER == 0 : s == 0 || strs[s - 1].img != strs[s].img; }
+    __device__ __forceinline__ bool ends_file(uint32_t s) const { return plain ? s % PER == PER - 1 : j2p_je_ends_file(strs, ns, s); }
+};
+
 // per tile: each block's bits, their exclusive scan in the tile, the tile's sum
-template <class Huff>
-__device__ __forceinline__ void sizes_body(const struct j2p_je_img *__restrict__ imgs, uint32_t n, const struct j2p_je_tables *__restrict__ t,
-                                           const int16_t *__restrict__ coef, uint32_t *__restrict__ intra, uint32_t *__restrict__ tsum, Huff huff) {
+template <uint32_t PER, class Huff>
+__device__ __forceinline__ void sizes_body(const StreamMap<PER> &sm, const struct j2p_je_tables *__restrict__ t, const int16_t *__restrict__ coef,
+                                           uint32_t *__restrict__ intra, uint32_t *__restrict__ tsum, Huff huff) {
     typedef cub::BlockScan<uint32_t, kTileThreads> Scan;
     __shared__ typename Scan::TempStorage tmp;
-    const uint32_t tile = blockIdx.x;
-    const uint32_t i = find_image(imgs, n, tile, 1);
-    const struct j2p_je_img *im = &imgs[i];
-    const struct j2p_je_huff *h = huff(i);
+    const uint32_t tile = blockIdx.x, s = find_image(sm.strs, sm.ns, tile, 1);
+    const struct j2p_je_img *im = &sm.strs[s];
+    const struct j2p_je_huff *h = huff(sm.img(s));
     const uint64_t b = (uint64_t)(tile - im->tile0) * J2P_JE_TILE + threadIdx.x;
     const uint64_t blk0 = im->blk0;
     uint32_t bits = 0;
@@ -102,7 +123,7 @@ __device__ __forceinline__ void sizes_body(const struct j2p_je_img *__restrict__
     if (threadIdx.x == 0) tsum[tile] = total;
 }
 
-// per image: the tiles' bit offsets, the image's bits, the padding 1-bits
+// per stream: the tiles' bit offsets, the stream's bits, the padding 1-bits
 __device__ __forceinline__ void scan_body(struct j2p_je_img *__restrict__ imgs, const uint32_t *__restrict__ tsum, uint64_t *__restrict__ toff,
                                           uint32_t *__restrict__ raw) {
     __shared__ typename ScanU64::TempStorage tmp;
@@ -118,11 +139,11 @@ __device__ __forceinline__ void scan_body(struct j2p_je_img *__restrict__ imgs, 
     }
 }
 
-__device__ __forceinline__ void emit_body(const struct j2p_je_img *__restrict__ imgs, uint32_t n, const struct j2p_je_tables *__restrict__ t,
+__device__ __forceinline__ void emit_body(const struct j2p_je_img *__restrict__ strs, uint32_t ns, const struct j2p_je_tables *__restrict__ t,
                                           const int16_t *__restrict__ coef, const uint32_t *__restrict__ intra, const uint64_t *__restrict__ toff,
                                           uint32_t *__restrict__ raw, const struct j2p_je_huff *huff) {
     const uint32_t tile = blockIdx.x;
-    const struct j2p_je_img *im = &imgs[find_image(imgs, n, tile, 1)];
+    const struct j2p_je_img *im = &strs[find_image(strs, ns, tile, 1)];
     const uint64_t b = (uint64_t)(tile - im->tile0) * J2P_JE_TILE + threadIdx.x;
     if (b >= im->nblk) return;
     const uint64_t blk0 = im->blk0;
@@ -149,11 +170,11 @@ __device__ __forceinline__ uint32_t chunk_bytes(const struct j2p_je_img *im, con
     return m;
 }
 
-__device__ __forceinline__ void ffcount_body(const struct j2p_je_img *__restrict__ imgs, uint32_t n, const uint32_t *__restrict__ raw,
+__device__ __forceinline__ void ffcount_body(const struct j2p_je_img *__restrict__ strs, uint32_t ns, const uint32_t *__restrict__ raw,
                                              uint32_t *__restrict__ ffc) {
     typedef cub::BlockReduce<uint32_t, kChunkThreads> Red;
     __shared__ typename Red::TempStorage tmp;
-    const struct j2p_je_img *im = &imgs[find_image(imgs, n, blockIdx.x, 2)];
+    const struct j2p_je_img *im = &strs[find_image(strs, ns, blockIdx.x, 2)];
     const uint32_t c = blockIdx.x - im->chunk0;
     if ((uint64_t)c * J2P_JE_CHUNK >= raw_bytes(im)) {
         if (threadIdx.x == 0) ffc[blockIdx.x] = 0;
@@ -167,52 +188,68 @@ __device__ __forceinline__ void ffcount_body(const struct j2p_je_img *__restrict
     if (threadIdx.x == 0) ffc[blockIdx.x] = s;
 }
 
-// one CTA: the scan of the 0xFF counts over the call, each file's length and offset
-template <class HeadLen>
-__device__ __forceinline__ void offsets_body(struct j2p_je_img *__restrict__ imgs, uint32_t n, const uint32_t *__restrict__ ffc, uint32_t nchunks,
-                                             uint64_t *__restrict__ ffpre, uint64_t *__restrict__ offsets, HeadLen head_len) {
+// one CTA: the scan of the 0xFF counts over the call, each stream's place in the output (its header:
+// its scan's, of head_len(s) bytes, or RST; its stuffed bytes; after an image's last stream, EOI) and
+// each file's offset
+template <uint32_t PER, class HeadLen>
+__device__ __forceinline__ void offsets_body(struct j2p_je_img *__restrict__ strs, const StreamMap<PER> &sm, uint32_t n,
+                                             const uint32_t *__restrict__ ffc, uint32_t nchunks, uint64_t *__restrict__ ffpre,
+                                             uint64_t *__restrict__ offsets, HeadLen head_len) {
     __shared__ typename ScanU64::TempStorage tmp;
+    const uint32_t ns = sm.ns;
     const uint64_t ff = scan_segment(nchunks, [&](uint32_t k) { return (uint64_t)ffc[k]; }, [&](uint32_t k, uint64_t v) { ffpre[k] = v; }, tmp);
     if (threadIdx.x == 0) ffpre[nchunks] = ff;
     __syncthreads();
     const uint64_t base = scan_segment(
-        n,
-        [&](uint32_t i) {
-            const struct j2p_je_img *im = &imgs[i];
-            return head_len(i) + raw_bytes(im) + (ffpre[im->chunk0 + im->nchunks] - ffpre[im->chunk0]) + 2;
+        ns,
+        [&](uint32_t s) {
+            const struct j2p_je_img *st = &strs[s];
+            return (sm.rst(s) ? J2P_JE_RST : head_len(s)) + raw_bytes(st) + (ffpre[st->chunk0 + st->nchunks] - ffpre[st->chunk0]) +
+                   (sm.ends_file(s) ? 2 : 0);
         },
-        [&](uint32_t i, uint64_t v) { imgs[i].file_off = v; offsets[i] = v; }, tmp);
+        [&](uint32_t s, uint64_t v) {
+            strs[s].file_off = v;
+            if (sm.first_of_file(s)) offsets[sm.img(s)] = v;
+        },
+        tmp);
     __syncthreads();
-    for (uint32_t i = threadIdx.x; i < n; i += kScanThreads) imgs[i].file_len = (i + 1 < n ? imgs[i + 1].file_off : base) - imgs[i].file_off;
+    for (uint32_t s = threadIdx.x; s < ns; s += kScanThreads) strs[s].file_len = (s + 1 < ns ? strs[s + 1].file_off : base) - strs[s].file_off;
     if (threadIdx.x == 0) offsets[n] = base;
 }
 
-// per chunk: its bytes into the file with a 0x00 after each 0xFF; the first chunk also writes the
-// header, the one holding the last byte the EOI
-template <class HeadLen, class HeadByte>
-__device__ __forceinline__ void stuff_body(const struct j2p_je_img *__restrict__ imgs, uint32_t n, const uint32_t *__restrict__ raw,
-                                           const uint64_t *__restrict__ ffpre, uint8_t *__restrict__ out, HeadLen head_len, HeadByte head_byte) {
+// per chunk: its bytes into the output with a 0x00 after each 0xFF; a stream's first chunk also
+// writes its header (its scan's, head_len(s) bytes head_byte(s, k), or RST), the chunk holding an
+// image's last byte the EOI
+template <uint32_t PER, class HeadLen, class HeadByte>
+__device__ __forceinline__ void stuff_body(const StreamMap<PER> &sm, const uint32_t *__restrict__ raw, const uint64_t *__restrict__ ffpre,
+                                           uint8_t *__restrict__ out, HeadLen head_len, HeadByte head_byte) {
     typedef cub::BlockScan<uint32_t, kChunkThreads> Scan;
     __shared__ typename Scan::TempStorage tmp;
-    const uint32_t i = find_image(imgs, n, blockIdx.x, 2);
-    const struct j2p_je_img *im = &imgs[i];
-    const uint32_t c = blockIdx.x - im->chunk0;
-    const uint64_t nbytes = raw_bytes(im);
+    const uint32_t s = find_image(sm.strs, sm.ns, blockIdx.x, 2);
+    const struct j2p_je_img *st = &sm.strs[s];
+    const bool rst = sm.rst(s);
+    const uint32_t c = blockIdx.x - st->chunk0, hl = rst ? J2P_JE_RST : head_len(s);
+    const uint64_t nbytes = raw_bytes(st);
     if ((uint64_t)c * J2P_JE_CHUNK >= nbytes) return;
-    uint8_t *file = out + im->file_off;
-    if (c == 0)
-        for (uint32_t k = threadIdx.x; k < head_len(i); k += kChunkThreads) file[k] = head_byte(i, im, k);
-    if (threadIdx.x == 0 && (uint64_t)(c + 1) * J2P_JE_CHUNK >= nbytes) {
-        file[im->file_len - 2] = 0xff;
-        file[im->file_len - 1] = 0xd9;
+    uint8_t *file = out + st->file_off;
+    if (c == 0) {
+        if (rst) {
+            if (threadIdx.x < J2P_JE_RST) file[threadIdx.x] = j2p_je_rst_byte(st->part, threadIdx.x);
+        } else {
+            for (uint32_t k = threadIdx.x; k < hl; k += kChunkThreads) file[k] = head_byte(s, k);
+        }
+    }
+    if (threadIdx.x == 0 && (uint64_t)(c + 1) * J2P_JE_CHUNK >= nbytes && sm.ends_file(s)) {
+        file[st->file_len - 2] = 0xff;
+        file[st->file_len - 1] = 0xd9;
     }
     uint64_t j0;
     uint32_t cnt;
     uint4 v;
-    const uint32_t m = chunk_bytes(im, raw, c, &j0, &cnt, &v);
+    const uint32_t m = chunk_bytes(st, raw, c, &j0, &cnt, &v);
     uint32_t before;
     Scan(tmp).ExclusiveSum(cnt, before);
-    uint8_t *o = file + head_len(i) + j0 + (ffpre[blockIdx.x] - ffpre[im->chunk0]) + before;
+    uint8_t *o = file + hl + j0 + (ffpre[blockIdx.x] - ffpre[st->chunk0]) + before;
     const uint32_t wv[4] = {v.x, v.y, v.z, v.w};
 #pragma unroll
     for (int q = 0; q < 16; q++) {

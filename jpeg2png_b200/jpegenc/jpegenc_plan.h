@@ -150,101 +150,232 @@ static void make_tables(const struct j2p_jpegenc_params *p, struct j2p_je_tables
     memcpy(o, sos, 14);
 }
 
+// ---- restart intervals -------------------------------------------------------------------------
+// libjpeg's rule: restart_marker_blocks = b gives every scan an interval of b MCUs; restart_marker_rows
+// = r (which overrides b, as libjpeg's restart_in_rows overrides restart_interval) gives a scan
+// min(r x its MCUs per row, 65535): mcux for an interleaved scan, the component's own block-grid
+// width for a non-interleaved one.  0: no restarts.
+static uint32_t restart_interval(const struct j2p_jpegenc_params *p, uint32_t per_row) {
+    if (p->restart_marker_rows) {
+        const uint64_t v = (uint64_t)p->restart_marker_rows * per_row;
+        return v < 65535 ? (uint32_t)v : 65535u;
+    }
+    return (uint32_t)p->restart_marker_blocks;
+}
+
+#define J2P_JE_DRI 6u                   // DRI: FF DD 00 04 Ri
+#define J2P_JE_RST 2u                   // RSTm: FF D0+m, not stuffed
+#define J2P_JE_SOS 14u                  // the SOS of the interleaved scan that ends a baseline header
+
+// byte k of DRI for the interval ri
+J2P_HD uint8_t j2p_je_dri_byte(uint32_t ri, uint32_t k) {
+    return (uint8_t)(k == 0 ? 0xff : k == 1 ? 0xdd : k == 2 ? 0 : k == 3 ? 4 : k == 4 ? ri >> 8 : ri);
+}
+
+// byte k of a header that is hl bytes without DRI and ends in an SOS of sos bytes, head(k), with DRI
+// for dri (0: no DRI) inserted before the SOS, as libjpeg's write_scan_header places it
+#ifdef __CUDACC__
+#pragma nv_exec_check_disable
+#endif
+template <class Head>
+J2P_HD uint8_t j2p_je_dri_head(uint32_t dri, uint32_t hl, uint32_t sos, uint32_t k, Head head) {
+    const uint32_t at = hl - sos;
+    if (!dri || k < at) return head(k);
+    return k < at + J2P_JE_DRI ? j2p_je_dri_byte(dri, k - at) : head(k - J2P_JE_DRI);
+}
+
+// byte k of the RST before interval `part` > 0 of a scan
+J2P_HD uint8_t j2p_je_rst_byte(uint32_t part, uint32_t k) { return (uint8_t)(k ? 0xd0 + ((part - 1) & 7) : 0xff); }
+
+// Byte k of a stream's header: the scan header head(k) before its first interval, RST0 + (part - 1)
+// mod 8 before interval `part` > 0 (the marker number counts the scan's boundaries from 0).
+#ifdef __CUDACC__
+#pragma nv_exec_check_disable
+#endif
+template <class Head>
+J2P_HD uint8_t j2p_je_stream_byte(const struct j2p_je_img *st, uint32_t k, Head head) {
+    return st->part ? j2p_je_rst_byte(st->part, k) : head(k);
+}
+
+// the length of a baseline stream's header with the call's template
+J2P_HD uint32_t j2p_je_fixed_head_len(const struct j2p_je_img *st) { return st->part ? J2P_JE_RST : J2P_JE_HEAD + (st->ri ? J2P_JE_DRI : 0); }
+
+// byte k of a baseline scan header with the call's template: SOI .. SOS with the image's size and
+// its DRI
+J2P_HD uint8_t j2p_je_scan_head_byte(const struct j2p_je_tables *t, const struct j2p_je_img *st, uint32_t k) {
+    return j2p_je_dri_head(st->ri, J2P_JE_HEAD, J2P_JE_SOS, k, [&](uint32_t k1) { return j2p_je_head_byte(t, st, k1); });
+}
+
+// byte k of a baseline stream's header: the scan header, or the stream's RST
+J2P_HD uint8_t j2p_je_fixed_head_byte(const struct j2p_je_tables *t, const struct j2p_je_img *st, uint32_t k) {
+    return j2p_je_stream_byte(st, k, [&](uint32_t k1) { return j2p_je_scan_head_byte(t, st, k1); });
+}
+
+// whether stream s ends its image's file (EOI follows it)
+J2P_HD bool j2p_je_ends_file(const struct j2p_je_img *strs, uint32_t ns, uint32_t s) { return s + 1 == ns || strs[s + 1].img != strs[s].img; }
+
 // ---- plan --------------------------------------------------------------------------------------
-// work: [images][tables] [tile sums][tile offsets][block offsets in the tile][coefficients]
+// work: [images][tables][streams] [tile sums][tile offsets][block offsets in the tile][coefficients]
 //       [0xFF counts per chunk][their exclusive scan][offsets]
 //       (own codes only: [derived tables][headers][header lengths][symbol counts])
 //       [entropy words][files]
-// The symbol counts sit just before the entropy words, so that one memset clears both.
+// A stream is an image's scan, or one restart interval of it.  Without restarts each image is one
+// stream and the streams are the images ([streams] is empty); with them, stream p of an image holds
+// its MCUs p Ri .. (p + 1) Ri - 1.  The symbol counts sit just before the entropy words, so that one
+// memset clears both.
 struct Layout {
-    uint32_t n, ntiles, nchunks;
+    uint32_t n, ns, ntiles, nchunks;
+    bool plain;                         // no restart intervals: the streams are the images
     uint64_t nblk, words;
-    size_t off_imgs, off_tab, off_tsum, off_toff, off_intra, off_coef, off_ffc, off_ffpre, off_offs, off_raw, off_out, total;
+    size_t off_imgs, off_tab, off_strs, off_tsum, off_toff, off_intra, off_coef, off_ffc, off_ffpre, off_offs, off_raw, off_out, total;
     size_t off_huff, off_head, off_hlen, off_hist;      // per image; empty without own codes
 };
 
 #define J2P_JE_SYMBOLS 256u             // symbol counts per table and image (4 tables)
+#define J2P_JE_HEAD_ROOM (J2P_JE_HEAD + J2P_JE_DRI)    // the longest header of a baseline file
 
-// wpb: entropy words per block of the worst case; own: room for per-image tables and headers
-static int make_plan(const struct j2p_jpegenc_image *im, unsigned n, const struct j2p_jpegenc_params *p, uint32_t wpb, bool own, Layout *L,
-                     struct j2p_je_img *imgs) {
+// the checks of a call's arguments
+static int check_call(const struct j2p_jpegenc_image *im, unsigned n, const struct j2p_jpegenc_params *p) {
     if (!im) return fail("null argument: images");
     if (!p) return fail("null argument: params");
     if (n == 0) return fail("no images");
     if (p->quality < 1 || p->quality > 100) return fail("quality must be 1 .. 100 (got %d)", p->quality);
     if (p->sampling != J2P_JPEGENC_444 && p->sampling != J2P_JPEGENC_422 && p->sampling != J2P_JPEGENC_420)
         return fail("unknown sampling %d (0: 4:4:4, 1: 4:2:2, 2: 4:2:0)", p->sampling);
-    const uint32_t hs = p->sampling == J2P_JPEGENC_444 ? 1 : 2, vs = p->sampling == J2P_JPEGENC_420 ? 2 : 1, bpm = hs * vs + 2;
-    uint64_t nblk = 0, words = 0, tiles = 0, chunks = 0, out = 0;
+    if (p->restart_marker_blocks < 0 || p->restart_marker_blocks > 65535)
+        return fail("restart_marker_blocks must be 0 .. 65535 (got %d)", p->restart_marker_blocks);
+    if (p->restart_marker_rows < 0 || p->restart_marker_rows > 65535)
+        return fail("restart_marker_rows must be 0 .. 65535 (got %d)", p->restart_marker_rows);
     for (unsigned i = 0; i < n; i++) {
         const struct j2p_jpegenc_image *x = &im[i];
         if (!x->data) return fail("image %u: null data pointer", i);
         if (x->width == 0 || x->height == 0 || x->width > 65535 || x->height > 65535)
             return fail("image %u: width and height must be 1 .. 65535 (got %u x %u)", i, x->width, x->height);
-        const uint32_t mcux = (x->width + 8 * hs - 1) / (8 * hs), mcuy = (x->height + 8 * vs - 1) / (8 * vs);
-        const uint64_t nb = (uint64_t)mcux * mcuy * bpm;
-        const uint64_t nt = (nb + J2P_JE_TILE - 1) / J2P_JE_TILE;
-        const uint64_t raw_bytes = nb * (wpb * 4);
+    }
+    return 0;
+}
+
+// image i's descriptor, its blocks from blk0: what the blocks step reads (the stream fields are 0)
+static void image_desc(const struct j2p_jpegenc_image *x, uint32_t i, const struct j2p_jpegenc_params *p, uint64_t blk0, struct j2p_je_img *g) {
+    const uint32_t hs = p->sampling == J2P_JPEGENC_444 ? 1 : 2, vs = p->sampling == J2P_JPEGENC_420 ? 2 : 1;
+    memset(g, 0, sizeof *g);
+    g->src = (const uint8_t *)x->data;
+    g->s_row = x->row_stride;
+    g->s_col = x->col_stride;
+    g->s_chan = x->chan_stride;
+    g->w = x->width;
+    g->h = x->height;
+    g->mcux = (x->width + 8 * hs - 1) / (8 * hs);
+    g->mcuy = (x->height + 8 * vs - 1) / (8 * vs);
+    g->blk0 = blk0;
+    g->nblk = (uint64_t)g->mcux * g->mcuy * (hs * vs + 2);
+    g->img = i;
+}
+
+// The running totals of a plan's streams.  add() appends a stream of nb blocks from blk0 (in the
+// call's block order of the stream's kind), with wpb words a block of room, a header of at most
+// `head` bytes and `tail` bytes after it (EOI), and writes its descriptor into g when g is given.
+struct StreamPlan {
+    uint64_t ns = 0, tiles = 0, chunks = 0, words = 0, out = 0;
+    void add(const struct j2p_je_img &im, uint64_t blk0, uint64_t nb, uint32_t wpb, uint32_t head, uint32_t tail, uint32_t scan, uint32_t part,
+             uint32_t ri, struct j2p_je_img *g) {
+        const uint64_t nt = (nb + J2P_JE_TILE - 1) / J2P_JE_TILE, raw_bytes = nb * (wpb * 4);
         const uint64_t nc = (raw_bytes + J2P_JE_CHUNK - 1) / J2P_JE_CHUNK;
-        if (imgs) {
-            struct j2p_je_img *g = &imgs[i];
-            memset(g, 0, sizeof *g);
-            g->src = (const uint8_t *)x->data;
-            g->s_row = x->row_stride;
-            g->s_col = x->col_stride;
-            g->s_chan = x->chan_stride;
-            g->w = x->width;
-            g->h = x->height;
-            g->mcux = mcux;
-            g->mcuy = mcuy;
-            g->blk0 = nblk;
+        if (g) {
+            *g = im;
+            g->blk0 = blk0;
             g->nblk = nb;
             g->tile0 = (uint32_t)tiles;
             g->ntiles = (uint32_t)nt;
             g->chunk0 = (uint32_t)chunks;
             g->nchunks = (uint32_t)nc;
             g->raw_off = words;
-            g->out_cap = J2P_JE_HEAD + 2 * raw_bytes + 2;
+            g->scan = (uint8_t)scan;
+            g->part = part;
+            g->ri = (uint16_t)ri;
         }
-        nblk += nb;
+        ns++;
         tiles += nt;
         chunks += nc;
         words += (nb * wpb + 3) / 4 * 4 + 4;   // raw_off stays a multiple of 4 words: chunk_bytes reads uint4
-        out += J2P_JE_HEAD + 2 * raw_bytes + 2;
+        out += head + 2 * raw_bytes + tail;
     }
-    if (tiles >= 0x7fffffffu || chunks >= 0x7fffffffu) return fail("too many blocks for one call (%llu)", (unsigned long long)nblk);
-    const size_t m = own ? n : 0;
-    L->n = n;
-    L->nblk = nblk;
-    L->ntiles = (uint32_t)tiles;
-    L->nchunks = (uint32_t)chunks;
-    L->words = words;
+    int check(uint64_t nblk) const {
+        if (ns >= 0x7fffffffu || tiles >= 0x7fffffffu || chunks >= 0x7fffffffu)
+            return fail("too many blocks or restart intervals for one call (%llu blocks, %llu streams)", (unsigned long long)nblk,
+                        (unsigned long long)ns);
+        return 0;
+    }
+};
+
+// The plan of a call: wpb entropy words per block of the worst case; own: room for per-image tables
+// and headers.  With w, also the plan region (images, streams) at w.
+static int make_plan(const struct j2p_jpegenc_image *im, unsigned n, const struct j2p_jpegenc_params *p, uint32_t wpb, bool own, Layout *L,
+                     uint8_t *w) {
+    if (check_call(im, n, p) != 0) return -1;
+    const bool restarts = p->restart_marker_blocks || p->restart_marker_rows;
+    uint64_t ns = 0, nblk = 0;
+    for (unsigned i = 0; i < n; i++) {          // the streams, to place the arrays
+        struct j2p_je_img g;
+        image_desc(&im[i], i, p, 0, &g);
+        const uint64_t ri = restart_interval(p, g.mcux), mcus = (uint64_t)g.mcux * g.mcuy;
+        ns += ri ? (mcus + ri - 1) / ri : 1;
+    }
+    if (ns >= 0x7fffffffu) return fail("too many restart intervals for one call (%llu)", (unsigned long long)ns);
     size_t o = 0;
     L->off_imgs = o;  o = align16(o + n * sizeof(struct j2p_je_img));
     L->off_tab = o;   o = align16(o + sizeof(struct j2p_je_tables));
-    L->off_tsum = o;  o = align16(o + tiles * sizeof(uint32_t));
-    L->off_toff = o;  o = align16(o + tiles * sizeof(uint64_t));
+    o = (o + 127) & ~(size_t)127;       // each descriptor on one 128-byte line
+    L->plain = !restarts;
+    L->off_strs = restarts ? o : L->off_imgs;
+    if (restarts) o = align16(o + ns * sizeof(struct j2p_je_img));
+    struct j2p_je_img *imgs = w ? (struct j2p_je_img *)(w + L->off_imgs) : nullptr, *strs = w ? (struct j2p_je_img *)(w + L->off_strs) : nullptr;
+    StreamPlan sp;
+    for (unsigned i = 0; i < n; i++) {
+        struct j2p_je_img g;
+        image_desc(&im[i], i, p, nblk, &g);
+        const uint32_t bpm = (uint32_t)(g.nblk / ((uint64_t)g.mcux * g.mcuy)), ri = restart_interval(p, g.mcux);
+        const uint64_t mcus = (uint64_t)g.mcux * g.mcuy, parts = ri ? (mcus + ri - 1) / ri : 1;
+        g.ri = (uint16_t)ri;
+        if (imgs && restarts) imgs[i] = g;
+        for (uint64_t q = 0; q < parts; q++) {
+            const uint64_t m0 = q * ri, m1 = ri && m0 + ri < mcus ? m0 + ri : mcus;
+            sp.add(g, nblk + m0 * bpm, (m1 - m0) * bpm, wpb, q ? J2P_JE_RST : J2P_JE_HEAD + (ri ? J2P_JE_DRI : 0), q + 1 == parts ? 2 : 0, 0,
+                   (uint32_t)q, ri, strs ? &strs[sp.ns] : nullptr);
+        }
+        nblk += g.nblk;
+    }
+    if (sp.check(nblk) != 0) return -1;
+    const size_t m = own ? n : 0;
+    L->n = n;
+    L->ns = (uint32_t)ns;
+    L->nblk = nblk;
+    L->ntiles = (uint32_t)sp.tiles;
+    L->nchunks = (uint32_t)sp.chunks;
+    L->words = sp.words;
+    L->off_tsum = o;  o = align16(o + sp.tiles * sizeof(uint32_t));
+    L->off_toff = o;  o = align16(o + sp.tiles * sizeof(uint64_t));
     L->off_intra = o; o = align16(o + nblk * sizeof(uint32_t));
     L->off_coef = o;  o = align16(o + nblk * 64 * sizeof(int16_t));
-    L->off_ffc = o;   o = align16(o + chunks * sizeof(uint32_t));
-    L->off_ffpre = o; o = align16(o + (chunks + 1) * sizeof(uint64_t));
+    L->off_ffc = o;   o = align16(o + sp.chunks * sizeof(uint32_t));
+    L->off_ffpre = o; o = align16(o + (sp.chunks + 1) * sizeof(uint64_t));
     L->off_offs = o;  o = align16(o + (n + 1) * sizeof(uint64_t));
     L->off_huff = o;  o = align16(o + m * sizeof(struct j2p_je_huff));
-    L->off_head = o;  o = align16(o + m * J2P_JE_HEAD);
+    L->off_head = o;  o = align16(o + m * J2P_JE_HEAD_ROOM);
     L->off_hlen = o;  o = align16(o + m * sizeof(uint32_t));
     L->off_hist = o;  o = align16(o + m * 4 * J2P_JE_SYMBOLS * sizeof(uint64_t));
-    L->off_raw = o;   o = align16(o + words * sizeof(uint32_t));
-    L->off_out = o;   o = align16(o + out);
+    L->off_raw = o;   o = align16(o + sp.words * sizeof(uint32_t));
+    L->off_out = o;   o = align16(o + sp.out);
     L->total = o;
     return 0;
 }
 
-// the plan region (images, tables) in host memory
-static int fill_plan(const struct j2p_jpegenc_image *im, unsigned n, const struct j2p_jpegenc_params *p, uint32_t wpb, bool own, const Layout &L,
+// the plan region (images, tables, streams) in host memory
+static int fill_plan(const struct j2p_jpegenc_image *im, unsigned n, const struct j2p_jpegenc_params *p, uint32_t wpb, bool own, const Layout &,
                      uint8_t *w) {
     Layout tmp;
-    if (make_plan(im, n, p, wpb, own, &tmp, (struct j2p_je_img *)(w + L.off_imgs)) != 0) return -1;
-    make_tables(p, (struct j2p_je_tables *)(w + L.off_tab));
+    if (make_plan(im, n, p, wpb, own, &tmp, w) != 0) return -1;
+    make_tables(p, (struct j2p_je_tables *)(w + tmp.off_tab));
     return 0;
 }
 
@@ -296,13 +427,14 @@ static void host_blocks(const struct j2p_je_img *im, const struct j2p_je_tables 
 struct FixedCodes {
     const struct j2p_je_tables *t;
     const struct j2p_je_huff *huff(uint32_t) const { return &t->huff; }
-    uint32_t head_len(uint32_t) const { return J2P_JE_HEAD; }
-    uint8_t head_byte(uint32_t, const struct j2p_je_img *im, uint32_t k) const { return j2p_je_head_byte(t, im, k); }
+    uint32_t head_len(const struct j2p_je_img *st) const { return j2p_je_fixed_head_len(st); }
+    uint8_t head_byte(const struct j2p_je_img *st, uint32_t k) const { return j2p_je_fixed_head_byte(t, st, k); }
 };
 
-// The steps of the kernels run serially on host memory.  codes(L, w, imgs, t, coef) runs between
-// the blocks and the sizes and returns where each image's Huffman tables and header come from: an
-// object with huff(i), head_len(i) and head_byte(i, im, k), such as FixedCodes.
+// The steps of the kernels run serially on host memory.  codes(L, w, imgs, strs, t, coef) runs
+// between the blocks and the sizes and returns where each image's Huffman tables and each stream's
+// header come from: an object with huff(image), head_len(stream) and head_byte(stream, k), such as
+// FixedCodes.
 template <class Codes>
 static int encode_host_steps(const struct j2p_jpegenc_image *images, unsigned n, const struct j2p_jpegenc_params *params, uint32_t wpb, bool own,
                              void *work, size_t work_bytes, uint64_t *offsets, Codes codes) {
@@ -312,7 +444,8 @@ static int encode_host_steps(const struct j2p_jpegenc_image *images, unsigned n,
     if (work_bytes < L.total) return fail("work area of %zu bytes is smaller than the plan's %zu", work_bytes, L.total);
     uint8_t *w = (uint8_t *)work;
     if (fill_plan(images, n, params, wpb, own, L, w) != 0) return -1;
-    struct j2p_je_img *imgs = (struct j2p_je_img *)(w + L.off_imgs);
+    const struct j2p_je_img *imgs = (const struct j2p_je_img *)(w + L.off_imgs);
+    struct j2p_je_img *strs = (struct j2p_je_img *)(w + L.off_strs);
     const struct j2p_je_tables *t = (const struct j2p_je_tables *)(w + L.off_tab);
     uint32_t *tsum = (uint32_t *)(w + L.off_tsum), *intra = (uint32_t *)(w + L.off_intra), *ffc = (uint32_t *)(w + L.off_ffc);
     uint64_t *toff = (uint64_t *)(w + L.off_toff), *ffpre = (uint64_t *)(w + L.off_ffpre);
@@ -321,36 +454,36 @@ static int encode_host_steps(const struct j2p_jpegenc_image *images, unsigned n,
     uint8_t *out = w + L.off_out;
     memset(w + L.off_hist, 0, L.off_raw - L.off_hist + L.words * sizeof(uint32_t));
     for (unsigned i = 0; i < n; i++) host_blocks(&imgs[i], t, coef);   // blocks
-    const auto c = codes(L, w, (const struct j2p_je_img *)imgs, t, (const int16_t *)coef);
-    for (unsigned i = 0; i < n; i++) {                                  // sizes and scans
-        struct j2p_je_img *im = &imgs[i];
+    const auto c = codes(L, w, imgs, (const struct j2p_je_img *)strs, t, (const int16_t *)coef);
+    for (uint32_t s = 0; s < L.ns; s++) {                               // sizes and scans
+        struct j2p_je_img *im = &strs[s];
         uint64_t bits = 0;
         for (uint32_t k = 0; k < im->ntiles; k++) {
-            uint32_t s = 0;
+            uint32_t sum = 0;
             for (uint64_t b = (uint64_t)k * J2P_JE_TILE; b < im->nblk && b < (uint64_t)(k + 1) * J2P_JE_TILE; b++) {
-                intra[im->blk0 + b] = s;
-                s += j2p_je_block_bits(coef + (im->blk0 + b) * 64, pred_of(t, coef, im->blk0, b), c.huff(i), comp_of(t, b));
+                intra[im->blk0 + b] = sum;
+                sum += j2p_je_block_bits(coef + (im->blk0 + b) * 64, pred_of(t, coef, im->blk0, b), c.huff(im->img), comp_of(t, b));
             }
-            tsum[im->tile0 + k] = s;
+            tsum[im->tile0 + k] = sum;
             toff[im->tile0 + k] = bits;
-            bits += s;
+            bits += sum;
         }
         im->bits = bits;
         uint64_t pw;
         const uint32_t mask = j2p_je_pad(bits, &pw);
         raw[im->raw_off + pw] |= mask;
     }
-    for (unsigned i = 0; i < n; i++) {                                  // emit
-        const struct j2p_je_img *im = &imgs[i];
+    for (uint32_t s = 0; s < L.ns; s++) {                               // emit
+        const struct j2p_je_img *im = &strs[s];
         for (uint64_t b = 0; b < im->nblk; b++) {
             const uint64_t pos = toff[im->tile0 + b / J2P_JE_TILE] + intra[im->blk0 + b];
-            j2p_je_emit(coef + (im->blk0 + b) * 64, pred_of(t, coef, im->blk0, b), c.huff(i), comp_of(t, b), pos,
+            j2p_je_emit(coef + (im->blk0 + b) * 64, pred_of(t, coef, im->blk0, b), c.huff(im->img), comp_of(t, b), pos,
                         [&](uint64_t k, uint32_t v) { raw[im->raw_off + k] |= v; });
         }
     }
-    uint64_t ff = 0, off = 0;                                           // 0xFF counts, file offsets
-    for (unsigned i = 0; i < n; i++) {
-        struct j2p_je_img *im = &imgs[i];
+    uint64_t ff = 0, off = 0;                                           // 0xFF counts, stream and file offsets
+    for (uint32_t s = 0; s < L.ns; s++) {
+        struct j2p_je_img *im = &strs[s];
         const uint32_t *rw = raw + im->raw_off;
         const uint64_t nbytes = raw_bytes(im);
         for (uint32_t k = 0; k < im->nchunks; k++) {
@@ -361,25 +494,27 @@ static int encode_host_steps(const struct j2p_jpegenc_image *images, unsigned n,
             ff += cnt;
         }
         const uint64_t ffi = ff - ffpre[im->chunk0];
-        im->file_len = c.head_len(i) + nbytes + ffi + 2;
+        im->file_len = c.head_len(im) + nbytes + ffi + (j2p_je_ends_file(strs, L.ns, s) ? 2 : 0);
         im->file_off = off;
-        offsets[i] = off;
+        if (s == 0 || strs[s - 1].img != im->img) offsets[im->img] = off;
         off += im->file_len;
     }
     ffpre[L.nchunks] = ff;
     offsets[n] = off;
-    for (unsigned i = 0; i < n; i++) {                                  // files
-        const struct j2p_je_img *im = &imgs[i];
+    for (uint32_t s = 0; s < L.ns; s++) {                               // files
+        const struct j2p_je_img *im = &strs[s];
         uint8_t *o = out + im->file_off;
-        for (uint32_t k = 0; k < c.head_len(i); k++) *o++ = c.head_byte(i, im, k);
+        for (uint32_t k = 0; k < c.head_len(im); k++) *o++ = c.head_byte(im, k);
         const uint32_t *rw = raw + im->raw_off;
         for (uint64_t j = 0; j < raw_bytes(im); j++) {
             const uint8_t v = j2p_je_byte(rw, j);
             *o++ = v;
             if (v == 0xff) *o++ = 0;
         }
-        *o++ = 0xff;
-        *o++ = 0xd9;
+        if (j2p_je_ends_file(strs, L.ns, s)) {
+            *o++ = 0xff;
+            *o++ = 0xd9;
+        }
     }
     return 0;
 }

@@ -208,4 +208,11 @@ J2P_HD uint8_t j2p_jo_head_byte(const struct j2p_je_tables *t, const struct j2p_
         return t->head[J2P_JE_HEAD - J2P_JO_SOS + k];
 }
 
+// an image's file header: j2p_jo_head_byte with the image's DRI before the SOS when it has restarts
+J2P_HD uint32_t j2p_jo_file_head_len(const struct j2p_je_img *im, const struct j2p_jo_dht *d) { return j2p_jo_head_len(d) + (im->ri ? J2P_JE_DRI : 0); }
+
+J2P_HD uint8_t j2p_jo_file_head_byte(const struct j2p_je_tables *t, const struct j2p_je_img *im, const struct j2p_jo_dht *d, uint32_t k) {
+        return j2p_je_dri_head(im->ri, j2p_jo_head_len(d), J2P_JO_SOS, k, [&](uint32_t k1) { return j2p_jo_head_byte(t, im, d, k1); });
+}
+
 #endif  // J2P_JPEGOPT_CORE_H

@@ -9,7 +9,7 @@
  * scan script and the coding rules are in jpegprog_core.h.
  *
  * The images, parameters and statistics are jpegenc.h's structs, and the calls mirror its calls.
- * Every (image, scan) pair is its own bit stream.  One call queues a memset and
+ * Every (image, scan) pair, or every restart interval of it, is its own bit stream.  One call queues a memset and
  * J2P_JPEGPROG_LAUNCHES kernels, whatever the number and sizes of the images: blocks (and each AC
  * scan's block summaries), runs (the EOB-run state each block of an AC scan receives), hist (symbol
  * counts per image and table), tables (ten per image, and each stream's DHT and SOS header), sizes,
@@ -19,6 +19,14 @@
  * Work-area bound: a block of the AC first scan over 63 coefficients costs at most 63 x (16 + 10)
  * bits and one EOB-run emission of 16 + 14, J2P_JPEGPROG_BLOCK_BITS = 1668; every other scan's bound
  * is smaller (jpegprog_core.h), and each stream gets its own.
+ *
+ * Restart markers (jpegenc.h's restart fields): each scan gets the interval libjpeg gives it, in that
+ * scan's MCUs (an MCU of a non-interleaved AC scan is one block of its component's own grid), and
+ * its DRI, before the SOS, when the interval differs from the last DRI of the file.  Every (image,
+ * scan, interval) is then its own bit stream: the EOB run and its correction bits are flushed at the
+ * interval's end, and DC predictions, the run and BE restart at 0.  The per-block bounds still hold,
+ * because an interval's last EOB-run emission covers at least one of its blocks; an interval adds at
+ * most 7 pad bits and the 2 unstuffed bytes of its RST.  Scan headers stay per (image, scan).
  */
 #ifndef J2P_JPEGPROG_H
 #define J2P_JPEGPROG_H

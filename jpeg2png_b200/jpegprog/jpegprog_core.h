@@ -23,7 +23,8 @@
 //   DC first   the difference of successive shifted DCs of a component, coded as in a baseline scan;
 //   DC refine  one raw bit per block, (DC >> Al) & 1;
 //   AC first   a block ending in zeros adds one to the pending EOB run; the run is emitted before the
-//              next symbol, when it reaches 0x7FFF and at the end of the scan, as the symbol n << 4
+//              next symbol, when it reaches 0x7FFF and at the end of the scan or of a restart
+//              interval (the stream's last block, `last`), as the symbol n << 4
 //              (n = floor(log2 run)) and the run's low n bits;
 //   AC refine  a coefficient of shifted magnitude 1 is new: (r << 4) | 1, its sign, then the
 //              correction bits (magnitude & 1 of the already nonzero coefficients) buffered since
@@ -32,7 +33,7 @@
 //              coefficient the block adds one to the EOB run and its correction bits to the run's
 //              buffer, BE; the run and BE go out before the next emission of a block, when the run
 //              reaches 0x7FFF, when BE exceeds 937 (libjpeg's 1000-bit buffer less 63) and at the
-//              end of the scan.
+//              end of the scan or of a restart interval.
 //
 // A block of an AC scan takes the run state (EOB run, BE) left by the block before it.  A block with
 // a nonzero coefficient (AC first) or a new one (AC refine) emits the incoming state before anything
@@ -46,8 +47,8 @@
 
 #define J2P_JP_SCANS 10u                // scans, and so bit streams, per image
 #define J2P_JP_TABLES 10u               // Huffman tables per image
-#define J2P_JP_HEAD 752u                // room for a stream's header: SOI .. SOF2, two DHTs, SOS
-static_assert(J2P_JP_HEAD >= J2P_JO_HEAD_PRE + 2 * (21 + 256) + 14 && J2P_JP_HEAD % 16 == 0, "a stream's header fits");
+#define J2P_JP_HEAD 752u                // room for a scan's header: SOI .. SOF2, two DHTs, DRI, SOS
+static_assert(J2P_JP_HEAD >= J2P_JO_HEAD_PRE + 2 * (21 + 256) + J2P_JE_DRI + 14 && J2P_JP_HEAD % 16 == 0, "a scan's header fits");
 #define J2P_JP_MAX_RUN 0x7fffu          // the longest EOB run
 #define J2P_JP_MAX_BE 937u              // correction bits an EOB run may buffer before it is emitted
 #define J2P_JP_RESET 0x80u              // summary: the block emits the incoming state and sets its own
@@ -65,6 +66,13 @@ static_assert(J2P_JP_HEAD >= J2P_JO_HEAD_PRE + 2 * (21 + 256) + 14 && J2P_JP_HEA
 static_assert(J2P_JP_AC_FIRST_BITS(63u) == J2P_JPEGPROG_BLOCK_BITS && J2P_JP_AC_REFINE_BITS(63u) < J2P_JPEGPROG_BLOCK_BITS &&
                   J2P_JP_DC_FIRST_BITS < J2P_JPEGPROG_BLOCK_BITS,
               "J2P_JPEGPROG_BLOCK_BITS is the worst scan's bound");
+// With restart intervals each interval is a stream of its own, and its bound is still per block: its
+// last EOB-run emission covers at least one of its blocks.  The byte padding at the interval's end
+// costs no room: a stream of nb blocks gets nb x j2p_jp_bound_words(k) whole words, a multiple of 8
+// bits that its coded bits never exceed, so rounding them up to a byte stays inside it, even where
+// the bound fills its words exactly (scan 1: J2P_JP_AC_FIRST_BITS(5) is 160 bits, 5 words).  The RST
+// is the stream's 2-byte header, counted in the output outside its words.
+static_assert(J2P_JP_AC_FIRST_BITS(5u) == 5u * 32u && 32u % 8u == 0u, "a bound in whole words is whole bytes: padding stays inside it");
 
 struct j2p_jp_scan {
         uint32_t comp;                  // 0 Y, 1 Cb, 2 Cr; 3 all three, interleaved
@@ -220,7 +228,7 @@ J2P_HD void j2p_jp_eobrun(Out &o, uint32_t run, uint32_t be, uint64_t first) {
 }
 
 // Block j of scan s, coefficients c (zig-zag), of component comp, with the DC prediction pred (DC
-// first) or the incoming run state st (AC scans); last: the scan's last block.
+// first) or the incoming run state st (AC scans); last: the last block of the scan or restart interval.
 #ifdef __CUDACC__
 #pragma nv_exec_check_disable
 #endif
@@ -330,7 +338,7 @@ J2P_HD uint32_t j2p_jp_dht_len(const struct j2p_jp_dht *d, uint32_t tb) { return
 
 J2P_HD uint32_t j2p_jp_sos_len(uint32_t k) { return j2p_jp_scan_of(k).comp == 3 ? 14 : 10; }
 
-// the header of scan k's stream: SOI .. SOF2 before scan 0, the DHTs of its tables, its SOS
+// the header of scan k: SOI .. SOF2 before scan 0, the DHTs of its tables, its SOS (without DRI)
 J2P_HD uint32_t j2p_jp_head_len(const struct j2p_jp_dht *d, uint32_t k) {
         if (k == 0) return J2P_JO_HEAD_PRE + j2p_jp_dht_len(d, 0) + j2p_jp_dht_len(d, 1) + j2p_jp_sos_len(0);
         return (k == 6 ? 0 : j2p_jp_dht_len(d, j2p_jp_slot(k))) + j2p_jp_sos_len(k);
@@ -379,6 +387,14 @@ J2P_HD uint8_t j2p_jp_head_byte(const struct j2p_je_tables *t, const struct j2p_
                 b -= j2p_jp_dht_len(d, tb);
         }
         return j2p_jp_sos_byte(k, b);
+}
+
+// scan k's header with DRI for dri (0: none) before its SOS
+J2P_HD uint32_t j2p_jp_scan_head_len(const struct j2p_jp_dht *d, uint32_t k, uint32_t dri) { return j2p_jp_head_len(d, k) + (dri ? J2P_JE_DRI : 0); }
+
+J2P_HD uint8_t j2p_jp_scan_head_byte(const struct j2p_je_tables *t, const struct j2p_je_img *im, const struct j2p_jp_dht *d, uint32_t k,
+                                     uint32_t dri, uint32_t b) {
+        return j2p_je_dri_head(dri, j2p_jp_head_len(d, k), j2p_jp_sos_len(k), b, [&](uint32_t b1) { return j2p_jp_head_byte(t, im, d, k, b1); });
 }
 
 #endif  // J2P_JPEGPROG_CORE_H

@@ -28,6 +28,11 @@ Under "progressive_workloads", the same figures for encode_jpeg(..., progressive
 (libj2pjpegprog.so, ten kernels) against Pillow with progressive=True, on (a) at q90 4:2:0 and q95
 4:4:4, (b) at q75 4:2:0, (c), and one flat 7680x4320 image at q90 4:2:0 (every AC scan one EOB-run
 segment, walked by one thread of k_jp_runs).  --progressive-only measures only these.
+Under "restart_workloads" (last in the full run), for each of the three encoders on (a) at q90 4:2:0: restart_marker_rows=1
+(the encoder call against the same mode without restarts, and encode_jpeg against Pillow with the
+same options), and restart_marker_blocks=1, one stream per MCU, the worst case (the encoder call
+alone); and the flat 7680x4320 image, progressive, restart_marker_rows=1, against the same without
+restarts.  --restart-only measures only these.
 Wall-clock figures are the best of R after one warm-up.  Also the card's name and power limit
 (read-only nvidia-smi query in the same run).  Writes nothing.
 """
@@ -59,34 +64,35 @@ KERNELS_PROG = ('k_jp_blocks', 'k_jp_runs', 'k_jp_hist', 'k_jp_tables', 'k_jp_si
                 'k_jp_offsets', 'k_jp_stuff')
 
 
-def jpeg_encoder_ms(tensors, quality, subsampling, calls, optimize=False, progressive=False):
+def jpeg_encoder_ms(tensors, quality, subsampling, calls, optimize=False, progressive=False, **restart):
     """encoder_ms of one j2p_jpegenc_encode (or j2p_jpegopt_encode, j2p_jpegprog_encode) call on all
-    images, and the size of its work area."""
-    call, work_bytes = encoder_call(J.codec(J.params(quality, subsampling), optimize, progressive), tensors)
+    images, and the size of its work area; restart: the restart keywords."""
+    call, work_bytes = encoder_call(J.codec(J.params(quality, subsampling, **restart), optimize, progressive), tensors)
     out = encoder_ms(call, KERNELS_PROG if progressive else KERNELS_OPT if optimize else KERNELS, calls)
     return {'ms_per_call': out['ms_per_call'], 'work_bytes': work_bytes, 'kernel_ms_per_call': out['kernel_ms_per_call']}
 
 
-def pillow(hwc, quality, subsampling, optimize=False, progressive=False):
+def pillow(hwc, quality, subsampling, optimize=False, progressive=False, restart=(0, 0)):
     buf = io.BytesIO()
     if optimize or progressive:     # libjpeg cannot suspend in a multi-pass file's last pass: room for the whole file
         ImageFile.MAXBLOCK = max(ImageFile.MAXBLOCK, 4 * hwc.shape[0] * hwc.shape[1] * 3 + 65536)
-    Image.fromarray(hwc, 'RGB').save(buf, 'JPEG', quality=quality, subsampling=subsampling, optimize=optimize, progressive=progressive)
+    kw = dict(restart_marker_blocks=restart[0], restart_marker_rows=restart[1]) if any(restart) else {}
+    Image.fromarray(hwc, 'RGB').save(buf, 'JPEG', quality=quality, subsampling=subsampling, optimize=optimize, progressive=progressive, **kw)
     return buf.getvalue()
 
 
 _shm = {}
 
 
-def _pillow_shared(name, size, offset, h, w, quality, subsampling, optimize=False, progressive=False):
+def _pillow_shared(name, size, offset, h, w, quality, subsampling, optimize=False, progressive=False, restart=(0, 0)):
     """In a worker process: Pillow on image (h, w, 3) at `offset` of the shared buffer `name`."""
     if name not in _shm:
         _shm[name] = shared_memory.SharedMemory(name=name)
     hwc = np.ndarray((h, w, 3), np.uint8, buffer=_shm[name].buf[:size], offset=offset)
-    return pillow(hwc, quality, subsampling, optimize, progressive)
+    return pillow(hwc, quality, subsampling, optimize, progressive, restart)
 
 
-def host_arm(tensors, quality, subsampling, reps, procs, optimize=False, progressive=False):
+def host_arm(tensors, quality, subsampling, reps, procs, optimize=False, progressive=False, restart=(0, 0)):
     """Best-of-`reps` seconds and files of the host arm (copies, then Pillow in `procs` worker
     processes), and apart the copies alone and Pillow on the first image in this process."""
     shapes = [(t.shape[1], t.shape[2]) for t in tensors]
@@ -107,10 +113,11 @@ def host_arm(tensors, quality, subsampling, reps, procs, optimize=False, progres
                 copies()
                 return list(pool.map(_pillow_shared, [shm.name] * len(shapes), [offs[-1]] * len(shapes), offs[:-1],
                                      [h for h, _ in shapes], [w for _, w in shapes], [quality] * len(shapes),
-                                     [subsampling] * len(shapes), [optimize] * len(shapes), [progressive] * len(shapes)))
+                                     [subsampling] * len(shapes), [optimize] * len(shapes), [progressive] * len(shapes),
+                                     [restart] * len(shapes)))
             t_host, host_files = best_of(arm, reps)
         t_copy, _ = best_of(copies, reps)
-        t_one, _ = best_of(lambda: pillow(views[0].numpy(), quality, subsampling, optimize, progressive), reps)
+        t_one, _ = best_of(lambda: pillow(views[0].numpy(), quality, subsampling, optimize, progressive, restart), reps)
         del buf, views
     finally:
         shm.close()
@@ -170,6 +177,38 @@ def run_progressive(tensors, label, quality, subsampling, reps, calls, threads):
     return out
 
 
+def run_restart(tensors, label, quality, subsampling, mode, restart, reps, calls, threads, host=True):
+    """For one encoder (mode: {} or optimize= or progressive=) and the restart keywords: the encoder
+    call with and without them and, with host, encode_jpeg against Pillow with the same options."""
+    out = {'workload': label, 'images': len(tensors), 'quality': quality, 'subsampling': subsampling, **mode, **restart}
+    out['encoder'] = jpeg_encoder_ms(tensors, quality, subsampling, calls, **mode, **restart)
+    out['encoder_without_restarts'] = jpeg_encoder_ms(tensors, quality, subsampling, calls, **mode)
+    if not host:
+        return out
+    t_gpu, files = best_of(lambda: encode_jpeg(tensors, quality=quality, subsampling=subsampling, **mode, **restart), reps)
+    t_host, host_files, t_copy, t_one = host_arm(tensors, quality, subsampling, reps, threads, mode.get('optimize', False),
+                                                 mode.get('progressive', False),
+                                                 (restart.get('restart_marker_blocks', 0), restart.get('restart_marker_rows', 0)))
+    out['encode_jpeg'] = {'wall_ms': t_gpu * 1e3, 'ms_per_image': t_gpu / len(tensors) * 1e3, 'total_bytes': sum(map(len, files))}
+    out['host_pillow'] = {'wall_ms': t_host * 1e3, 'ms_per_image': t_host / len(tensors) * 1e3, 'processes': threads,
+                          'copies_alone_ms': t_copy * 1e3, 'one_image_one_thread_ms': t_one * 1e3}
+    out['speedup_vs_host'] = t_host / t_gpu
+    out['identical_to_host'] = files == host_files
+    return out
+
+
+def restart_workloads(big, flat8k, n, args, threads):
+    """The restart figures: each encoder on (a) at q90 4:2:0 with one interval per MCU row (against
+    Pillow too) and per MCU, and the flat 8K image, progressive, one interval per MCU row."""
+    out, label = [], f'{n} x 1920x1080 Q75 4:2:0, -i 100'
+    for mode in ({}, {'optimize': True}, {'progressive': True}):
+        out.append(run_restart(big, label, 90, '4:2:0', mode, {'restart_marker_rows': 1}, args.reps, args.calls, threads))
+        out.append(run_restart(big, label, 90, '4:2:0', mode, {'restart_marker_blocks': 1}, args.reps, args.calls, threads, host=False))
+    out.append(run_restart([flat8k], '1 x 7680x4320 flat', 90, '4:2:0', {'progressive': True}, {'restart_marker_rows': 1}, args.reps, args.calls,
+                           threads, host=False))
+    return out
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--device', type=int, default=0)
@@ -177,6 +216,7 @@ def main():
     ap.add_argument('--reps', type=int, default=3)
     ap.add_argument('--calls', type=int, default=20)
     ap.add_argument('--progressive-only', action='store_true')
+    ap.add_argument('--restart-only', action='store_true')
     args = ap.parse_args()
     if abi.load_product().j2p_device_count() <= 0 or not torch.cuda.is_available():
         raise SystemExit('jpegenc_bench.py: no CUDA device')
@@ -190,6 +230,10 @@ def main():
     img8k = torch.from_numpy(synth.cartoon_image(7680, 4320, 9).round().astype(np.uint8).transpose(2, 0, 1).copy()).cuda()
     flat8k = torch.full((3, 4320, 7680), 77, dtype=torch.uint8, device='cuda')
     torch.cuda.synchronize()
+    if args.restart_only:
+        line['restart_workloads'] = restart_workloads(big, flat8k, n, args, threads)
+        print(json.dumps(line), flush=True)
+        return
     line['progressive_workloads'] = []
     for tensors, label, cases in ((big, f'{n} x 1920x1080 Q75 4:2:0, -i 100', ((90, '4:2:0'), (95, '4:4:4'))),
                                   (small, f'{n} x 256x256 Q10 4:2:0, -i 50', ((75, '4:2:0'),)),
@@ -212,6 +256,7 @@ def main():
                                   ([img8k], '1 x 7680x4320 cartoon', ((90, '4:2:0'),))):
         for q, s in cases:
             line['optimize_workloads'].append(run_optimized(tensors, label, q, s, args.reps, args.calls, threads))
+    line['restart_workloads'] = restart_workloads(big, flat8k, n, args, threads)
     print(json.dumps(line), flush=True)
 
 
