@@ -1,6 +1,6 @@
 /* Host restatement of the shared-reciprocal division of jpeg2png_b200/csrc/numerics.cuh
  * (qdiv_core and qdiv4_core + their guard), checked against IEEE float division on this CPU.  The GPU-side twin is
- * tools/divcheck.cu; this one runs in the CPU suite and pins the ALGORITHM (Markstein's sequence
+ * tests/test_gpu_device_arith.py; this one runs in the CPU suite and pins the ALGORITHM (Markstein's sequence
  * with y = RN(1/b)) independently of any GPU.  fmaf() is the correctly rounded fused multiply-add
  * of C99; the file is compiled with -ffp-contract=off so nothing else is fused. */
 #include <math.h>

@@ -44,50 +44,15 @@ def test_host_driver_equals_pillow_optimize(quality, subsampling):
                         f'byte {k} ({JC.turbo_version()})')
 
 
-def _fib(n):
-    a, b, out = 1, 1, []
-    for _ in range(n):
-        out.append(a)
-        a, b = b, a + b
-    return out
-
-
-def _crafted():
-    """name -> 256 counts."""
-    rng = np.random.default_rng(11)
-    out = {}
-    for m in (20, 24, 30, 36, 40):                      # Fibonacci: K.2 lengths past 16 from 36 symbols
-        c = [0] * 256
-        for k, f in enumerate(_fib(m)):
-            c[(k * 37 + 5) % 256] = f
-        out[f'fibonacci{m}'] = c
-    out['one symbol'] = [0] * 255 + [9]
-    out['one symbol at 0'] = [1] + [0] * 255
-    out['two symbols'] = [0] * 17 + [3] + [0] * 100 + [3] + [0] * 137
-    out['256 equal'] = [5] * 256
-    out['ties at several levels'] = [(k % 3 + 1) * (1 + (k % 7 == 0)) for k in range(256)]
-    out['powers of two'] = [1 << (k % 20) for k in range(256)]
-    out['above 2^32'] = [int(v) for v in rng.integers(1 << 32, 1 << 40, 256)]
-    out['above 2^32 and small'] = [int(v) if k % 5 else 1 for k, v in enumerate(rng.integers(1 << 32, 1 << 36, 256))]
-    for s in range(4):
-        c = rng.integers(0, 50, 256) * (rng.random(256) < 0.4)
-        c[s] += 1
-        out[f'sparse random {s}'] = [int(v) for v in c]
-    return out
-
-
-LONG = ('fibonacci36', 'fibonacci40', 'powers of two', 'above 2^32 and small')
-
-
-@pytest.mark.parametrize('name', list(_crafted()))
+@pytest.mark.parametrize('name', list(OC.crafted()))
 def test_table_builder_equals_restatement(name):
-    counts = _crafted()[name]
+    counts = OC.crafted()[name]
     bits, vals = J.build_table(counts)
     want_bits, want_vals, longest = OC.restated_table(counts)
     assert (bits, vals) == (want_bits, want_vals)
     assert sorted(vals) == [k for k in range(256) if counts[k]]
     assert sum(bits) == len(vals)
-    if name in LONG:
+    if name in OC.LONG:
         assert longest > 16                             # the K.3 limit did the work
 
 

@@ -1,5 +1,6 @@
 """The exact shared-reciprocal division of numerics.cuh, restated for the host and checked against
-IEEE division on the CPU (tests/qdiv_check.c); the exhaustive GPU-side check is tools/divcheck.cu."""
+IEEE division on the CPU (tests/qdiv_check.c); tests/test_gpu_device_arith.py checks the device
+sequences themselves on the GPU."""
 import os
 import subprocess
 
