@@ -285,6 +285,13 @@ int j2p_session_export(j2p_session *s, unsigned frame0, unsigned nframes,
 int j2p_session_export_separate(j2p_session *y, j2p_session *cb, j2p_session *cr, unsigned frame0,
                                 unsigned nframes, const struct j2p_image_out *o, void *dst,
                                 void *stream);
+/* gray: one sample per pixel from plane 0 alone, x = clamp(float((double)(Y + 128))), which is the
+ * R (= G = B) sample of the RGB export for that luma with zero chroma; the same sample types, and
+ * HWC and CHW are the same bytes ((h, w, 1) or (1, h, w)).  `s`: a whole-frame session with one
+ * plane (a gray file, or a separate-mode luma session) or three (joint mode: its luma).  Streams
+ * and refusals as j2p_session_export, the refusal of nchannel being "not 1 or 3". */
+int j2p_session_export_gray(j2p_session *s, unsigned frame0, unsigned nframes,
+                            const struct j2p_image_out *o, void *dst, void *stream);
 
 /* Objective terms of the most recent iteration, as logged by the reference (compute.c:271-272):
  * out[0]=objective, out[1]=prob_dist, out[2]=tv, out[3]=tv2.  Only tracked when logging was

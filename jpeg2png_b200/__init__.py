@@ -1,5 +1,6 @@
 """jpeg2png_b200: the jpeg2png solver on H100.  `decode_jpeg` (jpeg2png_b200.decode) turns JPEG files
-into CUDA tensors, `encode_png` (jpeg2png_b200.encode) and `encode_jpeg` (jpeg2png_b200.jpeg_encode)
+into CUDA tensors (RGB, or one channel for grayscale files and `mode='GRAY'`), `encode_png`
+(jpeg2png_b200.encode, RGB or gray) and `encode_jpeg` (jpeg2png_b200.jpeg_encode, RGB)
 turn such tensors into PNG or JPEG files on the device (`encode_jpeg(..., optimize=True)` with
 per-image optimized Huffman tables, as Pillow's `optimize=True`, and `encode_jpeg(...,
 progressive=True)` with Pillow's progressive files); torch is imported only when one of

@@ -20,13 +20,16 @@ class Codec:
 
     image: the ctypes image struct (data, width, height and row, column and channel strides);
     check_size(shape, h, w): raises ValueError for a size the encoder refuses;
-    fill(d, x): sets the struct's other fields from the array or tensor x, if it has any."""
+    fill(d, x, channels): sets the struct's other fields from the array or tensor x and its channel
+    count, if it has any;
+    channels: the channel counts the encoder accepts, in the order its messages name them."""
     name: str
     load: Callable[[], C.CDLL]
     image: type
     check_size: Callable
     fill: Callable | None = None
     params: tuple = ()
+    channels: tuple = (3,)
 
     def call(self, fn, descs, *args, error=RuntimeError):
         """j2p_<name>_<fn>(descs, len(descs), *params, *args); `error` with the library's message
@@ -48,16 +51,19 @@ def check_layout(layout):
         raise ValueError(f"layout must be 'CHW' or 'HWC', not {layout!r}")
 
 
-def axes(shape, layout):
-    """(h, w, row axis, column axis, channel axis) of a (3, h, w) CHW or (h, w, 3) HWC shape."""
+def axes(shape, layout, channels=(3,)):
+    """(h, w, row axis, column axis, channel axis) of a (c, h, w) CHW or (h, w, c) HWC shape, c one
+    of `channels`."""
     if len(shape) != 3:
         raise ValueError(f'an image is 3-dimensional, (3, h, w) or (h, w, 3); got shape {tuple(shape)}')
     if layout == 'CHW':
-        if shape[0] != 3:
-            raise ValueError(f"layout 'CHW' wants shape (3, h, w); got {tuple(shape)}")
+        if shape[0] not in channels:
+            wanted = ' or '.join(f'({c}, h, w)' for c in channels)
+            raise ValueError(f"layout 'CHW' wants shape {wanted}; got {tuple(shape)}")
         return shape[1], shape[2], 1, 2, 0
-    if shape[2] != 3:
-        raise ValueError(f"layout 'HWC' wants shape (h, w, 3); got {tuple(shape)}")
+    if shape[2] not in channels:
+        wanted = ' or '.join(f'(h, w, {c})' for c in channels)
+        raise ValueError(f"layout 'HWC' wants shape {wanted}; got {tuple(shape)}")
     return shape[0], shape[1], 0, 1, 2
 
 
@@ -66,13 +72,13 @@ def descs(codec, items, layout, ptr=lambda x: x.data_ptr(), strides=lambda x: x.
     whose address and strides in elements ptr(x) and strides(x) give."""
     out = (codec.image * len(items))()
     for d, x in zip(out, items):
-        h, w, ra, ca, ka = axes(x.shape, layout)
+        h, w, ra, ca, ka = axes(x.shape, layout, codec.channels)
         codec.check_size(x.shape, h, w)
         st = strides(x)
         d.data, d.width, d.height = ptr(x), w, h
         d.row_stride, d.col_stride, d.chan_stride = st[ra], st[ca], st[ka]
         if codec.fill:
-            codec.fill(d, x)
+            codec.fill(d, x, x.shape[ka])
     return out
 
 
@@ -137,7 +143,7 @@ def encode_tensors(fn, codec, images, layout, dtypes):
             raise ValueError(f'{fn} takes torch tensors, not {type(x).__name__}')
         if x.dtype not in dtypes:
             raise ValueError(f'{fn} takes {" or ".join(map(str, dtypes))} tensors, not {x.dtype}')
-        h, w, *_ = axes(x.shape, layout)
+        h, w, *_ = axes(x.shape, layout, codec.channels)
         codec.check_size(x.shape, h, w)
         if x.device.type != 'cuda':
             raise ValueError(f'{fn} encodes CUDA tensors; this one is on {x.device}')

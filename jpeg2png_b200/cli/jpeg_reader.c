@@ -41,6 +41,7 @@ struct dec {
         struct huff dc[4], ac[4];
         struct comp c[3];
         int ncomp, progressive;
+        unsigned flags;                /* J2P_READ_* */
         unsigned W, H, maxh, maxv, mcux, mcuy;
         unsigned restart_interval;
         char *err;
@@ -375,11 +376,13 @@ static int parse_sof(struct dec *d, const uint8_t *s, unsigned len) {
         d->H = be16(s + 1);
         d->W = be16(s + 3);
         d->ncomp = s[5];
-        if (d->ncomp != 3) return fail(d, "only 3 component jpegs are supported");            /* jpeg.c:34 */
+        if (d->flags & J2P_READ_GRAY) {
+                if (d->ncomp != 1 && d->ncomp != 3) return fail(d, "only 1 and 3 component jpegs are supported");
+        } else if (d->ncomp != 3) return fail(d, "only 3 component jpegs are supported");    /* jpeg.c:34 */
         if (d->W == 0 || d->H == 0) return fail(d, "unsupported jpeg: empty image or DNL-defined height");
         if (len < 6 + 3u * d->ncomp) return fail(d, "corrupt jpeg: short SOF");
         d->maxh = d->maxv = 1;
-        for (int i = 0; i < 3; i++) {
+        for (int i = 0; i < d->ncomp; i++) {
                 struct comp *c = &d->c[i];
                 c->id = s[6 + 3 * i];
                 c->h = s[7 + 3 * i] >> 4;
@@ -391,7 +394,7 @@ static int parse_sof(struct dec *d, const uint8_t *s, unsigned len) {
         }
         d->mcux = (d->W + 8 * d->maxh - 1) / (8 * d->maxh);
         d->mcuy = (d->H + 8 * d->maxv - 1) / (8 * d->maxv);
-        for (int i = 0; i < 3; i++) {
+        for (int i = 0; i < d->ncomp; i++) {
                 struct comp *c = &d->c[i];
                 const unsigned cw = (d->W * c->h + d->maxh - 1) / d->maxh, ch = (d->H * c->v + d->maxv - 1) / d->maxv;   /* A.1.1 */
                 c->wb = (cw + 7) / 8;
@@ -446,7 +449,7 @@ static int read_markers(struct dec *d, const uint8_t *buf, size_t len) {
                         struct comp *sc[3];
                         for (int i = 0; i < ns; i++) {
                                 sc[i] = NULL;
-                                for (int k = 0; k < 3; k++) if (d->c[k].id == s[1 + 2 * i]) sc[i] = &d->c[k];
+                                for (int k = 0; k < d->ncomp; k++) if (d->c[k].id == s[1 + 2 * i]) sc[i] = &d->c[k];
                                 if (!sc[i]) { fail(d, "corrupt jpeg: scan names an unknown component"); break; }
                                 sc[i]->td = s[2 + 2 * i] >> 4;
                                 sc[i]->ta = s[2 + 2 * i] & 15;
@@ -491,7 +494,7 @@ static int read_markers(struct dec *d, const uint8_t *buf, size_t len) {
 
 /* the reference's checks of the frame (jpeg.c:40-64) and the planes' geometry and tables */
 static void check_planes(struct dec *d, struct coef *coefs) {
-        for (int i = 0; i < 3 && !d->failed; i++) {
+        for (int i = 0; i < d->ncomp && !d->failed; i++) {
                 struct comp *c = &d->c[i];
                 struct coef *o = &coefs[i];
                 if (!d->qt_present[c->tq]) { fail(d, "weird jpeg: no quant table pointer"); break; }          /* jpeg.c:40 */
@@ -509,10 +512,19 @@ static void check_planes(struct dec *d, struct coef *coefs) {
         }
 }
 
+/* Writes only the fields before ncomp (always 3 here), so callers that mirror the struct as it was
+ * before ncomp was appended (ctypes users of this entry point) stay within their buffer. */
 int j2p_read_jpeg_mem(const uint8_t *buf, size_t len, struct j2p_jpeg *out, char *err, size_t errlen) {
+        struct j2p_jpeg j;
+        const int rc = j2p_read_jpeg_mem_ex(buf, len, 0, &j, err, errlen);
+        memcpy(out, &j, offsetof(struct j2p_jpeg, ncomp));
+        return rc;
+}
+
+int j2p_read_jpeg_mem_ex(const uint8_t *buf, size_t len, unsigned flags, struct j2p_jpeg *out, char *err, size_t errlen) {
         struct dec *d = calloc(1, sizeof *d);
         if (!d) return -1;
-        d->p = buf; d->end = buf + len; d->err = err; d->errlen = errlen;
+        d->p = buf; d->end = buf + len; d->err = err; d->errlen = errlen; d->flags = flags;
         if (err && errlen) err[0] = 0;
         memset(out, 0, sizeof *out);
         read_markers(d, buf, len);
@@ -520,7 +532,8 @@ int j2p_read_jpeg_mem(const uint8_t *buf, size_t len, struct j2p_jpeg *out, char
         if (!d->failed) {
                 out->w = d->W;
                 out->h = d->H;
-                for (int i = 0; i < 3; i++) {
+                out->ncomp = (unsigned)d->ncomp;
+                for (int i = 0; i < d->ncomp; i++) {
                         struct comp *c = &d->c[i];
                         struct coef *o = &out->coefs[i];
                         o->data = malloc((size_t)o->w * o->h * sizeof(int16_t));
@@ -537,20 +550,25 @@ int j2p_read_jpeg_mem(const uint8_t *buf, size_t len, struct j2p_jpeg *out, char
 }
 
 int j2p_read_jpeg_layout(const uint8_t *buf, size_t len, struct j2p_jpeg_layout *out, char *err, size_t errlen) {
+        return j2p_read_jpeg_layout_ex(buf, len, 0, out, err, errlen);
+}
+
+int j2p_read_jpeg_layout_ex(const uint8_t *buf, size_t len, unsigned flags, struct j2p_jpeg_layout *out, char *err, size_t errlen) {
         struct dec *d = calloc(1, sizeof *d);
         if (!d) return -1;
-        d->p = buf; d->end = buf + len; d->err = err; d->errlen = errlen;
+        d->p = buf; d->end = buf + len; d->err = err; d->errlen = errlen; d->flags = flags;
         if (err && errlen) err[0] = 0;
         memset(out, 0, sizeof *out);
         d->lay = out;
         const int stopped = read_markers(d, buf, len);
         int decodable = !stopped && !d->failed;
-        for (int i = 0; i < 3 && decodable; i++) decodable = d->scans_of[i] == 1;
+        for (int i = 0; i < d->ncomp && decodable; i++) decodable = d->scans_of[i] == 1;
         if (decodable) {
                 check_planes(d, out->coefs);
                 out->w = d->W;
                 out->h = d->H;
-                for (int i = 0; i < 3; i++) { out->comp_h[i] = (unsigned)d->c[i].h; out->comp_v[i] = (unsigned)d->c[i].v; }
+                out->ncomp = (unsigned)d->ncomp;
+                for (int i = 0; i < d->ncomp; i++) { out->comp_h[i] = (unsigned)d->c[i].h; out->comp_v[i] = (unsigned)d->c[i].v; }
         }
         const int rc = d->failed ? -1 : 0;
         out->device_decodable = rc == 0 && decodable;
@@ -563,9 +581,14 @@ int j2p_read_jpeg_layout(const uint8_t *buf, size_t len, struct j2p_jpeg_layout 
 }
 
 int j2p_read_jpeg_prog_layout(const uint8_t *buf, size_t len, struct j2p_jpeg_prog_layout *out, char *err, size_t errlen) {
+        return j2p_read_jpeg_prog_layout_ex(buf, len, 0, out, err, errlen);
+}
+
+int j2p_read_jpeg_prog_layout_ex(const uint8_t *buf, size_t len, unsigned flags, struct j2p_jpeg_prog_layout *out, char *err,
+                                 size_t errlen) {
         struct dec *d = calloc(1, sizeof *d);
         if (!d) return -1;
-        d->p = buf; d->end = buf + len; d->err = err; d->errlen = errlen;
+        d->p = buf; d->end = buf + len; d->err = err; d->errlen = errlen; d->flags = flags;
         if (err && errlen) err[0] = 0;
         memset(out, 0, sizeof *out);
         d->play = out;
@@ -575,7 +598,8 @@ int j2p_read_jpeg_prog_layout(const uint8_t *buf, size_t len, struct j2p_jpeg_pr
                 check_planes(d, out->coefs);
                 out->w = d->W;
                 out->h = d->H;
-                for (int i = 0; i < 3; i++) { out->comp_h[i] = (unsigned)d->c[i].h; out->comp_v[i] = (unsigned)d->c[i].v; }
+                out->ncomp = (unsigned)d->ncomp;
+                for (int i = 0; i < d->ncomp; i++) { out->comp_h[i] = (unsigned)d->c[i].h; out->comp_v[i] = (unsigned)d->c[i].v; }
         }
         const int rc = d->failed ? -1 : 0;
         out->progressive_decodable = rc == 0 && decodable;

@@ -25,13 +25,23 @@
 struct j2p_jpeg {
         unsigned w, h;              /* image size in pixels */
         struct coef coefs[3];       /* data malloc'd (caller frees), fdata NULL */
+        unsigned ncomp;             /* 3, or 1 (J2P_READ_GRAY): coefs[1..2] empty (w = h = 0, data NULL) */
 };
 
 /* Returns 0 on success; on failure returns non-zero and writes a message into err (if non-NULL).
  * The messages for the reference's own rejections are the reference's (jpeg.c:34,43,60,63). */
 int j2p_read_jpeg_mem(const uint8_t *buf, size_t len, struct j2p_jpeg *out, char *err, size_t errlen);
 
+/* Flags of the _ex entry points; the plain ones pass 0.
+ * J2P_READ_GRAY: accept one-component (grayscale) files as well as three-component ones, and refuse
+ * every other count with "only 1 and 3 component jpegs are supported".  A gray file's plane is
+ * coefs[0] with w_samp = h_samp = 1 (whatever sampling factor its SOF gives it) and its scans are
+ * non-interleaved over the plane's real block grid; coefs[1..2] stay empty. */
+enum { J2P_READ_GRAY = 1u };
+int j2p_read_jpeg_mem_ex(const uint8_t *buf, size_t len, unsigned flags, struct j2p_jpeg *out, char *err, size_t errlen);
+
 /* ---- layout pass: the headers and the entropy-coded data of a file, without Huffman decoding ----
+ * (the _ex variant takes the J2P_READ_* flags of j2p_read_jpeg_mem_ex)
  *
  * j2p_read_jpeg_layout runs the marker loop and header checks of j2p_read_jpeg_mem (the same code)
  * and, instead of decoding each scan, cuts its entropy-coded data into segments, one per restart
@@ -40,8 +50,8 @@ int j2p_read_jpeg_mem(const uint8_t *buf, size_t len, struct j2p_jpeg *out, char
  * past its end read as zero.  The restart markers between segments are checked by the reader's own
  * restart rule, so "missing restart marker", "out of sequence" and "truncated" fail here as there.
  *
- * device_decodable: the file is sequential Huffman (SOF0/SOF1) and each of the three components is
- * in exactly one scan.  Only then are coefs (geometry and tables, data NULL), scans and segments
+ * device_decodable: the file is sequential Huffman (SOF0/SOF1) and each of its components is in
+ * exactly one scan.  Only then are coefs (geometry and tables, data NULL), scans and segments
  * filled; for every other file the pass stops as soon as that is known (a progressive SOF, a
  * component's second scan) and returns 0 with device_decodable = 0: such files are for
  * j2p_read_jpeg_mem.  A non-zero return means j2p_read_jpeg_mem rejects the file too (it may name an
@@ -74,8 +84,10 @@ struct j2p_jpeg_layout {
         struct j2p_jpeg_segment *seg;    /* malloc'd */
         uint8_t *data;                   /* malloc'd */
         size_t data_len;
+        unsigned ncomp;                  /* as struct j2p_jpeg; set when device_decodable */
 };
 int j2p_read_jpeg_layout(const uint8_t *buf, size_t len, struct j2p_jpeg_layout *out, char *err, size_t errlen);
+int j2p_read_jpeg_layout_ex(const uint8_t *buf, size_t len, unsigned flags, struct j2p_jpeg_layout *out, char *err, size_t errlen);
 void j2p_free_jpeg_layout(struct j2p_jpeg_layout *l);
 
 /* ---- progressive layout pass: every scan of a progressive file, cut as above ----
@@ -102,8 +114,11 @@ struct j2p_jpeg_prog_layout {
         struct j2p_jpeg_segment *seg;        /* malloc'd */
         uint8_t *data;                       /* malloc'd */
         size_t data_len;
+        unsigned ncomp;                      /* as struct j2p_jpeg; set when progressive_decodable */
 };
 int j2p_read_jpeg_prog_layout(const uint8_t *buf, size_t len, struct j2p_jpeg_prog_layout *out, char *err, size_t errlen);
+int j2p_read_jpeg_prog_layout_ex(const uint8_t *buf, size_t len, unsigned flags, struct j2p_jpeg_prog_layout *out, char *err,
+                                 size_t errlen);
 void j2p_free_jpeg_prog_layout(struct j2p_jpeg_prog_layout *l);
 
 #endif

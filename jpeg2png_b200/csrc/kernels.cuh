@@ -117,10 +117,12 @@ inline FrameDev frame_view(const FrameDev &F, int f) {
 // ---- the colour epilogue (kernels_epilogue.cu, k_scanlines): YCbCr planes of `nframes` frames ->
 // RGB in one of three output forms.  Each plane has its own base, row stride and frame stride, so
 // the three planes may come from one joint session or from three separate-mode sessions whose
-// frames differ in size.
+// frames differ in size.  With nc == 1 only the luma plane is read and each pixel is one sample:
+// the R (= G = B) sample of that luma with zero chroma.
 enum EpilogueMode { EP_SCANLINES = 0, EP_HWC = 1, EP_CHW = 2 };
 struct EpilogueArgs {
-    const float *plane[3];               // frame 0's Y, Cb, Cr (current iterates)
+    const float *plane[3];               // frame 0's Y, Cb, Cr (current iterates); Y alone when nc == 1
+    int nc;                              // samples per pixel: 3 (RGB) or 1 (gray)
     unsigned long long frame_stride[3];  // elements from one frame's plane to the next frame's
     int ld[3];                           // row stride of each plane, elements
     int w, h;                            // visible image, at most every plane's frame

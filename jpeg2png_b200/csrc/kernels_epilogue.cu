@@ -9,6 +9,9 @@
 //                 has to deflate it (3 or 6 bytes per pixel cross PCIe instead of 12)
 //   EP_HWC/EP_CHW interleaved or planar samples for a tensor: 8 bit = the 8-bit PNG sample,
 //                 16 bit = the 16-bit PNG sample in native byte order, 32 bit = the clamped float
+// With a.nc == 1 (gray export) only the luma is read and written: clamp(float(double(Y + 128))),
+// which is the RGB expression with zero chroma (1.402 * 0 and the other products are exact zeros,
+// and adding +0 to a double that is not -0 leaves it unchanged).  The branch is uniform per launch.
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -47,25 +50,33 @@ __global__ void __launch_bounds__(EP_NT) k_scanlines(const EpilogueArgs a) {
     __shared__ __align__(16) uint8_t sm[EP_NT * 12 + 16];               // + one word read past the end by store_bytes
     const int row = blockIdx.y, frame = blockIdx.z, x0 = blockIdx.x * EP_NT, tid = threadIdx.x;
     const int es = a.sample >> 3, npx = min(EP_NT, a.w - x0);           // bytes per sample, pixels of this CTA
+    const bool gray = a.nc == 1;
+    const int nc = gray ? 1 : 3;                                        // samples per pixel
     if (tid < npx) {
         const int px = x0 + tid;
         float v[3];
         {
             const float *Y = a.plane[0] + (size_t)frame * a.frame_stride[0] + (size_t)row * a.ld[0];
-            const float *Cb = a.plane[1] + (size_t)frame * a.frame_stride[1] + (size_t)row * a.ld[1];
-            const float *Cr = a.plane[2] + (size_t)frame * a.frame_stride[2] + (size_t)row * a.ld[2];
             const float yi = __fadd_rn(Y[px], 128.f);                                                     // jpeg2png.c:158
-            const double dy = (double)yi, dcb = (double)Cb[px], dcr = (double)Cr[px];
-            v[0] = clamp_sample(__dadd_rn(dy, __dmul_rn(1.402, dcr)));                                       // png.c:44
-            v[1] = clamp_sample(__dsub_rn(__dsub_rn(dy, __dmul_rn(0.34414, dcb)), __dmul_rn(0.71414, dcr))); // png.c:45
-            v[2] = clamp_sample(__dadd_rn(dy, __dmul_rn(1.772, dcb)));                                       // png.c:46
+            const double dy = (double)yi;
+            if (gray) {
+                v[0] = v[1] = v[2] = clamp_sample(dy);                                                       // png.c:44-46, zero chroma
+            } else {
+                const float *Cb = a.plane[1] + (size_t)frame * a.frame_stride[1] + (size_t)row * a.ld[1];
+                const float *Cr = a.plane[2] + (size_t)frame * a.frame_stride[2] + (size_t)row * a.ld[2];
+                const double dcb = (double)Cb[px], dcr = (double)Cr[px];
+                v[0] = clamp_sample(__dadd_rn(dy, __dmul_rn(1.402, dcr)));                                       // png.c:44
+                v[1] = clamp_sample(__dsub_rn(__dsub_rn(dy, __dmul_rn(0.34414, dcb)), __dmul_rn(0.71414, dcr))); // png.c:45
+                v[2] = clamp_sample(__dadd_rn(dy, __dmul_rn(1.772, dcb)));                                       // png.c:46
+            }
         }
         const float bitfactor = a.sample == 8 ? 1.0f : 256.0f;                                               // (1 << bits) / 256.
 #pragma unroll
         for (int k = 0; k < 3; k++) {
+            if (k >= nc) break;
             uint32_t s = a.sample == 32 ? __float_as_uint(v[k]) : __float2uint_rz(__fmul_rn(v[k], bitfactor));   // png.c:44-46 truncation
             if (a.mode == EP_SCANLINES && es == 2) s = ((s >> 8) & 0xffu) | ((s & 0xffu) << 8);                // png.c:58-60 big-endian
-            const int e = a.mode == EP_CHW ? k * EP_NT + tid : tid * 3 + k;                                   // staged element
+            const int e = a.mode == EP_CHW ? k * EP_NT + tid : tid * nc + k;                                  // staged element
             if (es == 1) sm[e] = (uint8_t)s;
             else if (es == 2) reinterpret_cast<uint16_t *>(sm)[e] = (uint16_t)s;
             else reinterpret_cast<uint32_t *>(sm)[e] = s;
@@ -75,13 +86,13 @@ __global__ void __launch_bounds__(EP_NT) k_scanlines(const EpilogueArgs a) {
     uint8_t *base = a.out + (size_t)frame * a.frame_bytes;
     if (a.mode == EP_CHW) {
         const size_t plane_bytes = (size_t)a.w * a.h * es, at = ((size_t)row * a.w + x0) * es;
-        for (int k = 0; k < 3; k++) store_bytes(base + k * plane_bytes + at, sm + k * EP_NT * es, npx * es, tid);
+        for (int k = 0; k < nc; k++) store_bytes(base + k * plane_bytes + at, sm + k * EP_NT * es, npx * es, tid);
         return;
     }
     const int filter = a.mode == EP_SCANLINES;                                                               // one filter byte per scanline
-    uint8_t *dst = base + (size_t)row * ((size_t)a.w * 3 * es + filter);
+    uint8_t *dst = base + (size_t)row * ((size_t)a.w * nc * es + filter);
     if (filter && x0 == 0 && tid == 0) dst[0] = 0;                                                           // PNG filter type 0 (None)
-    store_bytes(dst + filter + (size_t)x0 * 3 * es, sm, npx * 3 * es, tid);
+    store_bytes(dst + filter + (size_t)x0 * nc * es, sm, npx * nc * es, tid);
 }
 
 cudaError_t launch_scanlines(const EpilogueArgs &a, int nframes, cudaStream_t s) {

@@ -985,6 +985,7 @@ extern "C" int j2p_session_download_frame_scanlines(j2p_session *s, unsigned fra
     uint8_t *dev = nullptr;
     CK(dev_alloc(s, &dev, bytes));                   // returns to the device cache with the session
     EpilogueArgs a{};
+    a.nc = 3;
     for (int c = 0; c < 3; c++) {
         a.plane[c] = plane_x(s, frame * 3 + (unsigned)c);
         a.frame_stride[c] = s->F.frame_stride;
@@ -1003,9 +1004,10 @@ extern "C" int j2p_session_download_frame_scanlines(j2p_session *s, unsigned fra
 
 // ---- export into caller device memory: the colour epilogue with a tensor layout, on the caller's
 // stream, ordered after the solve that produced the planes and before anything later queued on a
-// session stream can overwrite them.  `ss`: one joint session, or the Y, Cb, Cr separate sessions.
-static int export_impl(j2p_session *const *ss, int nsess, unsigned frame0, unsigned nframes, const struct j2p_image_out *o, void *dst,
-                       void *stream) {
+// session stream can overwrite them.  `ss`: one joint session, or the Y, Cb, Cr separate sessions;
+// nout: samples per pixel, 3 (RGB) or 1 (gray: plane 0 of the one session ss[0] alone).
+static int export_impl(j2p_session *const *ss, int nsess, int nout, unsigned frame0, unsigned nframes, const struct j2p_image_out *o,
+                       void *dst, void *stream) {
     if (!o || !dst) return fail(J2P_ERR_ARG, "null argument");
     j2p_session *s0 = ss[0];
     if (nframes == 0) return fail(J2P_ERR_ARG, "nframes must be at least 1");
@@ -1015,15 +1017,16 @@ static int export_impl(j2p_session *const *ss, int nsess, unsigned frame0, unsig
     if (o->layout != J2P_LAYOUT_HWC && o->layout != J2P_LAYOUT_CHW) return fail(J2P_ERR_ARG, "unknown layout %u", o->layout);
     if (o->w == 0 || o->h == 0) return fail(J2P_ERR_ARG, "image %ux%u is empty", o->w, o->h);
     EpilogueArgs a{};
-    for (int c = 0; c < 3; c++) {
+    a.nc = nout;
+    for (int c = 0; c < nout; c++) {
         j2p_session *s = ss[nsess == 1 ? 0 : c];
         const int W = s->F.W, H = s->F.Hg;
         if (o->w > (unsigned)W || o->h > (unsigned)H) return fail(J2P_ERR_ARG, "image %ux%u does not fit the %dx%d frame of plane %d", o->w, o->h, W, H, c);
-        a.plane[c] = plane_x(s, nsess == 1 ? frame0 * 3 + (unsigned)c : frame0);
+        a.plane[c] = plane_x(s, nsess == 1 ? frame0 * (unsigned)s->F.nc + (unsigned)c : frame0);
         a.frame_stride[c] = s->F.frame_stride;
         a.ld[c] = W;
     }
-    const size_t image_bytes = (size_t)o->w * o->h * 3 * (o->sample / 8);
+    const size_t image_bytes = (size_t)o->w * o->h * (size_t)nout * (o->sample / 8);
     if (o->frame_bytes < image_bytes) return fail(J2P_ERR_ARG, "frame_bytes %zu is smaller than one image (%zu bytes)", o->frame_bytes, image_bytes);
     a.w = (int)o->w;
     a.h = (int)o->h;
@@ -1057,7 +1060,15 @@ extern "C" int j2p_session_export(j2p_session *s, unsigned frame0, unsigned nfra
                                   void *stream) {
     if (!s) return fail(J2P_ERR_ARG, "null session");
     if (s->F.nc != 3 || s->strip) return fail(J2P_ERR_ARG, "j2p_session_export needs a whole-frame session with three planes (joint mode)");
-    return export_impl(&s, 1, frame0, nframes, o, dst, stream);
+    return export_impl(&s, 1, 3, frame0, nframes, o, dst, stream);
+}
+
+extern "C" int j2p_session_export_gray(j2p_session *s, unsigned frame0, unsigned nframes, const struct j2p_image_out *o, void *dst,
+                                       void *stream) {
+    if (!s) return fail(J2P_ERR_ARG, "null session");
+    if ((s->F.nc != 1 && s->F.nc != 3) || s->strip)
+        return fail(J2P_ERR_ARG, "j2p_session_export_gray needs a whole-frame session with one or three planes (has %d)", s->F.nc);
+    return export_impl(&s, 1, 1, frame0, nframes, o, dst, stream);
 }
 
 extern "C" int j2p_session_export_separate(j2p_session *y, j2p_session *cb, j2p_session *cr, unsigned frame0, unsigned nframes,
@@ -1070,7 +1081,7 @@ extern "C" int j2p_session_export_separate(j2p_session *y, j2p_session *cb, j2p_
         if (ss[c]->nframes != y->nframes) return fail(J2P_ERR_ARG, "the separate sessions hold different frame counts (%u, %u)", y->nframes, ss[c]->nframes);
         if (ss[c]->device != y->device) return fail(J2P_ERR_ARG, "the separate sessions live on different devices (%d, %d)", y->device, ss[c]->device);
     }
-    return export_impl(ss, 3, frame0, nframes, o, dst, stream);
+    return export_impl(ss, 3, 3, frame0, nframes, o, dst, stream);
 }
 
 extern "C" int j2p_session_sync(j2p_session *s) {

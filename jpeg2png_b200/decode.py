@@ -1,4 +1,4 @@
-"""decode_jpeg: JPEG files in, RGB CUDA tensors out, through the solver.
+"""decode_jpeg: JPEG files in, RGB or gray CUDA tensors out, through the solver.
 
 Every input's headers are read on the host with the JPEG reader of the command line
 (libj2pcodecs.so) before any device work: sequential files whose components are each in one scan
@@ -7,7 +7,9 @@ go through its layout pass (j2p_read_jpeg_layout) and are Huffman-decoded on the
 together in batch sessions (j2p_session_create_batch), with the conventional decode on the device as
 the command line does it, and the colour conversion writes straight into one freshly allocated tensor
 per chunk (j2p_session_export) on the caller's current stream.  The returned tensors of a chunk are
-views of that tensor and share its storage.
+views of that tensor and share its storage.  With mode='UNCHANGED' or 'GRAY' the reader also takes
+one-component (grayscale) files (J2P_READ_GRAY); those are solved as the luma of separate mode and,
+like the luma of colour files in mode='GRAY', exported as one channel (j2p_session_export_gray).
 
 The samples are those of the PNG the command line writes for the same file and flags:
 torch.uint8 the 8-bit PNG samples, torch.uint16 the 16-bit (-1) samples in native byte order,
@@ -31,11 +33,13 @@ MAX_BATCH = 65535                   # frames per batch session (j2p_session_crea
 
 _SAMPLE = {torch.uint8: 8, torch.uint16: 16, torch.float32: 32}
 _LAYOUT = {'HWC': abi.LAYOUT_HWC, 'CHW': abi.LAYOUT_CHW}
+MODES = ('RGB', 'UNCHANGED', 'GRAY')
+READ_GRAY = 1                       # J2P_READ_GRAY (jpeg_reader.h)
 
 
 class Jpeg(C.Structure):
     """struct j2p_jpeg — jpeg2png_b200/cli/jpeg_reader.h."""
-    _fields_ = [('w', C.c_uint), ('h', C.c_uint), ('coefs', abi.Coef * 3)]
+    _fields_ = [('w', C.c_uint), ('h', C.c_uint), ('coefs', abi.Coef * 3), ('ncomp', C.c_uint)]
 
 
 class Huff(C.Structure):
@@ -60,7 +64,7 @@ class Layout(C.Structure):
     _fields_ = [('w', C.c_uint), ('h', C.c_uint), ('coefs', abi.Coef * 3), ('comp_h', C.c_uint * 3),
                 ('comp_v', C.c_uint * 3), ('device_decodable', C.c_int), ('nscan', C.c_uint), ('scan', Scan * 3),
                 ('nseg', C.c_uint), ('seg', C.POINTER(Segment)), ('data', C.POINTER(C.c_uint8)),
-                ('data_len', C.c_size_t)]
+                ('data_len', C.c_size_t), ('ncomp', C.c_uint)]
 
 
 class ProgScan(C.Structure):
@@ -73,7 +77,7 @@ class ProgLayout(C.Structure):
     _fields_ = [('w', C.c_uint), ('h', C.c_uint), ('coefs', abi.Coef * 3), ('comp_h', C.c_uint * 3),
                 ('comp_v', C.c_uint * 3), ('progressive_decodable', C.c_int), ('nscan', C.c_uint),
                 ('scan', C.POINTER(ProgScan)), ('nseg', C.c_uint), ('seg', C.POINTER(Segment)),
-                ('data', C.POINTER(C.c_uint8)), ('data_len', C.c_size_t)]
+                ('data', C.POINTER(C.c_uint8)), ('data_len', C.c_size_t), ('ncomp', C.c_uint)]
 
 
 class EntropyStats(C.Structure):
@@ -101,6 +105,12 @@ def _declare_codecs(lib):
     lib.j2p_free_jpeg_layout.argtypes = [C.POINTER(Layout)]
     lib.j2p_read_jpeg_prog_layout.restype = C.c_int
     lib.j2p_read_jpeg_prog_layout.argtypes = [C.c_char_p, C.c_size_t, C.POINTER(ProgLayout), C.c_char_p, C.c_size_t]
+    lib.j2p_read_jpeg_mem_ex.restype = C.c_int
+    lib.j2p_read_jpeg_mem_ex.argtypes = [C.c_char_p, C.c_size_t, C.c_uint, C.POINTER(Jpeg), C.c_char_p, C.c_size_t]
+    lib.j2p_read_jpeg_layout_ex.restype = C.c_int
+    lib.j2p_read_jpeg_layout_ex.argtypes = [C.c_char_p, C.c_size_t, C.c_uint, C.POINTER(Layout), C.c_char_p, C.c_size_t]
+    lib.j2p_read_jpeg_prog_layout_ex.restype = C.c_int
+    lib.j2p_read_jpeg_prog_layout_ex.argtypes = [C.c_char_p, C.c_size_t, C.c_uint, C.POINTER(ProgLayout), C.c_char_p, C.c_size_t]
     lib.j2p_free_jpeg_prog_layout.restype = None
     lib.j2p_free_jpeg_prog_layout.argtypes = [C.POINTER(ProgLayout)]
 
@@ -149,19 +159,20 @@ def load_progressive() -> C.CDLL:
 
 
 class FileLayout:
-    """A file's layout (j2p_read_jpeg_layout); frees the C buffers when collected."""
+    """A file's layout (j2p_read_jpeg_layout_ex with the J2P_READ_* `flags`); frees the C buffers
+    when collected.  planes: one per component of a device-decodable file."""
 
-    def __init__(self, data: bytes):
+    def __init__(self, data: bytes, flags: int = 0):
         lib = load_codecs()
         self.lay = Layout()
         err = C.create_string_buffer(256)
-        if lib.j2p_read_jpeg_layout(data, len(data), C.byref(self.lay), err, 256) != 0:
+        if lib.j2p_read_jpeg_layout_ex(data, len(data), flags, C.byref(self.lay), err, 256) != 0:
             raise ValueError(err.value.decode(errors='replace'))
         self.device_decodable = bool(self.lay.device_decodable)
         self.w, self.h = int(self.lay.w), int(self.lay.h)
         self.compressed = int(self.lay.data_len)
         self.planes = [Plane(int(c.w), int(c.h), int(c.w_samp), int(c.h_samp), None,
-                             np.array(list(c.quant_table), np.uint16)) for c in self.lay.coefs]
+                             np.array(list(c.quant_table), np.uint16)) for c in self.lay.coefs[:self.lay.ncomp]]
 
     def key(self):
         return Parsed.key(self)
@@ -174,19 +185,20 @@ class FileLayout:
 
 
 class ProgFileLayout:
-    """A progressive file's layout (j2p_read_jpeg_prog_layout); frees the C buffers when collected."""
+    """A progressive file's layout (j2p_read_jpeg_prog_layout_ex with the J2P_READ_* `flags`); frees
+    the C buffers when collected."""
 
-    def __init__(self, data: bytes):
+    def __init__(self, data: bytes, flags: int = 0):
         lib = load_codecs()
         self.lay = ProgLayout()
         err = C.create_string_buffer(256)
-        if lib.j2p_read_jpeg_prog_layout(data, len(data), C.byref(self.lay), err, 256) != 0:
+        if lib.j2p_read_jpeg_prog_layout_ex(data, len(data), flags, C.byref(self.lay), err, 256) != 0:
             raise ValueError(err.value.decode(errors='replace'))
         self.progressive_decodable = bool(self.lay.progressive_decodable)
         self.w, self.h = int(self.lay.w), int(self.lay.h)
         self.compressed = int(self.lay.data_len)
         self.planes = [Plane(int(c.w), int(c.h), int(c.w_samp), int(c.h_samp), None,
-                             np.array(list(c.quant_table), np.uint16)) for c in self.lay.coefs]
+                             np.array(list(c.quant_table), np.uint16)) for c in self.lay.coefs[:self.lay.ncomp]]
 
     def key(self):
         return Parsed.key(self)
@@ -204,7 +216,7 @@ def _layout_ptrs(layouts):
 
 def entropy_plan(layouts, outs, subseq_bits=SUBSEQ_BITS, pinned=False):
     """Pack `layouts` (FileLayout) into a plan for libj2pentropy.so; outs[3 * i + c]: address of
-    file i's plane c.  Returns (plan buffer: a pinned uint8 tensor or a numpy array, its address,
+    file i's plane c (any value for the planes a gray file does not have).  Returns (plan buffer: a pinned uint8 tensor or a numpy array, its address,
     plan bytes, work bytes)."""
     lib = load_entropy()
     ptrs = _layout_ptrs(layouts)
@@ -256,7 +268,7 @@ class Plane:
 
 @dataclass
 class Parsed:
-    """One parsed JPEG: the visible size and its three coefficient planes."""
+    """One parsed JPEG: the visible size and its coefficient planes (three, or one for a gray file)."""
     w: int
     h: int
     planes: list
@@ -266,15 +278,16 @@ class Parsed:
         return (self.w, self.h, tuple((p.w, p.h, p.w_samp, p.h_samp) for p in self.planes))
 
 
-def parse_jpeg(data: bytes) -> Parsed:
-    """Parse JPEG bytes with j2p_read_jpeg_mem; ValueError carries the reader's message."""
+def parse_jpeg(data: bytes, flags: int = 0) -> Parsed:
+    """Parse JPEG bytes with j2p_read_jpeg_mem_ex and the J2P_READ_* `flags`; ValueError carries the
+    reader's message."""
     lib = load_codecs()
     j = Jpeg()
     err = C.create_string_buffer(256)
-    if lib.j2p_read_jpeg_mem(data, len(data), C.byref(j), err, 256) != 0:
+    if lib.j2p_read_jpeg_mem_ex(data, len(data), flags, C.byref(j), err, 256) != 0:
         raise ValueError(err.value.decode(errors='replace'))
     planes = []
-    for c in j.coefs:
+    for c in j.coefs[:j.ncomp]:
         n = c.w * c.h
         d = np.ctypeslib.as_array(c.data, shape=(n,)).copy() if n else np.zeros(0, np.int16)
         abi.free_ptr(c.data)
@@ -317,11 +330,26 @@ def solver_flags(iterations, weight, pweight, separate):
     return tuple(int(n) for n in iters), weights, pweights
 
 
-def frame_footprint(key, separate: bool, sample_bytes: int) -> int:
+def solved_planes(key, separate: bool, mode: str = 'RGB'):
+    """(planes solved, output channels) of a frame of `key` in `mode`: a gray file's one plane and
+    one channel; for a colour file all three planes and three channels, or one channel in mode
+    'GRAY', from the luma alone when separate."""
+    planes = key[2]
+    if len(planes) == 1:
+        return 1, 1
+    if mode == 'GRAY':
+        return (1 if separate else 3), 1
+    return 3, 3
+
+
+def frame_footprint(key, separate: bool, sample_bytes: int, mode: str = 'RGB') -> int:
     """Estimated device bytes one frame of `key` takes in its batch session(s) (DESIGN §4: x, xp, g,
     gp at frame size per plane; coefficients int16 and the conventional decode fp32 at plane size;
-    the reduction state) plus its part of the output tensor."""
+    the reduction state) plus its part of the output tensor, for the planes solved and the channels
+    written in `mode` (solved_planes)."""
     w, h, planes = key
+    nsolved, nout = solved_planes(key, separate, mode)
+    planes = planes[:nsolved]
 
     def session(pl):
         W = max(pw * ws for pw, ph, ws, hs in pl)
@@ -333,15 +361,15 @@ def frame_footprint(key, separate: bool, sample_bytes: int) -> int:
         return n + (16 << 10)
 
     total = sum(session([p]) for p in planes) if separate else session(list(planes))
-    return total + w * h * 3 * sample_bytes
+    return total + w * h * nout * sample_bytes
 
 
-def chunk_frames(key, separate: bool, sample_bytes: int, max_frames, free_bytes: int) -> int:
+def chunk_frames(key, separate: bool, sample_bytes: int, max_frames, free_bytes: int, mode: str = 'RGB') -> int:
     """Frames per batch of `key`: max_frames, or as many as keep the estimated footprint of two
     chunks in flight (one solving while the next is uploaded) under half of `free_bytes`."""
     if max_frames is not None:
         return min(int(max_frames), MAX_BATCH)
-    per = frame_footprint(key, separate, sample_bytes)
+    per = frame_footprint(key, separate, sample_bytes, mode)
     return max(1, min(MAX_BATCH, free_bytes // 4 // per))
 
 
@@ -394,7 +422,8 @@ class _DeviceCoefs:
 
     def _decode(self, device, layouts, stream, subseq_bits, make_plan, lib, name, stats):
         dev = torch.device('cuda', device)
-        sizes = [p.w * p.h for lay in layouts for p in lay.planes]
+        # three planes per file, the ones a gray file does not have empty
+        sizes = [lay.planes[c].w * lay.planes[c].h if c < len(lay.planes) else 0 for lay in layouts for c in range(3)]
         offs = np.concatenate([[0], np.cumsum(sizes, dtype=np.int64)])
         with torch.cuda.stream(stream):
             self.coefs = torch.empty(max(int(offs[-1]), 1), dtype=torch.int16, device=dev)
@@ -435,14 +464,16 @@ class _Chunk:
     """The batch session(s) of one chunk: created, uploaded, iterated and exported by the
     constructor; close() waits for them and returns their blocks to the device cache.
     coefs: {item index: (_DeviceCoefs, its file index)} for items whose coefficients are on the
-    device (uploaded with j2p_session_upload_device after `coef_stream`)."""
+    device (uploaded with j2p_session_upload_device after `coef_stream`).  A gray file is solved as
+    the luma of separate mode; the output has the channels solved_planes gives for `mode`."""
 
-    def __init__(self, lib, device, items, flags, separate, dtype, layout, coefs=None, coef_stream=None):
+    def __init__(self, lib, device, items, flags, separate, dtype, layout, coefs=None, coef_stream=None, mode='RGB'):
         iters, weights, pweights = flags
         self.lib, self.sessions, self.coefs = lib, [], coefs or {}
         first, n = items[0], len(items)
-        if separate:
-            work = [(_frame_desc(first, [c], weights[c], pweights, iters[c]), [c], iters[c]) for c in range(3)]
+        nsolved, nout = solved_planes(first.key(), separate, mode)
+        if nsolved == 1 or separate:
+            work = [(_frame_desc(first, [c], weights[c], pweights, iters[c]), [c], iters[c]) for c in range(nsolved)]
         else:
             work = [(_frame_desc(first, [0, 1, 2], weights[0], pweights, iters[0]), [0, 1, 2], iters[0])]
         try:
@@ -463,14 +494,16 @@ class _Chunk:
                                                                p.quant.ctypes.data, None))     # conventional decode on the device
                 self._check(lib.j2p_session_iterate(s, 0, it))
             w, h = first.w, first.h
-            shape = (n, 3, h, w) if layout == abi.LAYOUT_CHW else (n, h, w, 3)
+            shape = (n, nout, h, w) if layout == abi.LAYOUT_CHW else (n, h, w, nout)
             self.out = torch.empty(shape, dtype=dtype, device=torch.device('cuda', device))
-            o = abi.ImageOut(w, h, _SAMPLE[dtype], layout, 3 * h * w * self.out.element_size())
+            o = abi.ImageOut(w, h, _SAMPLE[dtype], layout, nout * h * w * self.out.element_size())
             # torch's default stream is handle 0, which the ABI reads as "the session stream":
             # name it cudaStreamLegacy (1) instead
             stream = C.c_void_p(torch.cuda.current_stream(device).cuda_stream or 1)
             dst = C.c_void_p(self.out.data_ptr())
-            if separate:
+            if nout == 1:
+                self._check(lib.j2p_session_export_gray(self.sessions[0], 0, n, C.byref(o), dst, stream))
+            elif separate:
                 self._check(lib.j2p_session_export_separate(*self.sessions, 0, n, C.byref(o), dst, stream))
             else:
                 self._check(lib.j2p_session_export(self.sessions[0], 0, n, C.byref(o), dst, stream))
@@ -499,20 +532,21 @@ def _where(i, path):
     return f'input {i} ({path})' if path is not None else f'input {i}'
 
 
-def _front_end(data, device_ok, progressive=False):
+def _front_end(data, device_ok, progressive=False, flags=0):
     """The host part of one input: a FileLayout for the device decoder, a ProgFileLayout for the
     progressive device decoder (progressive=True), a Parsed from the host reader, or the ValueError
-    (always the host reader's message) or RuntimeError to raise."""
+    (always the host reader's message) or RuntimeError to raise.  flags: J2P_READ_*, for every
+    reader."""
     if not device_ok or _host_front_end:
         try:
-            return parse_jpeg(data)
+            return parse_jpeg(data, flags)
         except ValueError as e:
             return e
     try:
-        lay = FileLayout(data)
+        lay = FileLayout(data, flags)
     except ValueError:
         try:
-            parse_jpeg(data)
+            parse_jpeg(data, flags)
         except ValueError as e:
             return e
         return RuntimeError('the layout pass rejected a file the host reader accepts')
@@ -520,30 +554,39 @@ def _front_end(data, device_ok, progressive=False):
         return lay
     if progressive:
         try:
-            prog = ProgFileLayout(data)
+            prog = ProgFileLayout(data, flags)
         except ValueError:
             try:
-                parse_jpeg(data)
+                parse_jpeg(data, flags)
             except ValueError as e:
                 return e
             return RuntimeError('the progressive layout pass rejected a file the host reader accepts')
         if prog.progressive_decodable:
             return prog
     try:
-        return parse_jpeg(data)
+        return parse_jpeg(data, flags)
     except ValueError as e:
         return e
 
 
 def decode_jpeg(inputs, *, iterations=50, weight=0.3, pweight=0.001, separate=False,
-                dtype=torch.uint8, layout='CHW', device=None, max_frames=None, progressive_on_device=False):
-    """Decode JPEG files into RGB tensors on a CUDA device, deblocked by the solver.
+                dtype=torch.uint8, layout='CHW', device=None, max_frames=None, progressive_on_device=False,
+                mode='RGB'):
+    """Decode JPEG files into RGB or gray tensors on a CUDA device, deblocked by the solver.
 
     inputs: bytes-like, a path (str / os.PathLike), or a list or tuple of them.  A single input
-    returns one tensor, a list returns a list in input order.  Each tensor is (3, h, w) for
-    layout='CHW' or (h, w, 3) for 'HWC' at the image's visible size, on `device` (default: the
+    returns one tensor, a list returns a list in input order.  Each tensor is (c, h, w) for
+    layout='CHW' or (h, w, c) for 'HWC' at the image's visible size, on `device` (default: the
     current CUDA device).  dtype: torch.uint8 (the 8-bit PNG samples), torch.uint16 (the 16-bit
     PNG samples) or torch.float32 (the clamped samples before truncation).
+
+    mode: 'RGB' (c = 3; a grayscale file is refused with the reader's "only 3 component jpegs are
+    supported"), 'UNCHANGED' (c = 1 for a grayscale file, 3 for a colour file) or 'GRAY' (c = 1
+    for every file).  A one-channel sample is the RGB sample of its luma with zero chroma, so a gray
+    tensor t gives the RGB image as t.expand(3, -1, -1) (CHW).  A grayscale file is solved as the
+    luma of separate mode, with the first of three iterations, weights and pweights, so its result
+    does not depend on `separate`.  For a colour file, mode='GRAY' gives the luma of the joint solve,
+    or with separate=True the luma solve alone: its chroma planes are neither uploaded nor solved.
 
     iterations, weight, pweight, separate: the command line's -i, -w, -p and -s.  Scalars as there:
     a scalar weight sets luma only; three weights or three iteration counts need separate=True.
@@ -553,7 +596,7 @@ def decode_jpeg(inputs, *, iterations=50, weight=0.3, pweight=0.001, separate=Fa
     allocation and share its storage.  The result is written on the current torch stream and can
     be used there without synchronising.
 
-    Sequential (baseline or extended) files whose three components are each coded in one scan are
+    Sequential (baseline or extended) files whose components are each coded in one scan are
     Huffman-decoded on the device: only their compressed bytes are uploaded.  progressive_on_device:
     progressive files are Huffman-decoded on the device too (libj2pprogressive.so, DESIGN §7g);
     by default they are parsed on the host, as is every other file.  Raises ValueError for bad arguments and
@@ -562,6 +605,9 @@ def decode_jpeg(inputs, *, iterations=50, weight=0.3, pweight=0.001, separate=Fa
     is solved.  Raises RuntimeError when no CUDA device is usable.
     """
     flags = solver_flags(iterations, weight, pweight, separate)
+    if not isinstance(mode, str) or mode not in MODES:
+        raise ValueError(f"mode must be 'RGB', 'UNCHANGED' or 'GRAY', not {mode!r}")
+    read_flags = 0 if mode == 'RGB' else READ_GRAY
     if dtype not in _SAMPLE:
         raise ValueError(f'dtype must be torch.uint8, torch.uint16 or torch.float32, not {dtype}')
     if layout not in _LAYOUT:
@@ -584,9 +630,10 @@ def decode_jpeg(inputs, *, iterations=50, weight=0.3, pweight=0.001, separate=Fa
     workers = min(len(read), os.cpu_count() or 1, 16)
     if workers > 1:
         with ThreadPoolExecutor(workers) as pool:
-            parsed = list(pool.map(lambda d: _front_end(d, device_ok, progressive_on_device), [data for data, _ in read]))
+            parsed = list(pool.map(lambda d: _front_end(d, device_ok, progressive_on_device, read_flags),
+                                   [data for data, _ in read]))
     else:
-        parsed = [_front_end(data, device_ok, progressive_on_device) for data, _ in read]
+        parsed = [_front_end(data, device_ok, progressive_on_device, read_flags) for data, _ in read]
     for i, (p, (_, path)) in enumerate(zip(parsed, read)):
         if isinstance(p, ValueError):
             raise ValueError(f'{_where(i, path)}: {p}')
@@ -600,7 +647,7 @@ def decode_jpeg(inputs, *, iterations=50, weight=0.3, pweight=0.001, separate=Fa
     sample_bytes = _SAMPLE[dtype] // 8
     free = torch.cuda.mem_get_info(index)[0] if max_frames is None else 0
     chunks = plan([p.key() for p in parsed],
-                  lambda k: chunk_frames(k, separate, sample_bytes, max_frames, free))
+                  lambda k: chunk_frames(k, separate, sample_bytes, max_frames, free, mode))
 
     results = [None] * len(parsed)
     layout_id = _LAYOUT[layout]
@@ -622,14 +669,14 @@ def decode_jpeg(inputs, *, iterations=50, weight=0.3, pweight=0.001, separate=Fa
                             i = idx[j]
                             where = _where(i, read[i][1])
                             try:
-                                parse_jpeg(read[i][0])
+                                parse_jpeg(read[i][0], read_flags)
                             except ValueError as e:
                                 raise ValueError(f'{where}: {e}') from None
                             raise RuntimeError(f'{where}: the device entropy decoder failed '
                                                f'({ENT_FAILURES.get(int(dc.status[k]), int(dc.status[k]))}) on a file '
                                                'the host reader accepts (a decoder bug)')
                         coefs[j] = (dc, k)
-                chunk = _Chunk(lib, index, [parsed[i] for i in idx], flags, separate, dtype, layout_id, coefs, coef_stream)
+                chunk = _Chunk(lib, index, [parsed[i] for i in idx], flags, separate, dtype, layout_id, coefs, coef_stream, mode)
                 for j, i in enumerate(idx):
                     results[i] = chunk.out[j]
                 if previous is not None:        # this chunk is queued: let the previous one finish

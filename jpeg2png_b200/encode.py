@@ -1,4 +1,4 @@
-"""encode_png: RGB CUDA tensors in, PNG files (bytes) out, encoded on the device.
+"""encode_png: RGB or gray CUDA tensors in, PNG files (bytes) out, encoded on the device.
 
 The encoder is libj2ppng.so (jpeg2png_b200/png, DESIGN §7e): every row gets the PNG filter with
 the smallest sum of |residual|, the filtered stream is deflated in pieces of 64 KiB with zlib's
@@ -26,7 +26,8 @@ _NP_DTYPES = (np.dtype(np.uint8), np.dtype(np.uint16))
 class Image(C.Structure):
     """struct j2p_png_image — jpeg2png_b200/png/png.h."""
     _fields_ = [('data', C.c_void_p), ('width', C.c_uint32), ('height', C.c_uint32), ('sample_bytes', C.c_uint32),
-                ('row_stride', C.c_int64), ('col_stride', C.c_int64), ('chan_stride', C.c_int64)]
+                ('row_stride', C.c_int64), ('col_stride', C.c_int64), ('chan_stride', C.c_int64),
+                ('channels', C.c_uint32)]
 
 
 class Stats(C.Structure):
@@ -57,17 +58,18 @@ def _check_size(shape, h, w):
         raise ValueError(f'an image needs at least one pixel; got shape {tuple(shape)}')
 
 
-def _fill(d, x):
+def _fill(d, x, channels):
     d.sample_bytes = x.itemsize
+    d.channels = channels
 
 
 # j2p_png_plan's refusal of an image too large for one IDAT chunk reaches the caller as a ValueError
-CODEC = B.Codec('png', load_png, Image, _check_size, _fill)
+CODEC = B.Codec('png', load_png, Image, _check_size, _fill, channels=(3, 1))
 
 
 def encode_host(images, layout='HWC'):
-    """The serial host driver (j2p_png_encode_host) on numpy uint8 / uint16 arrays: a list of PNG
-    files as bytes, the same bytes the device writes."""
+    """The serial host driver (j2p_png_encode_host) on numpy uint8 / uint16 arrays, RGB or gray
+    as encode_png takes them: a list of PNG files as bytes, the same bytes the device writes."""
     B.check_layout(layout)
     for x in images:
         if x.dtype not in _NP_DTYPES:
@@ -76,12 +78,13 @@ def encode_host(images, layout='HWC'):
 
 
 def encode_png(images, *, layout='CHW'):
-    """Encode RGB CUDA tensors as PNG files on the device.
+    """Encode RGB or gray CUDA tensors as PNG files on the device.
 
     images: one tensor or a list or tuple of them, torch.uint8 or torch.uint16 (native-endian
     16-bit samples, written as 16-bit PNG), shaped (3, h, w) for layout='CHW' or (h, w, 3) for
-    'HWC', with any strides: what decode_jpeg returns.  Returns the PNG file as bytes, or a list of
-    bytes in input order.
+    'HWC', with any strides: what decode_jpeg returns.  A tensor with one channel, (1, h, w) or
+    (h, w, 1), is written as a gray PNG (colour type 0); gray and RGB images mix in one call.
+    Returns the PNG file as bytes, or a list of bytes in input order.
 
     The work is queued on torch's current stream, after what is already there, so a tensor just
     written on that stream needs no synchronisation.  Images of any mix of sizes go into one call;

@@ -139,9 +139,9 @@ extern "C" int j2p_entropy_pack(const struct j2p_jpeg_layout *const *L, unsigned
         const struct j2p_jpeg_layout *l = L[i];
         j2p_ent_file *f = &files[i];
         for (int p = 0; p < 3; p++) {
-            f->out[p] = out[3 * i + p];
             f->wb[p] = l->coefs[p].w / 8;
             f->hb[p] = l->coefs[p].h / 8;
+            f->out[p] = f->wb[p] ? out[3 * i + p] : nullptr;     // a gray file's planes 1 and 2 are empty
         }
         for (unsigned k = 0; k < l->nscan; k++, iscan++) {
             const struct j2p_jpeg_scan *ls = &l->scan[k];

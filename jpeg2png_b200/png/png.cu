@@ -34,7 +34,9 @@ static int make_plan(const struct j2p_png_image *im, unsigned n, Layout *L, stru
         if (x->width == 0 || x->height == 0 || x->width > 0x7fffffffu || x->height > 0x7fffffffu)
             return fail("image %u: width and height must be 1 .. 2^31 - 1 (got %u x %u)", i, x->width, x->height);
         if (x->sample_bytes != 1 && x->sample_bytes != 2) return fail("image %u: unknown sample size %u (1 or 2 bytes)", i, x->sample_bytes);
-        const uint64_t len = (uint64_t)x->height * (1 + (uint64_t)x->width * 3 * x->sample_bytes);
+        if (x->channels != 0 && x->channels != 1 && x->channels != 3) return fail("image %u: %u channels (1 or 3)", i, x->channels);
+        const uint32_t nc = x->channels == 1 ? 1 : 3;
+        const uint64_t len = (uint64_t)x->height * (1 + (uint64_t)x->width * nc * x->sample_bytes);
         const uint64_t np = (len + J2P_PNG_PIECE - 1) / J2P_PNG_PIECE;
         // PNG caps a chunk at 2^31 - 1 bytes and the file has one IDAT: refuse an image whose
         // IDAT could exceed it (every piece at its bound), before anything is sized from it
@@ -53,6 +55,7 @@ static int make_plan(const struct j2p_png_image *im, unsigned n, Layout *L, stru
             g->w = x->width;
             g->h = x->height;
             g->sb = x->sample_bytes;
+            g->nc = nc;
             g->piece0 = (uint32_t)pieces;
             g->npieces = (uint32_t)np;
             g->row0 = rows;
@@ -153,16 +156,21 @@ J2P_HD void write_frame(uint8_t *out, const struct j2p_png_img *im, const uint32
 }
 
 // ---- host driver -------------------------------------------------------------------------------
-static void filter_host(const struct j2p_png_img *im, uint8_t *filt) {
-    const uint64_t rb = j2p_png_row_bytes(im);
+template <uint32_t NC> static void filter_host_nc(const struct j2p_png_img *im, uint8_t *filt) {
+    const uint64_t rb = j2p_png_row_bytes<NC>(im);
     for (uint32_t y = 0; y < im->h; y++) {
         uint64_t sum[5] = {0, 0, 0, 0, 0};
-        for (uint64_t i = 0; i < rb; i++) j2p_png_filter_sums(im, y, (int64_t)i, sum);
+        for (uint64_t i = 0; i < rb; i++) j2p_png_filter_sums<NC>(im, y, (int64_t)i, sum);
         const int t = j2p_png_pick(sum);
         uint8_t *o = filt + im->filt_off + (uint64_t)y * (rb + 1);
         o[0] = (uint8_t)t;
-        for (uint64_t i = 0; i < rb; i++) o[1 + i] = j2p_png_filtered(im, t, y, (int64_t)i);
+        for (uint64_t i = 0; i < rb; i++) o[1 + i] = j2p_png_filtered<NC>(im, t, y, (int64_t)i);
     }
+}
+
+static void filter_host(const struct j2p_png_img *im, uint8_t *filt) {
+    if (im->nc == 1) filter_host_nc<1>(im, filt);
+    else filter_host_nc<3>(im, filt);
 }
 
 static void piece_host(const uint8_t *src, uint32_t n, bool last, uint32_t *out, const uint32_t *tab, const uint32_t *x2k, PieceResult *res,
@@ -277,16 +285,11 @@ __device__ __forceinline__ uint32_t find_image(const struct j2p_png_img *imgs, u
     return lo;
 }
 
-__global__ void __launch_bounds__(kFilterThreads) k_png_filter(const struct j2p_png_img *__restrict__ imgs, uint32_t n, uint64_t rows,
-                                                              uint8_t *__restrict__ filt) {
-    const uint64_t row = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-    const uint32_t lane = threadIdx.x & 31;
-    if (row >= rows) return;
-    const struct j2p_png_img im = imgs[find_image(imgs, n, row)];
-    const int64_t y = (int64_t)(row - im.row0);
-    const uint64_t rb = j2p_png_row_bytes(&im);
+// one row on one warp; NC: the image's channel count (im.nc), the same for the whole warp
+template <uint32_t NC> __device__ __forceinline__ void filter_row(const struct j2p_png_img &im, int64_t y, uint32_t lane, uint8_t *__restrict__ filt) {
+    const uint64_t rb = j2p_png_row_bytes<NC>(&im);
     uint64_t sum[5] = {0, 0, 0, 0, 0};
-    for (uint64_t i = lane; i < rb; i += 32) j2p_png_filter_sums(&im, y, (int64_t)i, sum);
+    for (uint64_t i = lane; i < rb; i += 32) j2p_png_filter_sums<NC>(&im, y, (int64_t)i, sum);
 #pragma unroll
     for (int t = 0; t < 5; t++)
 #pragma unroll
@@ -294,7 +297,18 @@ __global__ void __launch_bounds__(kFilterThreads) k_png_filter(const struct j2p_
     const int t = j2p_png_pick(sum);
     uint8_t *o = filt + im.filt_off + (uint64_t)y * (rb + 1);
     if (lane == 0) o[0] = (uint8_t)t;
-    for (uint64_t i = lane; i < rb; i += 32) o[1 + i] = j2p_png_filtered(&im, t, y, (int64_t)i);
+    for (uint64_t i = lane; i < rb; i += 32) o[1 + i] = j2p_png_filtered<NC>(&im, t, y, (int64_t)i);
+}
+
+__global__ void __launch_bounds__(kFilterThreads) k_png_filter(const struct j2p_png_img *__restrict__ imgs, uint32_t n, uint64_t rows,
+                                                              uint8_t *__restrict__ filt) {
+    const uint64_t row = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const uint32_t lane = threadIdx.x & 31;
+    if (row >= rows) return;
+    const struct j2p_png_img im = imgs[find_image(imgs, n, row)];
+    const int64_t y = (int64_t)(row - im.row0);
+    if (im.nc == 1) filter_row<1>(im, y, lane, filt);
+    else filter_row<3>(im, y, lane, filt);
 }
 
 struct PieceShared {

@@ -1,8 +1,9 @@
-/* png.h — libj2ppng.so: RGB images in device memory to PNG files, encoded on the device.
+/* png.h — libj2ppng.so: RGB and gray images in device memory to PNG files, encoded on the device.
  *
- * Each image is 8-bit or 16-bit RGB (16-bit samples in native byte order, written big-endian),
- * addressed with element strides for row, column and channel, so HWC, CHW and strided views are
- * read in place.  The file holds the signature, IHDR (colour type 2, no interlace), one IDAT (zlib
+ * Each image is 8-bit or 16-bit RGB or gray (16-bit samples in native byte order, written
+ * big-endian), addressed with element strides for row, column and channel, so HWC, CHW and strided
+ * views are read in place.  One call may mix RGB and gray images.  The file holds the signature,
+ * IHDR (colour type 2 for RGB, 0 for gray, no interlace), one IDAT (zlib
  * header 78 01, the deflate stream, the Adler-32) and IEND.  png_core.h states the encoding.
  *
  * One call: j2p_png_plan gives the size of the device work area for a list of images;
@@ -26,6 +27,7 @@ struct j2p_png_image {
         uint32_t width, height;         /* 1 .. 2^31 - 1 */
         uint32_t sample_bytes;          /* 1 (uint8) or 2 (native-endian uint16) */
         int64_t row_stride, col_stride, chan_stride;      /* in samples */
+        uint32_t channels;              /* 3 (RGB) or 1 (gray; chan_stride unused); 0 reads as 3 */
 };
 
 struct j2p_png_stats {
@@ -34,11 +36,12 @@ struct j2p_png_stats {
 };
 
 /* Work area for the n images: work_bytes in all, the files at out_offset in it.  Refuses null
- * pointers, n == 0, a width or height of 0 or above 2^31 - 1, a sample size other than 1 or 2, and
+ * pointers, n == 0, a width or height of 0 or above 2^31 - 1, a sample size other than 1 or 2, a
+ * channel count other than 0, 1 or 3, and
  * an image whose IDAT could exceed PNG's chunk limit of 2^31 - 1 bytes: the file has one IDAT, so
  * the image's worst-case deflate stream (every block stored, see j2p_png_piece_bound) plus the zlib
- * header and checksum must fit.  That admits about 2.14e9 filtered bytes, e.g. 26,700 x 26,700 at
- * 8 bits or 18,900 x 18,900 at 16 bits.  Returns 0, or -1 (j2p_png_last_error). */
+ * header and checksum must fit.  That admits about 2.14e9 filtered bytes, e.g. 26,700 x 26,700 RGB at
+ * 8 bits or 18,900 x 18,900 at 16 bits (three times the pixels in gray).  Returns 0, or -1 (j2p_png_last_error). */
 int j2p_png_plan(const struct j2p_png_image *images, unsigned n, size_t *work_bytes, size_t *out_offset);
 
 /* Encodes on `stream` (a cudaStream_t; NULL: the legacy default stream) into `work` (device memory

@@ -39,6 +39,7 @@ struct j2p_png_img {
         const uint8_t *src;
         int64_t s_row, s_col, s_chan;     /* element strides */
         uint32_t w, h, sb;                /* sample bytes: 1 or 2 */
+        uint32_t nc;                      /* samples per pixel: 3 (RGB) or 1 (gray) */
         uint32_t piece0, npieces;
         uint64_t row0;                    /* first row among all rows of the call */
         uint64_t filt_off, filt_len;      /* the filtered stream in the filtered buffer */
@@ -47,15 +48,18 @@ struct j2p_png_img {
 };
 
 /* ---- filtering ------------------------------------------------------------------------------ */
-J2P_HD uint64_t j2p_png_row_bytes(const struct j2p_png_img *im) { return (uint64_t)im->w * 3u * im->sb; }
+/* The steps below take the image's channel count NC (im->nc: 3 or 1) as a template argument:
+ * callers branch on it once per row, so each byte's address arithmetic has a constant divisor
+ * (none for gray) and the RGB code is what it is with 3 written in. */
+template <uint32_t NC> J2P_HD uint64_t j2p_png_row_bytes(const struct j2p_png_img *im) { return (uint64_t)im->w * NC * im->sb; }
 
 /* Byte i of row y of the unfiltered scanline (16-bit samples big-endian); 0 outside the image. */
-J2P_HD uint32_t j2p_png_raw(const struct j2p_png_img *im, int64_t y, int64_t i) {
+template <uint32_t NC> J2P_HD uint32_t j2p_png_raw(const struct j2p_png_img *im, int64_t y, int64_t i) {
         if (y < 0 || i < 0) return 0;
         /* a row holds fewer than J2P_PNG_MAX_IDAT bytes (the plan refuses larger images), so the
          * byte index fits 32 bits and its divisions are 32-bit ones */
         const uint32_t u = (uint32_t)i, s = im->sb == 2 ? u >> 1 : u, k = u - s * im->sb;
-        const uint32_t x = s / 3, c = s - x * 3;
+        const uint32_t x = s / NC, c = s - x * NC;
         const int64_t e = y * im->s_row + (int64_t)x * im->s_col + (int64_t)c * im->s_chan;
         if (im->sb == 1) return im->src[e];
         const uint16_t v = ((const uint16_t *)im->src)[e];
@@ -83,10 +87,10 @@ J2P_HD uint32_t j2p_png_residual(int t, uint32_t x, uint32_t a, uint32_t b, uint
 J2P_HD uint32_t j2p_png_cost(uint32_t r) { return r < 128 ? r : 256 - r; }
 
 /* Adds byte i of row y to the five filter sums. */
-J2P_HD void j2p_png_filter_sums(const struct j2p_png_img *im, int64_t y, int64_t i, uint64_t sum[5]) {
-        const int64_t bpp = 3 * (int64_t)im->sb;
-        const uint32_t x = j2p_png_raw(im, y, i), a = j2p_png_raw(im, y, i - bpp), b = j2p_png_raw(im, y - 1, i),
-                       c = j2p_png_raw(im, y - 1, i - bpp);
+template <uint32_t NC> J2P_HD void j2p_png_filter_sums(const struct j2p_png_img *im, int64_t y, int64_t i, uint64_t sum[5]) {
+        const int64_t bpp = NC * (int64_t)im->sb;
+        const uint32_t x = j2p_png_raw<NC>(im, y, i), a = j2p_png_raw<NC>(im, y, i - bpp), b = j2p_png_raw<NC>(im, y - 1, i),
+                       c = j2p_png_raw<NC>(im, y - 1, i - bpp);
 #ifdef __CUDA_ARCH__
 #pragma unroll
 #endif
@@ -104,10 +108,10 @@ J2P_HD int j2p_png_pick(const uint64_t sum[5]) {
         return best;
 }
 
-J2P_HD uint8_t j2p_png_filtered(const struct j2p_png_img *im, int t, int64_t y, int64_t i) {
-        const int64_t bpp = 3 * (int64_t)im->sb;
-        return (uint8_t)j2p_png_residual(t, j2p_png_raw(im, y, i), j2p_png_raw(im, y, i - bpp), j2p_png_raw(im, y - 1, i),
-                                         j2p_png_raw(im, y - 1, i - bpp));
+template <uint32_t NC> J2P_HD uint8_t j2p_png_filtered(const struct j2p_png_img *im, int t, int64_t y, int64_t i) {
+        const int64_t bpp = NC * (int64_t)im->sb;
+        return (uint8_t)j2p_png_residual(t, j2p_png_raw<NC>(im, y, i), j2p_png_raw<NC>(im, y, i - bpp), j2p_png_raw<NC>(im, y - 1, i),
+                                         j2p_png_raw<NC>(im, y - 1, i - bpp));
 }
 
 /* ---- parse ---------------------------------------------------------------------------------- */
@@ -532,7 +536,7 @@ J2P_HD void j2p_png_head(uint8_t *o, const struct j2p_png_img *im, uint32_t idat
         o[12] = 'I'; o[13] = 'H'; o[14] = 'D'; o[15] = 'R';
         j2p_png_be32(o + 16, im->w);
         j2p_png_be32(o + 20, im->h);
-        o[24] = (uint8_t)(8 * im->sb); o[25] = 2; o[26] = 0; o[27] = 0; o[28] = 0;
+        o[24] = (uint8_t)(8 * im->sb); o[25] = im->nc == 1 ? 0 : 2; o[26] = 0; o[27] = 0; o[28] = 0;     /* colour type: gray or RGB */
         j2p_png_be32(o + 29, j2p_png_crc(0, o + 12, 17, table));
         j2p_png_be32(o + 33, idat_len);
         o[37] = 'I'; o[38] = 'D'; o[39] = 'A'; o[40] = 'T';

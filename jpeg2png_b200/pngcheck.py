@@ -1,5 +1,5 @@
 """A numpy restatement of PNG row filtering, for checking encoded files without a PNG decoder
-(16-bit RGB included): the scanlines of an image, the five filters' residuals, the filter
+(16-bit RGB and gray included): the scanlines of an image, the five filters' residuals, the filter
 heuristic of encode_png, and whether a file's inflated scanlines are an image's pixels filtered as
 the file's filter bytes say (filtering is invertible, so that is pixel equality)."""
 import zlib
@@ -8,12 +8,12 @@ import numpy as np
 
 
 def scanlines(x):
-    """(h, row bytes) uint8: the unfiltered PNG samples of an (h, w, 3) uint8 / uint16 array,
-    16-bit samples big-endian."""
-    h, w, _ = x.shape
+    """(h, row bytes) uint8: the unfiltered PNG samples of an (h, w, c) uint8 / uint16 array (c = 3
+    for RGB, 1 for gray), 16-bit samples big-endian."""
+    h, w, c = x.shape
     if x.dtype == np.uint16:
-        return np.ascontiguousarray(x).astype('>u2').view(np.uint8).reshape(h, w * 6)
-    return np.ascontiguousarray(x).reshape(h, w * 3)
+        return np.ascontiguousarray(x).astype('>u2').view(np.uint8).reshape(h, w * c * 2)
+    return np.ascontiguousarray(x).reshape(h, w * c)
 
 
 def residuals(raw, bpp):
@@ -59,8 +59,10 @@ def idat(png):
     return z
 
 
-def holds_pixels(png, x):
-    """Whether the non-interlaced RGB PNG file `png` holds the (h, w, 3) uint8 / uint16 array x."""
+def holds_pixels(png, x, bpp=None):
+    """Whether the non-interlaced PNG file `png` holds the (h, w, c) uint8 / uint16 array x.  bpp:
+    the filters' bytes per pixel, by default c times the sample size (3 or 6 for RGB, 1 or 2 for
+    gray)."""
     raw = scanlines(x)
     h = raw.shape[0]
     s = np.frombuffer(zlib.decompress(idat(png)), np.uint8)
@@ -70,4 +72,6 @@ def holds_pixels(png, x):
     types = s[:, 0].astype(np.int64)
     if types.max() > 4:
         return False
-    return filtered(residuals(raw, 3 * x.itemsize), types) == s.tobytes()
+    if bpp is None:
+        bpp = x.shape[2] * x.itemsize
+    return filtered(residuals(raw, bpp), types) == s.tobytes()

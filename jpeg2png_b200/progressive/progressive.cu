@@ -181,9 +181,9 @@ extern "C" int j2p_progressive_pack(const struct j2p_jpeg_prog_layout *const *L,
     uint8_t *data = b + h->off_data;
     for (unsigned i = 0; i < n; i++) {
         for (int p = 0; p < 3; p++) {
-            files[i].out[p] = out[3 * i + p];
             files[i].wb[p] = L[i]->coefs[p].w / 8;
             files[i].hb[p] = L[i]->coefs[p].h / 8;
+            files[i].out[p] = files[i].wb[p] ? out[3 * i + p] : nullptr;     // a gray file's planes 1 and 2 are empty
         }
     }
     // everything in step order, files in input order within a step
@@ -297,7 +297,8 @@ extern "C" int j2p_progressive_decode_host(const void *plan, void *work, uint32_
     if (view_of(plan, plan, work, status, &v, &h) != 0) return -1;
     memset(status, 0, h->nfiles * sizeof(uint32_t));
     for (uint32_t i = 0; i < h->nfiles; i++)
-        for (int c = 0; c < 3; c++) memset(v.files[i].out[c], 0, (size_t)v.files[i].wb[c] * v.files[i].hb[c] * 64 * sizeof(int16_t));
+        for (int c = 0; c < 3; c++)
+            if (v.files[i].out[c]) memset(v.files[i].out[c], 0, (size_t)v.files[i].wb[c] * v.files[i].hb[c] * 64 * sizeof(int16_t));
     unsigned rounds = 0;
     if (h->nsub) {
         for (;;) {

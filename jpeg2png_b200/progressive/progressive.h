@@ -43,7 +43,8 @@ struct j2p_progressive_stats {
 int j2p_progressive_plan_size(const struct j2p_jpeg_prog_layout *const *layouts, unsigned n, unsigned subseq_bits, size_t *plan_bytes,
                               size_t *work_bytes);
 /* Writes the plan into `dst` (plan_bytes, 16-byte aligned).  out[3 * i + c]: where plane c of
- * file i goes (w/8 * h/8 * 64 int16, 16-byte aligned). */
+ * file i goes (w/8 * h/8 * 64 int16, 16-byte aligned).  The empty planes 1 and 2 of a gray file
+ * (J2P_READ_GRAY, w = h = 0) are never written and their out entries are not read. */
 int j2p_progressive_pack(const struct j2p_jpeg_prog_layout *const *layouts, unsigned n, unsigned subseq_bits, int16_t *const *out,
                          void *dst, size_t plan_bytes);
 /* Decodes on `stream` (a cudaStream_t; NULL: the legacy default stream).  plan_host: the packed
