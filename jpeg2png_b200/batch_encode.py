@@ -133,9 +133,24 @@ def encode_device(codec, descs, device):
     return results
 
 
+def by_codec(codecs, items, layout):
+    """The calls a list of images makes when each channel count has its codec, codecs = {channel
+    count: Codec}: [(codec, indices of its images, in input order)], a codec that several counts
+    share taking all their images."""
+    groups = {}
+    for i, x in enumerate(items):
+        c = codecs[x.shape[axes(x.shape, layout, tuple(codecs))[4]]]
+        groups.setdefault(id(c), (c, []))[1].append(i)
+    return list(groups.values())
+
+
 def encode_tensors(fn, codec, images, layout, dtypes):
     """The body of the public encoder `fn` once its own arguments are checked: images is one CUDA
-    tensor or a list or tuple of them, of one of `dtypes`.  Returns bytes or a list of bytes."""
+    tensor or a list or tuple of them, of one of `dtypes`.  codec: a Codec, or {channel count:
+    Codec} for an encoder whose library call takes one kind of image (the images of each kind go
+    to their own calls).  Returns bytes or a list of bytes, in input order."""
+    codecs = codec if isinstance(codec, dict) else {c: codec for c in codec.channels}
+    channels = tuple(codecs)
     single = not isinstance(images, (list, tuple))
     items = [images] if single else list(images)
     for x in items:
@@ -143,8 +158,8 @@ def encode_tensors(fn, codec, images, layout, dtypes):
             raise ValueError(f'{fn} takes torch tensors, not {type(x).__name__}')
         if x.dtype not in dtypes:
             raise ValueError(f'{fn} takes {" or ".join(map(str, dtypes))} tensors, not {x.dtype}')
-        h, w, *_ = axes(x.shape, layout, codec.channels)
-        codec.check_size(x.shape, h, w)
+        h, w, *_ = axes(x.shape, layout, channels)
+        codecs[channels[0]].check_size(x.shape, h, w)
         if x.device.type != 'cuda':
             raise ValueError(f'{fn} encodes CUDA tensors; this one is on {x.device}')
     if not torch.cuda.is_available() or torch.cuda.device_count() <= 0:
@@ -154,5 +169,8 @@ def encode_tensors(fn, codec, images, layout, dtypes):
     device = items[0].device
     if any(x.device != device for x in items):
         raise ValueError('all images of one call must be on the same device')
-    results = encode_device(codec, descs(codec, items, layout), device)
+    results = [None] * len(items)
+    for c, idx in by_codec(codecs, items, layout):
+        for i, r in zip(idx, encode_device(c, descs(c, [items[i] for i in idx], layout), device)):
+            results[i] = r
     return results[0] if single else results

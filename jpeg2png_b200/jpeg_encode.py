@@ -1,4 +1,4 @@
-"""encode_jpeg: RGB CUDA tensors in, baseline JPEG files (bytes) out, encoded on the device.
+"""encode_jpeg: RGB or gray CUDA tensors in, JPEG files (bytes) out, encoded on the device.
 
 The encoder is libj2pjpegenc.so (jpeg2png_b200/jpegenc, DESIGN §7f).  It writes the file that
 Pillow writes for the same pixels with `quality` and `subsampling` and no other options (libjpeg's
@@ -9,7 +9,9 @@ per image from its own symbol counts.  With `progressive=True` the encoder is li
 (jpeg2png_b200/jpegprog), which writes Pillow's `progressive=True` file: the same coefficients in
 libjpeg's ten-scan progression, each scan with tables built from its own symbol counts.
 `restart_marker_blocks` and `restart_marker_rows` add restart intervals to any of the three files,
-as Pillow's keywords of the same names do (DESIGN §7i).  Colour conversion, downsampling, DCT,
+as Pillow's keywords of the same names do (DESIGN §7i).  One-channel tensors are written as
+Pillow's one-component ('L') files by the same three libraries, one call per kind (DESIGN §7k).
+Colour conversion, downsampling, DCT,
 quantisation, the tables, Huffman coding and byte stuffing all run on the device; only the finished
 files cross PCIe.
 `encode_host` runs the same steps serially on numpy arrays and gives the same bytes.
@@ -44,7 +46,8 @@ class Image(C.Structure):
 
 class Params(C.Structure):
     """struct j2p_jpegenc_params — jpeg2png_b200/jpegenc/jpegenc.h."""
-    _fields_ = [('quality', C.c_int), ('sampling', C.c_int), ('restart_marker_blocks', C.c_int), ('restart_marker_rows', C.c_int)]
+    _fields_ = [('quality', C.c_int), ('sampling', C.c_int), ('restart_marker_blocks', C.c_int), ('restart_marker_rows', C.c_int),
+                ('components', C.c_int)]
 
 
 class Stats(C.Structure):
@@ -104,16 +107,19 @@ def _check_restart(name, v):
     return int(v)
 
 
-def params(quality, subsampling, restart_marker_blocks=0, restart_marker_rows=0) -> Params:
+def params(quality, subsampling, restart_marker_blocks=0, restart_marker_rows=0, components=3) -> Params:
     """Checked call parameters: quality an integer in 1..100, subsampling '4:4:4', '4:2:2' or '4:2:0',
-    the restart keywords integers in 0..65535."""
+    the restart keywords integers in 0..65535, components 3 (RGB images, YCbCr files) or 1 (gray
+    images, one-component files)."""
     if isinstance(quality, bool) or not isinstance(quality, (int, np.integer)) or not 1 <= quality <= 100:
         raise ValueError(f'quality must be an integer in 1..100, not {quality!r}')
     if subsampling not in SAMPLINGS:
         raise ValueError(f"subsampling must be '4:4:4', '4:2:2' or '4:2:0', not {subsampling!r}")
     blocks = _check_restart('restart_marker_blocks', restart_marker_blocks)
     rows = _check_restart('restart_marker_rows', restart_marker_rows)
-    return Params(int(quality), SAMPLINGS[subsampling], blocks, rows)
+    if components not in (1, 3) or isinstance(components, bool):
+        raise ValueError(f'components must be 3 or 1, not {components!r}')
+    return Params(int(quality), SAMPLINGS[subsampling], blocks, rows, int(components))
 
 
 def _check_size(shape, h, w):
@@ -128,9 +134,15 @@ CODEC_PROG = B.Codec('jpegprog', lambda: load_jpegprog(), Image, _check_size)
 
 def codec(p: Params, optimize=False, progressive=False) -> B.Codec:
     """libj2pjpegenc.so, or libj2pjpegopt.so when optimize, or libj2pjpegprog.so when progressive
-    (whatever optimize), for the shared driver, with the call parameters p."""
+    (whatever optimize), for the shared driver, with the call parameters p: it takes one-channel
+    images when p is gray (p.components == 1), three-channel ones otherwise."""
     c = CODEC_PROG if progressive else CODEC_OPT if optimize else CODEC
-    return dataclasses.replace(c, params=(C.byref(p),))
+    return dataclasses.replace(c, params=(C.byref(p),), channels=(1,) if p.components == 1 else c.channels)
+
+
+def _codecs(quality, subsampling, optimize, progressive, restart_marker_blocks, restart_marker_rows):
+    """The codec of each channel count encode_jpeg takes: {3: RGB, 1: gray}."""
+    return {c: codec(params(quality, subsampling, restart_marker_blocks, restart_marker_rows, c), optimize, progressive) for c in (3, 1)}
 
 
 def check_optimize(optimize):
@@ -165,12 +177,15 @@ def _work_bytes(descs, p):
 
 
 def encode_host(images, quality=75, subsampling='4:2:0', layout='HWC', optimize=False, progressive=False, restart_marker_blocks=0,
-                restart_marker_rows=0):
+                restart_marker_rows=0, gray=False):
     """The serial host driver (j2p_jpegenc_encode_host, or j2p_jpegopt_encode_host when optimize,
     or j2p_jpegprog_encode_host when progressive) on numpy uint8 arrays: a list of JPEG files as
-    bytes, the same bytes the device writes."""
+    bytes, the same bytes the device writes.  The arrays are RGB, or with gray=True all gray,
+    (h, w, 1) or (1, h, w), written as one-component files."""
     B.check_layout(layout)
-    p = params(quality, subsampling, restart_marker_blocks, restart_marker_rows)
+    if not isinstance(gray, bool):
+        raise ValueError(f'gray must be True or False, not {gray!r}')
+    p = params(quality, subsampling, restart_marker_blocks, restart_marker_rows, 1 if gray else 3)
     check_optimize(optimize)
     check_progressive(progressive)
     for x in images:
@@ -181,7 +196,7 @@ def encode_host(images, quality=75, subsampling='4:2:0', layout='HWC', optimize=
 
 def encode_jpeg(images, *, quality=75, subsampling='4:2:0', layout='CHW', optimize=False, progressive=False, restart_marker_blocks=0,
                 restart_marker_rows=0):
-    """Encode RGB CUDA tensors as baseline or progressive JPEG files on the device.
+    """Encode RGB or gray CUDA tensors as baseline or progressive JPEG files on the device.
 
     images: one tensor or a list or tuple of them, torch.uint8, shaped (3, h, w) for layout='CHW'
     or (h, w, 3) for 'HWC', with any strides, 1..65535 pixels high and wide.  quality: an integer
@@ -190,6 +205,14 @@ def encode_jpeg(images, *, quality=75, subsampling='4:2:0', layout='CHW', optimi
     `save(f, 'JPEG', quality=quality, subsampling=subsampling, optimize=optimize,
     progressive=progressive, restart_marker_blocks=restart_marker_blocks,
     restart_marker_rows=restart_marker_rows)`.
+
+    A tensor with one channel, (1, h, w) or (h, w, 1) (what decode_jpeg(mode='UNCHANGED' or
+    'GRAY') returns), is written as a one-component file: Pillow's file of the 'L' image, with every
+    keyword applied as to a colour image.  subsampling changes no coded byte of a gray file, only
+    the sampling factors its SOF declares (2 x 2 for the default '4:2:0', as Pillow writes them).
+    Pillow saving an 'L' image without a subsampling keyword declares 1 x 1: that file is
+    subsampling='4:4:4' here.
+    Gray and RGB images mix in one list; each kind is one library call.
 
     optimize: False writes the Annex K Huffman tables; True builds each image's tables from its own
     symbol counts, on the device, as libjpeg does for `optimize=True`: the same coefficients, files
@@ -219,7 +242,7 @@ def encode_jpeg(images, *, quality=75, subsampling='4:2:0', layout='CHW', optimi
     a CUDA device, and RuntimeError when no CUDA device is usable.
     """
     B.check_layout(layout)
-    p = params(quality, subsampling, restart_marker_blocks, restart_marker_rows)
+    codecs = _codecs(quality, subsampling, optimize, progressive, restart_marker_blocks, restart_marker_rows)
     check_optimize(optimize)
     check_progressive(progressive)
-    return B.encode_tensors('encode_jpeg', codec(p, optimize, progressive), images, layout, (torch.uint8,))
+    return B.encode_tensors('encode_jpeg', codecs, images, layout, (torch.uint8,))

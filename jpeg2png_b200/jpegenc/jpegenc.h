@@ -33,6 +33,17 @@
  * bound above, and each costs a stream descriptor, a 256-block tile, an 8 KiB stuffing chunk and
  * 16 bytes of rounding words of work area (jpegenc_plan.h).  Values above 65535 are refused, where
  * libjpeg would write DRI mod 65536 and count the full value (a corrupt file).
+ *
+ * Gray images (params->components == 1; 0 or 3 is colour): each image is one 8-bit channel, data
+ * its first sample, chan_stride not read.  The file is the one libjpeg writes for a one-component
+ * (Pillow 'L') image: SOI; the same APP0; DQT of table 0 only; SOF0 with component 1 and sampling
+ * byte 0x11, 0x21 or 0x22 for 4:4:4, 4:2:2 and 4:2:0 (it changes no coded byte); DHT DC0 and AC0;
+ * SOS of one component, 01 01 00 00 3f 00; 328 bytes before the entropy-coded data.  The scan walks
+ * the component's own ceil(w/8) x ceil(h/8) block grid in raster order, one block per MCU, with no
+ * dummy blocks; the samples are the pixels minus 128 (no colour conversion), the last row and
+ * column repeated past the image.  With restart_marker_rows = r an interval is min(r x ceil(w/8),
+ * 65535) blocks.  A block costs at most the luma bound, 1658 bits.  The kind belongs to the call,
+ * so a list of gray and colour images is two calls.  Any other components value is refused.
  */
 #ifndef J2P_JPEGENC_H
 #define J2P_JPEGENC_H
@@ -49,7 +60,7 @@ extern "C" {
 enum j2p_jpegenc_sampling { J2P_JPEGENC_444 = 0, J2P_JPEGENC_422 = 1, J2P_JPEGENC_420 = 2 };
 
 struct j2p_jpegenc_image {
-        const void *data;               /* first sample (R of the top-left pixel), uint8 */
+        const void *data;               /* first sample (R of the top-left pixel, or its gray value), uint8 */
         uint32_t width, height;         /* 1 .. 65535 */
         int64_t row_stride, col_stride, chan_stride;      /* in samples */
 };
@@ -60,6 +71,7 @@ struct j2p_jpegenc_params {
         int restart_marker_blocks;      /* 0 .. 65535: a restart interval of this many MCUs in every scan; 0 none */
         int restart_marker_rows;        /* 0 .. 65535: one of this many MCU rows per scan (capped at 65535
                                            MCUs); overrides restart_marker_blocks; 0 none */
+        int components;                 /* 0 or 3: RGB images, YCbCr files; 1: gray images, one-component files */
 };
 
 struct j2p_jpegenc_stats {
@@ -69,8 +81,8 @@ struct j2p_jpegenc_stats {
 
 /* Work area for the n images: work_bytes in all, the files at out_offset in it.  Refuses null
  * pointers, n == 0, a width or height of 0 or above 65535 (SOF's 16-bit fields), a quality outside
- * 1 .. 100, an unknown sampling and a restart field outside 0 .. 65535.  Returns 0, or -1
- * (j2p_jpegenc_last_error). */
+ * 1 .. 100, an unknown sampling, a restart field outside 0 .. 65535 and components other than 0, 1
+ * or 3.  Returns 0, or -1 (j2p_jpegenc_last_error). */
 int j2p_jpegenc_plan(const struct j2p_jpegenc_image *images, unsigned n, const struct j2p_jpegenc_params *params, size_t *work_bytes,
                      size_t *out_offset);
 

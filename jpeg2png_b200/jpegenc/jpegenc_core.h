@@ -17,6 +17,10 @@
 //   quantise   libjpeg-turbo's reciprocal multiply by (q << 3), with its rounding correction;
 //   coding     DC predicted along the scan order per component, the Annex K tables, ZRL and EOB,
 //              the last byte padded with 1-bits, each 0xFF followed by a stuffed 0x00.
+//
+// A gray call (j2p_je_tables.nc == 1) is the same steps for one component: libjpeg's null gray
+// conversion (the pixel minus 128), luma sampling 1 x 1 whatever the SOF declares, one block per
+// MCU, so the MCU grid is the block grid, no dummies, and the DC predicted along the raster.
 #ifndef J2P_JPEGENC_CORE_H
 #define J2P_JPEGENC_CORE_H
 
@@ -36,6 +40,8 @@ static_assert(J2P_JE_WORDS_PER_BLOCK * 32 % 8 == 0, "the padding of a stream's l
 #define J2P_JE_CHUNK 8192u              // entropy bytes per chunk of the stuffing kernels
 #define J2P_JE_HEAD 623u                // SOI .. SOS: 2 + 18 + 2 x 69 + 19 + 2 x 33 + 2 x 183 + 14
 #define J2P_JE_SOF_AT 158u              // offset of SOF0 in the header (its height follows at + 5)
+#define J2P_JE_HEAD_GRAY 328u           // a gray file's: 2 + 18 + 69 + 13 + 33 + 183 + 10
+#define J2P_JE_SOF_AT_GRAY 89u
 
 // per image of a call, or per bit stream (host plan, read by the kernels).  A stream is an image's
 // scan, or one restart interval of it; it carries its image's fields, and blk0, nblk, the tiles,
@@ -73,11 +79,18 @@ struct j2p_je_tables {
         uint8_t shift[2][64];           // total right shift of the product
         struct j2p_je_huff huff;        // the Annex K tables
         uint8_t zz[64];                 // zig-zag position of each natural index
-        uint32_t hs, vs;                // luma sampling factors (chroma 1 x 1)
+        uint32_t hs, vs;                // luma sampling factors (chroma 1 x 1); 1 x 1 for gray
+        uint32_t nc;                    // components: 3, or 1 for gray
+        uint32_t head_len, sof_at;      // the header template's length and the offset of its SOF
         uint8_t head[J2P_JE_HEAD];
 };
 
-J2P_HD uint32_t j2p_je_bpm(const struct j2p_je_tables *t) { return t->hs * t->vs + 2; }
+// blocks per MCU: the luma blocks and two chroma blocks, or a gray file's one block
+J2P_HD uint32_t j2p_je_bpm(const struct j2p_je_tables *t) { return t->hs * t->vs + t->nc - 1; }
+
+// the end of the template's SOF (10 + 3 bytes per component) and the length of the SOS that ends it
+J2P_HD uint32_t j2p_je_sof_end(const struct j2p_je_tables *t) { return t->sof_at + 10 + 3 * t->nc; }
+J2P_HD uint32_t j2p_je_sos_len(const struct j2p_je_tables *t) { return 8 + 2 * t->nc; }
 
 
 // ---- geometry -------------------------------------------------------------------------------------
@@ -148,6 +161,8 @@ J2P_HD int j2p_je_conv(int comp, int r, int g, int b) {
 J2P_HD int j2p_je_sample(const struct j2p_je_img *im, const struct j2p_je_tables *t, uint32_t comp, uint32_t y, uint32_t x) {
         int r, g, b;
         const uint32_t W = im->w - 1, H = im->h - 1;
+        if (t->nc == 1)                                 // gray: the pixel itself
+                return im->src[(int64_t)(y < H ? y : H) * im->s_row + (int64_t)(x < W ? x : W) * im->s_col] - 128;
         if (comp == 0 || t->hs == 1) {                  // full size
                 j2p_je_rgb(im, y < H ? y : H, x < W ? x : W, &r, &g, &b);
                 return j2p_je_conv((int)comp, r, g, b) - 128;
@@ -325,7 +340,7 @@ J2P_HD uint32_t j2p_je_pad(uint64_t bits, uint64_t *word) {
 
 // the header with the image's size in SOF0
 J2P_HD uint8_t j2p_je_head_byte(const struct j2p_je_tables *t, const struct j2p_je_img *im, uint32_t k) {
-        const uint32_t s = J2P_JE_SOF_AT;
+        const uint32_t s = t->sof_at;
         if (k == s + 5) return (uint8_t)(im->h >> 8);
         if (k == s + 6) return (uint8_t)im->h;
         if (k == s + 7) return (uint8_t)(im->w >> 8);

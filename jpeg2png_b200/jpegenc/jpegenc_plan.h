@@ -107,10 +107,25 @@ static uint8_t *put_dht(uint8_t *o, int index, const uint8_t *bits, const uint8_
     return o + 16 + n;
 }
 
+// whether a call is gray (one-component files)
+static bool is_gray(const struct j2p_jpegenc_params *p) { return p->components == 1; }
+
+// the luma sampling factors the SOF declares
+static uint32_t sof_hs(const struct j2p_jpegenc_params *p) { return p->sampling == J2P_JPEGENC_444 ? 1 : 2; }
+static uint32_t sof_vs(const struct j2p_jpegenc_params *p) { return p->sampling == J2P_JPEGENC_420 ? 2 : 1; }
+
+// the length of the call's header template
+static uint32_t head_len_of(const struct j2p_jpegenc_params *p) { return is_gray(p) ? J2P_JE_HEAD_GRAY : J2P_JE_HEAD; }
+
 static void make_tables(const struct j2p_jpegenc_params *p, struct j2p_je_tables *t) {
     memset(t, 0, sizeof *t);
-    t->hs = p->sampling == J2P_JPEGENC_444 ? 1 : 2;
-    t->vs = p->sampling == J2P_JPEGENC_420 ? 2 : 1;
+    const bool gray = is_gray(p);
+    t->hs = gray ? 1 : sof_hs(p);       // a gray component is sampled 1 x 1 whatever the SOF says
+    t->vs = gray ? 1 : sof_vs(p);
+    t->nc = gray ? 1 : 3;
+    t->head_len = head_len_of(p);
+    t->sof_at = gray ? J2P_JE_SOF_AT_GRAY : J2P_JE_SOF_AT;
+    const int ntbl = gray ? 1 : 2;
     uint16_t q[2][64];
     for (int tbl = 0; tbl < 2; tbl++) {
         quant_table(p->quality, tbl, q[tbl]);
@@ -127,27 +142,30 @@ static void make_tables(const struct j2p_jpegenc_params *p, struct j2p_je_tables
     static const uint8_t app0[18] = {0xff, 0xe0, 0, 16, 'J', 'F', 'I', 'F', 0, 1, 1, 0, 0, 1, 0, 1, 0, 0};
     memcpy(o, app0, 18);
     o += 18;
-    for (int tbl = 0; tbl < 2; tbl++) {
+    for (int tbl = 0; tbl < ntbl; tbl++) {
         o = put16(o, 0xffdb);
         o = put16(o, 67);
         *o++ = (uint8_t)tbl;
         for (int k = 0; k < 64; k++) *o++ = (uint8_t)q[tbl][kNatural[k]];
     }
     o = put16(o, 0xffc0);               // the size is patched per image (j2p_je_head_byte)
-    o = put16(o, 17);
+    o = put16(o, 8 + 3 * t->nc);
     *o++ = 8;
     o = put16(o, 0);
     o = put16(o, 0);
-    *o++ = 3;
-    const uint8_t comps[9] = {1, (uint8_t)(t->hs << 4 | t->vs), 0, 2, 0x11, 1, 3, 0x11, 1};
-    memcpy(o, comps, 9);
-    o += 9;
+    *o++ = (uint8_t)t->nc;
+    const uint8_t comps[9] = {1, (uint8_t)(sof_hs(p) << 4 | sof_vs(p)), 0, 2, 0x11, 1, 3, 0x11, 1};
+    memcpy(o, comps, 3 * t->nc);
+    o += 3 * t->nc;
     o = put_dht(o, 0x00, kDcBits[0], kDcVals);
     o = put_dht(o, 0x10, kAcBits[0], kAcVals[0]);
-    o = put_dht(o, 0x01, kDcBits[1], kDcVals);
-    o = put_dht(o, 0x11, kAcBits[1], kAcVals[1]);
+    if (!gray) {
+        o = put_dht(o, 0x01, kDcBits[1], kDcVals);
+        o = put_dht(o, 0x11, kAcBits[1], kAcVals[1]);
+    }
     static const uint8_t sos[14] = {0xff, 0xda, 0, 12, 3, 1, 0x00, 2, 0x11, 3, 0x11, 0, 63, 0};
-    memcpy(o, sos, 14);
+    static const uint8_t sos_gray[10] = {0xff, 0xda, 0, 8, 1, 1, 0x00, 0, 63, 0};
+    memcpy(o, gray ? sos_gray : sos, j2p_je_sos_len(t));
 }
 
 // ---- restart intervals -------------------------------------------------------------------------
@@ -165,7 +183,6 @@ static uint32_t restart_interval(const struct j2p_jpegenc_params *p, uint32_t pe
 
 #define J2P_JE_DRI 6u                   // DRI: FF DD 00 04 Ri
 #define J2P_JE_RST 2u                   // RSTm: FF D0+m, not stuffed
-#define J2P_JE_SOS 14u                  // the SOS of the interleaved scan that ends a baseline header
 
 // byte k of DRI for the interval ri
 J2P_HD uint8_t j2p_je_dri_byte(uint32_t ri, uint32_t k) {
@@ -198,12 +215,14 @@ J2P_HD uint8_t j2p_je_stream_byte(const struct j2p_je_img *st, uint32_t k, Head 
 }
 
 // the length of a baseline stream's header with the call's template
-J2P_HD uint32_t j2p_je_fixed_head_len(const struct j2p_je_img *st) { return st->part ? J2P_JE_RST : J2P_JE_HEAD + (st->ri ? J2P_JE_DRI : 0); }
+J2P_HD uint32_t j2p_je_fixed_head_len(const struct j2p_je_tables *t, const struct j2p_je_img *st) {
+    return st->part ? J2P_JE_RST : t->head_len + (st->ri ? J2P_JE_DRI : 0);
+}
 
 // byte k of a baseline scan header with the call's template: SOI .. SOS with the image's size and
 // its DRI
 J2P_HD uint8_t j2p_je_scan_head_byte(const struct j2p_je_tables *t, const struct j2p_je_img *st, uint32_t k) {
-    return j2p_je_dri_head(st->ri, J2P_JE_HEAD, J2P_JE_SOS, k, [&](uint32_t k1) { return j2p_je_head_byte(t, st, k1); });
+    return j2p_je_dri_head(st->ri, t->head_len, j2p_je_sos_len(t), k, [&](uint32_t k1) { return j2p_je_head_byte(t, st, k1); });
 }
 
 // byte k of a baseline stream's header: the scan header, or the stream's RST
@@ -246,6 +265,8 @@ static int check_call(const struct j2p_jpegenc_image *im, unsigned n, const stru
         return fail("restart_marker_blocks must be 0 .. 65535 (got %d)", p->restart_marker_blocks);
     if (p->restart_marker_rows < 0 || p->restart_marker_rows > 65535)
         return fail("restart_marker_rows must be 0 .. 65535 (got %d)", p->restart_marker_rows);
+    if (p->components != 0 && p->components != 1 && p->components != 3)
+        return fail("components must be 0 or 3 (colour) or 1 (gray) (got %d)", p->components);
     for (unsigned i = 0; i < n; i++) {
         const struct j2p_jpegenc_image *x = &im[i];
         if (!x->data) return fail("image %u: null data pointer", i);
@@ -255,20 +276,22 @@ static int check_call(const struct j2p_jpegenc_image *im, unsigned n, const stru
     return 0;
 }
 
-// image i's descriptor, its blocks from blk0: what the blocks step reads (the stream fields are 0)
+// image i's descriptor, its blocks from blk0: what the blocks step reads (the stream fields are 0).
+// A gray image's MCU is one block, so its MCU grid is its block grid.
 static void image_desc(const struct j2p_jpegenc_image *x, uint32_t i, const struct j2p_jpegenc_params *p, uint64_t blk0, struct j2p_je_img *g) {
-    const uint32_t hs = p->sampling == J2P_JPEGENC_444 ? 1 : 2, vs = p->sampling == J2P_JPEGENC_420 ? 2 : 1;
+    const bool gray = is_gray(p);
+    const uint32_t hs = gray ? 1 : sof_hs(p), vs = gray ? 1 : sof_vs(p), bpm = gray ? 1 : hs * vs + 2;
     memset(g, 0, sizeof *g);
     g->src = (const uint8_t *)x->data;
     g->s_row = x->row_stride;
     g->s_col = x->col_stride;
-    g->s_chan = x->chan_stride;
+    g->s_chan = gray ? 0 : x->chan_stride;
     g->w = x->width;
     g->h = x->height;
     g->mcux = (x->width + 8 * hs - 1) / (8 * hs);
     g->mcuy = (x->height + 8 * vs - 1) / (8 * vs);
     g->blk0 = blk0;
-    g->nblk = (uint64_t)g->mcux * g->mcuy * (hs * vs + 2);
+    g->nblk = (uint64_t)g->mcux * g->mcuy * bpm;
     g->img = i;
 }
 
@@ -340,7 +363,7 @@ static int make_plan(const struct j2p_jpegenc_image *im, unsigned n, const struc
         if (imgs && restarts) imgs[i] = g;
         for (uint64_t q = 0; q < parts; q++) {
             const uint64_t m0 = q * ri, m1 = ri && m0 + ri < mcus ? m0 + ri : mcus;
-            sp.add(g, nblk + m0 * bpm, (m1 - m0) * bpm, wpb, q ? J2P_JE_RST : J2P_JE_HEAD + (ri ? J2P_JE_DRI : 0), q + 1 == parts ? 2 : 0, 0,
+            sp.add(g, nblk + m0 * bpm, (m1 - m0) * bpm, wpb, q ? J2P_JE_RST : head_len_of(p) + (ri ? J2P_JE_DRI : 0), q + 1 == parts ? 2 : 0, 0,
                    (uint32_t)q, ri, strs ? &strs[sp.ns] : nullptr);
         }
         nblk += g.nblk;
@@ -427,7 +450,7 @@ static void host_blocks(const struct j2p_je_img *im, const struct j2p_je_tables 
 struct FixedCodes {
     const struct j2p_je_tables *t;
     const struct j2p_je_huff *huff(uint32_t) const { return &t->huff; }
-    uint32_t head_len(const struct j2p_je_img *st) const { return j2p_je_fixed_head_len(st); }
+    uint32_t head_len(const struct j2p_je_img *st) const { return j2p_je_fixed_head_len(t, st); }
     uint8_t head_byte(const struct j2p_je_img *st, uint32_t k) const { return j2p_je_fixed_head_byte(t, st, k); }
 };
 

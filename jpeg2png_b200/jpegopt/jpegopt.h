@@ -18,6 +18,10 @@
  * Work-area bound: with optimized tables any code can be 16 bits long, so a block costs at most
  * 16 + 11 bits of DC and 63 x (16 + 10) of AC, J2P_JPEGOPT_BLOCK_BITS = 1665 (jpegenc.h's bound,
  * 1658, holds for the Annex K tables only).
+ *
+ * Gray calls (components == 1, jpegenc.h): each image counts and builds two tables, DC0 and AC0,
+ * and its header is jpegenc.h's gray header with its own DHT 0x00 and 0x10.  The work-area bound
+ * is the same J2P_JPEGOPT_BLOCK_BITS per block, and a call still runs the nine kernels once.
  */
 #ifndef J2P_JPEGOPT_H
 #define J2P_JPEGOPT_H

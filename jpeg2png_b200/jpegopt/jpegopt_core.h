@@ -4,7 +4,8 @@
 //
 //   counts     per image and table, the symbols j2p_je_symbols walks (dummy blocks included): table
 //              0 counts the luma DC categories, 1 the luma AC symbols, 2 and 3 those of Cb and Cr
-//              together; a pseudo-symbol 256 with count 1 keeps any real code from being all 1-bits;
+//              together (a gray image has tables 0 and 1 only, and its header DHTs 0x00 and 0x10);
+//              a pseudo-symbol 256 with count 1 keeps any real code from being all 1-bits;
 //   lengths    T.81 Annex K.2: merge the two least counts until one node is left, lengthening both
 //              chains through others[].  V1 is the highest-numbered symbol among those of least
 //              nonzero count (a `<=` scan from 0 to 256), V2 the same without V1;
@@ -186,15 +187,21 @@ J2P_HD void j2p_jo_table(const uint64_t *counts, struct j2p_jo_scratch *s, struc
         if (L.lane == 0) j2p_je_derive(d->bits[tb], d->vals[tb], h->code[tb], h->size[tb]);
 }
 
-J2P_HD uint32_t j2p_jo_head_len(const struct j2p_jo_dht *d) {
-        return J2P_JO_HEAD_PRE + 4 * 21 + d->nvals[0] + d->nvals[1] + d->nvals[2] + d->nvals[3] + J2P_JO_SOS;
+// the tables of an image of the call: DC0, AC0, DC1, AC1, or a gray image's DC0 and AC0
+J2P_HD uint32_t j2p_jo_ntables(const struct j2p_je_tables *t) { return t->nc == 1 ? 2 : 4; }
+
+J2P_HD uint32_t j2p_jo_head_len(const struct j2p_je_tables *t, const struct j2p_jo_dht *d) {
+        uint32_t n = j2p_je_sof_end(t) + j2p_je_sos_len(t);
+        for (uint32_t tb = 0; tb < j2p_jo_ntables(t); tb++) n += 21 + d->nvals[tb];
+        return n;
 }
 
 // byte k of an image's header: the template's SOI .. SOF0 with the image's size, its own DHTs, SOS
 J2P_HD uint8_t j2p_jo_head_byte(const struct j2p_je_tables *t, const struct j2p_je_img *im, const struct j2p_jo_dht *d, uint32_t k) {
-        if (k < J2P_JO_HEAD_PRE) return j2p_je_head_byte(t, im, k);
-        k -= J2P_JO_HEAD_PRE;
-        for (int tb = 0; tb < 4; tb++) {
+        const uint32_t pre = j2p_je_sof_end(t);
+        if (k < pre) return j2p_je_head_byte(t, im, k);
+        k -= pre;
+        for (int tb = 0; tb < (int)j2p_jo_ntables(t); tb++) {
                 const uint32_t nv = d->nvals[tb], len = 2 + 2 + 1 + 16 + nv;
                 if (k < len) {
                         if (k < 2) return k ? 0xc4 : 0xff;
@@ -205,14 +212,16 @@ J2P_HD uint8_t j2p_jo_head_byte(const struct j2p_je_tables *t, const struct j2p_
                 }
                 k -= len;
         }
-        return t->head[J2P_JE_HEAD - J2P_JO_SOS + k];
+        return t->head[t->head_len - j2p_je_sos_len(t) + k];
 }
 
 // an image's file header: j2p_jo_head_byte with the image's DRI before the SOS when it has restarts
-J2P_HD uint32_t j2p_jo_file_head_len(const struct j2p_je_img *im, const struct j2p_jo_dht *d) { return j2p_jo_head_len(d) + (im->ri ? J2P_JE_DRI : 0); }
+J2P_HD uint32_t j2p_jo_file_head_len(const struct j2p_je_tables *t, const struct j2p_je_img *im, const struct j2p_jo_dht *d) {
+        return j2p_jo_head_len(t, d) + (im->ri ? J2P_JE_DRI : 0);
+}
 
 J2P_HD uint8_t j2p_jo_file_head_byte(const struct j2p_je_tables *t, const struct j2p_je_img *im, const struct j2p_jo_dht *d, uint32_t k) {
-        return j2p_je_dri_head(im->ri, j2p_jo_head_len(d), J2P_JO_SOS, k, [&](uint32_t k1) { return j2p_jo_head_byte(t, im, d, k1); });
+        return j2p_je_dri_head(im->ri, j2p_jo_head_len(t, d), j2p_je_sos_len(t), k, [&](uint32_t k1) { return j2p_jo_head_byte(t, im, d, k1); });
 }
 
 #endif  // J2P_JPEGOPT_CORE_H

@@ -38,22 +38,24 @@ static StreamPlan prog_streams(const struct j2p_je_img *imgs, unsigned n, const 
                                struct j2p_je_img *strs, struct j2p_jp_scanplan *scs, uint64_t *nsblk) {
     StreamPlan sp;
     uint64_t sblk = 0;
+    const bool g = j2p_jp_gray(t);
+    const uint32_t per = j2p_jp_nscans(g);
     for (unsigned i = 0; i < n; i++) {
         const struct j2p_je_img *im = &imgs[i];
         uint32_t last_ri = 0;                                   // the interval of the last DRI written
-        for (uint32_t k = 0; k < J2P_JP_SCANS; k++) {
-            const bool ac = j2p_jp_is_ac(k);
-            const uint32_t comp = j2p_jp_scan_of(k).comp, wpb = j2p_jp_bound_words(k);
+        for (uint32_t k = 0; k < per; k++) {
+            const bool ac = j2p_jp_is_ac(g, k);
+            const uint32_t comp = j2p_jp_scan_of(g, k).comp, wpb = j2p_jp_bound_words(g, k);
             // an MCU of an AC scan is one block of the component's own grid; of a DC scan, an MCU of the image
             const uint32_t per_row = ac ? j2p_jp_grid_w(im, t, comp) : im->mcux, upm = ac ? 1 : j2p_je_bpm(t);
             const uint64_t mcus = ac ? (uint64_t)per_row * j2p_jp_grid_h(im, t, comp) : (uint64_t)im->mcux * im->mcuy;
             const uint32_t ri = restart_interval(p, per_row);
             const uint64_t parts = ri ? (mcus + ri - 1) / ri : 1;
-            if (scs) scs[(size_t)i * J2P_JP_SCANS + k] = {(uint32_t)sp.ns, ri != last_ri ? ri : 0u};
+            if (scs) scs[(size_t)i * per + k] = {(uint32_t)sp.ns, ri != last_ri ? ri : 0u};
             last_ri = ri;
             for (uint64_t q = 0; q < parts; q++) {
                 const uint64_t m0 = q * ri, m1 = ri && m0 + ri < mcus ? m0 + ri : mcus;
-                sp.add(*im, sblk + m0 * upm, (m1 - m0) * upm, wpb, q ? J2P_JE_RST : J2P_JP_HEAD, k + 1 == J2P_JP_SCANS && q + 1 == parts ? 2 : 0, k,
+                sp.add(*im, sblk + m0 * upm, (m1 - m0) * upm, wpb, q ? J2P_JE_RST : J2P_JP_HEAD, k + 1 == per && q + 1 == parts ? 2 : 0, k,
                        (uint32_t)q, ri, strs ? &strs[sp.ns] : nullptr);
             }
             sblk += mcus * upm;
@@ -77,7 +79,7 @@ static int prog_plan(const struct j2p_jpegenc_image *im, unsigned n, const struc
     uint64_t sblk;
     const StreamPlan sp = prog_streams(imgs.data(), n, p, &t, nullptr, nullptr, &sblk);
     if (sp.check(nblk) != 0) return -1;
-    const size_t nsc = (size_t)n * J2P_JP_SCANS;
+    const size_t nsc = (size_t)n * j2p_jp_nscans(j2p_jp_gray(&t));
     size_t o = 0;
     P->off_imgs = o;  o = align16(o + n * sizeof(struct j2p_je_img));
     P->off_tab = o;   o = align16(o + sizeof(struct j2p_je_tables));
@@ -133,19 +135,24 @@ struct Ctx {
     const int16_t *coef;
     const uint8_t *summ;
     const uint32_t *state;
-    bool plain;                         // no restart intervals: stream s is scan s % 10 of image s / 10
+    bool plain;                         // no restart intervals: stream s is scan s % 10 of image s / 10 (6 for gray)
+    bool gray;                          // the call's images are gray: the six-scan script
 };
 
 // the scan and the image of stream s: arithmetic without restart intervals, the descriptor with them
-J2P_HD uint32_t scan_of(const Ctx &x, uint32_t s) { return x.plain ? s % J2P_JP_SCANS : x.strs[s].scan; }
-J2P_HD uint32_t image_of(const Ctx &x, uint32_t s) { return x.plain ? s / J2P_JP_SCANS : x.strs[s].img; }
+J2P_HD uint32_t scan_of(const Ctx &x, uint32_t s) {
+    return x.plain ? (x.gray ? s % J2P_JP_SCANS_GRAY : s % J2P_JP_SCANS) : x.strs[s].scan;
+}
+J2P_HD uint32_t image_of(const Ctx &x, uint32_t s) {
+    return x.plain ? (x.gray ? s / J2P_JP_SCANS_GRAY : s / J2P_JP_SCANS) : x.strs[s].img;
+}
 
 // the first block of stream s in its scan's order (the MCU grid's stored order for a DC scan, the
 // component's raster order for an AC scan): a multiple of an MCU, so a DC prediction restarts there
 J2P_HD uint64_t stream_first(const Ctx &x, uint32_t s) {
     if (x.plain) return 0;
     const struct j2p_je_img *st = &x.strs[s];
-    return (uint64_t)st->part * st->ri * (j2p_jp_is_ac(st->scan) ? 1u : j2p_je_bpm(x.t));
+    return (uint64_t)st->part * st->ri * (j2p_jp_is_ac(x.gray, st->scan) ? 1u : j2p_je_bpm(x.t));
 }
 
 // the coefficients of block j of an AC scan over component comp of image im
@@ -161,10 +168,10 @@ template <class Out>
 J2P_HD void code_block(const Ctx &x, uint32_t s, uint64_t j, Out &o) {
     const uint32_t k = scan_of(x, s);
     const struct j2p_je_img *st = &x.strs[s], *im = &x.imgs[image_of(x, s)];
-    const struct j2p_jp_scan sc = j2p_jp_scan_of(k);
+    const struct j2p_jp_scan sc = j2p_jp_scan_of(x.gray, k);
     const uint64_t f = stream_first(x, s);
     const bool last = j + 1 == st->nblk;
-    if (j2p_jp_is_ac(k))
+    if (j2p_jp_is_ac(x.gray, k))
         j2p_jp_code(sc, ac_coef(x, im, sc.comp, f + j), 0, sc.comp, x.state[st->blk0 + j], j, last, o);
     else
         j2p_jp_code(sc, x.coef + (im->blk0 + f + j) * 64, pred_of(x.t, x.coef, im->blk0 + f, j), comp_of(x.t, j), 0, j, last, o);
@@ -172,7 +179,7 @@ J2P_HD void code_block(const Ctx &x, uint32_t s, uint64_t j, Out &o) {
 
 // the summary of block j of AC stream s
 J2P_HD uint32_t summary_of(const Ctx &x, uint32_t s, uint64_t j) {
-    const struct j2p_jp_scan sc = j2p_jp_scan_of(scan_of(x, s));
+    const struct j2p_jp_scan sc = j2p_jp_scan_of(x.gray, scan_of(x, s));
     return j2p_jp_summary(sc, ac_coef(x, &x.imgs[image_of(x, s)], sc.comp, stream_first(x, s) + j));
 }
 
@@ -207,20 +214,21 @@ struct EmitBits {
     // the correction bits of the run's blocks that have any, in order
     J2P_HD void deferred(uint64_t first, uint32_t run, uint32_t) {
         const struct j2p_je_img *st = &x.strs[s], *im = &x.imgs[image_of(x, s)];
-        const struct j2p_jp_scan sc = j2p_jp_scan_of(scan_of(x, s));
+        const struct j2p_jp_scan sc = j2p_jp_scan_of(x.gray, scan_of(x, s));
         const uint64_t f = stream_first(x, s);
         for (uint64_t q = first; q < first + run; q++)
             if (x.summ[st->blk0 + q] & 63u) j2p_jp_tail(sc, ac_coef(x, im, sc.comp, f + q), *this);
     }
 };
 
-// the header of stream st: its scan's header (in heads, its length in hlens), or RST
-J2P_HD uint32_t prog_head_len(const uint32_t *hlens, const struct j2p_je_img *st) {
-    return st->part ? J2P_JE_RST : hlens[(size_t)st->img * J2P_JP_SCANS + st->scan];
+// the header of stream st: its scan's header (in heads, its length in hlens; per scans an image),
+// or RST
+static uint32_t prog_head_len(const uint32_t *hlens, uint32_t per, const struct j2p_je_img *st) {
+    return st->part ? J2P_JE_RST : hlens[(size_t)st->img * per + st->scan];
 }
 
-J2P_HD uint8_t prog_head_byte(const uint8_t *heads, const struct j2p_je_img *st, uint32_t k) {
-    return j2p_je_stream_byte(st, k, [&](uint32_t k1) { return heads[((size_t)st->img * J2P_JP_SCANS + st->scan) * J2P_JP_HEAD + k1]; });
+static uint8_t prog_head_byte(const uint8_t *heads, uint32_t per, const struct j2p_je_img *st, uint32_t k) {
+    return j2p_je_stream_byte(st, k, [&](uint32_t k1) { return heads[((size_t)st->img * per + st->scan) * J2P_JP_HEAD + k1]; });
 }
 
 // ---- host driver -------------------------------------------------------------------------------
@@ -242,11 +250,13 @@ extern "C" int j2p_jpegprog_encode_host(const struct j2p_jpegenc_image *images, 
     struct j2p_jp_huff *huffs = (struct j2p_jp_huff *)(w + P.off_huff);
     uint8_t *heads = w + P.off_head, *out = w + P.off_out;
     memset(w + P.off_hist, 0, P.off_raw - P.off_hist + P.words * sizeof(uint32_t));
-    const Ctx x = {imgs, strs, t, coef, summ, state, P.plain};
+    const bool g = j2p_jp_gray(t);
+    const uint32_t per = j2p_jp_nscans(g);
+    const Ctx x = {imgs, strs, t, coef, summ, state, P.plain, g};
     for (unsigned i = 0; i < n; i++) host_blocks(&imgs[i], t, coef);   // blocks
     for (uint32_t s = 0; s < P.ns; s++) {                               // summaries, runs
         const struct j2p_je_img *st = &strs[s];
-        if (!j2p_jp_is_ac(st->scan)) continue;
+        if (!j2p_jp_is_ac(g, st->scan)) continue;
         for (uint64_t j = 0; j < st->nblk; j++) summ[st->blk0 + j] = (uint8_t)summary_of(x, s, j);
         for (uint64_t j = 0; j < st->nblk; j++)
             if (j == 0 || (summ[st->blk0 + j - 1] & J2P_JP_RESET))
@@ -254,7 +264,7 @@ extern "C" int j2p_jpegprog_encode_host(const struct j2p_jpegenc_image *images, 
                             [&](uint64_t q, uint32_t v) { state[st->blk0 + q] = v; });
     }
     for (uint32_t s = 0; s < P.ns; s++) {                               // hist
-        uint64_t *h = hist + ((size_t)strs[s].img * J2P_JP_TABLES + j2p_jp_slot(strs[s].scan)) * 256;
+        uint64_t *h = hist + ((size_t)strs[s].img * J2P_JP_TABLES + j2p_jp_slot(g, strs[s].scan)) * 256;
         const auto count = [h](int tb, int v) { h[tb * 256 + v]++; };
         CountSymbols<decltype(count)> o = {count};
         for (uint64_t j = 0; j < strs[s].nblk; j++) code_block(x, s, j, o);
@@ -262,17 +272,17 @@ extern "C" int j2p_jpegprog_encode_host(const struct j2p_jpegenc_image *images, 
     for (unsigned i = 0; i < n; i++) {                                  // tables, scan headers
         struct j2p_jo_scratch scr;
         struct j2p_jp_dht d;
-        for (uint32_t tb = 0; tb < J2P_JP_TABLES; tb++)
+        for (uint32_t tb = 0; tb < j2p_jp_ntables(g); tb++)
             j2p_jp_table(hist + ((size_t)i * J2P_JP_TABLES + tb) * 256, &scr, &d, &huffs[(size_t)i * J2P_JP_TABLES + tb], tb, j2p_jo_serial());
-        for (uint32_t k = 0; k < J2P_JP_SCANS; k++) {
-            const size_t q = (size_t)i * J2P_JP_SCANS + k;
-            hlens[q] = j2p_jp_scan_head_len(&d, k, scs[q].dri);
+        for (uint32_t k = 0; k < per; k++) {
+            const size_t q = (size_t)i * per + k;
+            hlens[q] = j2p_jp_scan_head_len(t, &d, k, scs[q].dri);
             for (uint32_t b = 0; b < hlens[q]; b++) heads[q * J2P_JP_HEAD + b] = j2p_jp_scan_head_byte(t, &imgs[i], &d, k, scs[q].dri, b);
         }
     }
     for (uint32_t s = 0; s < P.ns; s++) {                               // sizes, emit, padding
         struct j2p_je_img *st = &strs[s];
-        const struct j2p_jp_huff *h = huffs + (size_t)st->img * J2P_JP_TABLES + j2p_jp_slot(st->scan);
+        const struct j2p_jp_huff *h = huffs + (size_t)st->img * J2P_JP_TABLES + j2p_jp_slot(g, st->scan);
         uint64_t pos = 0;
         for (uint64_t j = 0; j < st->nblk; j++) {
             CountBits c = {h, 0};
@@ -292,7 +302,7 @@ extern "C" int j2p_jpegprog_encode_host(const struct j2p_jpegenc_image *images, 
     for (uint32_t s = 0; s < P.ns; s++) {
         const struct j2p_je_img *st = &strs[s];
         if (s == 0 || strs[s - 1].img != st->img) offsets[st->img] = (uint64_t)(o - out);
-        for (uint32_t b = 0; b < prog_head_len(hlens, st); b++) *o++ = prog_head_byte(heads, st, b);
+        for (uint32_t b = 0; b < prog_head_len(hlens, per, st); b++) *o++ = prog_head_byte(heads, per, st, b);
         const uint32_t *rw = raw + st->raw_off;
         for (uint64_t j = 0; j < raw_bytes(st); j++) {
             const uint8_t v = j2p_je_byte(rw, j);
@@ -311,11 +321,11 @@ extern "C" int j2p_jpegprog_encode_host(const struct j2p_jpegenc_image *images, 
 // ---- device ------------------------------------------------------------------------------------
 static const int kTableThreads = 32 * J2P_JP_TABLES;    // one warp per table of an image
 
-// the derived tables of stream s (two for scan 0, one for an AC scan, none for the DC refine) into
-// shared memory, by every thread of the CTA
+// the derived tables of stream s (two for a colour scan 0, one for an AC scan or a gray scan 0, none
+// for the DC refine) into shared memory, by every thread of the CTA
 __device__ __forceinline__ const struct j2p_jp_huff *stage(struct j2p_jp_huff *sh, const struct j2p_jp_huff *huffs, const Ctx &x, uint32_t s) {
-    const uint32_t k = scan_of(x, s), nt = k == 0 ? 2 : j2p_jp_is_ac(k) ? 1 : 0;
-    const uint4 *src = (const uint4 *)(huffs + (size_t)image_of(x, s) * J2P_JP_TABLES + j2p_jp_slot(k));
+    const uint32_t k = scan_of(x, s), nt = j2p_jp_ntab(x.gray, k);
+    const uint4 *src = (const uint4 *)(huffs + (size_t)image_of(x, s) * J2P_JP_TABLES + j2p_jp_slot(x.gray, k));
     uint4 *dst = (uint4 *)sh;
     for (uint32_t q = threadIdx.x; q < nt * sizeof(struct j2p_jp_huff) / 16; q += blockDim.x) dst[q] = src[q];
     __syncthreads();
@@ -329,48 +339,74 @@ __device__ __forceinline__ uint32_t tile_block(const struct j2p_je_img *strs, ui
     return s;
 }
 
-// kBlockThreads threads, 8 per block: the shared blocks body, then each real block's summary in
-// each AC scan of its component (a lane per scan)
-__global__ void __launch_bounds__(kBlockThreads) k_jp_blocks(const struct j2p_je_img *__restrict__ imgs, uint32_t n,
-                                                            const struct j2p_je_tables *__restrict__ t, uint64_t nblk,
-                                                            int16_t *__restrict__ coef, const struct j2p_je_img *__restrict__ strs,
-                                                            const struct j2p_jp_scanplan *__restrict__ scs, bool plain,
-                                                            uint8_t *__restrict__ summ) {
-    blocks_body(imgs, n, t, nblk, coef);
-    __syncthreads();
+// x with the call's kind as the constant G.  k_jp_hist and k_jp_emit branch once on the kind, which
+// is uniform over the launch, and run their body with as_kind<true> or as_kind<false>, so each
+// kind's body is compiled for it alone; k_jp_blocks does the same with its summaries.
+template <bool G>
+__device__ __forceinline__ Ctx as_kind(Ctx x) {
+    x.gray = G;
+    return x;
+}
+
+// each real block's summary in each AC scan of its component (a lane per scan), G: gray
+template <bool G>
+__device__ __forceinline__ void summaries(const struct j2p_je_img *__restrict__ imgs, uint32_t n, const struct j2p_je_tables *__restrict__ t,
+                                          uint64_t nblk, const int16_t *__restrict__ coef, const struct j2p_je_img *__restrict__ strs,
+                                          const struct j2p_jp_scanplan *__restrict__ scs, bool plain, uint8_t *__restrict__ summ) {
     const uint64_t g = ((uint64_t)blockIdx.x * kBlockThreads + threadIdx.x) >> 3;
     if (g >= nblk) return;
     const uint32_t i = find_image(imgs, n, g, 0);
     const struct j2p_je_img *im = &imgs[i];
     const struct j2p_je_where wh = j2p_je_locate(im, t, g - im->blk0);
-    const int k = j2p_jp_comp_scan(wh.comp, threadIdx.x & 7);
+    const int k = j2p_jp_comp_scan(G, wh.comp, threadIdx.x & 7);
     if (wh.dummy || k < 0) return;
     const uint64_t j = (uint64_t)wh.row * j2p_jp_grid_w(im, t, wh.comp) + wh.col;
-    const size_t q = (size_t)i * J2P_JP_SCANS + k;
-    summ[strs[plain ? q : scs[q].s0].blk0 + j] = (uint8_t)j2p_jp_summary(j2p_jp_scan_of((uint32_t)k), coef + g * 64);
+    const size_t q = (size_t)i * j2p_jp_nscans(G) + k;
+    summ[strs[plain ? q : scs[q].s0].blk0 + j] = (uint8_t)j2p_jp_summary(j2p_jp_scan_of(G, (uint32_t)k), coef + g * 64);
 }
 
-// per block of an AC stream that starts a segment: the walk to the segment's end (a RESET block or
-// the stream's end, which a restart marker follows)
-__global__ void __launch_bounds__(kTileThreads) k_jp_runs(const struct j2p_je_img *__restrict__ strs, uint32_t ns, bool plain, const uint8_t *__restrict__ summ,
-                                                         uint32_t *__restrict__ state) {
-    const StreamMap<J2P_JP_SCANS> sm = {strs, ns, plain};
+// kBlockThreads threads, 8 per block: the shared blocks body, then the summaries.  Six CTAs per SM
+// (40 registers, as with colour summaries alone): the two summary bodies would otherwise take 48.
+__global__ void __launch_bounds__(kBlockThreads, 6) k_jp_blocks(const struct j2p_je_img *__restrict__ imgs, uint32_t n,
+                                                            const struct j2p_je_tables *__restrict__ t, uint64_t nblk,
+                                                            int16_t *__restrict__ coef, const struct j2p_je_img *__restrict__ strs,
+                                                            const struct j2p_jp_scanplan *__restrict__ scs, bool plain,
+                                                            uint8_t *__restrict__ summ, bool gray) {
+    blocks_body(imgs, n, t, nblk, coef);
+    __syncthreads();
+    if (gray) summaries<true>(imgs, n, t, nblk, coef, strs, scs, plain, summ);
+    else summaries<false>(imgs, n, t, nblk, coef, strs, scs, plain, summ);
+}
+
+// The stream-arithmetic kernels take the call's kind as a flag and run the body with PER = its
+// scans per image, J2P_JP_SCANS or J2P_JP_SCANS_GRAY: two instantiations in one kernel.
+template <uint32_t PER>
+__device__ __forceinline__ void runs_body(const struct j2p_je_img *__restrict__ strs, uint32_t ns, bool plain, const uint8_t *__restrict__ summ,
+                                          uint32_t *__restrict__ state) {
+    const StreamMap<PER> sm = {strs, ns, plain};
     uint64_t j;
     const uint32_t s = tile_block(sm.strs, sm.ns, &j);
     const struct j2p_je_img *st = &sm.strs[s];
-    if (!j2p_jp_is_ac(sm.scan(s)) || j >= st->nblk) return;
+    if (!j2p_jp_is_ac(PER == J2P_JP_SCANS_GRAY, sm.scan(s)) || j >= st->nblk) return;
     const uint8_t *m = summ + st->blk0;
     if (j && !(m[j - 1] & J2P_JP_RESET)) return;
     uint32_t *out = state + st->blk0;
     j2p_jp_walk(j, st->nblk, [&](uint64_t q) { return (uint32_t)m[q]; }, [&](uint64_t q, uint32_t v) { out[q] = v; });
 }
 
+// per block of an AC stream that starts a segment: the walk to the segment's end (a RESET block or
+// the stream's end, which a restart marker follows)
+__global__ void __launch_bounds__(kTileThreads) k_jp_runs(const struct j2p_je_img *__restrict__ strs, uint32_t ns, bool plain, const uint8_t *__restrict__ summ,
+                                                         uint32_t *__restrict__ state, bool gray) {
+    if (gray) runs_body<J2P_JP_SCANS_GRAY>(strs, ns, plain, summ, state);
+    else runs_body<J2P_JP_SCANS>(strs, ns, plain, summ, state);
+}
+
 // per tile: the symbols of its blocks counted in shared memory, then added to the image's counts
-__global__ void __launch_bounds__(kTileThreads) k_jp_hist(const Ctx x, uint32_t ns, unsigned long long *__restrict__ hist) {
-    __shared__ uint32_t cnt[2 * 256];
+__device__ __forceinline__ void hist_body(const Ctx &x, uint32_t ns, unsigned long long *__restrict__ hist, uint32_t *cnt) {
     uint64_t j;
     const uint32_t s = tile_block(x.strs, ns, &j), k = scan_of(x, s);
-    if (k == 6) return;                                 // the DC refine has no symbols
+    if (!j2p_jp_ntab(x.gray, k)) return;                // the DC refine has no symbols
     for (uint32_t q = threadIdx.x; q < 2 * 256; q += kTileThreads) cnt[q] = 0;
     __syncthreads();
     if (j < x.strs[s].nblk) {
@@ -379,12 +415,19 @@ __global__ void __launch_bounds__(kTileThreads) k_jp_hist(const Ctx x, uint32_t 
         code_block(x, s, j, o);
     }
     __syncthreads();
-    unsigned long long *h = hist + ((size_t)image_of(x, s) * J2P_JP_TABLES + j2p_jp_slot(k)) * 256;
+    unsigned long long *h = hist + ((size_t)image_of(x, s) * J2P_JP_TABLES + j2p_jp_slot(x.gray, k)) * 256;
     for (uint32_t q = threadIdx.x; q < 2 * 256; q += kTileThreads)
         if (cnt[q]) atomicAdd(h + q, (unsigned long long)cnt[q]);
 }
 
-// per image, a warp per table: code lengths, symbols and codes; then its scans' headers
+__global__ void __launch_bounds__(kTileThreads) k_jp_hist(const Ctx x, uint32_t ns, unsigned long long *__restrict__ hist) {
+    __shared__ uint32_t cnt[2 * 256];
+    if (x.gray) hist_body(as_kind<true>(x), ns, hist, cnt);
+    else hist_body(as_kind<false>(x), ns, hist, cnt);
+}
+
+// per image, a warp per table: code lengths, symbols and codes; then its scans' headers.  A gray
+// image's warps past its five tables have none to build.
 __global__ void __launch_bounds__(kTableThreads) k_jp_tables(const struct j2p_je_img *__restrict__ imgs, const struct j2p_je_tables *__restrict__ t,
                                                             const struct j2p_jp_scanplan *__restrict__ scs, const uint64_t *__restrict__ hist,
                                                             struct j2p_jp_huff *__restrict__ huffs, uint8_t *__restrict__ heads,
@@ -392,19 +435,22 @@ __global__ void __launch_bounds__(kTableThreads) k_jp_tables(const struct j2p_je
     __shared__ struct j2p_jo_scratch scr[J2P_JP_TABLES];
     __shared__ struct j2p_jp_dht d;
     const uint32_t i = blockIdx.x, tb = threadIdx.x >> 5;
+    const bool gray = j2p_jp_gray(t);
+    const uint32_t per = j2p_jp_nscans(gray);
     const WarpLanes L = {threadIdx.x & 31, 32};
     const size_t tab = (size_t)i * J2P_JP_TABLES + tb;
-    j2p_jp_table(hist + tab * 256, &scr[tb], &d, &huffs[tab], tb, L);
+    if (tb < j2p_jp_ntables(gray)) j2p_jp_table(hist + tab * 256, &scr[tb], &d, &huffs[tab], tb, L);
     __syncthreads();
-    for (uint32_t k = 0; k < J2P_JP_SCANS; k++) {
-        const size_t q = (size_t)i * J2P_JP_SCANS + k;
-        const uint32_t dri = scs[q].dri, len = j2p_jp_scan_head_len(&d, k, dri);
+    for (uint32_t k = 0; k < per; k++) {
+        const size_t q = (size_t)i * per + k;
+        const uint32_t dri = scs[q].dri, len = j2p_jp_scan_head_len(t, &d, k, dri);
         for (uint32_t b = threadIdx.x; b < len; b += kTableThreads) heads[q * J2P_JP_HEAD + b] = j2p_jp_scan_head_byte(t, &imgs[i], &d, k, dri, b);
         if (threadIdx.x == 0) hlens[q] = len;
     }
 }
 
-// per tile: each block's bits, their exclusive scan in the tile, the tile's sum
+// per tile: each block's bits, their exclusive scan in the tile, the tile's sum.  One body with the
+// kind as a runtime flag: two specialised bodies would take more registers.
 __global__ void __launch_bounds__(kTileThreads) k_jp_sizes(const Ctx x, uint32_t ns, const struct j2p_jp_huff *__restrict__ huffs,
                                                           uint32_t *__restrict__ intra, uint32_t *__restrict__ tsum) {
     typedef cub::BlockScan<uint32_t, kTileThreads> Scan;
@@ -426,10 +472,9 @@ __global__ void __launch_bounds__(kScanThreads) k_jp_scan(struct j2p_je_img *__r
     scan_body(strs, tsum, toff, raw);
 }
 
-__global__ void __launch_bounds__(kTileThreads) k_jp_emit(const Ctx x, uint32_t ns, const struct j2p_jp_huff *__restrict__ huffs,
-                                                         const uint32_t *__restrict__ intra, const uint64_t *__restrict__ toff,
-                                                         uint32_t *__restrict__ raw) {
-    __shared__ __align__(16) struct j2p_jp_huff sh[2];
+__device__ __forceinline__ void emit_kind_body(const Ctx &x, uint32_t ns, const struct j2p_jp_huff *__restrict__ huffs,
+                                               const uint32_t *__restrict__ intra, const uint64_t *__restrict__ toff, uint32_t *__restrict__ raw,
+                                               struct j2p_jp_huff *sh) {
     uint64_t j;
     const uint32_t s = tile_block(x.strs, ns, &j);
     const struct j2p_je_img *st = &x.strs[s];
@@ -443,24 +488,48 @@ __global__ void __launch_bounds__(kTileThreads) k_jp_emit(const Ctx x, uint32_t 
     if (e.w.fill) orw(e.w.word, (uint32_t)(e.w.acc >> 32));
 }
 
+__global__ void __launch_bounds__(kTileThreads) k_jp_emit(const Ctx x, uint32_t ns, const struct j2p_jp_huff *__restrict__ huffs,
+                                                         const uint32_t *__restrict__ intra, const uint64_t *__restrict__ toff,
+                                                         uint32_t *__restrict__ raw) {
+    __shared__ __align__(16) struct j2p_jp_huff sh[2];
+    if (x.gray) emit_kind_body(as_kind<true>(x), ns, huffs, intra, toff, raw, sh);
+    else emit_kind_body(as_kind<false>(x), ns, huffs, intra, toff, raw, sh);
+}
+
 __global__ void __launch_bounds__(kChunkThreads) k_jp_ffcount(const struct j2p_je_img *__restrict__ strs, uint32_t ns,
                                                              const uint32_t *__restrict__ raw, uint32_t *__restrict__ ffc) {
     ffcount_body(strs, ns, raw, ffc);
 }
 
+template <uint32_t PER>
+__device__ __forceinline__ void prog_offsets_body(struct j2p_je_img *__restrict__ strs, uint32_t ns, bool plain, uint32_t n,
+                                                  const uint32_t *__restrict__ ffc, uint32_t nchunks, const uint32_t *__restrict__ hlens,
+                                                  uint64_t *__restrict__ ffpre, uint64_t *__restrict__ offsets) {
+    const StreamMap<PER> sm = {strs, ns, plain};
+    offsets_body(strs, sm, n, ffc, nchunks, ffpre, offsets, [&](uint32_t s) { return hlens[sm.scan_index(s)]; });
+}
+
 __global__ void __launch_bounds__(kScanThreads) k_jp_offsets(struct j2p_je_img *__restrict__ strs, uint32_t ns, bool plain, uint32_t n,
                                                             const uint32_t *__restrict__ ffc, uint32_t nchunks, const uint32_t *__restrict__ hlens,
-                                                            uint64_t *__restrict__ ffpre, uint64_t *__restrict__ offsets) {
-    const StreamMap<J2P_JP_SCANS> sm = {strs, ns, plain};
-    offsets_body(strs, sm, n, ffc, nchunks, ffpre, offsets, [&](uint32_t s) { return hlens[sm.scan_index(s)]; });
+                                                            uint64_t *__restrict__ ffpre, uint64_t *__restrict__ offsets, bool gray) {
+    if (gray) prog_offsets_body<J2P_JP_SCANS_GRAY>(strs, ns, plain, n, ffc, nchunks, hlens, ffpre, offsets);
+    else prog_offsets_body<J2P_JP_SCANS>(strs, ns, plain, n, ffc, nchunks, hlens, ffpre, offsets);
+}
+
+template <uint32_t PER>
+__device__ __forceinline__ void prog_stuff_body(const struct j2p_je_img *__restrict__ strs, uint32_t ns, bool plain, const uint8_t *__restrict__ heads,
+                                                const uint32_t *__restrict__ hlens, const uint32_t *__restrict__ raw,
+                                                const uint64_t *__restrict__ ffpre, uint8_t *__restrict__ out) {
+    const StreamMap<PER> sm = {strs, ns, plain};
+    stuff_body(sm, raw, ffpre, out, [&](uint32_t s) { return hlens[sm.scan_index(s)]; },
+               [&](uint32_t s, uint32_t k) { return heads[(size_t)sm.scan_index(s) * J2P_JP_HEAD + k]; });
 }
 
 __global__ void __launch_bounds__(kChunkThreads) k_jp_stuff(const struct j2p_je_img *__restrict__ strs, uint32_t ns, bool plain, const uint8_t *__restrict__ heads,
                                                            const uint32_t *__restrict__ hlens, const uint32_t *__restrict__ raw,
-                                                           const uint64_t *__restrict__ ffpre, uint8_t *__restrict__ out) {
-    const StreamMap<J2P_JP_SCANS> sm = {strs, ns, plain};
-    stuff_body(sm, raw, ffpre, out, [&](uint32_t s) { return hlens[sm.scan_index(s)]; },
-               [&](uint32_t s, uint32_t k) { return heads[(size_t)sm.scan_index(s) * J2P_JP_HEAD + k]; });
+                                                           const uint64_t *__restrict__ ffpre, uint8_t *__restrict__ out, bool gray) {
+    if (gray) prog_stuff_body<J2P_JP_SCANS_GRAY>(strs, ns, plain, heads, hlens, raw, ffpre, out);
+    else prog_stuff_body<J2P_JP_SCANS>(strs, ns, plain, heads, hlens, raw, ffpre, out);
 }
 
 extern "C" int j2p_jpegprog_encode(const struct j2p_jpegenc_image *images, unsigned n, const struct j2p_jpegenc_params *params, void *work,
@@ -479,14 +548,15 @@ extern "C" int j2p_jpegprog_encode(const struct j2p_jpegenc_image *images, unsig
         int16_t *coef = (int16_t *)(w + P.off_coef);
         uint8_t *summ = w + P.off_summ, *heads = w + P.off_head;
         struct j2p_jp_huff *huffs = (struct j2p_jp_huff *)(w + P.off_huff);
-        const Ctx x = {imgs, strs, t, coef, summ, state, P.plain};
+        const bool gray = is_gray(params);
+        const Ctx x = {imgs, strs, t, coef, summ, state, P.plain, gray};
         // the symbol counts and the entropy words, which follow them
         const cudaError_t em = cudaMemsetAsync(hist, 0, P.off_raw - P.off_hist + P.words * sizeof(uint32_t), st);
         if (em != cudaSuccess) return fail("clearing the symbol counts and entropy words: %s", cudaGetErrorString(em));
         const uint64_t bgrid = (P.nblk * 8 + kBlockThreads - 1) / kBlockThreads;
-        k_jp_blocks<<<(unsigned)bgrid, kBlockThreads, 0, st>>>(imgs, n, t, P.nblk, coef, strs, scs, P.plain, summ);
+        k_jp_blocks<<<(unsigned)bgrid, kBlockThreads, 0, st>>>(imgs, n, t, P.nblk, coef, strs, scs, P.plain, summ, gray);
         counted();
-        k_jp_runs<<<P.ntiles, kTileThreads, 0, st>>>(strs, P.ns, P.plain, summ, state);
+        k_jp_runs<<<P.ntiles, kTileThreads, 0, st>>>(strs, P.ns, P.plain, summ, state, gray);
         counted();
         k_jp_hist<<<P.ntiles, kTileThreads, 0, st>>>(x, P.ns, (unsigned long long *)hist);
         counted();
@@ -500,9 +570,9 @@ extern "C" int j2p_jpegprog_encode(const struct j2p_jpegenc_image *images, unsig
         counted();
         k_jp_ffcount<<<P.nchunks, kChunkThreads, 0, st>>>(strs, P.ns, raw, ffc);
         counted();
-        k_jp_offsets<<<1, kScanThreads, 0, st>>>(strs, P.ns, P.plain, n, ffc, P.nchunks, hlens, ffpre, offs);
+        k_jp_offsets<<<1, kScanThreads, 0, st>>>(strs, P.ns, P.plain, n, ffc, P.nchunks, hlens, ffpre, offs, gray);
         counted();
-        k_jp_stuff<<<P.nchunks, kChunkThreads, 0, st>>>(strs, P.ns, P.plain, heads, hlens, raw, ffpre, w + P.off_out);
+        k_jp_stuff<<<P.nchunks, kChunkThreads, 0, st>>>(strs, P.ns, P.plain, heads, hlens, raw, ffpre, w + P.off_out, gray);
         counted();
         return 0;
     };

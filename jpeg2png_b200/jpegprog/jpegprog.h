@@ -27,6 +27,13 @@
  * interval's end, and DC predictions, the run and BE restart at 0.  The per-block bounds still hold,
  * because an interval's last EOB-run emission covers at least one of its blocks; an interval adds at
  * most 7 pad bits and the 2 unstuffed bytes of its RST.  Scan headers stay per (image, scan).
+ *
+ * Gray calls (components == 1, jpegenc.h): SOF2 with one component, then libjpeg's six scans for
+ * one component (Ss Se Ah Al: 0 0 0 1, 1 5 0 2, 6 63 0 2, 1 63 2 1, 0 0 1 0, 1 63 1 0), five
+ * tables per image (the DC refine has none), every scan non-interleaved over the real block grid in
+ * raster order.  Per-scan bounds: 27, 160, 1538, 1101, 1 and 1101 bits a block, all within
+ * J2P_JPEGPROG_BLOCK_BITS.  Every scan has the same restart interval, so a file has one DRI.  A call
+ * still runs the J2P_JPEGPROG_LAUNCHES kernels once each.
  */
 #ifndef J2P_JPEGPROG_H
 #define J2P_JPEGPROG_H

@@ -15,6 +15,20 @@
 //   8     Cb          1..63   1  0   8: 0x11
 //   9     Y           1..63   1  0   9: 0x10
 //
+// and, for a gray call (j2p_je_tables.nc == 1), as jpeg_simple_progression scripts one component:
+//
+//   scan  components  Ss..Se  Ah Al  tables (slot: DHT index)
+//   0     Y           0..0    0  1   0: 0x00                           DC first
+//   1     Y           1..5    0  2   1: 0x10
+//   2     Y           6..63   0  2   2: 0x10
+//   3     Y           1..63   2  1   3: 0x10                           AC refine
+//   4     Y           0..0    1  0   none                              DC refine
+//   5     Y           1..63   1  0   4: 0x10
+//
+// Every gray scan is non-interleaved over the component's block grid, which is also its MCU grid,
+// so the stored order is the raster and every scan has the same restart interval.  The kind is
+// the call's: the kernels take it as a launch-uniform flag (`g` below).
+//
 // The coding is T.81 Annex G as libjpeg's progressive Huffman encoder applies it:
 //
 //   point      DC: arithmetic shift right by Al; AC: the magnitude shifted, the sign kept;
@@ -45,8 +59,10 @@
 #include "../jpegopt/jpegopt_core.h"
 #include "jpegprog.h"
 
-#define J2P_JP_SCANS 10u                // scans, and so bit streams, per image
-#define J2P_JP_TABLES 10u               // Huffman tables per image
+#define J2P_JP_SCANS 10u                // scans, and so bit streams, per colour image
+#define J2P_JP_SCANS_GRAY 6u            // per gray image
+#define J2P_JP_TABLES 10u               // Huffman table slots per image (a gray image uses 5)
+#define J2P_JP_TABLES_GRAY 5u
 #define J2P_JP_HEAD 752u                // room for a scan's header: SOI .. SOF2, two DHTs, DRI, SOS
 static_assert(J2P_JP_HEAD >= J2P_JO_HEAD_PRE + 2 * (21 + 256) + J2P_JE_DRI + 14 && J2P_JP_HEAD % 16 == 0, "a scan's header fits");
 #define J2P_JP_MAX_RUN 0x7fffu          // the longest EOB run
@@ -73,13 +89,30 @@ static_assert(J2P_JP_AC_FIRST_BITS(63u) == J2P_JPEGPROG_BLOCK_BITS && J2P_JP_AC_
 // the bound fills its words exactly (scan 1: J2P_JP_AC_FIRST_BITS(5) is 160 bits, 5 words).  The RST
 // is the stream's 2-byte header, counted in the output outside its words.
 static_assert(J2P_JP_AC_FIRST_BITS(5u) == 5u * 32u && 32u % 8u == 0u, "a bound in whole words is whole bytes: padding stays inside it");
+// The gray script's per-scan bounds: DC first 27, AC first over 1..5 160 and over 6..63 1538, AC
+// refine over 1..63 1101, DC refine 1 bit a block.
+static_assert(J2P_JP_AC_FIRST_BITS(58u) == 1538u && J2P_JP_AC_FIRST_BITS(58u) < J2P_JPEGPROG_BLOCK_BITS, "the gray scans are within the bound");
 
 struct j2p_jp_scan {
         uint32_t comp;                  // 0 Y, 1 Cb, 2 Cr; 3 all three, interleaved
         uint32_t ss, se, ah, al;
 };
 
-J2P_HD struct j2p_jp_scan j2p_jp_scan_of(uint32_t k) {
+// the scans and the table slots of an image of the call (g: gray)
+J2P_HD uint32_t j2p_jp_nscans(bool g) { return g ? J2P_JP_SCANS_GRAY : J2P_JP_SCANS; }
+J2P_HD uint32_t j2p_jp_ntables(bool g) { return g ? J2P_JP_TABLES_GRAY : J2P_JP_TABLES; }
+
+J2P_HD struct j2p_jp_scan j2p_jp_scan_of(bool g, uint32_t k) {
+        if (g) {
+                switch (k) {
+                case 0: return {0, 0, 0, 0, 1};
+                case 1: return {0, 1, 5, 0, 2};
+                case 2: return {0, 6, 63, 0, 2};
+                case 3: return {0, 1, 63, 2, 1};
+                case 4: return {0, 0, 0, 1, 0};
+                default: return {0, 1, 63, 1, 0};
+                }
+        }
         switch (k) {
         case 0: return {3, 0, 0, 0, 1};
         case 1: return {0, 1, 5, 0, 2};
@@ -94,22 +127,28 @@ J2P_HD struct j2p_jp_scan j2p_jp_scan_of(uint32_t k) {
         }
 }
 
-J2P_HD bool j2p_jp_is_ac(uint32_t k) { return k != 0 && k != 6; }
+// the DC refine scan: 6, or a gray image's 4
+J2P_HD bool j2p_jp_is_ac(bool g, uint32_t k) { return k != 0 && k != (g ? 4u : 6u); }
 
-// the table slot of scan k's first table (scan 0: luma 0, chroma 1); scan 6 has none
-J2P_HD uint32_t j2p_jp_slot(uint32_t k) { return k == 0 ? 0 : k < 6 ? k + 1 : k; }
+// the table slot of scan k's first table (scan 0: luma 0, chroma 1); the DC refine has none (its
+// slot is the next scan's, and it counts no symbols there)
+J2P_HD uint32_t j2p_jp_slot(bool g, uint32_t k) { return g ? (k < 4 ? k : 4) : k == 0 ? 0 : k < 6 ? k + 1 : k; }
+
+// the tables scan k codes with: two for a colour DC first scan, none for the DC refine, else one
+J2P_HD uint32_t j2p_jp_ntab(bool g, uint32_t k) { return j2p_jp_is_ac(g, k) ? 1 : k ? 0 : g ? 1 : 2; }
 
 // the worst case of a block of scan k, in bits and in 32-bit words
-J2P_HD uint32_t j2p_jp_bound_bits(uint32_t k) {
-        const struct j2p_jp_scan s = j2p_jp_scan_of(k);
-        if (!j2p_jp_is_ac(k)) return s.ah ? J2P_JP_DC_REFINE_BITS : J2P_JP_DC_FIRST_BITS;
+J2P_HD uint32_t j2p_jp_bound_bits(bool g, uint32_t k) {
+        const struct j2p_jp_scan s = j2p_jp_scan_of(g, k);
+        if (!j2p_jp_is_ac(g, k)) return s.ah ? J2P_JP_DC_REFINE_BITS : J2P_JP_DC_FIRST_BITS;
         return s.ah ? J2P_JP_AC_REFINE_BITS(s.se - s.ss + 1) : J2P_JP_AC_FIRST_BITS(s.se - s.ss + 1);
 }
 
-J2P_HD uint32_t j2p_jp_bound_words(uint32_t k) { return (j2p_jp_bound_bits(k) + 31) / 32; }
+J2P_HD uint32_t j2p_jp_bound_words(bool g, uint32_t k) { return (j2p_jp_bound_bits(g, k) + 31) / 32; }
 
 // the AC scans of component comp, q = 0, 1, ...; -1 past the last
-J2P_HD int j2p_jp_comp_scan(uint32_t comp, uint32_t q) {
+J2P_HD int j2p_jp_comp_scan(bool g, uint32_t comp, uint32_t q) {
+        if (g) return q == 0 ? 1 : q == 1 ? 2 : q == 2 ? 3 : q == 3 ? 5 : -1;
         if (comp == 0) return q == 0 ? 1 : q == 1 ? 4 : q == 2 ? 5 : q == 3 ? 9 : -1;
         if (comp == 1) return q == 0 ? 3 : q == 1 ? 8 : -1;
         return q == 0 ? 2 : q == 1 ? 7 : -1;
@@ -336,12 +375,15 @@ J2P_HD void j2p_jp_table(const uint64_t *counts, struct j2p_jo_scratch *s, struc
 
 J2P_HD uint32_t j2p_jp_dht_len(const struct j2p_jp_dht *d, uint32_t tb) { return 21 + d->nvals[tb]; }
 
-J2P_HD uint32_t j2p_jp_sos_len(uint32_t k) { return j2p_jp_scan_of(k).comp == 3 ? 14 : 10; }
+J2P_HD uint32_t j2p_jp_sos_len(bool g, uint32_t k) { return j2p_jp_scan_of(g, k).comp == 3 ? 14 : 10; }
+
+J2P_HD bool j2p_jp_gray(const struct j2p_je_tables *t) { return t->nc == 1; }
 
 // the header of scan k: SOI .. SOF2 before scan 0, the DHTs of its tables, its SOS (without DRI)
-J2P_HD uint32_t j2p_jp_head_len(const struct j2p_jp_dht *d, uint32_t k) {
-        if (k == 0) return J2P_JO_HEAD_PRE + j2p_jp_dht_len(d, 0) + j2p_jp_dht_len(d, 1) + j2p_jp_sos_len(0);
-        return (k == 6 ? 0 : j2p_jp_dht_len(d, j2p_jp_slot(k))) + j2p_jp_sos_len(k);
+J2P_HD uint32_t j2p_jp_head_len(const struct j2p_je_tables *t, const struct j2p_jp_dht *d, uint32_t k) {
+        const bool g = j2p_jp_gray(t);
+        if (k == 0) return j2p_je_sof_end(t) + j2p_jp_dht_len(d, 0) + (g ? 0 : j2p_jp_dht_len(d, 1)) + j2p_jp_sos_len(g, 0);
+        return (j2p_jp_is_ac(g, k) ? j2p_jp_dht_len(d, j2p_jp_slot(g, k)) : 0) + j2p_jp_sos_len(g, k);
 }
 
 J2P_HD uint8_t j2p_jp_dht_byte(const struct j2p_jp_dht *d, uint32_t tb, uint32_t index, uint32_t k) {
@@ -355,8 +397,8 @@ J2P_HD uint8_t j2p_jp_dht_byte(const struct j2p_jp_dht *d, uint32_t tb, uint32_t
 
 // SOS: the components with their table selectors (td << 4 | ta, 0 where the scan uses none), Ss,
 // Se, Ah << 4 | Al
-J2P_HD uint8_t j2p_jp_sos_byte(uint32_t k, uint32_t b) {
-        const struct j2p_jp_scan s = j2p_jp_scan_of(k);
+J2P_HD uint8_t j2p_jp_sos_byte(bool g, uint32_t k, uint32_t b) {
+        const struct j2p_jp_scan s = j2p_jp_scan_of(g, k);
         const uint32_t ns = s.comp == 3 ? 3 : 1, len = 6 + 2 * ns;
         if (b < 2) return b ? 0xda : 0xff;
         if (b < 4) return (uint8_t)(b == 2 ? 0 : len);
@@ -372,29 +414,34 @@ J2P_HD uint8_t j2p_jp_sos_byte(uint32_t k, uint32_t b) {
 }
 
 J2P_HD uint8_t j2p_jp_head_byte(const struct j2p_je_tables *t, const struct j2p_je_img *im, const struct j2p_jp_dht *d, uint32_t k, uint32_t b) {
+        const bool g = j2p_jp_gray(t);
         if (k == 0) {
-                if (b < J2P_JO_HEAD_PRE) return b == J2P_JE_SOF_AT + 1 ? 0xc2 : j2p_je_head_byte(t, im, b);
-                b -= J2P_JO_HEAD_PRE;
-                for (uint32_t tb = 0; tb < 2; tb++) {
+                const uint32_t pre = j2p_je_sof_end(t);
+                if (b < pre) return b == t->sof_at + 1 ? 0xc2 : j2p_je_head_byte(t, im, b);
+                b -= pre;
+                for (uint32_t tb = 0; tb < j2p_jp_ntab(g, 0); tb++) {
                         if (b < j2p_jp_dht_len(d, tb)) return j2p_jp_dht_byte(d, tb, tb, b);
                         b -= j2p_jp_dht_len(d, tb);
                 }
-                return j2p_jp_sos_byte(0, b);
+                return j2p_jp_sos_byte(g, 0, b);
         }
-        if (k != 6) {
-                const uint32_t tb = j2p_jp_slot(k);
-                if (b < j2p_jp_dht_len(d, tb)) return j2p_jp_dht_byte(d, tb, j2p_jp_scan_of(k).comp ? 0x11 : 0x10, b);
+        if (j2p_jp_is_ac(g, k)) {
+                const uint32_t tb = j2p_jp_slot(g, k);
+                if (b < j2p_jp_dht_len(d, tb)) return j2p_jp_dht_byte(d, tb, j2p_jp_scan_of(g, k).comp ? 0x11 : 0x10, b);
                 b -= j2p_jp_dht_len(d, tb);
         }
-        return j2p_jp_sos_byte(k, b);
+        return j2p_jp_sos_byte(g, k, b);
 }
 
 // scan k's header with DRI for dri (0: none) before its SOS
-J2P_HD uint32_t j2p_jp_scan_head_len(const struct j2p_jp_dht *d, uint32_t k, uint32_t dri) { return j2p_jp_head_len(d, k) + (dri ? J2P_JE_DRI : 0); }
+J2P_HD uint32_t j2p_jp_scan_head_len(const struct j2p_je_tables *t, const struct j2p_jp_dht *d, uint32_t k, uint32_t dri) {
+        return j2p_jp_head_len(t, d, k) + (dri ? J2P_JE_DRI : 0);
+}
 
 J2P_HD uint8_t j2p_jp_scan_head_byte(const struct j2p_je_tables *t, const struct j2p_je_img *im, const struct j2p_jp_dht *d, uint32_t k,
                                      uint32_t dri, uint32_t b) {
-        return j2p_je_dri_head(dri, j2p_jp_head_len(d, k), j2p_jp_sos_len(k), b, [&](uint32_t b1) { return j2p_jp_head_byte(t, im, d, k, b1); });
+        return j2p_je_dri_head(dri, j2p_jp_head_len(t, d, k), j2p_jp_sos_len(j2p_jp_gray(t), k), b,
+                               [&](uint32_t b1) { return j2p_jp_head_byte(t, im, d, k, b1); });
 }
 
 #endif  // J2P_JPEGPROG_CORE_H
