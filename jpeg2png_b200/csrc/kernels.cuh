@@ -114,6 +114,33 @@ inline FrameDev frame_view(const FrameDev &F, int f) {
     return V;
 }
 
+// CUDA caps gridDim.y and gridDim.z at 65535.  The projection and epilogue grids have one CTA row
+// per block row (or pixel row) of a plane, so a taller plane is covered by several launches of at
+// most kMaxGridRows CTA rows each, every one on a view that starts further down the frame.
+constexpr int kMaxGridRows = 65535;
+
+// Planes [c0, c0 + count) seen from coefficient block row `brow` on; a block row spans `frame_rows`
+// frame rows (8 * the vertical sampling factor).  Strip borders: only the view that holds a border
+// row delivers it to the neighbour.  The kernels address every array relative to the plane
+// pointers, so the offsets here are the only 64-bit products the split needs.
+inline FrameDev rows_view(const FrameDev &F, int c0, int count, int brow, int frame_rows, bool last) {
+    FrameDev V = F;
+    const size_t px = (size_t)brow * frame_rows * (size_t)F.W;
+    for (int c = c0; c < c0 + count; c++) {
+        PlaneDev &P = V.pl[c];
+        P.x += px;
+        P.xp += px;
+        P.g += px;
+        P.gp += (size_t)brow * 8 * P.cw;
+        P.data += (size_t)brow * (P.cw >> 3) * 64;
+        P.ch = P.ch > 8 * brow ? P.ch - 8 * brow : 0;
+    }
+    V.H = F.H - brow * frame_rows;
+    if (brow > 0) V.sync.has_up = 0;
+    if (!last) V.sync.has_down = 0;
+    return V;
+}
+
 // ---- the colour epilogue (kernels_epilogue.cu, k_scanlines): YCbCr planes of `nframes` frames ->
 // RGB in one of three output forms.  Each plane has its own base, row stride and frame stride, so
 // the three planes may come from one joint session or from three separate-mode sessions whose
@@ -126,6 +153,7 @@ struct EpilogueArgs {
     unsigned long long frame_stride[3];  // elements from one frame's plane to the next frame's
     int ld[3];                           // row stride of each plane, elements
     int w, h;                            // visible image, at most every plane's frame
+    int row0;                            // first image row of this launch (launch_scanlines)
     int mode;                            // EpilogueMode
     int sample;                          // bits per sample: 8 or 16 (scanlines), 8, 16 or 32 (HWC / CHW)
     unsigned long long frame_bytes;      // output bytes from one frame to the next

@@ -44,11 +44,11 @@ __device__ __forceinline__ void store_bytes(uint8_t *dst, const uint8_t *src, in
     if (tid < nbytes - done) dst[done + tid] = src[done + tid];
 }
 
-// one CTA = EP_NT consecutive pixels of one row (blockIdx.y) of one frame (blockIdx.z); samples are
-// staged in shared memory in output order and written out with coalesced word stores
+// one CTA = EP_NT consecutive pixels of one row (a.row0 + blockIdx.y) of one frame (blockIdx.z); samples
+// are staged in shared memory in output order and written out with coalesced word stores
 __global__ void __launch_bounds__(EP_NT) k_scanlines(const EpilogueArgs a) {
     __shared__ __align__(16) uint8_t sm[EP_NT * 12 + 16];               // + one word read past the end by store_bytes
-    const int row = blockIdx.y, frame = blockIdx.z, x0 = blockIdx.x * EP_NT, tid = threadIdx.x;
+    const int row = a.row0 + (int)blockIdx.y, frame = blockIdx.z, x0 = blockIdx.x * EP_NT, tid = threadIdx.x;
     const int es = a.sample >> 3, npx = min(EP_NT, a.w - x0);           // bytes per sample, pixels of this CTA
     const bool gray = a.nc == 1;
     const int nc = gray ? 1 : 3;                                        // samples per pixel
@@ -95,10 +95,17 @@ __global__ void __launch_bounds__(EP_NT) k_scanlines(const EpilogueArgs a) {
     store_bytes(dst + filter + (size_t)x0 * nc * es, sm, npx * nc * es, tid);
 }
 
-cudaError_t launch_scanlines(const EpilogueArgs &a, int nframes, cudaStream_t s) {
-    const dim3 grid((a.w + EP_NT - 1) / EP_NT, a.h, nframes);
-    k_scanlines<<<grid, EP_NT, 0, s>>>(a);
-    return cudaGetLastError();
+// rows in launches of at most kMaxGridRows (kernels.cuh); *nlaunch: launches made
+cudaError_t launch_scanlines(const EpilogueArgs &a, int nframes, cudaStream_t s, int *nlaunch) {
+    EpilogueArgs b = a;
+    for (b.row0 = 0; b.row0 < a.h; b.row0 += kMaxGridRows) {
+        const int rows = a.h - b.row0 < kMaxGridRows ? a.h - b.row0 : kMaxGridRows;
+        k_scanlines<<<dim3((a.w + EP_NT - 1) / EP_NT, rows, nframes), EP_NT, 0, s>>>(b);
+        *nlaunch += 1;
+        const cudaError_t e = cudaGetLastError();
+        if (e != cudaSuccess) return e;
+    }
+    return cudaSuccess;
 }
 
 }  // namespace j2p

@@ -366,12 +366,19 @@ cudaError_t launch_project(const FrameDev &Fin, float factor, cudaStream_t s, in
         ProjPlane G;
         G.c = c;
         G.gx = (F.W + tw - 1) / tw;
-        const dim3 grid(G.gx, (F.H + th - 1) / th);
-        const int before = *nlaunch;
+        const int gy = (F.H + th - 1) / th;
+        // k_project's CTA rows in launches of at most kMaxGridRows (one launch unless the plane is that tall)
+        auto each_rows = [&](const FrameDev &V, auto launch) {
+            for (int y0 = 0; y0 < gy; y0 += kMaxGridRows) {
+                const int rows = gy - y0 < kMaxGridRows ? gy - y0 : kMaxGridRows;
+                launch(y0 == 0 && rows == gy ? V : rows_view(V, c, 1, y0 * P_BH, 8 * P.sh, y0 + rows == gy), dim3(G.gx, rows));
+                *nlaunch += 1;
+            }
+        };
         if (F.log_on && P.sw == 1 && P.sh == 1) {
-            k_project<1, 1><<<grid, P_NT, 0, s>>>(F, G, factor);                // the variant that also sums the log terms
+            each_rows(F, [&](const FrameDev &V, dim3 grid) { k_project<1, 1><<<grid, P_NT, 0, s>>>(V, G, factor); });   // the variant that also sums the log terms
         } else if (P.sw == 1 && P.sh == 1) {
-            int count = 1;      // following planes of identical geometry ride in the same launch (grid.z)
+            int count = 1;      // following planes of identical geometry ride in the same launch (grid.z; a batch: grid.x)
             while (c + count < F.nc && F.pl[c + count].sw == 1 && F.pl[c + count].sh == 1 && F.pl[c + count].cw == P.cw &&
                    F.pl[c + count].ch == P.ch)
                 count++;
@@ -398,15 +405,14 @@ cudaError_t launch_project(const FrameDev &Fin, float factor, cudaStream_t s, in
         else {
             // k_project<> handles one frame: a batch launches it once per frame on that frame's view
             for (int f = 0; f < F.nframes; f++) {
-                const FrameDev &V = F.nframes > 1 ? frame_view(F, f) : F;
-                if (P.sw == 2 && P.sh == 2) k_project<2, 2><<<grid, P_NT, 0, s>>>(V, G, factor);
-                else if (P.sw == 2 && P.sh == 1) k_project<2, 1><<<grid, P_NT, 0, s>>>(V, G, factor);
-                else if (P.sw == 1 && P.sh == 2) k_project<1, 2><<<grid, P_NT, 0, s>>>(V, G, factor);
-                else k_project<0, 0><<<grid, P_NT, 0, s>>>(V, G, factor);
-                *nlaunch += 1;
+                each_rows(F.nframes > 1 ? frame_view(F, f) : F, [&](const FrameDev &V, dim3 grid) {
+                    if (P.sw == 2 && P.sh == 2) k_project<2, 2><<<grid, P_NT, 0, s>>>(V, G, factor);
+                    else if (P.sw == 2 && P.sh == 1) k_project<2, 1><<<grid, P_NT, 0, s>>>(V, G, factor);
+                    else if (P.sw == 1 && P.sh == 2) k_project<1, 2><<<grid, P_NT, 0, s>>>(V, G, factor);
+                    else k_project<0, 0><<<grid, P_NT, 0, s>>>(V, G, factor);
+                });
             }
         }
-        if (*nlaunch == before) *nlaunch += 1;                       // the logging k_project<1, 1> launch above
         const cudaError_t e = cudaGetLastError();
         if (e != cudaSuccess) return e;
     }

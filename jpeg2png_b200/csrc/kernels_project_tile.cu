@@ -38,7 +38,9 @@ static_assert(PT_C4 == 1 << PT_SH, "tile width");
 #define J2P_TILE_MIN_CTAS (256 / J2P_TILE_BLOCKS / 2)      // 32 warps per SM either way (64 registers)
 #endif
 // RES: the plane's coefficient grid is smaller than the frame (compute.c:338), e.g. 1080p luma.
-// BATCH: a batch session (FrameDev::nframes); blockIdx.z = frame * count + k for planes c0 + k.
+// BATCH: a batch session (FrameDev::nframes); blockIdx.z = frame, blockIdx.x = k * (CTA columns) +
+// column for planes c0 + k (a single frame: blockIdx.z = k).  A batch keeps gridDim.z for the frames,
+// which may number 65535.
 template <bool RES, bool BATCH>
 __global__ void __launch_bounds__(PT_NT, J2P_TILE_MIN_CTAS) k_project_tile(const __grid_constant__ FrameDev F, const int c0, const float factor) {
     __shared__ __align__(16) float4 sx[8][PT_C4];                // x_k          -> later x_{k+1}
@@ -48,14 +50,16 @@ __global__ void __launch_bounds__(PT_NT, J2P_TILE_MIN_CTAS) k_project_tile(const
     __shared__ __align__(16) float sq[3][64];
     __shared__ float snorm[2];
     const int tid = threadIdx.x;
-    const int count = BATCH ? (int)gridDim.z / F.nframes : 1;
-    const int frame = BATCH ? (int)blockIdx.z / count : 0;
-    const int c = c0 + (int)blockIdx.z - frame * count;          // planes of equal geometry share one launch
+    const int frame = BATCH ? (int)blockIdx.z : 0;
+    const int gx = BATCH ? ((F.pl[c0].cw >> 3) + PT_NB - 1) / PT_NB : 0;   // CTA columns per plane
+    const int k = BATCH ? (int)blockIdx.x / gx : (int)blockIdx.z;
+    const int c = c0 + k;                                        // planes of equal geometry share one launch
     const PlaneDev &P = F.pl[c];
     const size_t fo = BATCH ? (size_t)frame * F.frame_stride : 0;
     const int W = F.W;
     const int bw = P.cw >> 3;
-    const int bx0 = blockIdx.x * PT_NB, by = strip_row_order(F.sync, blockIdx.y, gridDim.y);   // the grid covers real blocks only
+    const int bx0 = (BATCH ? (int)blockIdx.x - k * gx : (int)blockIdx.x) * PT_NB;
+    const int by = strip_row_order(F.sync, blockIdx.y, gridDim.y);   // the grid covers real blocks only
     const int nbx = min(PT_NB, bw - bx0);                           // blocks of this tile that exist
     const int valid_c4 = nbx * 2;
     const size_t row0 = (size_t)(by * 8) * W + (size_t)bx0 * 8;  // first pixel of the tile
@@ -302,14 +306,17 @@ int project_tile_border_units(const PlaneDev &P) { return ((P.cw >> 3) + PT_NB -
 // uncovered_only: the tiles have been projected by the TMA kernel; only the stepped-only pixels remain
 cudaError_t launch_project_tile(const FrameDev &F, int c, int count, float factor, cudaStream_t s, int *nlaunch, bool uncovered_only) {
     const PlaneDev &P = F.pl[c];
-    const int bw = P.cw >> 3, bh = P.ch >> 3;
-    const dim3 grid((bw + PT_NB - 1) / PT_NB, bh, count * F.nframes);
+    const int bw = P.cw >> 3, bh = P.ch >> 3, gx = (bw + PT_NB - 1) / PT_NB;
+    const bool batch = F.nframes > 1;
     cudaError_t e = cudaSuccess;
-    if (!uncovered_only && F.nframes > 1) {
-        e = P.resample ? launch_chain(k_project_tile<true, true>, grid, dim3(PT_NT), 0, s, F, c, factor) : launch_chain(k_project_tile<false, true>, grid, dim3(PT_NT), 0, s, F, c, factor);
-        *nlaunch += 1;
-    } else if (!uncovered_only) {
-        e = P.resample ? launch_chain(k_project_tile<true, false>, grid, dim3(PT_NT), 0, s, F, c, factor) : launch_chain(k_project_tile<false, false>, grid, dim3(PT_NT), 0, s, F, c, factor);
+    for (int y0 = 0; y0 < bh && !uncovered_only && e == cudaSuccess; y0 += kMaxGridRows) {   // one launch unless bh > 65535
+        const int rows = bh - y0 < kMaxGridRows ? bh - y0 : kMaxGridRows;
+        const FrameDev V = y0 == 0 && rows == bh ? F : rows_view(F, c, count, y0, 8, y0 + rows == bh);
+        const dim3 grid = batch ? dim3(gx * count, rows, F.nframes) : dim3(gx, rows, count);
+        if (batch)
+            e = P.resample ? launch_chain(k_project_tile<true, true>, grid, dim3(PT_NT), 0, s, V, c, factor) : launch_chain(k_project_tile<false, true>, grid, dim3(PT_NT), 0, s, V, c, factor);
+        else
+            e = P.resample ? launch_chain(k_project_tile<true, false>, grid, dim3(PT_NT), 0, s, V, c, factor) : launch_chain(k_project_tile<false, false>, grid, dim3(PT_NT), 0, s, V, c, factor);
         *nlaunch += 1;
     }
     for (int k = c; k < c + count && e == cudaSuccess; k++)

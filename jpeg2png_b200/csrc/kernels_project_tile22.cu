@@ -32,7 +32,8 @@ constexpr size_t P22_SMEM = (size_t)3 * 16 * P22_C4 * sizeof(float4)      // x_k
                             + (size_t)P22_NB * TILE_STRIDE * sizeof(float) // transpose tiles
                             + 3 * 64 * sizeof(float) + 4 * sizeof(float);  // tables, norm
 
-// BATCH: a batch session (FrameDev::nframes); blockIdx.z = frame * count + k for planes c0 + k.
+// BATCH: a batch session (FrameDev::nframes); blockIdx.z = frame, blockIdx.x = k * (CTA columns) +
+// column for planes c0 + k (a single frame: blockIdx.z = k), as in k_project_tile.
 template <bool BATCH>
 __global__ void __launch_bounds__(P22_NT, 3) k_project_tile22(const __grid_constant__ FrameDev F, const int c0, const float factor) {
     extern __shared__ __align__(16) unsigned char smem22[];
@@ -45,14 +46,16 @@ __global__ void __launch_bounds__(P22_NT, 3) k_project_tile22(const __grid_const
     float *snorm = sq + 3 * 64;                                      // [2]
 
     const int tid = threadIdx.x;
-    const int count = BATCH ? (int)gridDim.z / F.nframes : 1;
-    const int frame = BATCH ? (int)blockIdx.z / count : 0;
-    const int c = c0 + (int)blockIdx.z - frame * count;              // planes of equal geometry share one launch
+    const int frame = BATCH ? (int)blockIdx.z : 0;
+    const int gx = BATCH ? ((F.pl[c0].cw >> 3) + P22_NB - 1) / P22_NB : 0;   // CTA columns per plane
+    const int k = BATCH ? (int)blockIdx.x / gx : (int)blockIdx.z;
+    const int c = c0 + k;                                            // planes of equal geometry share one launch
     const PlaneDev &P = F.pl[c];
     const size_t fo = BATCH ? (size_t)frame * F.frame_stride : 0;
     const int W = F.W;
     const int bw = P.cw >> 3;
-    const int bx0 = blockIdx.x * P22_NB, by = strip_row_order(F.sync, blockIdx.y, gridDim.y);   // the grid covers real blocks only
+    const int bx0 = (BATCH ? (int)blockIdx.x - k * gx : (int)blockIdx.x) * P22_NB;
+    const int by = strip_row_order(F.sync, blockIdx.y, gridDim.y);   // the grid covers real blocks only
     const int nbx = min(P22_NB, bw - bx0);
     const int valid_c4 = nbx * 4, valid_g4 = nbx * 2;
     const size_t row0 = (size_t)(by * 16) * W + (size_t)bx0 * 16;    // first frame pixel of the tile
@@ -305,12 +308,16 @@ cudaError_t configure_project_tile22() {
 // c .. c+count-1, which must all be 2x2 planes with the same coefficient grid.
 cudaError_t launch_project_tile22(const FrameDev &F, int c, int count, float factor, cudaStream_t s, int *nlaunch) {
     const PlaneDev &P = F.pl[c];
-    const int bw = P.cw >> 3, bh = P.ch >> 3;
+    const int bw = P.cw >> 3, bh = P.ch >> 3, gx = (bw + P22_NB - 1) / P22_NB;
     const bool batch = F.nframes > 1;
-    const dim3 grid((bw + P22_NB - 1) / P22_NB, bh, count * F.nframes);
-    cudaError_t e = batch ? launch_chain(k_project_tile22<true>, grid, dim3(P22_NT), P22_SMEM, s, F, c, factor)
-                          : launch_chain(k_project_tile22<false>, grid, dim3(P22_NT), P22_SMEM, s, F, c, factor);
-    *nlaunch += 1;
+    cudaError_t e = cudaSuccess;
+    for (int y0 = 0; y0 < bh && e == cudaSuccess; y0 += kMaxGridRows) {   // one launch unless bh > 65535
+        const int rows = bh - y0 < kMaxGridRows ? bh - y0 : kMaxGridRows;
+        const FrameDev V = y0 == 0 && rows == bh ? F : rows_view(F, c, count, y0, 16, y0 + rows == bh);
+        e = batch ? launch_chain(k_project_tile22<true>, dim3(gx * count, rows, F.nframes), dim3(P22_NT), P22_SMEM, s, V, c, factor)
+                  : launch_chain(k_project_tile22<false>, dim3(gx, rows, count), dim3(P22_NT), P22_SMEM, s, V, c, factor);
+        *nlaunch += 1;
+    }
     for (int k = c; k < c + count && e == cudaSuccess; k++) {
         const PlaneDev &Q = F.pl[k];
         if (2 * Q.cw < F.W || 2 * Q.ch < F.H) {

@@ -50,7 +50,7 @@ cudaError_t launch_init_plane(const float *fdata, float *x, float *xp, int W, in
 bool project_tma_enabled();
 int project_tma_border_units(const PlaneDev &P);
 int project_tile_border_units(const PlaneDev &P);
-cudaError_t launch_scanlines(const EpilogueArgs &a, int nframes, cudaStream_t s);
+cudaError_t launch_scanlines(const EpilogueArgs &a, int nframes, cudaStream_t s, int *nlaunch);
 // kernels_strip.cu: the strip exchanges over peer memory (parameter blocks in kernels.cuh)
 cudaError_t launch_halo_exchange(const HaloPeers &P, unsigned seq, unsigned *ticket, int *err, int wait_for_arrival, cudaStream_t s);
 }  // namespace j2p
@@ -70,8 +70,10 @@ static int fail(int code, const char *fmt, ...) {
 #define CK(call)                                                                                      \
     do {                                                                                              \
         cudaError_t e_ = (call);                                                                      \
-        if (e_ != cudaSuccess)                                                                        \
+        if (e_ != cudaSuccess) {                                                                      \
+            cudaGetLastError();   /* a refused launch also sets the thread's last error: later calls must not see it */ \
             return fail(J2P_ERR_CUDA, "%s failed: %s (%s:%d)", #call, cudaGetErrorString(e_), __FILE__, __LINE__); \
+        }                                                                                             \
     } while (0)
 
 constexpr int kEventRing = 32;
@@ -997,8 +999,9 @@ extern "C" int j2p_session_download_frame_scanlines(j2p_session *s, unsigned fra
     a.sample = (int)bits;
     a.frame_bytes = bytes;
     a.out = dev;
-    CK(launch_scanlines(a, 1, s->stream));
-    s->launches++;
+    int nep = 0;
+    CK(launch_scanlines(a, 1, s->stream, &nep));
+    s->launches += (unsigned)nep;
     return staged_d2h(s, out, dev, bytes);
 }
 
@@ -1044,8 +1047,9 @@ static int export_impl(j2p_session *const *ss, int nsess, int nout, unsigned fra
         CK(cudaEventRecord(s->export_ev, s->stream));
         CK(cudaStreamWaitEvent(st, s->export_ev, 0));
     }
-    CK(launch_scanlines(a, (int)nframes, st));
-    s0->launches++;
+    int nep = 0;
+    CK(launch_scanlines(a, (int)nframes, st, &nep));
+    s0->launches += (unsigned)nep;
     // ... and the session stream waits for the export before a later upload / reset / iterate
     for (int k = 0; k < nsess; k++) {
         j2p_session *s = ss[k];
