@@ -292,6 +292,23 @@ int j2p_session_export_separate(j2p_session *y, j2p_session *cb, j2p_session *cr
  * and refusals as j2p_session_export, the refusal of nchannel being "not 1 or 3". */
 int j2p_session_export_gray(j2p_session *s, unsigned frame0, unsigned nframes,
                             const struct j2p_image_out *o, void *dst, void *stream);
+/* oriented: the export of j2p_session_export (nsessions 1, channels 3), j2p_session_export_gray
+ * (nsessions 1, channels 1) or j2p_session_export_separate (nsessions 3: Y, Cb, Cr; channels 3),
+ * with frame frame0 + i flipped or rotated by its EXIF orientation orientation[i] as Pillow's
+ * ImageOps.exif_transpose does it: 2 FLIP_LEFT_RIGHT, 3 ROTATE_180, 4 FLIP_TOP_BOTTOM, 5 TRANSPOSE,
+ * 6 ROTATE_270, 7 TRANSVERSE, 8 ROTATE_90.
+ *   orientation: device pointer to nframes bytes on the sessions' device (values outside 1..8 are
+ *                written as 1); NULL = every frame 1.
+ * o->w x o->h is the stored (unrotated) image.  Frames with orientation 5..8 are o->h wide and o->w
+ * tall in dst, so HWC is (w, h, c) and CHW (c, w, h) for them; frame_bytes, the sample types and the
+ * channel order are as j2p_session_export.  The samples are bit-identical to the unoriented export;
+ * only their addresses change.  One launch for any mix of orientations.  Streams and refusals as
+ * the export each combination stands for, and J2P_ERR_ARG for a null `sessions` or session, a
+ * nsessions / channels combination that is none of the three, orientation memory that is not device
+ * memory on the sessions' device, and o->h above 2097120 (65535 rows of 32-pixel tiles). */
+int j2p_session_export_oriented(j2p_session *const *sessions, unsigned nsessions, unsigned channels,
+                                unsigned frame0, unsigned nframes, const unsigned char *orientation,
+                                const struct j2p_image_out *o, void *dst, void *stream);
 
 /* Objective terms of the most recent iteration, as logged by the reference (compute.c:271-272):
  * out[0]=objective, out[1]=prob_dist, out[2]=tv, out[3]=tv2.  Only tracked when logging was

@@ -628,3 +628,55 @@ void j2p_free_jpeg_layout(struct j2p_jpeg_layout *l) {
         l->nseg = 0;
         l->data_len = 0;
 }
+
+/* ---- EXIF orientation (tag 0x0112 of IFD0 in the first APP1 "Exif\0\0" segment before SOS) ---- */
+
+static unsigned tiff16(const uint8_t *p, int be) { return be ? ((unsigned)p[0] << 8) | p[1] : ((unsigned)p[1] << 8) | p[0]; }
+static uint32_t tiff32(const uint8_t *p, int be) {
+        return be ? ((uint32_t)p[0] << 24) | ((uint32_t)p[1] << 16) | ((uint32_t)p[2] << 8) | p[3]
+                  : ((uint32_t)p[3] << 24) | ((uint32_t)p[2] << 16) | ((uint32_t)p[1] << 8) | p[0];
+}
+
+/* t: the TIFF structure after "Exif\0\0", n bytes of it */
+static int tiff_orientation(const uint8_t *t, size_t n) {
+        if (n < 8) return 1;
+        int be;
+        if (t[0] == 'I' && t[1] == 'I') be = 0;
+        else if (t[0] == 'M' && t[1] == 'M') be = 1;
+        else return 1;
+        if (tiff16(t + 2, be) != 42) return 1;
+        const uint32_t ifd = tiff32(t + 4, be);
+        if (ifd > n || n - ifd < 2) return 1;
+        const unsigned count = tiff16(t + ifd, be);
+        if ((n - ifd - 2) / 12 < count) return 1;                     /* the entries run past the segment */
+        for (unsigned i = 0; i < count; i++) {
+                const uint8_t *e = t + ifd + 2 + 12u * i;
+                if (tiff16(e, be) != 0x0112) continue;
+                const unsigned type = tiff16(e + 2, be);
+                if (tiff32(e + 4, be) != 1 || (type != 3 && type != 4)) return 1;   /* SHORT or LONG, count 1 */
+                const uint32_t v = type == 3 ? tiff16(e + 8, be) : tiff32(e + 8, be);
+                return v >= 1 && v <= 8 ? (int)v : 1;
+        }
+        return 1;
+}
+
+int j2p_jpeg_exif_orientation(const void *data, size_t len) {
+        const uint8_t *p = data, *end = p + len;
+        if (!data || len < 4 || p[0] != 0xFF || p[1] != 0xD8) return 1;
+        p += 2;
+        for (;;) {
+                while (p < end && *p != 0xFF) p++;
+                while (p < end && *p == 0xFF) p++;
+                if (p >= end) return 1;
+                const unsigned m = *p++;
+                if (m == 0xD9 || m == 0xDA) return 1;                    /* EOI, SOS: no Exif before the image data */
+                if (m == 0x01 || (m >= 0xD0 && m <= 0xD7)) continue;      /* TEM, RSTn: no length */
+                if (end - p < 2) return 1;
+                const unsigned seglen = be16(p);
+                if (seglen < 2 || (size_t)(end - p) < seglen) return 1;
+                const uint8_t *s = p + 2;
+                const size_t sl = seglen - 2;
+                p += seglen;
+                if (m == 0xE1 && sl >= 6 && memcmp(s, "Exif\0\0", 6) == 0) return tiff_orientation(s + 6, sl - 6);
+        }
+}

@@ -121,4 +121,13 @@ int j2p_read_jpeg_prog_layout_ex(const uint8_t *buf, size_t len, unsigned flags,
                                  size_t errlen);
 void j2p_free_jpeg_prog_layout(struct j2p_jpeg_prog_layout *l);
 
+/* ---- EXIF orientation ----
+ * The Orientation tag (0x0112) of IFD0 in the first APP1 segment that starts with "Exif\0\0" before
+ * the first SOS: 1..8 as TIFF/EXIF define it (1 = upright; 2..8 the flip or rotation that makes the
+ * stored image upright, as Pillow's ImageOps.exif_transpose applies it).  Returns 1 when there is no
+ * such segment or tag, when the TIFF header (II or MM, 42, the IFD0 offset) or IFD0 runs past the
+ * segment or the buffer, when the tag is not one SHORT or LONG, and for values outside 1..8.
+ * Reads nothing outside [data, data + len) and does not look at any other header. */
+int j2p_jpeg_exif_orientation(const void *data, size_t len);
+
 #endif

@@ -146,6 +146,8 @@ inline FrameDev rows_view(const FrameDev &F, int c0, int count, int brow, int fr
 // the three planes may come from one joint session or from three separate-mode sessions whose
 // frames differ in size.  With nc == 1 only the luma plane is read and each pixel is one sample:
 // the R (= G = B) sample of that luma with zero chroma.
+// With `oriented` set (HWC / CHW only) a CTA covers a tile of the image instead of a row segment,
+// and each frame is written flipped or rotated by its EXIF orientation (orient[frame], 1..8).
 enum EpilogueMode { EP_SCANLINES = 0, EP_HWC = 1, EP_CHW = 2 };
 struct EpilogueArgs {
     const float *plane[3];               // frame 0's Y, Cb, Cr (current iterates); Y alone when nc == 1
@@ -158,6 +160,8 @@ struct EpilogueArgs {
     int sample;                          // bits per sample: 8 or 16 (scanlines), 8, 16 or 32 (HWC / CHW)
     unsigned long long frame_bytes;      // output bytes from one frame to the next
     uint8_t *out;
+    int oriented;                        // tiled mapping with per-frame orientation (HWC / CHW)
+    const uint8_t *orient;               // device, one value per launched frame; NULL: every frame 1
 };
 
 // ---- the stand-alone halo kernel (kernels_strip.cu); pointers into OTHER ranks' memory are cudaIpc

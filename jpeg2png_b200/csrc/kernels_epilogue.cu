@@ -12,6 +12,8 @@
 // With a.nc == 1 (gray export) only the luma is read and written: clamp(float(double(Y + 128))),
 // which is the RGB expression with zero chroma (1.402 * 0 and the other products are exact zeros,
 // and adding +0 to a double that is not -0 leaves it unchanged).  The branch is uniform per launch.
+// With a.oriented (HWC / CHW) the same samples are written flipped or rotated per frame by its EXIF
+// orientation (DESIGN §7l): a CTA converts a 32 x 32 tile and writes it where the orientation puts it.
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -21,6 +23,10 @@
 namespace j2p {
 
 constexpr int EP_NT = 256;
+constexpr int EP_TILE = 32;                                 // oriented mode: tiles of EP_TILE x EP_TILE pixels
+constexpr int EP_TILE_ROW = EP_TILE * 12 + 4;               // largest staged output row (HWC float), + a pad word
+constexpr int EP_STAGE = 3 * EP_TILE * (EP_TILE * 4 + 4);   // largest staged tile (CHW float), rows padded by a word
+static_assert(EP_STAGE >= EP_TILE * EP_TILE_ROW && EP_STAGE >= EP_NT * 12, "the staging buffer holds every mode");
 
 // png.c:15-17 + :44-46: the double expression is narrowed to float by the call to clamp() and
 // compared with the double bounds 0. and 255.
@@ -29,9 +35,10 @@ __device__ __forceinline__ float clamp_sample(double v) {
     return (double)x > 255. ? 255.f : ((double)x < 0. ? 0.f : x);
 }
 
-// nbytes staged bytes -> global memory, consecutive threads on consecutive 4-byte words; dst has
-// any alignment (a scanline starts after its filter byte, a CHW row segment at any pixel)
-__device__ __forceinline__ void store_bytes(uint8_t *dst, const uint8_t *src, int nbytes, int tid) {
+// nbytes staged bytes -> global memory, consecutive threads (nt of them: the CTA or a warp) on
+// consecutive 4-byte words; dst has any alignment (a scanline starts after its filter byte, a CHW row
+// segment at any pixel)
+__device__ __forceinline__ void store_bytes(uint8_t *dst, const uint8_t *src, int nbytes, int tid, int nt = EP_NT) {
     const int head = min(nbytes, (int)((4u - ((unsigned)(uintptr_t)dst & 3u)) & 3u));
     if (tid < head) dst[tid] = src[tid];
     const int words = (nbytes - head) >> 2;
@@ -39,47 +46,116 @@ __device__ __forceinline__ void store_bytes(uint8_t *dst, const uint8_t *src, in
     const unsigned o = (unsigned)(uintptr_t)s & 3u;
     const uint32_t *s4 = reinterpret_cast<const uint32_t *>(s - o);
     uint32_t *d4 = reinterpret_cast<uint32_t *>(dst + head);
-    for (int i = tid; i < words; i += EP_NT) d4[i] = __byte_perm(s4[i], s4[i + 1], 0x3210u + 0x1111u * o);
+    for (int i = tid; i < words; i += nt) d4[i] = __byte_perm(s4[i], s4[i + 1], 0x3210u + 0x1111u * o);
     const int done = head + 4 * words;
     if (tid < nbytes - done) dst[done + tid] = src[done + tid];
 }
 
+// the samples of pixel (px, row) of a frame: the unsigned value of each of the nc samples (the float's
+// bits at 32 bits), before any byte swap
+__device__ __forceinline__ void pixel_samples(const EpilogueArgs &a, int frame, int row, int px, bool gray, uint32_t s[3]) {
+    float v[3];
+    const float *Y = a.plane[0] + (size_t)frame * a.frame_stride[0] + (size_t)row * a.ld[0];
+    const float yi = __fadd_rn(Y[px], 128.f);                                                     // jpeg2png.c:158
+    const double dy = (double)yi;
+    if (gray) {
+        v[0] = v[1] = v[2] = clamp_sample(dy);                                                       // png.c:44-46, zero chroma
+    } else {
+        const float *Cb = a.plane[1] + (size_t)frame * a.frame_stride[1] + (size_t)row * a.ld[1];
+        const float *Cr = a.plane[2] + (size_t)frame * a.frame_stride[2] + (size_t)row * a.ld[2];
+        const double dcb = (double)Cb[px], dcr = (double)Cr[px];
+        v[0] = clamp_sample(__dadd_rn(dy, __dmul_rn(1.402, dcr)));                                       // png.c:44
+        v[1] = clamp_sample(__dsub_rn(__dsub_rn(dy, __dmul_rn(0.34414, dcb)), __dmul_rn(0.71414, dcr))); // png.c:45
+        v[2] = clamp_sample(__dadd_rn(dy, __dmul_rn(1.772, dcb)));                                       // png.c:46
+    }
+    const float bitfactor = a.sample == 8 ? 1.0f : 256.0f;                                               // (1 << bits) / 256.
+#pragma unroll
+    for (int k = 0; k < 3; k++)
+        s[k] = a.sample == 32 ? __float_as_uint(v[k]) : __float2uint_rz(__fmul_rn(v[k], bitfactor));    // png.c:44-46 truncation
+}
+
+__device__ __forceinline__ void stage_sample(uint8_t *p, uint32_t s, int es) {
+    if (es == 1) *p = (uint8_t)s;
+    else if (es == 2) *reinterpret_cast<uint16_t *>(p) = (uint16_t)s;
+    else *reinterpret_cast<uint32_t *>(p) = s;
+}
+
+// Oriented mode: one CTA = the tile (blockIdx.x, blockIdx.y) of frame blockIdx.z.  Each warp reads
+// whole tile rows of the planes; the samples are staged in output order for the frame's orientation
+// k (EXIF, as Pillow's ImageOps.exif_transpose applies it: k >= 5 transposes, then (k - 1) & 3 =
+// 1, 2, 3 flips the columns, both, the rows of the result), and each warp writes staged output rows
+// as contiguous segments.  A staged row is padded by one word so the transposed staging stores of a
+// warp fall in different banks.
+__device__ __forceinline__ void oriented_tile(const EpilogueArgs &a, uint8_t *sm) {
+    const int frame = blockIdx.z, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int tx0 = blockIdx.x * EP_TILE, ty0 = blockIdx.y * EP_TILE;
+    const int tw = min(EP_TILE, a.w - tx0), th = min(EP_TILE, a.h - ty0);
+    const int es = a.sample >> 3;
+    const bool gray = a.nc == 1, chw = a.mode == EP_CHW;
+    const int nc = gray ? 1 : 3;
+    int k = a.orient ? a.orient[frame] : 1;
+    if (k < 1 || k > 8) k = 1;
+    const bool tr = k >= 5;
+    const int fl = (k - 1) & 3;
+    const bool fx = fl == 1 || fl == 2, fy = fl >= 2;
+    const int ow = tr ? th : tw, oh = tr ? tw : th;                         // the tile as written
+    const int px_bytes = chw ? es : nc * es;                                // a staged pixel
+    const int row_bytes = EP_TILE * px_bytes + 4;                           // a staged output row
+    const int plane_stage = EP_TILE * row_bytes;                            // CHW: one channel's staged tile
+    if (lane < tw) {
+        for (int ly = warp; ly < th; ly += EP_NT / 32) {
+            uint32_t s[3];
+            pixel_samples(a, frame, ty0 + ly, tx0 + lane, gray, s);
+            const int sx = tr ? ly : lane, sy = tr ? lane : ly;
+            const int ox = fx ? ow - 1 - sx : sx, oy = fy ? oh - 1 - sy : sy;
+            uint8_t *e = sm + oy * row_bytes + ox * px_bytes;
+#pragma unroll
+            for (int c = 0; c < 3; c++) {
+                if (c >= nc) break;
+                stage_sample(chw ? e + c * plane_stage : e + c * es, s[c], es);
+            }
+        }
+    }
+    __syncthreads();
+    // the output image is SW x SH (transposed for k >= 5); the tile starts at (X0, Y0) there
+    const int SW = tr ? a.h : a.w, SH = tr ? a.w : a.h;
+    const int sx0 = tr ? ty0 : tx0, sy0 = tr ? tx0 : ty0;
+    const int X0 = fx ? SW - sx0 - ow : sx0, Y0 = fy ? SH - sy0 - oh : sy0;
+    uint8_t *base = a.out + (size_t)frame * a.frame_bytes;
+    const size_t plane_bytes = (size_t)a.w * a.h * es;
+    // g lanes per output row segment, so that a warp writes several short segments (CHW) at once
+    const int segs = chw ? nc * oh : oh, words = (ow * px_bytes + 3) >> 2;
+    const int g = words <= 8 ? 8 : (words <= 16 ? 16 : 32);
+    for (int r = warp * (32 / g) + lane / g; r < segs; r += EP_NT / g) {
+        const int c = chw ? r / oh : 0, oy = r - c * oh;
+        uint8_t *dst = base + c * plane_bytes + ((size_t)(Y0 + oy) * SW + X0) * px_bytes;
+        store_bytes(dst, sm + c * plane_stage + oy * row_bytes, ow * px_bytes, lane % g, g);
+    }
+}
+
 // one CTA = EP_NT consecutive pixels of one row (a.row0 + blockIdx.y) of one frame (blockIdx.z); samples
-// are staged in shared memory in output order and written out with coalesced word stores
+// are staged in shared memory in output order and written out with coalesced word stores.  With
+// a.oriented: one 32 x 32 tile per CTA (oriented_tile).
 __global__ void __launch_bounds__(EP_NT) k_scanlines(const EpilogueArgs a) {
-    __shared__ __align__(16) uint8_t sm[EP_NT * 12 + 16];               // + one word read past the end by store_bytes
+    __shared__ __align__(16) uint8_t sm[EP_STAGE + 16];                // + one word read past the end by store_bytes
+    if (a.oriented) {
+        oriented_tile(a, sm);
+        return;
+    }
     const int row = a.row0 + (int)blockIdx.y, frame = blockIdx.z, x0 = blockIdx.x * EP_NT, tid = threadIdx.x;
     const int es = a.sample >> 3, npx = min(EP_NT, a.w - x0);           // bytes per sample, pixels of this CTA
     const bool gray = a.nc == 1;
     const int nc = gray ? 1 : 3;                                        // samples per pixel
     if (tid < npx) {
-        const int px = x0 + tid;
-        float v[3];
-        {
-            const float *Y = a.plane[0] + (size_t)frame * a.frame_stride[0] + (size_t)row * a.ld[0];
-            const float yi = __fadd_rn(Y[px], 128.f);                                                     // jpeg2png.c:158
-            const double dy = (double)yi;
-            if (gray) {
-                v[0] = v[1] = v[2] = clamp_sample(dy);                                                       // png.c:44-46, zero chroma
-            } else {
-                const float *Cb = a.plane[1] + (size_t)frame * a.frame_stride[1] + (size_t)row * a.ld[1];
-                const float *Cr = a.plane[2] + (size_t)frame * a.frame_stride[2] + (size_t)row * a.ld[2];
-                const double dcb = (double)Cb[px], dcr = (double)Cr[px];
-                v[0] = clamp_sample(__dadd_rn(dy, __dmul_rn(1.402, dcr)));                                       // png.c:44
-                v[1] = clamp_sample(__dsub_rn(__dsub_rn(dy, __dmul_rn(0.34414, dcb)), __dmul_rn(0.71414, dcr))); // png.c:45
-                v[2] = clamp_sample(__dadd_rn(dy, __dmul_rn(1.772, dcb)));                                       // png.c:46
-            }
-        }
-        const float bitfactor = a.sample == 8 ? 1.0f : 256.0f;                                               // (1 << bits) / 256.
+        uint32_t v[3];
+        pixel_samples(a, frame, row, x0 + tid, gray, v);
 #pragma unroll
         for (int k = 0; k < 3; k++) {
             if (k >= nc) break;
-            uint32_t s = a.sample == 32 ? __float_as_uint(v[k]) : __float2uint_rz(__fmul_rn(v[k], bitfactor));   // png.c:44-46 truncation
+            uint32_t s = v[k];
             if (a.mode == EP_SCANLINES && es == 2) s = ((s >> 8) & 0xffu) | ((s & 0xffu) << 8);                // png.c:58-60 big-endian
             const int e = a.mode == EP_CHW ? k * EP_NT + tid : tid * nc + k;                                  // staged element
-            if (es == 1) sm[e] = (uint8_t)s;
-            else if (es == 2) reinterpret_cast<uint16_t *>(sm)[e] = (uint16_t)s;
-            else reinterpret_cast<uint32_t *>(sm)[e] = s;
+            stage_sample(sm + e * es, s, es);
         }
     }
     __syncthreads();
@@ -95,8 +171,14 @@ __global__ void __launch_bounds__(EP_NT) k_scanlines(const EpilogueArgs a) {
     store_bytes(dst + filter + (size_t)x0 * nc * es, sm, npx * nc * es, tid);
 }
 
-// rows in launches of at most kMaxGridRows (kernels.cuh); *nlaunch: launches made
+// rows in launches of at most kMaxGridRows (kernels.cuh); the oriented mode in one launch of tiles
+// (its caller keeps the tile rows within kMaxGridRows); *nlaunch: launches made
 cudaError_t launch_scanlines(const EpilogueArgs &a, int nframes, cudaStream_t s, int *nlaunch) {
+    if (a.oriented) {
+        k_scanlines<<<dim3((a.w + EP_TILE - 1) / EP_TILE, (a.h + EP_TILE - 1) / EP_TILE, nframes), EP_NT, 0, s>>>(a);
+        *nlaunch += 1;
+        return cudaGetLastError();
+    }
     EpilogueArgs b = a;
     for (b.row0 = 0; b.row0 < a.h; b.row0 += kMaxGridRows) {
         const int rows = a.h - b.row0 < kMaxGridRows ? a.h - b.row0 : kMaxGridRows;

@@ -1008,9 +1008,11 @@ extern "C" int j2p_session_download_frame_scanlines(j2p_session *s, unsigned fra
 // ---- export into caller device memory: the colour epilogue with a tensor layout, on the caller's
 // stream, ordered after the solve that produced the planes and before anything later queued on a
 // session stream can overwrite them.  `ss`: one joint session, or the Y, Cb, Cr separate sessions;
-// nout: samples per pixel, 3 (RGB) or 1 (gray: plane 0 of the one session ss[0] alone).
+// nout: samples per pixel, 3 (RGB) or 1 (gray: plane 0 of the one session ss[0] alone).  oriented:
+// the tiled mode of the epilogue, each frame flipped or rotated by orient[frame - frame0] (device
+// memory; NULL = every frame 1).
 static int export_impl(j2p_session *const *ss, int nsess, int nout, unsigned frame0, unsigned nframes, const struct j2p_image_out *o,
-                       void *dst, void *stream) {
+                       void *dst, void *stream, bool oriented = false, const unsigned char *orient = nullptr) {
     if (!o || !dst) return fail(J2P_ERR_ARG, "null argument");
     j2p_session *s0 = ss[0];
     if (nframes == 0) return fail(J2P_ERR_ARG, "nframes must be at least 1");
@@ -1037,7 +1039,20 @@ static int export_impl(j2p_session *const *ss, int nsess, int nout, unsigned fra
     a.sample = (int)o->sample;
     a.frame_bytes = o->frame_bytes;
     a.out = (uint8_t *)dst;
+    a.oriented = oriented;
+    a.orient = orient;
+    if (oriented && (o->h + 31) / 32 > (unsigned)kMaxGridRows)
+        return fail(J2P_ERR_ARG, "an oriented export of %u rows has more than %d rows of 32-pixel tiles", o->h, kMaxGridRows);
     CK(cudaSetDevice(s0->device));
+    if (orient) {
+        cudaPointerAttributes attr;
+        if (cudaPointerGetAttributes(&attr, orient) != cudaSuccess) {
+            cudaGetLastError();
+            return fail(J2P_ERR_ARG, "orientation is not a CUDA pointer");
+        }
+        if (attr.type != cudaMemoryTypeDevice || attr.device != s0->device)
+            return fail(J2P_ERR_ARG, "orientation is not device memory on device %d", s0->device);
+    }
     const cudaStream_t st = stream ? (cudaStream_t)stream : s0->stream;
     // every session stream other than the launch stream: the launch waits for its solve ...
     for (int k = 0; k < nsess; k++) {
@@ -1086,6 +1101,34 @@ extern "C" int j2p_session_export_separate(j2p_session *y, j2p_session *cb, j2p_
         if (ss[c]->device != y->device) return fail(J2P_ERR_ARG, "the separate sessions live on different devices (%d, %d)", y->device, ss[c]->device);
     }
     return export_impl(ss, 3, 3, frame0, nframes, o, dst, stream);
+}
+
+extern "C" int j2p_session_export_oriented(j2p_session *const *sessions, unsigned nsessions, unsigned channels, unsigned frame0,
+                                           unsigned nframes, const unsigned char *orientation, const struct j2p_image_out *o,
+                                           void *dst, void *stream) {
+    if (!sessions) return fail(J2P_ERR_ARG, "null argument");
+    if (!((nsessions == 1 && (channels == 1 || channels == 3)) || (nsessions == 3 && channels == 3)))
+        return fail(J2P_ERR_ARG, "j2p_session_export_oriented takes one session with 1 or 3 channels or three sessions with 3 (got %u, %u)",
+                    nsessions, channels);
+    for (unsigned k = 0; k < nsessions; k++)
+        if (!sessions[k]) return fail(J2P_ERR_ARG, "null session");
+    j2p_session *s = sessions[0];
+    if (nsessions == 3) {
+        for (int c = 0; c < 3; c++) {
+            if (sessions[c]->F.nc != 1 || sessions[c]->strip)
+                return fail(J2P_ERR_ARG, "a separate oriented export needs three whole-frame sessions with one plane each (plane %d has %d)", c,
+                            sessions[c]->F.nc);
+            if (sessions[c]->nframes != s->nframes)
+                return fail(J2P_ERR_ARG, "the separate sessions hold different frame counts (%u, %u)", s->nframes, sessions[c]->nframes);
+            if (sessions[c]->device != s->device)
+                return fail(J2P_ERR_ARG, "the separate sessions live on different devices (%d, %d)", s->device, sessions[c]->device);
+        }
+    } else if (channels == 3) {
+        if (s->F.nc != 3 || s->strip) return fail(J2P_ERR_ARG, "a joint oriented export needs a whole-frame session with three planes");
+    } else if ((s->F.nc != 1 && s->F.nc != 3) || s->strip) {
+        return fail(J2P_ERR_ARG, "a gray oriented export needs a whole-frame session with one or three planes (has %d)", s->F.nc);
+    }
+    return export_impl(sessions, (int)nsessions, (int)channels, frame0, nframes, o, dst, stream, true, orientation);
 }
 
 extern "C" int j2p_session_sync(j2p_session *s) {

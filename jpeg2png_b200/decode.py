@@ -10,6 +10,9 @@ per chunk (j2p_session_export) on the caller's current stream.  The returned ten
 views of that tensor and share its storage.  With mode='UNCHANGED' or 'GRAY' the reader also takes
 one-component (grayscale) files (J2P_READ_GRAY); those are solved as the luma of separate mode and,
 like the luma of colour files in mode='GRAY', exported as one channel (j2p_session_export_gray).
+With apply_exif_orientation=True each file's EXIF Orientation tag is read on the host
+(j2p_jpeg_exif_orientation) and a chunk that holds a file with an orientation other than 1 is exported
+in one call that flips or rotates every frame as it writes it (j2p_session_export_oriented, DESIGN §7l).
 
 The samples are those of the PNG the command line writes for the same file and flags:
 torch.uint8 the 8-bit PNG samples, torch.uint16 the 16-bit (-1) samples in native byte order,
@@ -113,6 +116,8 @@ def _declare_codecs(lib):
     lib.j2p_read_jpeg_prog_layout_ex.argtypes = [C.c_char_p, C.c_size_t, C.c_uint, C.POINTER(ProgLayout), C.c_char_p, C.c_size_t]
     lib.j2p_free_jpeg_prog_layout.restype = None
     lib.j2p_free_jpeg_prog_layout.argtypes = [C.POINTER(ProgLayout)]
+    lib.j2p_jpeg_exif_orientation.restype = C.c_int
+    lib.j2p_jpeg_exif_orientation.argtypes = [C.c_char_p, C.c_size_t]
 
 
 def load_codecs() -> C.CDLL:
@@ -295,6 +300,19 @@ def parse_jpeg(data: bytes, flags: int = 0) -> Parsed:
     return Parsed(int(j.w), int(j.h), planes)
 
 
+def exif_orientation(data: bytes) -> int:
+    """The EXIF Orientation of JPEG bytes (j2p_jpeg_exif_orientation): 1..8, 1 without a usable tag."""
+    return int(load_codecs().j2p_jpeg_exif_orientation(data, len(data)))
+
+
+def oriented_shape(shape, layout_id, orientation):
+    """The (c, h, w) or (h, w, c) shape of a frame of `shape` written with an EXIF orientation."""
+    if orientation < 5:
+        return shape
+    c, h, w = shape if layout_id == abi.LAYOUT_CHW else (shape[2], shape[0], shape[1])
+    return (c, w, h) if layout_id == abi.LAYOUT_CHW else (w, h, c)
+
+
 def solver_flags(iterations, weight, pweight, separate):
     """The command line's flags (reference jpeg2png.c:206-244): returns per-plane iterations,
     weights and pweights.  A scalar weight sets luma only (chroma 0); three weights or three
@@ -465,9 +483,13 @@ class _Chunk:
     constructor; close() waits for them and returns their blocks to the device cache.
     coefs: {item index: (_DeviceCoefs, its file index)} for items whose coefficients are on the
     device (uploaded with j2p_session_upload_device after `coef_stream`).  A gray file is solved as
-    the luma of separate mode; the output has the channels solved_planes gives for `mode`."""
+    the luma of separate mode; the output has the channels solved_planes gives for `mode`.
+    orientations: the EXIF orientation of each item, or None.  When one of them is not 1 the chunk is
+    exported by j2p_session_export_oriented into an (n, c * h * w) tensor; frame(j) is item j's
+    tensor either way."""
 
-    def __init__(self, lib, device, items, flags, separate, dtype, layout, coefs=None, coef_stream=None, mode='RGB'):
+    def __init__(self, lib, device, items, flags, separate, dtype, layout, coefs=None, coef_stream=None, mode='RGB',
+                 orientations=None):
         iters, weights, pweights = flags
         self.lib, self.sessions, self.coefs = lib, [], coefs or {}
         first, n = items[0], len(items)
@@ -494,14 +516,26 @@ class _Chunk:
                                                                p.quant.ctypes.data, None))     # conventional decode on the device
                 self._check(lib.j2p_session_iterate(s, 0, it))
             w, h = first.w, first.h
-            shape = (n, nout, h, w) if layout == abi.LAYOUT_CHW else (n, h, w, nout)
-            self.out = torch.empty(shape, dtype=dtype, device=torch.device('cuda', device))
+            shape = (nout, h, w) if layout == abi.LAYOUT_CHW else (h, w, nout)
+            cuda = torch.device('cuda', device)
+            self.shapes = None
+            if orientations is not None and any(k != 1 for k in orientations):
+                self.shapes = [oriented_shape(shape, layout, k) for k in orientations]
+                self.out = torch.empty((n, nout * h * w), dtype=dtype, device=cuda)
+            else:
+                self.out = torch.empty((n,) + shape, dtype=dtype, device=cuda)
             o = abi.ImageOut(w, h, _SAMPLE[dtype], layout, nout * h * w * self.out.element_size())
             # torch's default stream is handle 0, which the ABI reads as "the session stream":
             # name it cudaStreamLegacy (1) instead
             stream = C.c_void_p(torch.cuda.current_stream(device).cuda_stream or 1)
             dst = C.c_void_p(self.out.data_ptr())
-            if nout == 1:
+            if self.shapes is not None:
+                # uploaded on the current stream, which the export runs on
+                self.orient = torch.tensor(orientations, dtype=torch.uint8).to(cuda)
+                ss = self.sessions[:1] if nout == 1 else self.sessions
+                self._check(lib.j2p_session_export_oriented((C.c_void_p * len(ss))(*ss), len(ss), nout, 0, n,
+                                                            C.c_void_p(self.orient.data_ptr()), C.byref(o), dst, stream))
+            elif nout == 1:
                 self._check(lib.j2p_session_export_gray(self.sessions[0], 0, n, C.byref(o), dst, stream))
             elif separate:
                 self._check(lib.j2p_session_export_separate(*self.sessions, 0, n, C.byref(o), dst, stream))
@@ -514,6 +548,10 @@ class _Chunk:
     def _check(self, rc):
         if rc != 0:
             raise RuntimeError(self.lib.j2p_last_error().decode())
+
+    def frame(self, j):
+        """Item j's tensor: a view of out[j]."""
+        return self.out[j] if self.shapes is None else self.out[j].view(self.shapes[j])
 
     def close(self):
         for s in self.sessions:
@@ -571,7 +609,7 @@ def _front_end(data, device_ok, progressive=False, flags=0):
 
 def decode_jpeg(inputs, *, iterations=50, weight=0.3, pweight=0.001, separate=False,
                 dtype=torch.uint8, layout='CHW', device=None, max_frames=None, progressive_on_device=False,
-                mode='RGB'):
+                mode='RGB', apply_exif_orientation=False):
     """Decode JPEG files into RGB or gray tensors on a CUDA device, deblocked by the solver.
 
     inputs: bytes-like, a path (str / os.PathLike), or a list or tuple of them.  A single input
@@ -603,11 +641,21 @@ def decode_jpeg(inputs, *, iterations=50, weight=0.3, pweight=0.001, separate=Fa
     unreadable files, with the host reader's message: header errors before any device work, errors
     in a device-decoded file's entropy-coded data once its batch has been decoded, before that batch
     is solved.  Raises RuntimeError when no CUDA device is usable.
+
+    apply_exif_orientation: True or False (default).  With True, a file whose EXIF Orientation tag
+    (0x0112 of IFD0 in its first "Exif" APP1 segment) is 2..8 comes back flipped or rotated as
+    Pillow's ImageOps.exif_transpose shows it, at its rotated visible size: orientations 5..8 swap h
+    and w, giving (c, w, h) or (w, h, c).  Files without a usable tag read as 1 and are unchanged.
+    The samples are those of the unrotated decode, written to their rotated places by the export
+    itself; mode, separate, dtype, layout, max_frames and progressive_on_device work as without it,
+    and files of one geometry share a batch whatever their orientation.  Every tensor is contiguous.
     """
     flags = solver_flags(iterations, weight, pweight, separate)
     if not isinstance(mode, str) or mode not in MODES:
         raise ValueError(f"mode must be 'RGB', 'UNCHANGED' or 'GRAY', not {mode!r}")
     read_flags = 0 if mode == 'RGB' else READ_GRAY
+    if apply_exif_orientation is not True and apply_exif_orientation is not False:
+        raise ValueError(f'apply_exif_orientation must be True or False, not {apply_exif_orientation!r}')
     if dtype not in _SAMPLE:
         raise ValueError(f'dtype must be torch.uint8, torch.uint16 or torch.float32, not {dtype}')
     if layout not in _LAYOUT:
@@ -632,8 +680,11 @@ def decode_jpeg(inputs, *, iterations=50, weight=0.3, pweight=0.001, separate=Fa
         with ThreadPoolExecutor(workers) as pool:
             parsed = list(pool.map(lambda d: _front_end(d, device_ok, progressive_on_device, read_flags),
                                    [data for data, _ in read]))
+            orientations = (list(pool.map(exif_orientation, [data for data, _ in read]))
+                            if apply_exif_orientation else None)
     else:
         parsed = [_front_end(data, device_ok, progressive_on_device, read_flags) for data, _ in read]
+        orientations = [exif_orientation(data) for data, _ in read] if apply_exif_orientation else None
     for i, (p, (_, path)) in enumerate(zip(parsed, read)):
         if isinstance(p, ValueError):
             raise ValueError(f'{_where(i, path)}: {p}')
@@ -676,9 +727,10 @@ def decode_jpeg(inputs, *, iterations=50, weight=0.3, pweight=0.001, separate=Fa
                                                f'({ENT_FAILURES.get(int(dc.status[k]), int(dc.status[k]))}) on a file '
                                                'the host reader accepts (a decoder bug)')
                         coefs[j] = (dc, k)
-                chunk = _Chunk(lib, index, [parsed[i] for i in idx], flags, separate, dtype, layout_id, coefs, coef_stream, mode)
+                chunk = _Chunk(lib, index, [parsed[i] for i in idx], flags, separate, dtype, layout_id, coefs, coef_stream, mode,
+                               None if orientations is None else [orientations[i] for i in idx])
                 for j, i in enumerate(idx):
-                    results[i] = chunk.out[j]
+                    results[i] = chunk.frame(j)
                 if previous is not None:        # this chunk is queued: let the previous one finish
                     previous.close()
                 previous = chunk
