@@ -310,6 +310,22 @@ int j2p_session_export_oriented(j2p_session *const *sessions, unsigned nsessions
                                 unsigned frame0, unsigned nframes, const unsigned char *orientation,
                                 const struct j2p_image_out *o, void *dst, void *stream);
 
+/* Iterations [first, first + count) of every frame of every session of `sessions`, in one launch chain:
+ * each kernel of an iteration is launched once for all n sessions, whatever their frame sizes, on the
+ * first session's stream (the grouped kernels of libj2pmixed.so, loaded on first use).  Every frame's
+ * result is bit-identical to what j2p_session_iterate gives it: same CTAs, bands and tiles, its own sums
+ * of g^2 folded in the same order.  Each session's FISTA state, buffer parity, iteration counter and
+ * launch count advance as j2p_session_iterate would advance them, so j2p_session_iterate, the exports and
+ * later groups continue from there.  The launch stream first waits for what every other session's
+ * stream has queued (uploads, re-arm), and each other session's stream then waits for the group's last
+ * launch.  first == 0 re-arms a session as j2p_session_iterate does.
+ * Sessions join a group when they are whole-frame (batch or single-frame) sessions on one device, without
+ * objective logging, with equal nchannel, equal sampling factors per plane, every plane 1x1 or 2x2, and
+ * bitwise-equal weight, pweights and iterations, first is every session's next iteration, and the group
+ * holds at most 65535 frames.  Everything else is J2P_ERR_ARG with a message naming the first offending
+ * session; a missing libj2pmixed.so is J2P_ERR_CUDA. */
+int j2p_session_iterate_group(j2p_session *const *sessions, unsigned n, unsigned first, unsigned count);
+
 /* Objective terms of the most recent iteration, as logged by the reference (compute.c:271-272):
  * out[0]=objective, out[1]=prob_dist, out[2]=tv, out[3]=tv2.  Only tracked when logging was
  * enabled with j2p_session_set_logging(s, 1) before iterating. */

@@ -454,15 +454,6 @@ cudaError_t configure_project_kernels();
 int packed_gradient_occupancy();
 cudaError_t launch_gradient_packed(const FrameDev &F, float factor, cudaStream_t s);
 
-// J2P_PDL=0: launch the kernels of an iteration without the programmatic-dependent-launch attribute (pdl.cuh; A/B aid)
-bool pdl_enabled() {
-    static const bool on = [] {
-        const char *e = getenv("J2P_PDL");
-        return !(e && *e == '0');
-    }();
-    return on;
-}
-
 // J2P_GRAD_SCALAR=1: the scalar kernel for every session (A/B aid; it is always the -c csv build)
 static bool g_grad_scalar = false;
 

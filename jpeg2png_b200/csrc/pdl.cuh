@@ -15,6 +15,7 @@
 // A kernel launched without the attribute sees both instructions as no-ops.
 #pragma once
 #include <cuda_runtime.h>
+#include <stdlib.h>
 
 #include <utility>
 
@@ -25,7 +26,14 @@ __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;"
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 #endif
 
-bool pdl_enabled();      // J2P_PDL=0 switches the attribute off (A/B aid); kernels_gradient.cu
+// J2P_PDL=0: launch the kernels of an iteration without the programmatic-dependent-launch attribute (A/B aid)
+inline bool pdl_enabled() {
+    static const bool on = [] {
+        const char *e = getenv("J2P_PDL");
+        return !(e && *e == '0');
+    }();
+    return on;
+}
 
 template <typename... KArgs, typename... Args>
 inline cudaError_t launch_chain(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t s, Args &&...args) {

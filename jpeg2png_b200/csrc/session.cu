@@ -28,13 +28,17 @@
 #include <sys/mman.h>
 #include <time.h>
 
+#include <atomic>
+#include <algorithm>
 #include <map>
+#include <string>
 #include <mutex>
 #include <utility>
 #include <vector>
 
 #include "../../include/jpeg2png_b200.h"
 #include "copy_pool.h"
+#include "geometry.cuh"
 #include "kernels.cuh"
 #include "tma_maps.h"
 
@@ -53,6 +57,9 @@ int project_tile_border_units(const PlaneDev &P);
 cudaError_t launch_scanlines(const EpilogueArgs &a, int nframes, cudaStream_t s, int *nlaunch);
 // kernels_strip.cu: the strip exchanges over peer memory (parameter blocks in kernels.cuh)
 cudaError_t launch_halo_exchange(const HaloPeers &P, unsigned seq, unsigned *ticket, int *err, int wait_for_arrival, cudaStream_t s);
+// kernels_gradient_packed.cu: the packed gradient's GPM and grid for a frame (what a group gives it)
+int packed_gradient_gpm(const FrameDev &F);
+void packed_gradient_geometry(const FrameDev &F, int *cx, int *bands, int *rows);
 }  // namespace j2p
 
 using namespace j2p;
@@ -214,7 +221,12 @@ struct j2p_session {
     unsigned stage_next = 0;
     cudaEvent_t export_ev = nullptr;          // orders j2p_session_export on a caller stream with the session stream
     cudaEvent_t upload_ev = nullptr;          // orders j2p_session_upload_device after its producer stream
+    unsigned long long uid = 0;               // unique over the process (a group's plan names its sessions by it)
+    unsigned long long tables_gen = 0;        // bumped whenever a quantisation table is set
+    struct GroupPlan *group = nullptr;        // the plan of the last group this session led (j2p_session_iterate_group)
+    cudaEvent_t group_ev = nullptr;           // orders a group's launches with this session's stream
 };
+static void free_group_plan(GroupPlan *g);
 
 // x_k <-> x_{k-1} after an iteration (reference SWAP at compute.c:438); all planes together, which
 // keeps pl[c].x == pl[0].x + c * plane_stride
@@ -309,6 +321,8 @@ extern "C" void j2p_session_destroy(j2p_session *s) {
     }
     if (s->export_ev) cudaEventDestroy(s->export_ev);
     if (s->upload_ev) cudaEventDestroy(s->upload_ev);
+    if (s->group_ev) cudaEventDestroy(s->group_ev);
+    free_group_plan(s->group);                       // the stream is idle: no group launch reads the plan any more
     if (s->stream) cudaStreamDestroy(s->stream);
     delete s;
 }
@@ -487,6 +501,8 @@ static int create_session(j2p_session **out, int device, const struct j2p_frame_
     if (!out || !d) return fail(J2P_ERR_ARG, "null argument");
     *out = nullptr;
     j2p_session *s = new j2p_session();
+    static std::atomic<unsigned long long> uid_seq{0};
+    s->uid = ++uid_seq;
     const int rc = create_impl(s, device, d, row0, rows, nframes);
     if (rc != J2P_OK) {
         char keep[sizeof g_err];
@@ -685,6 +701,7 @@ static int set_tables(j2p_session *s, unsigned plane, const uint16_t *quant, flo
         }
     }
     s->tables_stale = true;
+    s->tables_gen++;
     *tab_out = tab;
     return J2P_OK;
 }
@@ -1567,6 +1584,303 @@ extern "C" int j2p_session_iterate_strip(j2p_session *s, j2p_comm *c, unsigned n
             if (c->fused_halo) c->seq_halo++;                            // delivered by the projection kernels
             else if ((rc = exchange_halos_p2p(s, c, 0)) != J2P_OK) return rc;   // stand-alone copy, no wait: the next gradient waits
         } else if ((rc = exchange_halos_nccl(s, c, api)) != J2P_OK) return rc;
+    }
+    return J2P_OK;
+}
+
+// ---- groups: sessions of different frame sizes iterated in one launch chain ----------------------
+// The grouped kernels live in libj2pmixed.so (mixed/mixed.cu), next to this library in the package
+// tree, loaded on first use.  A group's plan (geometry.cuh): one GroupFrame per session and parity,
+// one GroupCta per CTA of every grouped kernel, and device tables for one-frame sessions (their kernels
+// read the tables from the parameter block).  It is built once and kept in the first session until
+// the group's sessions or their arming change.
+namespace {
+struct MixedApi {
+    int (*configure)(void) = nullptr;
+    int (*iterate)(const GroupFrame *, const GroupCta *, const GroupLaunch *, int, int, float, void *, int *) = nullptr;
+    char err[400] = "";
+};
+const MixedApi &mixed_api() {
+    static const MixedApi api = [] {
+        MixedApi a;
+        Dl_info info;
+        if (!dladdr((void *)&j2p_session_iterate_group, &info) || !info.dli_fname) {
+            snprintf(a.err, sizeof a.err, "cannot locate libjpeg2png_b200.so to find libj2pmixed.so");
+            return a;
+        }
+        std::string path(info.dli_fname);
+        const size_t slash = path.rfind('/');
+        path = (slash == std::string::npos ? std::string(".") : path.substr(0, slash)) + "/../mixed/libj2pmixed.so";
+        void *h = dlopen(path.c_str(), RTLD_NOW | RTLD_LOCAL);
+        if (!h) {
+            snprintf(a.err, sizeof a.err, "libj2pmixed.so (the grouped kernels) cannot be loaded: %s", dlerror());
+            return a;
+        }
+        a.configure = (int (*)(void))dlsym(h, "j2p_mixed_configure");
+        a.iterate = (decltype(a.iterate))dlsym(h, "j2p_mixed_iterate");
+        if (!a.configure || !a.iterate) {
+            snprintf(a.err, sizeof a.err, "%s does not export j2p_mixed_configure / j2p_mixed_iterate", path.c_str());
+            a.configure = nullptr;
+            a.iterate = nullptr;
+        }
+        return a;
+    }();
+    return api;
+}
+std::once_flag g_mixed_once[64];
+int g_mixed_cfg[64];
+}  // namespace
+
+struct GroupPlan {
+    std::vector<unsigned long long> key;     // the sessions (uid): their geometry and buffers never change
+    std::vector<unsigned long long> tables_gen;   // the one-frame sessions' tables the device copy holds
+    GroupFrame *frames = nullptr;    // device [2][n]: parity 0, parity 1
+    GroupCta *ctas = nullptr;        // device, every grouped kernel's slice (L)
+    float *tables = nullptr;         // device tables of the one-frame sessions
+    GroupLaunch L{};
+    int gpm_nc = 0, tgv = 0;
+    std::vector<unsigned> launches;  // per session: what one j2p_session_iterate iteration adds to its count
+    std::vector<GroupFrame> h_frames;
+    std::vector<GroupCta> h_ctas;
+    std::vector<float> h_tables;
+};
+
+static void free_group_plan(GroupPlan *g) {
+    if (!g) return;
+    cudaFree(g->frames);
+    cudaFree(g->ctas);
+    cudaFree(g->tables);
+    delete g;
+}
+
+// the launches one iteration of `s` makes on its own (one_iteration: the gradient, then launch_project
+// for 1x1 / 2x2 planes, planes of one geometry sharing a launch, a launch per 65535 block rows, and one
+// per plane with pixels no block covers)
+static unsigned own_launches(const FrameDev &F) {
+    unsigned n = 1;
+    for (int c = 0; c < F.nc; c++) {
+        const PlaneDev &P = F.pl[c];
+        int count = 1;
+        while (c + count < F.nc && F.pl[c + count].sw == P.sw && F.pl[c + count].sh == P.sh && F.pl[c + count].cw == P.cw &&
+               F.pl[c + count].ch == P.ch)
+            count++;
+        n += (unsigned)(((P.ch >> 3) + kMaxGridRows - 1) / kMaxGridRows);
+        for (int k = c; k < c + count; k++)
+            n += F.pl[k].sw * F.pl[k].cw < F.W || F.pl[k].sh * F.pl[k].ch < F.H ? 1u : 0u;
+        c += count - 1;
+    }
+    return n;
+}
+
+static int build_group_plan(j2p_session *const *ss, unsigned n, GroupPlan *g) {
+    std::vector<GroupCta> slot[GK_COUNT];
+    size_t ntab = 0;
+    for (unsigned d = 0; d < n; d++)
+        if (ss[d]->nframes == 1) ntab += ss[d]->tables.size();
+    g->h_tables.reserve(ntab);
+    g->h_frames.assign(2 * (size_t)n, GroupFrame{});
+    g->launches.resize(n);
+    if (ntab) CK(cudaMalloc(&g->tables, ntab * sizeof(float)));
+    for (unsigned d = 0; d < n; d++) {
+        const j2p_session *s = ss[d];
+        FrameDev F = s->F;
+        for (int c = 0; c < F.nc; c++) {                    // parity 0: x_k in the first iterate buffer
+            F.pl[c].x = s->x[c];
+            F.pl[c].xp = s->xp[c];
+        }
+        F.buf_sel = 0;
+        if (s->nframes == 1) {
+            F.tables = g->tables + g->h_tables.size();
+            g->h_tables.insert(g->h_tables.end(), s->tables.begin(), s->tables.end());
+        }
+        int cx, bands, rows;
+        packed_gradient_geometry(F, &cx, &bands, &rows);
+        const int gpm = packed_gradient_gpm(F);
+        g->launches[d] = own_launches(F);
+        GroupFrame &G0 = g->h_frames[d], &G1 = g->h_frames[n + d];
+        G0.F = F;
+        G0.band_rows = rows;
+        G1 = G0;
+        for (int c = 0; c < F.nc; c++) std::swap(G1.F.pl[c].x, G1.F.pl[c].xp);
+        G1.F.buf_sel = 1;
+        for (unsigned f = 0; f < s->nframes; f++) {
+            for (int by = 0; by < bands; by++)
+                for (int bx = 0; bx < cx; bx++) slot[GK_GRAD + gpm].push_back({d, 0, (unsigned)bx, (unsigned)by, f, (unsigned)cx, (unsigned)bands, 0});
+            for (int c = 0; c < F.nc; c++) {
+                const PlaneDev &P = F.pl[c];
+                const bool p11 = P.sw == 1;                 // the join rules leave 1x1 and 2x2 planes only
+                const int bw = P.cw >> 3, bh = P.ch >> 3, gx = (bw + 15) / 16;   // PT_NB == P22_NB == 16 blocks per tile
+                std::vector<GroupCta> &tiles = slot[p11 ? GK_TILE + (P.resample ? 1 : 0) : GK_TILE22];
+                for (int by = 0; by < bh; by++)
+                    for (int bx = 0; bx < gx; bx++) tiles.push_back({d, (unsigned)c, (unsigned)bx, (unsigned)by, f, (unsigned)gx, (unsigned)bh, 0});
+                const size_t cwf = (size_t)P.sw * P.cw, chf = (size_t)P.sh * P.ch;
+                if (cwf < (size_t)F.W || chf < (size_t)F.H) {
+                    // any split of the region is the same per-pixel step; this is the batch path's
+                    const size_t px = ((size_t)F.H - chf) * F.W + chf * (F.W - cwf);
+                    const size_t cap = s->nframes > 1 ? (132 * 8 + s->nframes - 1) / s->nframes : 132 * 8;
+                    const size_t blocks = std::min((px + 255) / 256, cap);
+                    for (size_t b = 0; b < blocks; b++)
+                        slot[p11 ? GK_UNCOVERED : GK_UNCOVERED22].push_back({d, (unsigned)c, (unsigned)b, 0, f, (unsigned)blocks, 1, 0});
+                }
+            }
+        }
+    }
+    for (int k = 0; k < GK_COUNT; k++) {
+        if (slot[k].size() > 0x7fffffffu) return fail(J2P_ERR_ARG, "the group needs more than 2^31 CTAs in one launch");
+        g->L.first[k] = (unsigned)g->h_ctas.size();
+        g->L.count[k] = (unsigned)slot[k].size();
+        g->h_ctas.insert(g->h_ctas.end(), slot[k].begin(), slot[k].end());
+    }
+    j2p_session *s0 = ss[0];
+    CK(cudaMalloc(&g->frames, g->h_frames.size() * sizeof(GroupFrame)));
+    CK(cudaMalloc(&g->ctas, g->h_ctas.size() * sizeof(GroupCta)));
+    // host vectors live as long as the plan: the copies may still be in flight when this returns
+    CK(cudaMemcpyAsync(g->frames, g->h_frames.data(), g->h_frames.size() * sizeof(GroupFrame), cudaMemcpyHostToDevice, s0->stream));
+    CK(cudaMemcpyAsync(g->ctas, g->h_ctas.data(), g->h_ctas.size() * sizeof(GroupCta), cudaMemcpyHostToDevice, s0->stream));
+    if (ntab) CK(cudaMemcpyAsync(g->tables, g->h_tables.data(), ntab * sizeof(float), cudaMemcpyHostToDevice, s0->stream));
+    g->gpm_nc = s0->F.nc;
+    g->tgv = s0->F.use_tgv;
+    for (unsigned d = 0; d < n; d++) {
+        g->key.push_back(ss[d]->uid);
+        g->tables_gen.push_back(ss[d]->tables_gen);
+    }
+    return J2P_OK;
+}
+
+// After uploads: the one-frame sessions' tables into the plan's device copy again (the CTA table and the
+// descriptors depend on geometry and buffers only).  Ordered on the launch stream after earlier groups.
+static int refresh_group_tables(j2p_session *const *ss, unsigned n, GroupPlan *g) {
+    bool stale = false;
+    for (unsigned d = 0; d < n; d++) stale = stale || (ss[d]->nframes == 1 && g->tables_gen[d] != ss[d]->tables_gen);
+    if (!stale) return J2P_OK;
+    size_t at = 0;
+    for (unsigned d = 0; d < n; d++) {
+        if (ss[d]->nframes != 1) continue;
+        std::copy(ss[d]->tables.begin(), ss[d]->tables.end(), g->h_tables.begin() + at);
+        at += ss[d]->tables.size();
+        g->tables_gen[d] = ss[d]->tables_gen;
+    }
+    // pageable source: the copy has read h_tables when the call returns
+    CK(cudaMemcpyAsync(g->tables, g->h_tables.data(), g->h_tables.size() * sizeof(float), cudaMemcpyHostToDevice, ss[0]->stream));
+    return J2P_OK;
+}
+
+// the first reason `s` (index k) cannot join a group led by s0, or nullptr
+static int refuse_join(const j2p_session *s0, const j2p_session *s, unsigned k) {
+    const j2p_frame_desc &a = s0->desc, &b = s->desc;
+    if (s->device != s0->device) return fail(J2P_ERR_ARG, "group session %u is on device %d, session 0 on %d", k, s->device, s0->device);
+    if (s->strip) return fail(J2P_ERR_ARG, "group session %u is a strip session", k);
+    if (s->logging) return fail(J2P_ERR_ARG, "group session %u logs the objective", k);
+    if (b.nchannel != a.nchannel) return fail(J2P_ERR_ARG, "group session %u has %u planes, session 0 %u", k, b.nchannel, a.nchannel);
+    for (unsigned c = 0; c < b.nchannel; c++) {
+        if (!((b.w_samp[c] == 1 && b.h_samp[c] == 1) || (b.w_samp[c] == 2 && b.h_samp[c] == 2)))
+            return fail(J2P_ERR_ARG, "group session %u plane %u is sampled %ux%u; a group takes 1x1 and 2x2 planes only", k, c, b.w_samp[c], b.h_samp[c]);
+        if (b.w_samp[c] != a.w_samp[c] || b.h_samp[c] != a.h_samp[c])
+            return fail(J2P_ERR_ARG, "group session %u plane %u is sampled %ux%u, session 0 %ux%u", k, c, b.w_samp[c], b.h_samp[c], a.w_samp[c], a.h_samp[c]);
+        if (memcmp(&b.pweight[c], &a.pweight[c], sizeof(float)))
+            return fail(J2P_ERR_ARG, "group session %u plane %u has pweight %g, session 0 %g", k, c, b.pweight[c], a.pweight[c]);
+    }
+    if (memcmp(&b.weight, &a.weight, sizeof(float))) return fail(J2P_ERR_ARG, "group session %u has weight %g, session 0 %g", k, b.weight, a.weight);
+    if (b.iterations != a.iterations) return fail(J2P_ERR_ARG, "group session %u has %u iterations, session 0 %u", k, b.iterations, a.iterations);
+    return J2P_OK;
+}
+
+extern "C" int j2p_session_iterate_group(j2p_session *const *sessions, unsigned n, unsigned first, unsigned count) {
+    if (!sessions || n == 0) return fail(J2P_ERR_ARG, "a group needs at least one session");
+    for (unsigned k = 0; k < n; k++)
+        if (!sessions[k]) return fail(J2P_ERR_ARG, "group session %u is null", k);
+    j2p_session *s0 = sessions[0];
+    unsigned long long frames = 0;
+    for (unsigned k = 0; k < n; k++) {
+        const int rc = refuse_join(s0, sessions[k], k);
+        if (rc != J2P_OK) return rc;
+        for (unsigned j = 0; j < k; j++)
+            if (sessions[j] == sessions[k]) return fail(J2P_ERR_ARG, "group session %u is session %u again", k, j);
+        frames += sessions[k]->nframes;
+        if (frames > 65535) return fail(J2P_ERR_ARG, "group session %u takes the group past 65535 frames", k);
+    }
+    CK(cudaSetDevice(s0->device));
+    // every session is checked before any is re-armed: a refused call changes nothing
+    for (unsigned k = 0; k < n; k++) {
+        const j2p_session *s = sessions[k];
+        for (size_t p = 0; p < s->uploaded.size(); p++)
+            if (!s->uploaded[p]) return fail(J2P_ERR_ARG, "group session %u: plane %zu has not been uploaded", k, p);
+        const unsigned next = s->stale ? 0u : s->next_iter;      // a re-arm (check_ready) starts at 0
+        if (first != 0 && first != next)
+            return fail(J2P_ERR_ARG, "group session %u: iterations must be contiguous (expected %u, got %u)", k, next, first);
+    }
+    for (unsigned k = 0; k < n; k++) {
+        const int rc = check_ready(sessions[k], first);
+        if (rc != J2P_OK) {
+            char why[sizeof g_err];
+            memcpy(why, g_err, sizeof why);
+            return fail(rc, "group session %u: %s", k, why);
+        }
+    }
+    if (count == 0) return J2P_OK;
+    const MixedApi &api = mixed_api();
+    if (!api.iterate) return fail(J2P_ERR_CUDA, "%s", api.err);
+    std::call_once(g_mixed_once[s0->device & 63], [&] { g_mixed_cfg[s0->device & 63] = api.configure(); });
+    CK((cudaError_t)g_mixed_cfg[s0->device & 63]);
+
+    GroupPlan *g = s0->group;
+    bool same = g && g->key.size() == n;
+    for (unsigned k = 0; same && k < n; k++) same = g->key[k] == sessions[k]->uid;
+    if (!same) {
+        if (g) {
+            CK(cudaStreamSynchronize(s0->stream));      // the old plan may still be read by queued launches
+            free_group_plan(g);
+            s0->group = nullptr;
+        }
+        g = new GroupPlan();
+        const int rc = build_group_plan(sessions, n, g);
+        if (rc != J2P_OK) {
+            cudaStreamSynchronize(s0->stream);
+            free_group_plan(g);
+            return rc;
+        }
+        s0->group = g;
+    } else {
+        const int rc = refresh_group_tables(sessions, n, g);
+        if (rc != J2P_OK) return rc;
+    }
+    // the launch stream waits for what every other session's stream has queued (uploads, re-arm)
+    for (unsigned k = 1; k < n; k++) {
+        j2p_session *s = sessions[k];
+        if (s->stream == s0->stream) continue;
+        if (!s->group_ev) CK(cudaEventCreateWithFlags(&s->group_ev, cudaEventDisableTiming));
+        CK(cudaEventRecord(s->group_ev, s->stream));
+        CK(cudaStreamWaitEvent(s0->stream, s->group_ev, 0));
+    }
+    for (unsigned i = first; i < first + count; i++) {
+        // FISTA momentum (compute.c:431-432, :440): every session is at iteration i, so at the same t
+        const float tnext = (1 + sqrtf(1 + 4 * (s0->t * s0->t))) / 2;
+        const float factor = (s0->t - 1) / tnext;
+        int nl = 0;
+        const cudaError_t e = (cudaError_t)api.iterate(g->frames + (size_t)s0->F.buf_sel * n, g->ctas, &g->L, g->gpm_nc, g->tgv, factor, s0->stream, &nl);
+        CK(e);
+        for (unsigned k = 0; k < n; k++) {
+            j2p_session *s = sessions[k];
+            s->t = tnext;
+            s->launches += g->launches[k];
+            swap_iterates(s->F);                                             // compute.c:438
+        }
+    }
+    // ... and every other session's stream waits for the group's last launch
+    for (unsigned k = 0; k < n; k++) {
+        j2p_session *s = sessions[k];
+        if (k > 0 && s->stream != s0->stream) {
+            CK(cudaEventRecord(s->group_ev, s0->stream));
+            CK(cudaStreamWaitEvent(s->stream, s->group_ev, 0));
+        }
+        // the iterations j2p_session_wait_iteration may ask for: marked where the whole group is complete
+        for (unsigned i = first; i < first + count; i++)
+            if (i % kEventStride == kEventStride - 1) {
+                const int slot = (int)((i / kEventStride) % kEventRing);
+                CK(cudaEventRecord(s->ev[slot], s->stream));
+                s->ev_iter[slot] = (long long)i;
+            }
+        s->next_iter = first + count;
     }
     return J2P_OK;
 }

@@ -407,6 +407,60 @@ def plan(keys, frames_for_key):
     return chunks
 
 
+# Grouping (internal switch; tools/mixed_bench.py and the tests compare the two): chunks of different
+# geometries whose frames are small are iterated together, one j2p_session_iterate_group call per pack
+# (DESIGN §7m).  False solves every chunk on its own, as before grouping existed.
+_group_chunks = True
+# Frames up to this many pixels are grouped.  Measured on an H100 (DESIGN §7m): a group of 64 sizes
+# around 256² (65 536 px) is faster than its chunks one after another; at 512² (4:4:4) and at 1080p
+# the group's flat grids are slower than the per-size launches, so those chunks keep their own.
+GROUP_MAX_PIXELS = 1 << 17
+
+
+def group_class(key, separate: bool, mode: str = 'RGB'):
+    """The class of a chunk of `key` for grouping, or None when it is solved on its own: chunks of one
+    class may share a group (the join rules of j2p_session_iterate_group: one session per chunk, equal
+    plane count and sampling factors, every plane 1x1 or 2x2), and only frames of at most
+    GROUP_MAX_PIXELS pixels are grouped.  Separate-mode colour chunks (a session per plane) are not."""
+    w, h, planes = key
+    nsolved, _ = solved_planes(key, separate, mode)
+    if separate and len(planes) > 1:
+        return None
+    solved = planes[:nsolved]
+    if any((ws, hs) not in ((1, 1), (2, 2)) for _, _, ws, hs in solved):
+        return None
+    W = max(pw * ws for pw, _, ws, _ in solved)
+    H = max(ph * hs for _, ph, _, hs in solved)
+    if W * H > GROUP_MAX_PIXELS:
+        return None
+    return (nsolved, tuple((ws, hs) for _, _, ws, hs in solved))
+
+
+def pack(chunks, class_of, bytes_of, cap_bytes):
+    """Packs of the chunks of plan(): lists of chunk indices, each list in order and the packs in
+    order of their first chunk.  A chunk whose class_of(key) is None is a pack of its own.  Chunks of
+    one class share a pack while it holds no other chunk of their key, at most MAX_BATCH frames and at
+    most cap_bytes of bytes_of(key, frames) (a chunk alone may exceed it, as it does today)."""
+    packs, open_ = [], {}
+    for j, (key, idx) in enumerate(chunks):
+        cls = class_of(key)
+        if cls is None:
+            packs.append([j])
+            continue
+        cur = open_.get(cls)
+        if cur is not None:
+            p, keys, frames, nbytes = cur
+            b = bytes_of(key, len(idx))
+            if key not in keys and frames + len(idx) <= MAX_BATCH and nbytes + b <= cap_bytes:
+                p.append(j)
+                open_[cls] = (p, keys | {key}, frames + len(idx), nbytes + b)
+                continue
+        p = [j]
+        packs.append(p)
+        open_[cls] = (p, {key}, len(idx), bytes_of(key, len(idx)))
+    return packs
+
+
 def _read_input(x):
     if isinstance(x, (bytes, bytearray, memoryview)):
         return bytes(x), None
@@ -489,7 +543,8 @@ class _Chunk:
     tensor either way."""
 
     def __init__(self, lib, device, items, flags, separate, dtype, layout, coefs=None, coef_stream=None, mode='RGB',
-                 orientations=None):
+                 orientations=None, grouped=False):
+        """grouped: create and upload only; the caller iterates the sessions in a group, then calls export()."""
         iters, weights, pweights = flags
         self.lib, self.sessions, self.coefs = lib, [], coefs or {}
         first, n = items[0], len(items)
@@ -514,7 +569,21 @@ class _Chunk:
                         else:
                             self._check(lib.j2p_session_upload(s, f * len(channels) + k, p.data.ctypes.data,
                                                                p.quant.ctypes.data, None))     # conventional decode on the device
-                self._check(lib.j2p_session_iterate(s, 0, it))
+                if not grouped:
+                    self._check(lib.j2p_session_iterate(s, 0, it))
+            self.iterations = work[0][2]
+            self._export_args = (device, items, dtype, layout, nout, separate, orientations)
+            if not grouped:
+                self.export()
+        except BaseException:
+            self.close()
+            raise
+
+    def export(self):
+        """The chunk's tensor, written on the current torch stream after the sessions' solve."""
+        device, items, dtype, layout, nout, separate, orientations = self._export_args
+        lib, first, n = self.lib, items[0], len(items)
+        try:
             w, h = first.w, first.h
             shape = (nout, h, w) if layout == abi.LAYOUT_CHW else (h, w, nout)
             cuda = torch.device('cuda', device)
@@ -630,8 +699,9 @@ def decode_jpeg(inputs, *, iterations=50, weight=0.3, pweight=0.001, separate=Fa
     a scalar weight sets luma only; three weights or three iteration counts need separate=True.
 
     Inputs with the same geometry are solved together, max_frames per batch (default: as many as
-    fit in a quarter of the free device memory).  The tensors of one batch are views of one
-    allocation and share its storage.  The result is written on the current torch stream and can
+    fit in a quarter of the free device memory).  Batches of different small geometries (up to
+    GROUP_MAX_PIXELS pixels per frame, joint or gray) are iterated together in one group.  The
+    tensors of one batch are views of one allocation and share its storage.  The result is written on the current torch stream and can
     be used there without synchronising.
 
     Sequential (baseline or extended) files whose components are each coded in one scan are
@@ -700,15 +770,24 @@ def decode_jpeg(inputs, *, iterations=50, weight=0.3, pweight=0.001, separate=Fa
     chunks = plan([p.key() for p in parsed],
                   lambda k: chunk_frames(k, separate, sample_bytes, max_frames, free, mode))
 
+    # packs of chunks iterated in one group; a pack of one chunk is solved as the chunk alone
+    if _group_chunks:
+        cap = (free if max_frames is None else torch.cuda.mem_get_info(index)[0]) // 4
+        packs = pack(chunks, lambda k: group_class(k, separate, mode),
+                     lambda k, n: n * frame_footprint(k, separate, sample_bytes, mode), cap)
+    else:
+        packs = [[j] for j in range(len(chunks))]
+
     results = [None] * len(parsed)
     layout_id = _LAYOUT[layout]
-    previous = None
+    previous = []
     try:
         with torch.cuda.device(index):
             # the entropy decoder's own stream: waiting for a chunk's decode does not wait for the
             # solve of the chunk before it
             coef_stream = torch.cuda.Stream(index)
-            for _, idx in chunks:
+
+            def chunk_coefs(idx):
                 coefs = {}
                 for kind, decoder in ((FileLayout, _DeviceCoefs), (ProgFileLayout, _ProgCoefs)):
                     on_dev = [j for j, i in enumerate(idx) if isinstance(parsed[i], kind)]
@@ -727,14 +806,34 @@ def decode_jpeg(inputs, *, iterations=50, weight=0.3, pweight=0.001, separate=Fa
                                                f'({ENT_FAILURES.get(int(dc.status[k]), int(dc.status[k]))}) on a file '
                                                'the host reader accepts (a decoder bug)')
                         coefs[j] = (dc, k)
-                chunk = _Chunk(lib, index, [parsed[i] for i in idx], flags, separate, dtype, layout_id, coefs, coef_stream, mode,
-                               None if orientations is None else [orientations[i] for i in idx])
-                for j, i in enumerate(idx):
-                    results[i] = chunk.frame(j)
-                if previous is not None:        # this chunk is queued: let the previous one finish
-                    previous.close()
-                previous = chunk
+                return coefs
+
+            for p in packs:
+                made = []
+                try:
+                    for j in p:
+                        idx = chunks[j][1]
+                        made.append(_Chunk(lib, index, [parsed[i] for i in idx], flags, separate, dtype, layout_id,
+                                           chunk_coefs(idx), coef_stream, mode,
+                                           None if orientations is None else [orientations[i] for i in idx],
+                                           grouped=len(p) > 1))
+                    if len(p) > 1:
+                        ss = [c.sessions[0] for c in made]
+                        if lib.j2p_session_iterate_group((C.c_void_p * len(ss))(*ss), len(ss), 0, made[0].iterations) != 0:
+                            raise RuntimeError(lib.j2p_last_error().decode())
+                        for c in made:
+                            c.export()
+                except BaseException:
+                    for c in made:
+                        c.close()
+                    raise
+                for j, c in zip(p, made):
+                    for k, i in enumerate(chunks[j][1]):
+                        results[i] = c.frame(k)
+                for c in previous:              # this pack is queued: let the previous one finish
+                    c.close()
+                previous = made
     finally:
-        if previous is not None:
-            previous.close()
+        for c in previous:
+            c.close()
     return results[0] if single else results
