@@ -3,10 +3,12 @@ into CUDA tensors (RGB, or one channel for grayscale files and `mode='GRAY'`), `
 (jpeg2png_b200.encode, RGB or gray) and `encode_jpeg` (jpeg2png_b200.jpeg_encode, RGB)
 turn such tensors into PNG or JPEG files on the device (`encode_jpeg(..., optimize=True)` with
 per-image optimized Huffman tables, as Pillow's `optimize=True`, and `encode_jpeg(...,
-progressive=True)` with Pillow's progressive files); torch is imported only when one of
-them is first used."""
+progressive=True)` with Pillow's progressive files, and `encode_jpeg(..., qtables=)` with given
+quantisation tables, per image if need be); `keep_settings` reads a JPEG file's tables and
+sampling, as Pillow's quality='keep' re-uses them; torch is imported only when one of them is
+first used."""
 
-__all__ = ['decode_jpeg', 'encode_png', 'encode_jpeg']
+__all__ = ['decode_jpeg', 'encode_png', 'encode_jpeg', 'keep_settings']
 
 
 def __getattr__(name):
@@ -19,4 +21,7 @@ def __getattr__(name):
     if name == 'encode_jpeg':
         from .jpeg_encode import encode_jpeg
         return encode_jpeg
+    if name == 'keep_settings':
+        from .jpeg_encode import keep_settings
+        return keep_settings
     raise AttributeError(f'module {__name__!r} has no attribute {name!r}')

@@ -22,7 +22,9 @@ class Codec:
     check_size(shape, h, w): raises ValueError for a size the encoder refuses;
     fill(d, x, channels): sets the struct's other fields from the array or tensor x and its channel
     count, if it has any;
-    channels: the channel counts the encoder accepts, in the order its messages name them."""
+    channels: the channel counts the encoder accepts, in the order its messages name them;
+    place(descs): sets fields of the call's structs that depend on each image's place in the call
+    (the JPEG encoder's set of quantisation tables), if it has any."""
     name: str
     load: Callable[[], C.CDLL]
     image: type
@@ -30,6 +32,7 @@ class Codec:
     fill: Callable | None = None
     params: tuple = ()
     channels: tuple = (3,)
+    place: Callable | None = None
 
     def call(self, fn, descs, *args, error=RuntimeError):
         """j2p_<name>_<fn>(descs, len(descs), *params, *args); `error` with the library's message
@@ -82,9 +85,16 @@ def descs(codec, items, layout, ptr=lambda x: x.data_ptr(), strides=lambda x: x.
     return out
 
 
+def placed(codec, d):
+    """d after the codec's place(d), when it has one."""
+    if codec.place:
+        codec.place(d)
+    return d
+
+
 def encode_host(codec, images, layout):
     """The serial host driver on numpy arrays: a list of files as bytes."""
-    d = descs(codec, images, layout, lambda x: x.ctypes.data, lambda x: [s // x.itemsize for s in x.strides])
+    d = placed(codec, descs(codec, images, layout, lambda x: x.ctypes.data, lambda x: [s // x.itemsize for s in x.strides]))
     work_bytes, base = codec.plan(d)
     work = np.zeros(work_bytes, np.uint8)
     offs = (C.c_uint64 * (len(images) + 1))()
@@ -144,11 +154,13 @@ def by_codec(codecs, items, layout):
     return list(groups.values())
 
 
-def encode_tensors(fn, codec, images, layout, dtypes):
+def encode_tensors(fn, codec, images, layout, dtypes, calls=None):
     """The body of the public encoder `fn` once its own arguments are checked: images is one CUDA
     tensor or a list or tuple of them, of one of `dtypes`.  codec: a Codec, or {channel count:
     Codec} for an encoder whose library call takes one kind of image (the images of each kind go
-    to their own calls).  Returns bytes or a list of bytes, in input order."""
+    to their own calls).  calls(items), when given, replaces that split: [(Codec, indices of its
+    images, in input order)], once codec's checks have accepted the images.  Returns bytes or a
+    list of bytes, in input order."""
     codecs = codec if isinstance(codec, dict) else {c: codec for c in codec.channels}
     channels = tuple(codecs)
     single = not isinstance(images, (list, tuple))
@@ -170,7 +182,7 @@ def encode_tensors(fn, codec, images, layout, dtypes):
     if any(x.device != device for x in items):
         raise ValueError('all images of one call must be on the same device')
     results = [None] * len(items)
-    for c, idx in by_codec(codecs, items, layout):
-        for i, r in zip(idx, encode_device(c, descs(c, [items[i] for i in idx], layout), device)):
+    for c, idx in (calls or (lambda x: by_codec(codecs, x, layout)))(items):
+        for i, r in zip(idx, encode_device(c, placed(c, descs(c, [items[i] for i in idx], layout)), device)):
             results[i] = r
     return results[0] if single else results

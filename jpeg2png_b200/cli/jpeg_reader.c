@@ -50,6 +50,7 @@ struct dec {
         struct j2p_jpeg_layout *lay;   /* the layout pass (j2p_read_jpeg_layout), NULL for a full read */
         unsigned scans_of[3];          /* layout pass: scans that name each component */
         struct j2p_jpeg_prog_layout *play;   /* the progressive layout pass (j2p_read_jpeg_prog_layout) */
+        int headers_only;              /* j2p_jpeg_keep_settings: stop at the first SOS */
         size_t data_cap, seg_cap, scan_cap;
 };
 
@@ -401,7 +402,7 @@ static int parse_sof(struct dec *d, const uint8_t *s, unsigned len) {
                 c->hb = (ch + 7) / 8;
                 c->pwb = d->mcux * c->h;
                 c->phb = d->mcuy * c->v;
-                if (d->lay || d->play) continue;                                                        /* the layout passes store no blocks */
+                if (d->lay || d->play || d->headers_only) continue;                                     /* the layout passes store no blocks */
                 c->blk = calloc((size_t)c->pwb * c->phb * 64, sizeof(int16_t));
                 if (!c->blk) return fail(d, "could not allocate memory for coefs");                /* jpeg.c:69 */
         }
@@ -443,6 +444,7 @@ static int read_markers(struct dec *d, const uint8_t *buf, size_t len) {
                         if (sl < 2) fail(d, "corrupt jpeg: short DRI"); else d->restart_interval = be16(s);
                 } else if (m == 0xDA) {
                         if (!have_sof) { fail(d, "corrupt jpeg: scan before frame header"); break; }
+                        if (d->headers_only) break;
                         if (sl < 1) { fail(d, "corrupt jpeg: short SOS"); break; }
                         const int ns = s[0];
                         if (ns < 1 || ns > 3 || sl < 1 + 2u * ns + 3) { fail(d, "corrupt jpeg: bad SOS"); break; }
@@ -679,4 +681,29 @@ int j2p_jpeg_exif_orientation(const void *data, size_t len) {
                 p += seglen;
                 if (m == 0xE1 && sl >= 6 && memcmp(s, "Exif\0\0", 6) == 0) return tiff_orientation(s + 6, sl - 6);
         }
+}
+
+/* ---- the settings of Pillow's quality='keep' ---- */
+int j2p_jpeg_keep_settings(const void *data, size_t len, struct j2p_jpeg_keep *out, char *err, size_t errlen) {
+        struct dec *d = calloc(1, sizeof *d);
+        if (!d) return -1;
+        d->p = data; d->end = d->p + len; d->err = err; d->errlen = errlen; d->flags = J2P_READ_GRAY; d->headers_only = 1;
+        if (err && errlen) err[0] = 0;
+        memset(out, 0, sizeof *out);
+        read_markers(d, data, len);
+        struct coef coefs[3];
+        memset(coefs, 0, sizeof coefs);
+        if (!d->failed) check_planes(d, coefs);
+        if (!d->failed) {
+                for (int t = 0; t < 4; t++) {
+                        if (!d->qt_present[t]) continue;
+                        out->present |= 1u << t;
+                        memcpy(out->qt[t], d->qt[t], sizeof out->qt[t]);
+                }
+                out->ncomp = (unsigned)d->ncomp;
+                for (int i = 0; i < d->ncomp; i++) { out->comp_h[i] = (unsigned)d->c[i].h; out->comp_v[i] = (unsigned)d->c[i].v; }
+        }
+        const int rc = d->failed ? -1 : 0;
+        free(d);
+        return rc;
 }

@@ -130,4 +130,19 @@ void j2p_free_jpeg_prog_layout(struct j2p_jpeg_prog_layout *l);
  * Reads nothing outside [data, data + len) and does not look at any other header. */
 int j2p_jpeg_exif_orientation(const void *data, size_t len);
 
+/* ---- the settings of Pillow's quality='keep' ----
+ * The quantisation tables a file defines before its first SOS (natural order, bit t of present set
+ * for table t: Pillow's Image.quantization) and its frame's components and sampling factors (what
+ * Pillow's get_sampling reads).  The headers up to the first SOS go through the reader's own marker
+ * loop and segment parsers, and the frame through its table and geometry checks, with
+ * J2P_READ_GRAY: a file the reader refuses in its headers is refused with the reader's message, and
+ * nothing after the first SOS is read.  Returns 0, or -1 with the message in err. */
+struct j2p_jpeg_keep {
+        uint16_t qt[4][64];
+        unsigned present;
+        unsigned ncomp;             /* 1 or 3 */
+        unsigned comp_h[3], comp_v[3];
+};
+int j2p_jpeg_keep_settings(const void *data, size_t len, struct j2p_jpeg_keep *out, char *err, size_t errlen);
+
 #endif

@@ -99,6 +99,12 @@ ENTROPY_LIB = os.path.join(abi._PKG_DIR, 'entropy', 'libj2pentropy.so')
 SUBSEQ_BITS = 1024                  # bits per subsequence of the device decoder (DESIGN §7d)
 ENT_FAILURES = {1: 'bad huffman code', 2: 'bad magnitude category', 3: 'coefficient index out of range'}
 
+class Keep(C.Structure):
+    """struct j2p_jpeg_keep — jpeg2png_b200/cli/jpeg_reader.h."""
+    _fields_ = [('qt', (C.c_uint16 * 64) * 4), ('present', C.c_uint), ('ncomp', C.c_uint), ('comp_h', C.c_uint * 3),
+                ('comp_v', C.c_uint * 3)]
+
+
 def _declare_codecs(lib):
     lib.j2p_read_jpeg_mem.restype = C.c_int
     lib.j2p_read_jpeg_mem.argtypes = [C.c_char_p, C.c_size_t, C.POINTER(Jpeg), C.c_char_p, C.c_size_t]
@@ -118,6 +124,8 @@ def _declare_codecs(lib):
     lib.j2p_free_jpeg_prog_layout.argtypes = [C.POINTER(ProgLayout)]
     lib.j2p_jpeg_exif_orientation.restype = C.c_int
     lib.j2p_jpeg_exif_orientation.argtypes = [C.c_char_p, C.c_size_t]
+    lib.j2p_jpeg_keep_settings.restype = C.c_int
+    lib.j2p_jpeg_keep_settings.argtypes = [C.c_char_p, C.c_size_t, C.POINTER(Keep), C.c_char_p, C.c_size_t]
 
 
 def load_codecs() -> C.CDLL:

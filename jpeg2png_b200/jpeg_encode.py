@@ -11,6 +11,9 @@ libjpeg's ten-scan progression, each scan with tables built from its own symbol 
 `restart_marker_blocks` and `restart_marker_rows` add restart intervals to any of the three files,
 as Pillow's keywords of the same names do (DESIGN §7i).  One-channel tensors are written as
 Pillow's one-component ('L') files by the same three libraries, one call per kind (DESIGN §7k).
+`qtables` writes given quantisation tables, per image if need be, as Pillow's keyword of the same
+name does, and `keep_settings` reads a file's tables and sampling as Pillow's quality='keep' does
+(DESIGN §7n).
 Colour conversion, downsampling, DCT,
 quantisation, the tables, Huffman coding and byte stuffing all run on the device; only the finished
 files cross PCIe.
@@ -41,13 +44,18 @@ MAX_SIDE = 65535                    # SOF's 16-bit height and width
 class Image(C.Structure):
     """struct j2p_jpegenc_image — jpeg2png_b200/jpegenc/jpegenc.h."""
     _fields_ = [('data', C.c_void_p), ('width', C.c_uint32), ('height', C.c_uint32),
-                ('row_stride', C.c_int64), ('col_stride', C.c_int64), ('chan_stride', C.c_int64)]
+                ('row_stride', C.c_int64), ('col_stride', C.c_int64), ('chan_stride', C.c_int64), ('qtables', C.c_uint32)]
+
+
+class Qtables(C.Structure):
+    """struct j2p_jpegenc_qtables — jpeg2png_b200/jpegenc/jpegenc.h."""
+    _fields_ = [('table', (C.c_uint16 * 64) * 4), ('ntables', C.c_uint32)]
 
 
 class Params(C.Structure):
     """struct j2p_jpegenc_params — jpeg2png_b200/jpegenc/jpegenc.h."""
     _fields_ = [('quality', C.c_int), ('sampling', C.c_int), ('restart_marker_blocks', C.c_int), ('restart_marker_rows', C.c_int),
-                ('components', C.c_int)]
+                ('components', C.c_int), ('qtables', C.POINTER(Qtables)), ('nqtables', C.c_uint)]
 
 
 class Stats(C.Structure):
@@ -107,14 +115,24 @@ def _check_restart(name, v):
     return int(v)
 
 
+def check_quality(quality, allow_none=False):
+    if quality is None and allow_none:
+        return
+    if isinstance(quality, bool) or not isinstance(quality, (int, np.integer)) or not 1 <= quality <= 100:
+        raise ValueError(f'quality must be an integer in 1..100{" or None" if allow_none else ""}, not {quality!r}')
+
+
+def check_subsampling(subsampling):
+    if not isinstance(subsampling, str) or subsampling not in SAMPLINGS:
+        raise ValueError(f"subsampling must be '4:4:4', '4:2:2' or '4:2:0', not {subsampling!r}")
+
+
 def params(quality, subsampling, restart_marker_blocks=0, restart_marker_rows=0, components=3) -> Params:
     """Checked call parameters: quality an integer in 1..100, subsampling '4:4:4', '4:2:2' or '4:2:0',
     the restart keywords integers in 0..65535, components 3 (RGB images, YCbCr files) or 1 (gray
     images, one-component files)."""
-    if isinstance(quality, bool) or not isinstance(quality, (int, np.integer)) or not 1 <= quality <= 100:
-        raise ValueError(f'quality must be an integer in 1..100, not {quality!r}')
-    if subsampling not in SAMPLINGS:
-        raise ValueError(f"subsampling must be '4:4:4', '4:2:2' or '4:2:0', not {subsampling!r}")
+    check_quality(quality)
+    check_subsampling(subsampling)
     blocks = _check_restart('restart_marker_blocks', restart_marker_blocks)
     rows = _check_restart('restart_marker_rows', restart_marker_rows)
     if components not in (1, 3) or isinstance(components, bool):
@@ -132,12 +150,132 @@ CODEC_OPT = B.Codec('jpegopt', lambda: load_jpegopt(), Image, _check_size)
 CODEC_PROG = B.Codec('jpegprog', lambda: load_jpegprog(), Image, _check_size)
 
 
-def codec(p: Params, optimize=False, progressive=False) -> B.Codec:
+def codec(p: Params, optimize=False, progressive=False, sets=None) -> B.Codec:
     """libj2pjpegenc.so, or libj2pjpegopt.so when optimize, or libj2pjpegprog.so when progressive
     (whatever optimize), for the shared driver, with the call parameters p: it takes one-channel
-    images when p is gray (p.components == 1), three-channel ones otherwise."""
+    images when p is gray (p.components == 1), three-channel ones otherwise.  sets: None (the IJG
+    tables of p.quality), or each image's final tables in call order (lists of 64 integers in
+    natural order, or None for the IJG tables of p.quality); the distinct ones become the call's
+    sets, each stored once."""
     c = CODEC_PROG if progressive else CODEC_OPT if optimize else CODEC
-    return dataclasses.replace(c, params=(C.byref(p),), channels=(1,) if p.components == 1 else c.channels)
+    place = None
+    if sets is not None and any(t is not None for t in sets):
+        own = [tuple(map(tuple, t if t is not None else scaled_tables(IJG_TABLES, p.quality))) for t in sets]
+        distinct = list(dict.fromkeys(own))
+        arr = (Qtables * len(distinct))()
+        for q, t in zip(arr, distinct):
+            q.ntables = len(t)
+            for k, row in enumerate(t):
+                q.table[k][:] = row
+        p.qtables, p.nqtables = arr, len(distinct)
+        p.sets_ = arr                   # p, which the codec holds by reference, keeps them alive
+        index = [distinct.index(t) for t in own]
+
+        def place(d):
+            for x, k in zip(d, index):
+                x.qtables = k
+    return dataclasses.replace(c, params=(C.byref(p),), channels=(1,) if p.components == 1 else c.channels, place=place)
+
+
+# ---- quantisation tables ---------------------------------------------------------------------------
+# ITU-T T.81 Annex K.1 (natural order): libjpeg's tables before quality scaling
+IJG_TABLES = (
+    (16, 11, 10, 16, 24, 40, 51, 61, 12, 12, 14, 19, 26, 58, 60, 55, 14, 13, 16, 24, 40, 57, 69, 56, 14, 17, 22, 29, 51, 87, 80, 62,
+     18, 22, 37, 56, 68, 109, 103, 77, 24, 35, 55, 64, 81, 104, 113, 92, 49, 64, 78, 87, 103, 121, 120, 101, 72, 92, 95, 98, 112, 100,
+     103, 99),
+    (17, 18, 24, 47, 99, 99, 99, 99, 18, 21, 26, 66, 99, 99, 99, 99, 24, 26, 56, 99, 99, 99, 99, 99, 47, 66) + (99,) * 38)
+MAX_ENTRY = 8191                    # 8q must fit libjpeg-turbo's 16-bit divisor
+
+
+def scaled_tables(tables, quality):
+    """Final tables as Pillow makes them from given ones: without quality (None) each entry as
+    given, 0 raised to 1 and anything above 32767 lowered to it; with quality q each entry scaled as
+    jpeg_quality_scaling(q) scales the IJG tables, (t s + 50) / 100 with s = 5000 / q below 50 and
+    200 - 2q otherwise, then clamped to 1..255.  Raises ValueError for a final entry above 8191:
+    libjpeg-turbo divides by 8q in 16 bits, so Pillow writes such a file with coefficients that do
+    not match the table it declares."""
+    if quality is None:
+        out = [[min(max(v, 1), 32767) for v in t] for t in tables]
+    else:
+        s = 5000 // quality if quality < 50 else 200 - 2 * quality
+        out = [[min(max((v * s + 50) // 100, 1), 255) for v in t] for t in tables]
+    for k, t in enumerate(out):
+        if max(t) > MAX_ENTRY:
+            raise ValueError(f'quantisation table {k} has an entry of {max(t)} (quality {quality}); entries above {MAX_ENTRY} are refused: '
+                             f'libjpeg divides by 8q in 16 bits, so the file would not match its own tables')
+    return out
+
+
+def parse_qtables(value):
+    """Pillow's validate_qtables on a list, tuple or dict of 1..4 tables of 64 integers in 0..65535
+    (natural order): a list of lists of ints.  A dict keeps [d[k] for k in range(len(d)) if k in d].
+    Strings (Pillow's text tables and preset names) are refused."""
+    if isinstance(value, str):
+        raise ValueError('qtables as text or as a preset name is not supported; give a list, tuple or dict of tables')
+    if isinstance(value, dict):
+        value = [value[k] for k in range(len(value)) if k in value]
+    elif not isinstance(value, (list, tuple, np.ndarray)):
+        raise ValueError(f'qtables must be a list, tuple or dict of tables, not {type(value).__name__}')
+    if not 1 <= len(value) <= 4:
+        raise ValueError(f'qtables holds 1..4 tables, not {len(value)}')
+    out = []
+    for t in value:
+        if isinstance(t, (str, bytes, dict)) or not hasattr(t, '__len__') or len(t) != 64:
+            raise ValueError('a quantisation table is a sequence of 64 integers')
+        for v in t:
+            if isinstance(v, (bool, np.bool_)) or not isinstance(v, (int, np.integer)) or not 0 <= v <= 65535:
+                raise ValueError(f'quantisation table entries are integers in 0..65535, not {v!r}')
+        out.append([int(v) for v in t])
+    return out
+
+
+def _flat(e):
+    """Whether e is one table (a flat sequence), rather than an element of a per-image list."""
+    return isinstance(e, (list, tuple, np.ndarray)) and not any(v is None or isinstance(v, (list, tuple, dict, np.ndarray)) for v in e)
+
+
+def per_image(qtables, quality, n):
+    """Each of n images' final tables, or None for the IJG tables of quality: qtables is None, one
+    tables value for every image, or a list or tuple of n elements, each None or a tables value."""
+    if qtables is None:
+        return [None] * n
+    if isinstance(qtables, (list, tuple)) and qtables and not all(_flat(e) for e in qtables):
+        if len(qtables) != n:
+            raise ValueError(f'a per-image qtables list has {len(qtables)} elements for {n} images')
+        return [None if e is None else scaled_tables(parse_qtables(e), quality) for e in qtables]
+    return [scaled_tables(parse_qtables(qtables), quality)] * n
+
+
+def _subsamplings(subsampling, n):
+    """Each of n images' subsampling: one value, or a list or tuple of n."""
+    if isinstance(subsampling, (list, tuple)):
+        if len(subsampling) != n:
+            raise ValueError(f'a per-image subsampling list has {len(subsampling)} elements for {n} images')
+        subs = list(subsampling)
+    else:
+        subs = [subsampling] * n
+    for s in subs:
+        check_subsampling(s)
+    return subs
+
+
+def _calls(quality, subsampling, optimize, progressive, restart_marker_blocks, restart_marker_rows, qtables, n, channels):
+    """calls(items) for the shared driver: one library call per (channel count, subsampling) kind of
+    the n images, each with the distinct tables of its images as its sets; channels(x): x's channel
+    count."""
+    check_quality(quality, allow_none=True)
+    subs = _subsamplings(subsampling, n)
+    sets = per_image(qtables, quality, n)
+    blocks = _check_restart('restart_marker_blocks', restart_marker_blocks)
+    rows = _check_restart('restart_marker_rows', restart_marker_rows)
+    q = 75 if quality is None else int(quality)     # the IJG tables' quality, where an image has no tables
+
+    def calls(items):
+        kinds = {}
+        for i, x in enumerate(items):
+            kinds.setdefault((channels(x), subs[i]), []).append(i)
+        return [(codec(params(q, s, blocks, rows, c), optimize, progressive, [sets[i] for i in idx]), idx) for (c, s), idx in kinds.items()]
+    return calls
 
 
 def _codecs(quality, subsampling, optimize, progressive, restart_marker_blocks, restart_marker_rows):
@@ -176,35 +314,55 @@ def _work_bytes(descs, p):
     return codec(p).plan(descs)[0]
 
 
-def encode_host(images, quality=75, subsampling='4:2:0', layout='HWC', optimize=False, progressive=False, restart_marker_blocks=0,
-                restart_marker_rows=0, gray=False):
+def encode_host(images, quality=None, subsampling='4:2:0', layout='HWC', optimize=False, progressive=False, restart_marker_blocks=0,
+                restart_marker_rows=0, gray=False, qtables=None):
     """The serial host driver (j2p_jpegenc_encode_host, or j2p_jpegopt_encode_host when optimize,
     or j2p_jpegprog_encode_host when progressive) on numpy uint8 arrays: a list of JPEG files as
     bytes, the same bytes the device writes.  The arrays are RGB, or with gray=True all gray,
-    (h, w, 1) or (1, h, w), written as one-component files."""
+    (h, w, 1) or (1, h, w), written as one-component files.  quality, subsampling and qtables as
+    encode_jpeg takes them (per-image lists included: one call per subsampling)."""
     B.check_layout(layout)
     if not isinstance(gray, bool):
         raise ValueError(f'gray must be True or False, not {gray!r}')
-    p = params(quality, subsampling, restart_marker_blocks, restart_marker_rows, 1 if gray else 3)
     check_optimize(optimize)
     check_progressive(progressive)
     for x in images:
         if x.dtype != np.uint8:
             raise ValueError(f'samples are uint8, not {x.dtype}')
-    return B.encode_host(codec(p, optimize, progressive), images, layout)
+    calls = _calls(quality, subsampling, optimize, progressive, restart_marker_blocks, restart_marker_rows, qtables, len(images),
+                   lambda x: 1 if gray else 3)
+    out = [None] * len(images)
+    for c, idx in calls(images):
+        for i, f in zip(idx, B.encode_host(c, [images[i] for i in idx], layout)):
+            out[i] = f
+    return out
 
 
-def encode_jpeg(images, *, quality=75, subsampling='4:2:0', layout='CHW', optimize=False, progressive=False, restart_marker_blocks=0,
-                restart_marker_rows=0):
+def encode_jpeg(images, *, quality=None, subsampling='4:2:0', layout='CHW', optimize=False, progressive=False, restart_marker_blocks=0,
+                restart_marker_rows=0, qtables=None):
     """Encode RGB or gray CUDA tensors as baseline or progressive JPEG files on the device.
 
     images: one tensor or a list or tuple of them, torch.uint8, shaped (3, h, w) for layout='CHW'
     or (h, w, 3) for 'HWC', with any strides, 1..65535 pixels high and wide.  quality: an integer
-    in 1..100; subsampling: '4:4:4', '4:2:2' or '4:2:0'.  Returns the JPEG file as bytes, or a list
-    of bytes in input order: byte for byte the file Pillow writes for the same pixels with
-    `save(f, 'JPEG', quality=quality, subsampling=subsampling, optimize=optimize,
-    progressive=progressive, restart_marker_blocks=restart_marker_blocks,
-    restart_marker_rows=restart_marker_rows)`.
+    in 1..100, or None (75 without qtables); subsampling: '4:4:4', '4:2:2' or '4:2:0', or a list or
+    tuple of them, one per image.  Returns the JPEG file as bytes, or a list of bytes in input
+    order: byte for byte the file Pillow writes for the same pixels with `save(f, 'JPEG',
+    quality=quality, subsampling=subsampling, optimize=optimize, progressive=progressive,
+    restart_marker_blocks=restart_marker_blocks, restart_marker_rows=restart_marker_rows,
+    qtables=qtables)` (quality=None being Pillow's default, -1).
+
+    qtables: None (the IJG tables of quality), Pillow's form (a list, tuple or dict of 1..4 tables
+    of 64 integers in 0..65535, natural order) for every image, or a list or tuple with one element
+    per image, each None (the IJG tables of quality) or such a value, so that files from different
+    sources keep their own tables in one call.  As in Pillow, one table serves Y, Cb and Cr, two
+    serve Y and then Cb and Cr, and a third serves Cr (a fourth is not used); a gray image uses the
+    first.  Without quality the entries are used as given (0 becomes 1); with quality q they are
+    scaled as the IJG tables are and clamped to 1..255.  An entry that ends above 8191 is refused
+    with ValueError (Pillow writes a corrupt file: libjpeg divides by 8q in 16 bits), as are
+    strings (text tables and preset names).  A table with an entry above 255 is written as a 16-bit
+    DQT and makes the file SOF1 (extended sequential) unless it is progressive.
+    `encode_jpeg(decode_jpeg(files, mode='UNCHANGED'), **keep_settings(files))` re-encodes files
+    with their own tables and sampling, as Pillow's quality='keep' does.
 
     A tensor with one channel, (1, h, w) or (h, w, 1) (what decode_jpeg(mode='UNCHANGED' or
     'GRAY') returns), is written as a one-component file: Pillow's file of the 'L' image, with every
@@ -242,7 +400,38 @@ def encode_jpeg(images, *, quality=75, subsampling='4:2:0', layout='CHW', optimi
     a CUDA device, and RuntimeError when no CUDA device is usable.
     """
     B.check_layout(layout)
-    codecs = _codecs(quality, subsampling, optimize, progressive, restart_marker_blocks, restart_marker_rows)
     check_optimize(optimize)
     check_progressive(progressive)
-    return B.encode_tensors('encode_jpeg', codecs, images, layout, (torch.uint8,))
+    n = len(images) if isinstance(images, (list, tuple)) else 1
+    calls = _calls(quality, subsampling, optimize, progressive, restart_marker_blocks, restart_marker_rows, qtables, n,
+                   lambda x: x.shape[B.axes(x.shape, layout, (3, 1))[4]])
+    codecs = _codecs(75, '4:2:0', optimize, progressive, restart_marker_blocks, restart_marker_rows)      # the checks of the images
+    return B.encode_tensors('encode_jpeg', codecs, images, layout, (torch.uint8,), calls)
+
+
+def keep_settings(inputs):
+    """The settings Pillow's quality='keep' re-uses for JPEG files: inputs is bytes-like, a path
+    (str / os.PathLike), or a list or tuple of them, as decode_jpeg takes them.  For one input,
+    {'qtables': {table id: [64 ints, natural order]}, 'subsampling': s}: the quantisation tables
+    the file defines before its first scan (Pillow's Image.quantization) and its sampling as
+    Pillow's get_sampling reads it, '4:4:4', '4:2:2' or '4:2:0' for those colour layouts and, for
+    any other (a gray file, 4:4:0, ...), libjpeg's default that Pillow then writes: '4:2:0' for
+    colour, 1 x 1 ('4:4:4' here) for gray.  For a list, the same keys holding lists, which
+    encode_jpeg takes per image.  The headers are read by the project's JPEG reader
+    (j2p_jpeg_keep_settings): a file it refuses raises ValueError with its message."""
+    from . import decode as D
+    single = not isinstance(inputs, (list, tuple))
+    out = {'qtables': [], 'subsampling': []}
+    lib = D.load_codecs()
+    for i, x in enumerate([inputs] if single else inputs):
+        data, path = D._read_input(x)
+        k = D.Keep()
+        err = C.create_string_buffer(256)
+        if lib.j2p_jpeg_keep_settings(data, len(data), C.byref(k), err, 256) != 0:
+            raise ValueError(f'{D._where(i, path)}: {err.value.decode(errors="replace")}')
+        out['qtables'].append({t: list(k.qt[t]) for t in range(4) if k.present >> t & 1})
+        hv = tuple(v for c in range(k.ncomp) for v in (k.comp_h[c], k.comp_v[c]))
+        out['subsampling'].append({(1, 1, 1, 1, 1, 1): '4:4:4', (2, 1, 1, 1, 1, 1): '4:2:2', (2, 2, 1, 1, 1, 1): '4:2:0'}.get(
+            hv, '4:2:0' if k.ncomp == 3 else '4:4:4'))
+    return {key: v[0] for key, v in out.items()} if single else out
+

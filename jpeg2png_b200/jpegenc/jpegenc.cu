@@ -56,25 +56,28 @@ __global__ void __launch_bounds__(kChunkThreads) k_je_ffcount(const struct j2p_j
     ffcount_body(strs, ns, raw, ffc);
 }
 
-// the scan header's length: the template (head, the call's kind), with DRI when the image has
+// the scan header's length: its image's template (t: the call's sets), with DRI when the image has
 // restart intervals
-__device__ __forceinline__ uint32_t fixed_head_len(const StreamMap<1> &sm, uint32_t head, uint32_t s) {
-    return sm.plain ? head : head + (sm.strs[s].ri ? J2P_JE_DRI : 0);
+__device__ __forceinline__ uint32_t fixed_head_len(const StreamMap<1> &sm, const struct j2p_je_tables *t, uint32_t s) {
+    const struct j2p_je_img *st = &sm.strs[s];
+    return t[st->set].head_len + (!sm.plain && st->ri ? J2P_JE_DRI : 0);
 }
 
 __global__ void __launch_bounds__(kScanThreads) k_je_offsets(struct j2p_je_img *__restrict__ strs, uint32_t ns, bool plain, uint32_t n,
                                                             const uint32_t *__restrict__ ffc, uint32_t nchunks, uint64_t *__restrict__ ffpre,
-                                                            uint64_t *__restrict__ offsets, uint32_t head) {
+                                                            uint64_t *__restrict__ offsets, const struct j2p_je_tables *__restrict__ t) {
     const StreamMap<1> sm = {strs, ns, plain};
-    offsets_body(strs, sm, n, ffc, nchunks, ffpre, offsets, [&](uint32_t s) { return fixed_head_len(sm, head, s); });
+    offsets_body(strs, sm, n, ffc, nchunks, ffpre, offsets, [&](uint32_t s) { return fixed_head_len(sm, t, s); });
 }
 
 __global__ void __launch_bounds__(kChunkThreads) k_je_stuff(const struct j2p_je_img *__restrict__ strs, uint32_t ns, bool plain, const struct j2p_je_tables *__restrict__ t,
                                                            const uint32_t *__restrict__ raw, const uint64_t *__restrict__ ffpre,
-                                                           uint8_t *__restrict__ out, uint32_t head) {
+                                                           uint8_t *__restrict__ out) {
     const StreamMap<1> sm = {strs, ns, plain};
-    stuff_body(sm, raw, ffpre, out, [&](uint32_t s) { return fixed_head_len(sm, head, s); },
-               [&](uint32_t s, uint32_t k) { return sm.plain ? j2p_je_head_byte(t, &sm.strs[s], k) : j2p_je_scan_head_byte(t, &sm.strs[s], k); });
+    stuff_body(sm, raw, ffpre, out, [&](uint32_t s) { return fixed_head_len(sm, t, s); }, [&](uint32_t s, uint32_t k) {
+        const struct j2p_je_img *st = &sm.strs[s];
+        return sm.plain ? j2p_je_head_byte(t + st->set, st, k) : j2p_je_scan_head_byte(t + st->set, st, k);
+    });
 }
 
 extern "C" int j2p_jpegenc_encode(const struct j2p_jpegenc_image *images, unsigned n, const struct j2p_jpegenc_params *params, void *work,
@@ -102,9 +105,9 @@ extern "C" int j2p_jpegenc_encode(const struct j2p_jpegenc_image *images, unsign
         counted();
         k_je_ffcount<<<L.nchunks, kChunkThreads, 0, st>>>(strs, L.ns, raw, ffc);
         counted();
-        k_je_offsets<<<1, kScanThreads, 0, st>>>(strs, L.ns, L.plain, n, ffc, L.nchunks, ffpre, offs, head_len_of(params));
+        k_je_offsets<<<1, kScanThreads, 0, st>>>(strs, L.ns, L.plain, n, ffc, L.nchunks, ffpre, offs, t);
         counted();
-        k_je_stuff<<<L.nchunks, kChunkThreads, 0, st>>>(strs, L.ns, L.plain, t, raw, ffpre, w + L.off_out, head_len_of(params));
+        k_je_stuff<<<L.nchunks, kChunkThreads, 0, st>>>(strs, L.ns, L.plain, t, raw, ffpre, w + L.off_out);
         counted();
         return 0;
     };

@@ -44,6 +44,21 @@
  * column repeated past the image.  With restart_marker_rows = r an interval is min(r x ceil(w/8),
  * 65535) blocks.  A block costs at most the luma bound, 1658 bits.  The kind belongs to the call,
  * so a list of gray and colour images is two calls.  Any other components value is refused.
+ *
+ * Given quantisation tables (params->qtables; Pillow's qtables keyword): the call takes nqtables
+ * sets of 1 .. 4 tables of final values (natural order, 1 .. 8191: any parsing and quality scaling
+ * is the caller's), and image i is quantised with set images[i].qtables, so files from different
+ * sources keep their own tables in one call.  The components use the tables as Pillow maps them:
+ * one table: Y, Cb and Cr all table 0; two: Y 0, Cb and Cr 1; three or four: Y 0, Cb 1, Cr 2 (a
+ * fourth is neither written nor used); a gray image table 0.  The Huffman tables do not change (Cb
+ * and Cr share DC1 / AC1 even with three quantisation tables).  The header carries one DQT per used
+ * table in the order the components first use it, 16-bit (Pq = 1, 131 bytes) when one of its
+ * entries exceeds 255, else 8-bit (67 bytes), and the frame is SOF1 rather than SOF0 when any DQT is
+ * 16-bit (a progressive file stays SOF2).  Entries above 8191 are refused: libjpeg divides by 8q in
+ * 16 bits, so they wrap and its coefficients no longer match the table its file declares.  NULL
+ * qtables is the IJG tables of params->quality, one set that every image uses (the images' qtables
+ * fields are not read); a zero-initialised params keeps that meaning.  The header's length is per
+ * set, 623 bytes for the quality tables of a colour file, at most 884 with three 16-bit tables.
  */
 #ifndef J2P_JPEGENC_H
 #define J2P_JPEGENC_H
@@ -63,6 +78,13 @@ struct j2p_jpegenc_image {
         const void *data;               /* first sample (R of the top-left pixel, or its gray value), uint8 */
         uint32_t width, height;         /* 1 .. 65535 */
         int64_t row_stride, col_stride, chan_stride;      /* in samples */
+        uint32_t qtables;               /* the image's set of params->qtables; not read when that is NULL */
+};
+
+/* One set of quantisation tables: final values, natural (row-major) order. */
+struct j2p_jpegenc_qtables {
+        uint16_t table[4][64];          /* 1 .. 8191 */
+        uint32_t ntables;               /* 1 .. 4 */
 };
 
 struct j2p_jpegenc_params {
@@ -72,6 +94,8 @@ struct j2p_jpegenc_params {
         int restart_marker_rows;        /* 0 .. 65535: one of this many MCU rows per scan (capped at 65535
                                            MCUs); overrides restart_marker_blocks; 0 none */
         int components;                 /* 0 or 3: RGB images, YCbCr files; 1: gray images, one-component files */
+        const struct j2p_jpegenc_qtables *qtables;        /* nqtables sets, or NULL: the IJG tables of quality */
+        unsigned nqtables;
 };
 
 struct j2p_jpegenc_stats {
@@ -81,8 +105,9 @@ struct j2p_jpegenc_stats {
 
 /* Work area for the n images: work_bytes in all, the files at out_offset in it.  Refuses null
  * pointers, n == 0, a width or height of 0 or above 65535 (SOF's 16-bit fields), a quality outside
- * 1 .. 100, an unknown sampling, a restart field outside 0 .. 65535 and components other than 0, 1
- * or 3.  Returns 0, or -1 (j2p_jpegenc_last_error). */
+ * 1 .. 100, an unknown sampling, a restart field outside 0 .. 65535, components other than 0, 1
+ * or 3, and given tables with nqtables == 0, a set with ntables outside 1 .. 4 or an entry of 0 or
+ * above 8191, or an image whose set is not below nqtables.  Returns 0, or -1 (j2p_jpegenc_last_error). */
 int j2p_jpegenc_plan(const struct j2p_jpegenc_image *images, unsigned n, const struct j2p_jpegenc_params *params, size_t *work_bytes,
                      size_t *out_offset);
 

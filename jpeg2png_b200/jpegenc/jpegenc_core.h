@@ -38,10 +38,12 @@ static_assert(J2P_JE_WORDS_PER_BLOCK * 32 >= J2P_JPEGENC_BLOCK_BITS && (J2P_JE_W
 static_assert(J2P_JE_WORDS_PER_BLOCK * 32 % 8 == 0, "the padding of a stream's last byte fits its words");
 #define J2P_JE_TILE 256u                // blocks per tile of the size and emit kernels (never across images)
 #define J2P_JE_CHUNK 8192u              // entropy bytes per chunk of the stuffing kernels
-#define J2P_JE_HEAD 623u                // SOI .. SOS: 2 + 18 + 2 x 69 + 19 + 2 x 33 + 2 x 183 + 14
-#define J2P_JE_SOF_AT 158u              // offset of SOF0 in the header (its height follows at + 5)
-#define J2P_JE_HEAD_GRAY 328u           // a gray file's: 2 + 18 + 69 + 13 + 33 + 183 + 10
-#define J2P_JE_SOF_AT_GRAY 89u
+// A header template is SOI, APP0, one DQT per used quantisation table (67 bytes 8-bit, 131
+// 16-bit), SOF0 or SOF1, the DHTs and SOS; its length is its set's.  The quality tables give 2 + 18
+// + 2 x 67 + 19 + 2 x 33 + 2 x 183 + 14 = 623 bytes for a colour file, 2 + 18 + 67 + 13 + 33 + 183 +
+// 10 = 328 for a gray one.  The longest is a colour file's with three 16-bit tables:
+#define J2P_JE_PRE_MAX (2u + 18u + 3u * 133u + 19u)       // SOI .. the SOF's end, three 16-bit DQTs
+#define J2P_JE_HEAD_MAX (J2P_JE_PRE_MAX + 2u * 33u + 2u * 183u + 14u)
 
 // per image of a call, or per bit stream (host plan, read by the kernels).  A stream is an image's
 // scan, or one restart interval of it; it carries its image's fields, and blk0, nblk, the tiles,
@@ -60,6 +62,7 @@ struct j2p_je_img {
         uint16_t ri;                    // the scan's restart interval in MCUs, 0 without restarts
         uint8_t scan;                   // the scan of the file (progressive; 0 otherwise)
         uint8_t pad_;
+        uint32_t set;                   // the image's set of quantisation tables (its j2p_je_tables)
         // written by the encoder
         uint64_t bits;                  // entropy-coded bits before padding
         uint64_t file_off, file_len;
@@ -73,16 +76,19 @@ struct j2p_je_huff {
         uint8_t size[4][256];
 };
 
-// per call: quantisation reciprocals (natural order), derived Huffman codes, the header template
+// per set of quantisation tables of a call (the IJG tables of the call's quality are its one set):
+// the reciprocals of each component's table (natural order) and the header template.  The other
+// fields, the derived Huffman codes and the geometry, are the call's and the same in every set, so
+// the steps that read only them take set 0.
 struct j2p_je_tables {
-        uint16_t recip[2][64], corr[2][64];
-        uint8_t shift[2][64];           // total right shift of the product
+        uint16_t recip[3][64], corr[3][64];             // per component: Y, Cb, Cr
+        uint8_t shift[3][64];           // total right shift of the product
         struct j2p_je_huff huff;        // the Annex K tables
         uint8_t zz[64];                 // zig-zag position of each natural index
         uint32_t hs, vs;                // luma sampling factors (chroma 1 x 1); 1 x 1 for gray
         uint32_t nc;                    // components: 3, or 1 for gray
         uint32_t head_len, sof_at;      // the header template's length and the offset of its SOF
-        uint8_t head[J2P_JE_HEAD];
+        uint8_t head[J2P_JE_HEAD_MAX];
 };
 
 // blocks per MCU: the luma blocks and two chroma blocks, or a gray file's one block
@@ -235,10 +241,11 @@ J2P_HD void j2p_je_block_row(const struct j2p_je_img *im, const struct j2p_je_ta
         j2p_je_fdct_1d<1>(d);
 }
 
-// libjpeg-turbo's quantisation of coefficient v at natural index i
-J2P_HD int j2p_je_quant(const struct j2p_je_tables *t, int tbl, int i, int v) {
+// libjpeg-turbo's quantisation of coefficient v (|v| < 2^15) of component comp at natural index i.
+// (a + corr) < 2^16 and recip < 2^16 for every divisor 8q up to 65528, so the product fits 32 bits.
+J2P_HD int j2p_je_quant(const struct j2p_je_tables *t, int comp, int i, int v) {
         const uint32_t a = (uint32_t)(v < 0 ? -v : v);
-        const uint32_t q = ((a + t->corr[tbl][i]) * (uint32_t)t->recip[tbl][i]) >> t->shift[tbl][i];
+        const uint32_t q = ((a + t->corr[comp][i]) * (uint32_t)t->recip[comp][i]) >> t->shift[comp][i];
         return v < 0 ? -(int)q : (int)q;
 }
 
@@ -338,7 +345,7 @@ J2P_HD uint32_t j2p_je_pad(uint64_t bits, uint64_t *word) {
         return (0xffffffffu >> at) & ~(n + at >= 32 ? 0u : 0xffffffffu >> (at + n));
 }
 
-// the header with the image's size in SOF0
+// the header with the image's size in its SOF
 J2P_HD uint8_t j2p_je_head_byte(const struct j2p_je_tables *t, const struct j2p_je_img *im, uint32_t k) {
         const uint32_t s = t->sof_at;
         if (k == s + 5) return (uint8_t)(im->h >> 8);

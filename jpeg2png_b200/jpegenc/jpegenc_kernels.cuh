@@ -64,16 +64,19 @@ __device__ uint64_t scan_segment(uint32_t count, Ld ld, St st, typename ScanU64:
     return base;
 }
 
-// kBlockThreads threads, 8 per block: colour, downsampling, FDCT and quantisation
+// kBlockThreads threads, 8 per block: colour, downsampling, FDCT and quantisation with the tables
+// of the image's set (t: the call's sets)
 __device__ __forceinline__ void blocks_body(const struct j2p_je_img *__restrict__ imgs, uint32_t n, const struct j2p_je_tables *__restrict__ t,
                                             uint64_t nblk, int16_t *__restrict__ coef) {
     __shared__ int rows[kBlockThreads / 8][8 * 9];
+    __shared__ uint32_t sets[kBlockThreads / 8];   // each block's set, with its rows: no register holds it across the barrier
     const uint32_t grp = threadIdx.x >> 3, lane = threadIdx.x & 7;
     const uint64_t g = ((uint64_t)blockIdx.x * kBlockThreads + threadIdx.x) >> 3;
     const bool on = g < nblk;
     struct j2p_je_where wh;
-    if (on) {
+    if (on) {                           // the geometry is the same in every set: set 0's
         const struct j2p_je_img im = imgs[find_image(imgs, n, g, 0)];
+        if (lane == 0) sets[grp] = im.set;
         wh = j2p_je_locate(&im, t, g - im.blk0);
         int d[8];
         j2p_je_block_row(&im, t, &wh, (int)lane, d);
@@ -81,7 +84,7 @@ __device__ __forceinline__ void blocks_body(const struct j2p_je_img *__restrict_
         for (int x = 0; x < 8; x++) rows[grp][lane * 9 + x] = d[x];
     }
     __syncthreads();
-    if (on) finish_column(t, &wh, rows[grp], 9, (int)lane, coef + g * 64);
+    if (on) finish_column(t + sets[grp], &wh, rows[grp], 9, (int)lane, coef + g * 64);
 }
 
 // Where the kernels find a stream's image, scan and interval.  Without restart intervals (plain)

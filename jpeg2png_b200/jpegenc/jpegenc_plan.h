@@ -1,5 +1,5 @@
 // jpegenc_plan.h — the host side shared by libj2pjpegenc.so, libj2pjpegopt.so and libj2pjpegprog.so: the quantisation
-// tables and their reciprocals, the Annex K Huffman tables and the header template, the plan of a
+// tables and their reciprocals, the Annex K Huffman tables and the header templates, the plan of a
 // call (the layout of its work area), the steps that both the kernels and the host driver call per
 // block, and the serial host driver.  The first two libraries differ only in where an image's
 // Huffman tables and header come from: the call's Annex K ones, or the image's own optimized ones
@@ -9,6 +9,8 @@
 #define J2P_JPEGENC_PLAN_H
 
 #include <string.h>
+
+#include <vector>
 
 #include "../common/codec_host.h"
 #include "jpegenc_core.h"
@@ -49,13 +51,39 @@ static const uint8_t kAcVals[2][162] = {
      0xc2, 0xc3, 0xc4, 0xc5, 0xc6, 0xc7, 0xc8, 0xc9, 0xca, 0xd2, 0xd3, 0xd4, 0xd5, 0xd6, 0xd7, 0xd8, 0xd9, 0xda, 0xe2, 0xe3, 0xe4,
      0xe5, 0xe6, 0xe7, 0xe8, 0xe9, 0xea, 0xf2, 0xf3, 0xf4, 0xf5, 0xf6, 0xf7, 0xf8, 0xf9, 0xfa}};
 
-// IJG quality scaling (jpeg_quality_scaling, jpeg_add_quant_table with force_baseline)
-static void quant_table(int quality, int tbl, uint16_t *q) {
+// The call's one set without given tables: the two Annex K tables with IJG quality scaling
+// (jpeg_quality_scaling, jpeg_add_quant_table with force_baseline)
+static void quality_set(int quality, struct j2p_jpegenc_qtables *q) {
+    memset(q, 0, sizeof *q);
+    q->ntables = 2;
     const long s = quality < 50 ? 5000 / quality : 200 - 2 * quality;
-    for (int i = 0; i < 64; i++) {
-        long v = (kBaseQuant[tbl][i] * s + 50) / 100;
-        q[i] = (uint16_t)(v < 1 ? 1 : v > 255 ? 255 : v);
-    }
+    for (int tbl = 0; tbl < 2; tbl++)
+        for (int i = 0; i < 64; i++) {
+            const long v = (kBaseQuant[tbl][i] * s + 50) / 100;
+            q->table[tbl][i] = (uint16_t)(v < 1 ? 1 : v > 255 ? 255 : v);
+        }
+}
+
+// the sets of quantisation tables of a call, and set k of them
+static uint32_t nsets_of(const struct j2p_jpegenc_params *p) { return p->qtables ? p->nqtables : 1u; }
+
+static void set_of(const struct j2p_jpegenc_params *p, uint32_t k, struct j2p_jpegenc_qtables *q) {
+    if (p->qtables) *q = p->qtables[k];
+    else quality_set(p->quality, q);
+}
+
+// the table component c (0 Y, 1 Cb, 2 Cr) quantises with, as Pillow maps n tables onto them: one
+// for all; two, Y 0 and Cb, Cr 1; three or four, Y 0, Cb 1, Cr 2
+static uint32_t table_of(uint32_t n, uint32_t c) { return n == 1 || c == 0 ? 0u : n == 2 ? 1u : c; }
+
+// the tables a file of nc components writes (a DQT each, in this order): 0 .. dqts - 1
+static uint32_t dqts_of(const struct j2p_jpegenc_qtables *q, uint32_t nc) { return nc == 1 ? 1u : q->ntables < 3 ? q->ntables : 3u; }
+
+// whether table tb needs a 16-bit DQT
+static bool wide_table(const struct j2p_jpegenc_qtables *q, uint32_t tb) {
+    for (int i = 0; i < 64; i++)
+        if (q->table[tb][i] > 255) return true;
+    return false;
 }
 
 // libjpeg-turbo's reciprocal of a divisor d >= 2 (compute_reciprocal, 16-bit DCT elements):
@@ -114,22 +142,28 @@ static bool is_gray(const struct j2p_jpegenc_params *p) { return p->components =
 static uint32_t sof_hs(const struct j2p_jpegenc_params *p) { return p->sampling == J2P_JPEGENC_444 ? 1 : 2; }
 static uint32_t sof_vs(const struct j2p_jpegenc_params *p) { return p->sampling == J2P_JPEGENC_420 ? 2 : 1; }
 
-// the length of the call's header template
-static uint32_t head_len_of(const struct j2p_jpegenc_params *p) { return is_gray(p) ? J2P_JE_HEAD_GRAY : J2P_JE_HEAD; }
+// the length of set k's header template: SOI, APP0, its DQTs, SOF, DHTs, SOS
+static uint32_t head_len_of(const struct j2p_jpegenc_params *p, uint32_t k) {
+    struct j2p_jpegenc_qtables q;
+    set_of(p, k, &q);
+    const uint32_t nc = is_gray(p) ? 1 : 3;
+    uint32_t n = 2 + 18 + (10 + 3 * nc) + (nc == 1 ? 33 + 183 : 2 * 33 + 2 * 183) + (8 + 2 * nc);
+    for (uint32_t tb = 0; tb < dqts_of(&q, nc); tb++) n += wide_table(&q, tb) ? 133 : 69;
+    return n;
+}
 
-static void make_tables(const struct j2p_jpegenc_params *p, struct j2p_je_tables *t) {
+// set k of the call: each component's reciprocals, the call's codes and geometry, the header template
+static void make_tables(const struct j2p_jpegenc_params *p, uint32_t set, struct j2p_je_tables *t) {
     memset(t, 0, sizeof *t);
     const bool gray = is_gray(p);
     t->hs = gray ? 1 : sof_hs(p);       // a gray component is sampled 1 x 1 whatever the SOF says
     t->vs = gray ? 1 : sof_vs(p);
     t->nc = gray ? 1 : 3;
-    t->head_len = head_len_of(p);
-    t->sof_at = gray ? J2P_JE_SOF_AT_GRAY : J2P_JE_SOF_AT;
-    const int ntbl = gray ? 1 : 2;
-    uint16_t q[2][64];
-    for (int tbl = 0; tbl < 2; tbl++) {
-        quant_table(p->quality, tbl, q[tbl]);
-        for (int i = 0; i < 64; i++) reciprocal((uint32_t)q[tbl][i] << 3, &t->recip[tbl][i], &t->corr[tbl][i], &t->shift[tbl][i]);
+    struct j2p_jpegenc_qtables q;
+    set_of(p, set, &q);
+    for (uint32_t c = 0; c < 3; c++) {
+        const uint16_t *tb = q.table[table_of(q.ntables, c)];
+        for (int i = 0; i < 64; i++) reciprocal((uint32_t)tb[i] << 3, &t->recip[c][i], &t->corr[c][i], &t->shift[c][i]);
     }
     for (int k = 0; k < 64; k++) t->zz[kNatural[k]] = (uint8_t)k;
     j2p_je_derive(kDcBits[0], kDcVals, t->huff.code[0], t->huff.size[0]);
@@ -142,19 +176,28 @@ static void make_tables(const struct j2p_jpegenc_params *p, struct j2p_je_tables
     static const uint8_t app0[18] = {0xff, 0xe0, 0, 16, 'J', 'F', 'I', 'F', 0, 1, 1, 0, 0, 1, 0, 1, 0, 0};
     memcpy(o, app0, 18);
     o += 18;
-    for (int tbl = 0; tbl < ntbl; tbl++) {
+    bool sof1 = false;                  // libjpeg's frame is not baseline with a 16-bit table
+    for (uint32_t tbl = 0; tbl < dqts_of(&q, t->nc); tbl++) {
+        const bool wide = wide_table(&q, tbl);
+        sof1 |= wide;
         o = put16(o, 0xffdb);
-        o = put16(o, 67);
-        *o++ = (uint8_t)tbl;
-        for (int k = 0; k < 64; k++) *o++ = (uint8_t)q[tbl][kNatural[k]];
+        o = put16(o, wide ? 131 : 67);
+        *o++ = (uint8_t)(wide << 4 | tbl);
+        for (int k = 0; k < 64; k++) {
+            const uint16_t v = q.table[tbl][kNatural[k]];
+            if (wide) o = put16(o, v);
+            else *o++ = (uint8_t)v;
+        }
     }
-    o = put16(o, 0xffc0);               // the size is patched per image (j2p_je_head_byte)
+    t->sof_at = (uint32_t)(o - t->head);
+    o = put16(o, sof1 ? 0xffc1 : 0xffc0);   // the size is patched per image (j2p_je_head_byte)
     o = put16(o, 8 + 3 * t->nc);
     *o++ = 8;
     o = put16(o, 0);
     o = put16(o, 0);
     *o++ = (uint8_t)t->nc;
-    const uint8_t comps[9] = {1, (uint8_t)(sof_hs(p) << 4 | sof_vs(p)), 0, 2, 0x11, 1, 3, 0x11, 1};
+    const uint8_t comps[9] = {1, (uint8_t)(sof_hs(p) << 4 | sof_vs(p)), 0, 2, 0x11, (uint8_t)table_of(q.ntables, 1), 3, 0x11,
+                              (uint8_t)table_of(q.ntables, 2)};
     memcpy(o, comps, 3 * t->nc);
     o += 3 * t->nc;
     o = put_dht(o, 0x00, kDcBits[0], kDcVals);
@@ -166,6 +209,7 @@ static void make_tables(const struct j2p_jpegenc_params *p, struct j2p_je_tables
     static const uint8_t sos[14] = {0xff, 0xda, 0, 12, 3, 1, 0x00, 2, 0x11, 3, 0x11, 0, 63, 0};
     static const uint8_t sos_gray[10] = {0xff, 0xda, 0, 8, 1, 1, 0x00, 0, 63, 0};
     memcpy(o, gray ? sos_gray : sos, j2p_je_sos_len(t));
+    t->head_len = (uint32_t)(o - t->head) + j2p_je_sos_len(t);
 }
 
 // ---- restart intervals -------------------------------------------------------------------------
@@ -214,13 +258,13 @@ J2P_HD uint8_t j2p_je_stream_byte(const struct j2p_je_img *st, uint32_t k, Head 
     return st->part ? j2p_je_rst_byte(st->part, k) : head(k);
 }
 
-// the length of a baseline stream's header with the call's template
+// the length of a baseline stream's header with its image's template t
 J2P_HD uint32_t j2p_je_fixed_head_len(const struct j2p_je_tables *t, const struct j2p_je_img *st) {
     return st->part ? J2P_JE_RST : t->head_len + (st->ri ? J2P_JE_DRI : 0);
 }
 
-// byte k of a baseline scan header with the call's template: SOI .. SOS with the image's size and
-// its DRI
+// byte k of a baseline scan header with its image's template t: SOI .. SOS with the image's size
+// and its DRI
 J2P_HD uint8_t j2p_je_scan_head_byte(const struct j2p_je_tables *t, const struct j2p_je_img *st, uint32_t k) {
     return j2p_je_dri_head(st->ri, t->head_len, j2p_je_sos_len(t), k, [&](uint32_t k1) { return j2p_je_head_byte(t, st, k1); });
 }
@@ -234,7 +278,7 @@ J2P_HD uint8_t j2p_je_fixed_head_byte(const struct j2p_je_tables *t, const struc
 J2P_HD bool j2p_je_ends_file(const struct j2p_je_img *strs, uint32_t ns, uint32_t s) { return s + 1 == ns || strs[s + 1].img != strs[s].img; }
 
 // ---- plan --------------------------------------------------------------------------------------
-// work: [images][tables][streams] [tile sums][tile offsets][block offsets in the tile][coefficients]
+// work: [images][sets of tables][streams] [tile sums][tile offsets][block offsets in the tile][coefficients]
 //       [0xFF counts per chunk][their exclusive scan][offsets]
 //       (own codes only: [derived tables][headers][header lengths][symbol counts])
 //       [entropy words][files]
@@ -251,7 +295,7 @@ struct Layout {
 };
 
 #define J2P_JE_SYMBOLS 256u             // symbol counts per table and image (4 tables)
-#define J2P_JE_HEAD_ROOM (J2P_JE_HEAD + J2P_JE_DRI)    // the longest header of a baseline file
+#define J2P_JE_HEAD_ROOM (J2P_JE_HEAD_MAX + J2P_JE_DRI)        // the longest header of a baseline file
 
 // the checks of a call's arguments
 static int check_call(const struct j2p_jpegenc_image *im, unsigned n, const struct j2p_jpegenc_params *p) {
@@ -267,11 +311,22 @@ static int check_call(const struct j2p_jpegenc_image *im, unsigned n, const stru
         return fail("restart_marker_rows must be 0 .. 65535 (got %d)", p->restart_marker_rows);
     if (p->components != 0 && p->components != 1 && p->components != 3)
         return fail("components must be 0 or 3 (colour) or 1 (gray) (got %d)", p->components);
+    if (p->qtables && p->nqtables == 0) return fail("qtables given with nqtables 0");
+    for (unsigned k = 0; p->qtables && k < p->nqtables; k++) {
+        const struct j2p_jpegenc_qtables *q = &p->qtables[k];
+        if (q->ntables < 1 || q->ntables > 4) return fail("set %u: ntables must be 1 .. 4 (got %u)", k, q->ntables);
+        for (uint32_t tb = 0; tb < q->ntables; tb++)
+            for (int i = 0; i < 64; i++)
+                if (q->table[tb][i] < 1 || q->table[tb][i] > 8191)
+                    return fail("set %u: table %u entry %d is %u; entries must be 1 .. 8191 (8q must fit libjpeg's 16-bit divisor)", k, tb, i,
+                                q->table[tb][i]);
+    }
     for (unsigned i = 0; i < n; i++) {
         const struct j2p_jpegenc_image *x = &im[i];
         if (!x->data) return fail("image %u: null data pointer", i);
         if (x->width == 0 || x->height == 0 || x->width > 65535 || x->height > 65535)
             return fail("image %u: width and height must be 1 .. 65535 (got %u x %u)", i, x->width, x->height);
+        if (p->qtables && x->qtables >= p->nqtables) return fail("image %u: set %u of qtables, which has %u", i, x->qtables, p->nqtables);
     }
     return 0;
 }
@@ -293,6 +348,7 @@ static void image_desc(const struct j2p_jpegenc_image *x, uint32_t i, const stru
     g->blk0 = blk0;
     g->nblk = (uint64_t)g->mcux * g->mcuy * bpm;
     g->img = i;
+    g->set = p->qtables ? x->qtables : 0;
 }
 
 // The running totals of a plan's streams.  add() appends a stream of nb blocks from blk0 (in the
@@ -347,13 +403,15 @@ static int make_plan(const struct j2p_jpegenc_image *im, unsigned n, const struc
     if (ns >= 0x7fffffffu) return fail("too many restart intervals for one call (%llu)", (unsigned long long)ns);
     size_t o = 0;
     L->off_imgs = o;  o = align16(o + n * sizeof(struct j2p_je_img));
-    L->off_tab = o;   o = align16(o + sizeof(struct j2p_je_tables));
+    L->off_tab = o;   o = align16(o + nsets_of(p) * sizeof(struct j2p_je_tables));
     o = (o + 127) & ~(size_t)127;       // each descriptor on one 128-byte line
     L->plain = !restarts;
     L->off_strs = restarts ? o : L->off_imgs;
     if (restarts) o = align16(o + ns * sizeof(struct j2p_je_img));
     struct j2p_je_img *imgs = w ? (struct j2p_je_img *)(w + L->off_imgs) : nullptr, *strs = w ? (struct j2p_je_img *)(w + L->off_strs) : nullptr;
     StreamPlan sp;
+    std::vector<uint32_t> head(nsets_of(p));
+    for (uint32_t k = 0; k < nsets_of(p); k++) head[k] = head_len_of(p, k);
     for (unsigned i = 0; i < n; i++) {
         struct j2p_je_img g;
         image_desc(&im[i], i, p, nblk, &g);
@@ -363,7 +421,7 @@ static int make_plan(const struct j2p_jpegenc_image *im, unsigned n, const struc
         if (imgs && restarts) imgs[i] = g;
         for (uint64_t q = 0; q < parts; q++) {
             const uint64_t m0 = q * ri, m1 = ri && m0 + ri < mcus ? m0 + ri : mcus;
-            sp.add(g, nblk + m0 * bpm, (m1 - m0) * bpm, wpb, q ? J2P_JE_RST : head_len_of(p) + (ri ? J2P_JE_DRI : 0), q + 1 == parts ? 2 : 0, 0,
+            sp.add(g, nblk + m0 * bpm, (m1 - m0) * bpm, wpb, q ? J2P_JE_RST : head[g.set] + (ri ? J2P_JE_DRI : 0), q + 1 == parts ? 2 : 0, 0,
                    (uint32_t)q, ri, strs ? &strs[sp.ns] : nullptr);
         }
         nblk += g.nblk;
@@ -393,23 +451,29 @@ static int make_plan(const struct j2p_jpegenc_image *im, unsigned n, const struc
     return 0;
 }
 
-// the plan region (images, tables, streams) in host memory
+// the call's sets of tables at t
+static void make_sets(const struct j2p_jpegenc_params *p, struct j2p_je_tables *t) {
+    for (uint32_t k = 0; k < nsets_of(p); k++) make_tables(p, k, t + k);
+}
+
+// the plan region (images, sets, streams) in host memory
 static int fill_plan(const struct j2p_jpegenc_image *im, unsigned n, const struct j2p_jpegenc_params *p, uint32_t wpb, bool own, const Layout &,
                      uint8_t *w) {
     Layout tmp;
     if (make_plan(im, n, p, wpb, own, &tmp, w) != 0) return -1;
-    make_tables(p, (struct j2p_je_tables *)(w + tmp.off_tab));
+    make_sets(p, (struct j2p_je_tables *)(w + tmp.off_tab));
     return 0;
 }
 
 // ---- steps shared by the kernels and the host driver ----------------------------------------------
+// Geometry and codes are the same in every set: these read the call's set 0.
 J2P_HD uint32_t comp_of(const struct j2p_je_tables *t, uint64_t b) {
     const uint32_t k = (uint32_t)(b % j2p_je_bpm(t)), nl = t->hs * t->vs;
     return k < nl ? 0 : 1 + (k - nl);
 }
 
-// column x of a block whose rows are through pass 1 (rows[y * stride + x]): pass 2, quantise, and
-// store in zig-zag order; a dummy keeps only its DC
+// column x of a block whose rows are through pass 1 (rows[y * stride + x]): pass 2, quantise with
+// the tables of t (the image's set), and store in zig-zag order; a dummy keeps only its DC
 J2P_HD void finish_column(const struct j2p_je_tables *t, const struct j2p_je_where *w, const int *rows, int stride, int x, int16_t *coef) {
     int d[8];
 #ifdef __CUDA_ARCH__
@@ -417,13 +481,12 @@ J2P_HD void finish_column(const struct j2p_je_tables *t, const struct j2p_je_whe
 #endif
     for (int y = 0; y < 8; y++) d[y] = rows[y * stride + x];
     j2p_je_fdct_1d<2>(d);
-    const int tbl = w->comp ? 1 : 0;
 #ifdef __CUDA_ARCH__
 #pragma unroll
 #endif
     for (int y = 0; y < 8; y++) {
         const int i = y * 8 + x;
-        const int v = w->dummy && i ? 0 : j2p_je_quant(t, tbl, i, d[y]);
+        const int v = w->dummy && i ? 0 : j2p_je_quant(t, (int)w->comp, i, d[y]);
         coef[t->zz[i]] = (int16_t)v;
     }
 }
@@ -436,7 +499,8 @@ J2P_HD int pred_of(const struct j2p_je_tables *t, const int16_t *coef, uint64_t 
 J2P_HD uint64_t raw_bytes(const struct j2p_je_img *im) { return (im->bits + 7) / 8; }
 
 // ---- host driver -------------------------------------------------------------------------------
-// the blocks step of the kernels on one image, serially: its coefficients at coef + im->blk0 * 64
+// the blocks step of the kernels on one image with its set t, serially: its coefficients at coef +
+// im->blk0 * 64
 static void host_blocks(const struct j2p_je_img *im, const struct j2p_je_tables *t, int16_t *coef) {
     for (uint64_t b = 0; b < im->nblk; b++) {
         const struct j2p_je_where wh = j2p_je_locate(im, t, b);
@@ -446,15 +510,17 @@ static void host_blocks(const struct j2p_je_img *im, const struct j2p_je_tables 
     }
 }
 
-// encode_jpeg's default codes: the call's Annex K tables and header template for every image
+// encode_jpeg's default codes: the call's Annex K tables for every image, and the header template of
+// its set (t: the sets)
 struct FixedCodes {
     const struct j2p_je_tables *t;
     const struct j2p_je_huff *huff(uint32_t) const { return &t->huff; }
-    uint32_t head_len(const struct j2p_je_img *st) const { return j2p_je_fixed_head_len(t, st); }
-    uint8_t head_byte(const struct j2p_je_img *st, uint32_t k) const { return j2p_je_fixed_head_byte(t, st, k); }
+    uint32_t head_len(const struct j2p_je_img *st) const { return j2p_je_fixed_head_len(t + st->set, st); }
+    uint8_t head_byte(const struct j2p_je_img *st, uint32_t k) const { return j2p_je_fixed_head_byte(t + st->set, st, k); }
 };
 
-// The steps of the kernels run serially on host memory.  codes(L, w, imgs, strs, t, coef) runs
+// The steps of the kernels run serially on host memory.  codes(L, w, imgs, strs, t, coef) (t: the
+// sets) runs
 // between the blocks and the sizes and returns where each image's Huffman tables and each stream's
 // header come from: an object with huff(image), head_len(stream) and head_byte(stream, k), such as
 // FixedCodes.
@@ -476,7 +542,7 @@ static int encode_host_steps(const struct j2p_jpegenc_image *images, unsigned n,
     uint32_t *raw = (uint32_t *)(w + L.off_raw);
     uint8_t *out = w + L.off_out;
     memset(w + L.off_hist, 0, L.off_raw - L.off_hist + L.words * sizeof(uint32_t));
-    for (unsigned i = 0; i < n; i++) host_blocks(&imgs[i], t, coef);   // blocks
+    for (unsigned i = 0; i < n; i++) host_blocks(&imgs[i], t + imgs[i].set, coef);      // blocks
     const auto c = codes(L, w, imgs, (const struct j2p_je_img *)strs, t, (const int16_t *)coef);
     for (uint32_t s = 0; s < L.ns; s++) {                               // sizes and scans
         struct j2p_je_img *im = &strs[s];

@@ -70,8 +70,9 @@ extern "C" int j2p_jpegopt_encode_host(const struct j2p_jpegenc_image *images, u
             struct j2p_jo_scratch s;
             struct j2p_jo_dht d;
             for (int tb = 0; tb < (int)j2p_jo_ntables(t); tb++) j2p_jo_table(h + tb * J2P_JE_SYMBOLS, &s, &d, &huffs[i], tb, j2p_jo_serial());
-            hlens[i] = j2p_jo_file_head_len(t, im, &d);
-            for (uint32_t k = 0; k < hlens[i]; k++) heads[(size_t)i * J2P_JE_HEAD_ROOM + k] = j2p_jo_file_head_byte(t, im, &d, k);
+            const struct j2p_je_tables *ts = t + im->set;
+            hlens[i] = j2p_jo_file_head_len(ts, im, &d);
+            for (uint32_t k = 0; k < hlens[i]; k++) heads[(size_t)i * J2P_JE_HEAD_ROOM + k] = j2p_jo_file_head_byte(ts, im, &d, k);
         }
         return OwnCodes{huffs, heads, hlens};
     };
@@ -118,8 +119,9 @@ __global__ void __launch_bounds__(kTileThreads) k_jo_hist(const struct j2p_je_im
         if (cnt[k]) atomicAdd(h + k, (unsigned long long)cnt[k]);
 }
 
-// per image, a warp per table: code lengths, symbols and codes; then the image's header and its
-// length.  A gray image's warps 2 and 3 have no table (its chroma counts are all 0).
+// per image, a warp per table: code lengths, symbols and codes; then the image's header (from its
+// set's template) and its length.  A gray image's warps 2 and 3 have no table (its chroma counts are
+// all 0).
 __global__ void __launch_bounds__(kTableThreads) k_jo_tables(const struct j2p_je_img *__restrict__ imgs, const struct j2p_je_tables *__restrict__ t,
                                                             const uint64_t *__restrict__ hist, struct j2p_je_huff *__restrict__ huffs,
                                                             uint8_t *__restrict__ heads, uint32_t *__restrict__ hlens) {
@@ -129,8 +131,9 @@ __global__ void __launch_bounds__(kTableThreads) k_jo_tables(const struct j2p_je
     const WarpLanes L = {threadIdx.x & 31, 32};
     if (tb < j2p_jo_ntables(t)) j2p_jo_table(hist + ((size_t)i * 4 + tb) * J2P_JE_SYMBOLS, &scr[tb], &d, &huffs[i], (int)tb, L);
     __syncthreads();
-    const uint32_t len = j2p_jo_file_head_len(t, &imgs[i], &d);
-    for (uint32_t k = threadIdx.x; k < len; k += kTableThreads) heads[(size_t)i * J2P_JE_HEAD_ROOM + k] = j2p_jo_file_head_byte(t, &imgs[i], &d, k);
+    const struct j2p_je_tables *ts = t + imgs[i].set;
+    const uint32_t len = j2p_jo_file_head_len(ts, &imgs[i], &d);
+    for (uint32_t k = threadIdx.x; k < len; k += kTableThreads) heads[(size_t)i * J2P_JE_HEAD_ROOM + k] = j2p_jo_file_head_byte(ts, &imgs[i], &d, k);
     if (threadIdx.x == 0) hlens[i] = len;
 }
 

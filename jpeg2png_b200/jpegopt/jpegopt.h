@@ -6,8 +6,10 @@
  * order, as libj2pjpegenc.so's files (jpegenc.h), and the same entropy-coded coefficients, but each
  * image's four DHT segments hold its own tables, built from its own symbol counts (T.81 Annex K.2
  * with libjpeg's tie rule, the K.3 limit to 16 bits; jpegopt_core.h).  A DHT lists only the
- * symbols that occur, so the header is at most jpegenc.h's 623 bytes and its length varies by
- * image.
+ * symbols that occur, so the header is at most the length of its set's template (jpegenc.h: 623
+ * bytes for the quality tables of a colour file, 884 at most with given tables) and its length
+ * varies by image.  With given quantisation tables (params->qtables, jpegenc.h) each image's DQTs
+ * and SOF0 or SOF1 come from its own set, as in libj2pjpegenc.so's file.
  *
  * The images, parameters and statistics are jpegenc.h's structs, and the calls mirror its calls.
  * One call queues a memset and nine kernels, whatever the number and sizes of the images:

@@ -28,10 +28,6 @@
 
 #include "../jpegenc/jpegenc_plan.h"
 
-#define J2P_JO_HEAD_PRE 177u            // SOI .. SOF0 of the header template: J2P_JE_SOF_AT + 19
-#define J2P_JO_SOS 14u                  // the SOS segment that ends it
-static_assert(J2P_JO_HEAD_PRE + 2 * 33 + 2 * 183 + J2P_JO_SOS == J2P_JE_HEAD, "the header template is SOI .. SOF0, four DHTs, SOS");
-
 // scratch of one table's build
 struct j2p_jo_scratch {
         uint64_t freq[257];             // symbol 256 is the pseudo-symbol
@@ -196,7 +192,10 @@ J2P_HD uint32_t j2p_jo_head_len(const struct j2p_je_tables *t, const struct j2p_
         return n;
 }
 
-// byte k of an image's header: the template's SOI .. SOF0 with the image's size, its own DHTs, SOS
+// The header of an image whose set is t: the template's SOI .. SOF with the image's size (its length
+// is the set's: j2p_je_sof_end), the image's own DHTs, the template's SOS.  An optimized table codes
+// no more symbols than the Annex K one of its kind, so the header fits the template's room.
+// byte k of it:
 J2P_HD uint8_t j2p_jo_head_byte(const struct j2p_je_tables *t, const struct j2p_je_img *im, const struct j2p_jo_dht *d, uint32_t k) {
         const uint32_t pre = j2p_je_sof_end(t);
         if (k < pre) return j2p_je_head_byte(t, im, k);

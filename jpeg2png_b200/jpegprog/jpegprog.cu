@@ -15,7 +15,7 @@ extern "C" const char *j2p_jpegprog_last_error(void) { return g_err; }
 // stream blocks, its tiles, chunks, words, bits and place in the output.  Without restarts a scan is
 // one stream.  The streams of one scan are consecutive, and so are their stream blocks, and each
 // (image, scan) has a j2p_jp_scanplan: its first stream and the DRI its header carries.
-// work: [images][tables][streams][scans] [tile sums][tile offsets][block offsets in the tile][run states]
+// work: [images][sets of tables][streams][scans] [tile sums][tile offsets][block offsets in the tile][run states]
 //       [summaries][coefficients][0xFF counts per chunk][their exclusive scan][offsets]
 //       [derived tables][scan headers][their lengths][symbol counts][entropy words][files]
 // The symbol counts sit just before the entropy words, so that one memset clears both.
@@ -74,21 +74,21 @@ static int prog_plan(const struct j2p_jpegenc_image *im, unsigned n, const struc
         image_desc(&im[i], i, p, nblk, &imgs[i]);
         nblk += imgs[i].nblk;
     }
-    struct j2p_je_tables t;
-    make_tables(p, &t);
+    struct j2p_je_tables t;             // set 0: the geometry, the same in every set
+    make_tables(p, 0, &t);
     uint64_t sblk;
     const StreamPlan sp = prog_streams(imgs.data(), n, p, &t, nullptr, nullptr, &sblk);
     if (sp.check(nblk) != 0) return -1;
     const size_t nsc = (size_t)n * j2p_jp_nscans(j2p_jp_gray(&t));
     size_t o = 0;
     P->off_imgs = o;  o = align16(o + n * sizeof(struct j2p_je_img));
-    P->off_tab = o;   o = align16(o + sizeof(struct j2p_je_tables));
+    P->off_tab = o;   o = align16(o + nsets_of(p) * sizeof(struct j2p_je_tables));
     o = (o + 127) & ~(size_t)127;       // each descriptor on one 128-byte line
     P->off_str = o;   o = align16(o + sp.ns * sizeof(struct j2p_je_img));
     P->off_scan = o;  o = align16(o + nsc * sizeof(struct j2p_jp_scanplan));
     if (w) {
         memcpy(w + P->off_imgs, imgs.data(), n * sizeof(struct j2p_je_img));
-        memcpy(w + P->off_tab, &t, sizeof t);
+        make_sets(p, (struct j2p_je_tables *)(w + P->off_tab));
         prog_streams(imgs.data(), n, p, &t, (struct j2p_je_img *)(w + P->off_str), (struct j2p_jp_scanplan *)(w + P->off_scan), &sblk);
     }
     P->n = n;
@@ -253,7 +253,7 @@ extern "C" int j2p_jpegprog_encode_host(const struct j2p_jpegenc_image *images, 
     const bool g = j2p_jp_gray(t);
     const uint32_t per = j2p_jp_nscans(g);
     const Ctx x = {imgs, strs, t, coef, summ, state, P.plain, g};
-    for (unsigned i = 0; i < n; i++) host_blocks(&imgs[i], t, coef);   // blocks
+    for (unsigned i = 0; i < n; i++) host_blocks(&imgs[i], t + imgs[i].set, coef);      // blocks
     for (uint32_t s = 0; s < P.ns; s++) {                               // summaries, runs
         const struct j2p_je_img *st = &strs[s];
         if (!j2p_jp_is_ac(g, st->scan)) continue;
@@ -274,10 +274,11 @@ extern "C" int j2p_jpegprog_encode_host(const struct j2p_jpegenc_image *images, 
         struct j2p_jp_dht d;
         for (uint32_t tb = 0; tb < j2p_jp_ntables(g); tb++)
             j2p_jp_table(hist + ((size_t)i * J2P_JP_TABLES + tb) * 256, &scr, &d, &huffs[(size_t)i * J2P_JP_TABLES + tb], tb, j2p_jo_serial());
+        const struct j2p_je_tables *ts = t + imgs[i].set;
         for (uint32_t k = 0; k < per; k++) {
             const size_t q = (size_t)i * per + k;
-            hlens[q] = j2p_jp_scan_head_len(t, &d, k, scs[q].dri);
-            for (uint32_t b = 0; b < hlens[q]; b++) heads[q * J2P_JP_HEAD + b] = j2p_jp_scan_head_byte(t, &imgs[i], &d, k, scs[q].dri, b);
+            hlens[q] = j2p_jp_scan_head_len(ts, &d, k, scs[q].dri);
+            for (uint32_t b = 0; b < hlens[q]; b++) heads[q * J2P_JP_HEAD + b] = j2p_jp_scan_head_byte(ts, &imgs[i], &d, k, scs[q].dri, b);
         }
     }
     for (uint32_t s = 0; s < P.ns; s++) {                               // sizes, emit, padding
@@ -426,8 +427,8 @@ __global__ void __launch_bounds__(kTileThreads) k_jp_hist(const Ctx x, uint32_t 
     else hist_body(as_kind<false>(x), ns, hist, cnt);
 }
 
-// per image, a warp per table: code lengths, symbols and codes; then its scans' headers.  A gray
-// image's warps past its five tables have none to build.
+// per image, a warp per table: code lengths, symbols and codes; then its scans' headers, from its
+// set's template.  A gray image's warps past its five tables have none to build.
 __global__ void __launch_bounds__(kTableThreads) k_jp_tables(const struct j2p_je_img *__restrict__ imgs, const struct j2p_je_tables *__restrict__ t,
                                                             const struct j2p_jp_scanplan *__restrict__ scs, const uint64_t *__restrict__ hist,
                                                             struct j2p_jp_huff *__restrict__ huffs, uint8_t *__restrict__ heads,
@@ -441,10 +442,11 @@ __global__ void __launch_bounds__(kTableThreads) k_jp_tables(const struct j2p_je
     const size_t tab = (size_t)i * J2P_JP_TABLES + tb;
     if (tb < j2p_jp_ntables(gray)) j2p_jp_table(hist + tab * 256, &scr[tb], &d, &huffs[tab], tb, L);
     __syncthreads();
+    const struct j2p_je_tables *ts = t + imgs[i].set;
     for (uint32_t k = 0; k < per; k++) {
         const size_t q = (size_t)i * per + k;
-        const uint32_t dri = scs[q].dri, len = j2p_jp_scan_head_len(t, &d, k, dri);
-        for (uint32_t b = threadIdx.x; b < len; b += kTableThreads) heads[q * J2P_JP_HEAD + b] = j2p_jp_scan_head_byte(t, &imgs[i], &d, k, dri, b);
+        const uint32_t dri = scs[q].dri, len = j2p_jp_scan_head_len(ts, &d, k, dri);
+        for (uint32_t b = threadIdx.x; b < len; b += kTableThreads) heads[q * J2P_JP_HEAD + b] = j2p_jp_scan_head_byte(ts, &imgs[i], &d, k, dri, b);
         if (threadIdx.x == 0) hlens[q] = len;
     }
 }

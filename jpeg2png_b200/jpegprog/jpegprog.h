@@ -3,7 +3,8 @@
  *
  * The file is the one libjpeg's compressor writes with jpeg_simple_progression, as Pillow's JPEG
  * writer drives it with `progressive=True` (and quality q, subsampling s; `optimize` changes no
- * byte): SOI, JFIF APP0, the two DQTs and SOF2 of libj2pjpegenc.so's file (jpegenc.h), then ten
+ * byte): SOI, JFIF APP0, the DQTs of libj2pjpegenc.so's file (jpegenc.h: the image's set of
+ * quantisation tables, or the two quality tables) and SOF2 (whatever their precision), then ten
  * scans, each after the DHTs of the tables it uses, then EOI.  The coefficients are the baseline
  * file's; each scan's tables are built from that scan's own symbol counts (jpegopt_core.h).  The
  * scan script and the coding rules are in jpegprog_core.h.

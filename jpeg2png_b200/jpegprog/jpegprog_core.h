@@ -63,8 +63,8 @@
 #define J2P_JP_SCANS_GRAY 6u            // per gray image
 #define J2P_JP_TABLES 10u               // Huffman table slots per image (a gray image uses 5)
 #define J2P_JP_TABLES_GRAY 5u
-#define J2P_JP_HEAD 752u                // room for a scan's header: SOI .. SOF2, two DHTs, DRI, SOS
-static_assert(J2P_JP_HEAD >= J2P_JO_HEAD_PRE + 2 * (21 + 256) + J2P_JE_DRI + 14 && J2P_JP_HEAD % 16 == 0, "a scan's header fits");
+#define J2P_JP_HEAD 1024u               // room for a scan's header: SOI .. SOF2, two DHTs, DRI, SOS
+static_assert(J2P_JP_HEAD >= J2P_JE_PRE_MAX + 2 * (21 + 256) + J2P_JE_DRI + 14 && J2P_JP_HEAD % 16 == 0, "a scan's header fits");
 #define J2P_JP_MAX_RUN 0x7fffu          // the longest EOB run
 #define J2P_JP_MAX_BE 937u              // correction bits an EOB run may buffer before it is emitted
 #define J2P_JP_RESET 0x80u              // summary: the block emits the incoming state and sets its own
@@ -379,7 +379,8 @@ J2P_HD uint32_t j2p_jp_sos_len(bool g, uint32_t k) { return j2p_jp_scan_of(g, k)
 
 J2P_HD bool j2p_jp_gray(const struct j2p_je_tables *t) { return t->nc == 1; }
 
-// the header of scan k: SOI .. SOF2 before scan 0, the DHTs of its tables, its SOS (without DRI)
+// the header of scan k of an image whose set is t: SOI .. SOF2 (its set's DQTs) before scan 0, the
+// DHTs of its tables, its SOS (without DRI)
 J2P_HD uint32_t j2p_jp_head_len(const struct j2p_je_tables *t, const struct j2p_jp_dht *d, uint32_t k) {
         const bool g = j2p_jp_gray(t);
         if (k == 0) return j2p_je_sof_end(t) + j2p_jp_dht_len(d, 0) + (g ? 0 : j2p_jp_dht_len(d, 1)) + j2p_jp_sos_len(g, 0);
