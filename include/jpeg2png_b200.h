@@ -133,7 +133,7 @@ void j2p_session_destroy(j2p_session *s);
  * first j2p_session_iterate(s, 0, n) or j2p_session_reset after its planes were uploaded, so new
  * frames can be uploaded into a batch and solved again.  Objective logging and the strip calls are
  * refused on a batch of more than one frame (J2P_ERR_ARG); so are nframes == 0 and out-of-range
- * planes or frames. */
+ * planes or frames.  j2p_session_record_objective records the objective of every frame of a batch. */
 int j2p_session_create_batch(j2p_session **out, int device, const struct j2p_frame_desc *desc,
                              unsigned nframes);
 /* Frames of the session (1 for every session not made by j2p_session_create_batch). */
@@ -331,6 +331,20 @@ int j2p_session_iterate_group(j2p_session *const *sessions, unsigned n, unsigned
  * enabled with j2p_session_set_logging(s, 1) before iterating. */
 int j2p_session_set_logging(j2p_session *s, int enabled);
 int j2p_session_objective(j2p_session *s, double out[4]);
+
+/* Record the objective of every iteration on the device, for every frame of a whole-frame session
+ * (single-frame or batch): the numbers j2p_session_objective gives, without a host wait per
+ * iteration.  Set before iterating; re-arming (first == 0) clears the record.  Refused on strip
+ * sessions and on sessions with j2p_session_set_logging on (and vice versa); a missing
+ * libj2pobjective.so is J2P_ERR_CUDA.  A recording session iterates with the recording kernels of
+ * libj2pobjective.so (loaded on first use): the same launches and the same iterates, bit for bit.
+ * The record holds desc.iterations rows: iterating a recording session past them is J2P_ERR_ARG, and
+ * so is a group (j2p_session_iterate_group) that contains one. */
+int j2p_session_record_objective(j2p_session *s, int enabled);
+/* Iterations [first, first+count) of every frame: out[(f * count + i) * 4 + k], k = objective,
+ * prob_dist, tv, tv2.  Synchronises the session stream; one device-to-host copy.  Rows that have not
+ * been recorded since the last arm are J2P_ERR_ARG. */
+int j2p_session_objective_history(j2p_session *s, unsigned first, unsigned count, double *out);
 
 /* Block the host until everything queued on the session stream has finished. */
 int j2p_session_sync(j2p_session *s);

@@ -5,16 +5,20 @@ turn such tensors into PNG or JPEG files on the device (`encode_jpeg(..., optimi
 per-image optimized Huffman tables, as Pillow's `optimize=True`, and `encode_jpeg(...,
 progressive=True)` with Pillow's progressive files, and `encode_jpeg(..., qtables=)` with given
 quantisation tables, per image if need be); `keep_settings` reads a JPEG file's tables and
-sampling, as Pillow's quality='keep' re-uses them; torch is imported only when one of them is
-first used."""
+sampling, as Pillow's quality='keep' re-uses them; `write_objective_csv` writes the objective logs of
+`decode_jpeg(..., return_objective=True)` as the command line's -c file; torch is imported only when
+one of them is first used."""
 
-__all__ = ['decode_jpeg', 'encode_png', 'encode_jpeg', 'keep_settings']
+__all__ = ['decode_jpeg', 'encode_png', 'encode_jpeg', 'keep_settings', 'write_objective_csv']
 
 
 def __getattr__(name):
     if name == 'decode_jpeg':
         from .decode import decode_jpeg
         return decode_jpeg
+    if name == 'write_objective_csv':
+        from .decode import write_objective_csv
+        return write_objective_csv
     if name == 'encode_png':
         from .encode import encode_png
         return encode_png

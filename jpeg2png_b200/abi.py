@@ -221,6 +221,10 @@ def declare_product(lib: C.CDLL) -> C.CDLL:
     lib.j2p_session_set_logging.argtypes = [vp, C.c_int]
     lib.j2p_session_objective.restype = C.c_int
     lib.j2p_session_objective.argtypes = [vp, C.POINTER(C.c_double)]
+    lib.j2p_session_record_objective.restype = C.c_int
+    lib.j2p_session_record_objective.argtypes = [vp, C.c_int]
+    lib.j2p_session_objective_history.restype = C.c_int
+    lib.j2p_session_objective_history.argtypes = [vp, C.c_uint, C.c_uint, C.POINTER(C.c_double)]
     lib.j2p_session_sync.restype = C.c_int
     lib.j2p_session_sync.argtypes = [vp]
     lib.j2p_session_stream.restype = vp
@@ -247,6 +251,7 @@ HEADER_SYMBOLS = [
     'j2p_session_create_batch', 'j2p_session_frames', 'j2p_session_download_frame_scanlines',
     'j2p_session_export', 'j2p_session_export_separate', 'j2p_session_upload_device',
     'j2p_session_export_gray', 'j2p_session_export_oriented', 'j2p_session_iterate_group',
+    'j2p_session_record_objective', 'j2p_session_objective_history',
 ]
 
 _product = None

@@ -35,6 +35,8 @@ namespace j2p {
 template <int NC, bool TGV, int GPM, bool BATCH>
 __global__ void J2P_GRAD_BOUNDS k_gradient_packed(const __grid_constant__ FrameDev F, const float factor, const int band_rows) {
     const GridGeo geo{};
+    constexpr bool REC = false;          // the recording variant is k_gradient_packed_rec (libj2pobjective.so)
+    const RecDev R{};
 #include "gradient_packed_body.inc"
 }
 

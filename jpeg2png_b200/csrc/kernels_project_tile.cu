@@ -26,6 +26,8 @@ namespace j2p {
 template <bool RES, bool BATCH>
 __global__ void __launch_bounds__(PT_NT, J2P_TILE_MIN_CTAS) k_project_tile(const __grid_constant__ FrameDev F, const int c0, const float factor) {
     const GridGeo geo{};
+    constexpr bool REC = false;          // the recording variant is k_project_tile_rec (libj2pobjective.so)
+    const RecDev R{};
 #include "project_tile_body.inc"
 }
 

@@ -40,12 +40,14 @@ cudaError_t configure_project_tile22() {
 
 // F: already restricted to the rows the session owns (launch_project).  Projects planes
 // c .. c+count-1, which must all be 2x2 planes with the same coefficient grid.
-cudaError_t launch_project_tile22(const FrameDev &F, int c, int count, float factor, cudaStream_t s, int *nlaunch) {
+// uncovered_only: the tiles have been projected elsewhere (the recording kernels of
+// libj2pobjective.so); only the stepped-only pixels remain
+cudaError_t launch_project_tile22(const FrameDev &F, int c, int count, float factor, cudaStream_t s, int *nlaunch, bool uncovered_only) {
     const PlaneDev &P = F.pl[c];
     const int bw = P.cw >> 3, bh = P.ch >> 3, gx = (bw + P22_NB - 1) / P22_NB;
     const bool batch = F.nframes > 1;
     cudaError_t e = cudaSuccess;
-    for (int y0 = 0; y0 < bh && e == cudaSuccess; y0 += kMaxGridRows) {   // one launch unless bh > 65535
+    for (int y0 = 0; y0 < bh && !uncovered_only && e == cudaSuccess; y0 += kMaxGridRows) {   // one launch unless bh > 65535
         const int rows = bh - y0 < kMaxGridRows ? bh - y0 : kMaxGridRows;
         const FrameDev V = y0 == 0 && rows == bh ? F : rows_view(F, c, count, y0, 16, y0 + rows == bh);
         e = batch ? launch_chain(k_project_tile22<true>, dim3(gx * count, rows, F.nframes), dim3(P22_NT), P22_SMEM, s, V, c, factor)

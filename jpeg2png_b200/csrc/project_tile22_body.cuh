@@ -12,6 +12,7 @@
 #include "numerics.cuh"
 #include "pdl.cuh"
 #include "project_common.cuh"
+#include "record.cuh"
 #include "strip_sync.cuh"
 
 namespace j2p {
@@ -25,8 +26,11 @@ constexpr size_t P22_SMEM = (size_t)3 * 16 * P22_C4 * sizeof(float4)      // x_k
                             + (size_t)P22_NB * TILE_STRIDE * sizeof(float) // transpose tiles
                             + 3 * 64 * sizeof(float) + 4 * sizeof(float);  // tables, norm
 
-template <bool BATCH, class G>
-__device__ __forceinline__ void project_tile22_body(const FrameDev &F, const int c0, const float factor, const G &geo) {
+// REC (k_project_tile22_rec, objective/objective.cu; false everywhere else) also writes the CTA's sum of
+// (residual/q)^2 to R->pp (record.cuh), behind `if constexpr (REC)`.
+template <bool BATCH, class G, bool REC = false>
+__device__ __forceinline__ void project_tile22_body(const FrameDev &F, const int c0, const float factor, const G &geo, const RecDev *R = nullptr) {
+    __shared__ double rsum[REC ? P22_NB : 1];                        // REC: each block's sum of (residual/q)^2
     extern __shared__ __align__(16) unsigned char smem22[];
     float4 *sx = reinterpret_cast<float4 *>(smem22);                 // [16][P22_C4]  x_k  -> later x_{k+1}
     float4 *sp = sx + 16 * P22_C4;                                   // [16][P22_C4]  x_{k-1}
@@ -110,6 +114,7 @@ __device__ __forceinline__ void project_tile22_body(const FrameDev &F, const int
     const bool use_prob = P.use_prob != 0;
     const unsigned gmask = 0xffu << (tid & 24);
     float *tile = tiles + b * TILE_STRIDE;
+    double rloc = 0.;                                                // REC: this block's sum (0 for blocks beyond the plane)
 
     if (real) {
         // ---- stepped point of the 2 x 16 footprint (compute.c:436, :213) --------------------------
@@ -193,6 +198,15 @@ __device__ __forceinline__ void project_tile22_body(const FrameDev &F, const int
 #pragma unroll
                 for (int i = 0; i < 8; i++) r[i] = fdiv(num[i], qqv[i]);
             }
+            if constexpr (REC) {                                   // the block's sum of (residual/q)^2 (compute_simd_step.c:22-26), fp64
+                if (use_prob) {
+#pragma unroll
+                    for (int i = 0; i < 8; i++) rloc = __dadd_rn(rloc, (double)fsq(fdiv(num[i], qv[i])));
+                    rloc = __dadd_rn(rloc, __shfl_xor_sync(gmask, rloc, 1));
+                    rloc = __dadd_rn(rloc, __shfl_xor_sync(gmask, rloc, 2));
+                    rloc = __dadd_rn(rloc, __shfl_xor_sync(gmask, rloc, 4));
+                }
+            }
         }
 
         idct8x8_rows(v, tile, j, gmask);
@@ -221,7 +235,17 @@ __device__ __forceinline__ void project_tile22_body(const FrameDev &F, const int
                     make_float4(fmul(pa, r[h * 4 + 0]), fmul(pa, r[h * 4 + 1]), fmul(pa, r[h * 4 + 2]), fmul(pa, r[h * 4 + 3]));
         }
     }
+    if constexpr (REC) {
+        if (j == 0) rsum[b] = rloc;
+    }
     __syncthreads();
+    if constexpr (REC) {                                             // the CTA's partial, blocks in order (record.cuh)
+        if (tid == 0 && use_prob) {
+            double sum = 0.;
+            for (int k = 0; k < P22_NB; k++) sum = __dadd_rn(sum, rsum[k]);
+            R->pp[((size_t)frame * 3 + c) * R->pp_stride + (size_t)(R->row0 + by) * gx + bx0 / P22_NB] = sum;
+        }
+    }
 
     // ---- coalesced copy-out: x_{k+1} over x_{k-1} (compute.c:387), gp for the next iteration ------
 #pragma unroll

@@ -12,6 +12,7 @@
 #include "numerics.cuh"
 #include "pdl.cuh"
 #include "project_common.cuh"
+#include "record.cuh"
 #include "strip_sync.cuh"
 
 namespace j2p {

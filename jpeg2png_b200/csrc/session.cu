@@ -40,6 +40,7 @@
 #include "copy_pool.h"
 #include "geometry.cuh"
 #include "kernels.cuh"
+#include "record.cuh"
 #include "tma_maps.h"
 
 namespace j2p {
@@ -60,6 +61,9 @@ cudaError_t launch_halo_exchange(const HaloPeers &P, unsigned seq, unsigned *tic
 // kernels_gradient_packed.cu: the packed gradient's GPM and grid for a frame (what a group gives it)
 int packed_gradient_gpm(const FrameDev &F);
 void packed_gradient_geometry(const FrameDev &F, int *cx, int *bands, int *rows);
+// the stepped-only pixels of 1x1 / 2x2 planes (uncovered_only), next to the recording projection
+cudaError_t launch_project_tile(const FrameDev &F, int c, int count, float factor, cudaStream_t s, int *nlaunch, bool uncovered_only);
+cudaError_t launch_project_tile22(const FrameDev &F, int c, int count, float factor, cudaStream_t s, int *nlaunch, bool uncovered_only);
 }  // namespace j2p
 
 using namespace j2p;
@@ -225,6 +229,12 @@ struct j2p_session {
     unsigned long long tables_gen = 0;        // bumped whenever a quantisation table is set
     struct GroupPlan *group = nullptr;        // the plan of the last group this session led (j2p_session_iterate_group)
     cudaEvent_t group_ev = nullptr;           // orders a group's launches with this session's stream
+    // j2p_session_record_objective: the kernels of libj2pobjective.so and the device record (record.cuh)
+    bool recording = false;
+    bool rec_armed = false;                   // the record holds every iteration since the last arm
+    double *rec_hist = nullptr;               // [desc.iterations][nframes][REC_FIELDS]
+    double *rec_pp = nullptr;                 // projection partials [nframes][3][rec_pp_stride]
+    unsigned rec_pp_stride = 0, rec_pp_count[3] = {};
 };
 static void free_group_plan(GroupPlan *g);
 
@@ -569,6 +579,10 @@ static int reset_impl(j2p_session *s) {
     s->next_log_iter = 0;
     s->log_host_iter = -1;
     CK(cudaMemsetAsync(F.logsums, 0, sizeof(double) * 8, s->stream));    // iteration 0: DCT distance is exactly 0
+    if (s->rec_hist) {
+        CK(cudaMemsetAsync(s->rec_hist, 0, sizeof(double) * REC_FIELDS * s->desc.iterations * s->nframes, s->stream));
+        s->rec_armed = s->recording;
+    }
     return J2P_OK;
 }
 
@@ -786,14 +800,29 @@ extern "C" int j2p_session_upload_device(j2p_session *s, unsigned plane, const i
     return plane_uploaded(s, plane);
 }
 
-// one solver iteration on the session stream; optional events around each kernel
-static int one_iteration(j2p_session *s, cudaEvent_t e0, cudaEvent_t e1, cudaEvent_t e2) {
+static int record_gradient(j2p_session *s, unsigned iter, float factor);
+static int record_project(j2p_session *s, unsigned iter, float factor, int *nlaunch);
+
+// one solver iteration (number `iter`) on the session stream; optional events around each kernel
+static int one_iteration(j2p_session *s, unsigned iter, cudaEvent_t e0, cudaEvent_t e1, cudaEvent_t e2) {
     FrameDev &F = s->F;
     // FISTA momentum (compute.c:431-432, :440), host floats
     const float tnext = (1 + sqrtf(1 + 4 * (s->t * s->t))) / 2;
     const float factor = (s->t - 1) / tnext;
     s->t = tnext;
     if (e0) CK(cudaEventRecord(e0, s->stream));
+    if (s->recording) {                                                  // the same iteration with the objective recorded
+        int rc = record_gradient(s, iter, factor);
+        if (rc != J2P_OK) return rc;
+        if (e1) CK(cudaEventRecord(e1, s->stream));
+        int nproj = 0;
+        rc = record_project(s, iter, factor, &nproj);
+        if (rc != J2P_OK) return rc;
+        if (e2) CK(cudaEventRecord(e2, s->stream));
+        s->launches += 1 + (unsigned)nproj;
+        swap_iterates(F);                                                // compute.c:438
+        return J2P_OK;
+    }
     CK(launch_gradient(F, factor, s->stream));
     if (e1) CK(cudaEventRecord(e1, s->stream));
     if (F.log_on) {
@@ -910,10 +939,17 @@ extern "C" int j2p_session_iterate(j2p_session *s, unsigned first, unsigned n) {
     if (!s) return fail(J2P_ERR_ARG, "null session");
     if (s->strip) return fail(J2P_ERR_ARG, "a strip session is driven with j2p_session_gradient / j2p_session_project");
     CK(cudaSetDevice(s->device));
+    if (s->recording) {
+        if ((unsigned long long)first + n > s->desc.iterations)
+            return fail(J2P_ERR_ARG, "the objective record holds %u iterations; iterations %u..%llu asked for", s->desc.iterations, first,
+                        (unsigned long long)first + n - 1);
+        if (first != 0 && !s->rec_armed && !s->stale)
+            return fail(J2P_ERR_ARG, "recording was switched on after iteration 0: iterate from first == 0 to re-arm the record");
+    }
     int rc = check_ready(s, first);
     if (rc != J2P_OK) return rc;
     for (unsigned i = first; i < first + n; i++) {
-        rc = one_iteration(s, nullptr, nullptr, nullptr);
+        rc = one_iteration(s, i, nullptr, nullptr, nullptr);
         if (rc != J2P_OK) return rc;
         if (i % kEventStride == kEventStride - 1) {
             const int slot = (int)((i / kEventStride) % kEventRing);
@@ -928,13 +964,15 @@ extern "C" int j2p_session_iterate(j2p_session *s, unsigned first, unsigned n) {
 extern "C" int j2p_session_profile(j2p_session *s, unsigned n, float *ms_gradient, float *ms_project) {
     if (!s || !ms_gradient || !ms_project || n == 0) return fail(J2P_ERR_ARG, "bad argument");
     CK(cudaSetDevice(s->device));
+    if (s->recording && n > s->desc.iterations)
+        return fail(J2P_ERR_ARG, "the objective record holds %u iterations; %u asked for", s->desc.iterations, n);
     int rc = check_ready(s, 0);
     if (rc != J2P_OK) return rc;
     cudaEvent_t e[3];
     for (int k = 0; k < 3; k++) CK(cudaEventCreate(&e[k]));
     double sg = 0., sp = 0.;
     for (unsigned i = 0; i < n; i++) {
-        rc = one_iteration(s, e[0], e[1], e[2]);
+        rc = one_iteration(s, i, e[0], e[1], e[2]);
         if (rc != J2P_OK) return rc;
         CK(cudaEventSynchronize(e[2]));
         float a = 0.f, b = 0.f;
@@ -1159,6 +1197,7 @@ extern "C" int j2p_session_set_logging(j2p_session *s, int enabled) {
     if (!s) return fail(J2P_ERR_ARG, "null session");
     if (enabled && s->strip) return fail(J2P_ERR_ARG, "objective logging is not available on strip sessions");
     if (enabled && s->nframes > 1) return refuse_batch(s, "objective logging");
+    if (enabled && s->recording) return fail(J2P_ERR_ARG, "the session records the objective (j2p_session_record_objective); logging is the other way to get it");
     s->logging = enabled != 0;
     s->F.log_on = s->logging;
     return J2P_OK;
@@ -1168,33 +1207,191 @@ extern "C" int j2p_session_set_logging(j2p_session *s, int enabled) {
 // (compute.c:232-272, compute_simd_step.c:61): prob_dist = 0.5 * sum (residual/q)^2 over the
 // planes with pweight != 0, tv / tv2 = fp64 sums of alpha*norm, objective = their sum over the
 // float total_alpha.  Synchronises the session stream.
-extern "C" int j2p_session_objective(j2p_session *s, double out[4]) {
-    if (!s || !out) return fail(J2P_ERR_ARG, "null argument");
-    if (!s->logging || s->log_host_iter < 0) return fail(J2P_ERR_ARG, "no logged iteration (call j2p_session_set_logging(s, 1) before iterating)");
-    CK(cudaSetDevice(s->device));
-    CK(cudaStreamSynchronize(s->stream));
+// The four logged numbers from the raw sums of one iteration: tv, tv2 and each plane's sum of
+// (residual/q)^2.  Shared by j2p_session_objective and j2p_session_objective_history.
+static void objective_terms(const j2p_session *s, double tv, double tv2_raw, const double *prob_raw, double out[4]) {
     const FrameDev &F = s->F;
-    const int slot = (int)(s->log_host_iter & 1);
     double prob = 0.;
     float total_alpha = 0.f;
     for (int c = 0; c < F.nc; c++) {
         if (F.pl[c].use_prob) {                                         // compute.c:244-247
             total_alpha += F.pl[c].p_alpha;
-            prob += 0.5 * s->log_host[2 + 3 * slot + c];
+            prob += 0.5 * prob_raw[c];
         }
     }
     total_alpha += (float)F.nc;                                         // compute.c:252
-    const double tv = s->log_host[0];
     double tv2 = 0.;
     if (F.use_tgv) {                                                    // compute.c:257-260
         const float alpha = s->desc.weight / sqrtf((float)(4 / 2));
         total_alpha += alpha * (float)F.nc;
-        tv2 = s->log_host[1];
+        tv2 = tv2_raw;
     }
     out[0] = (tv + tv2 + prob) / (double)total_alpha;                   // compute.c:271
     out[1] = prob;
     out[2] = tv;
     out[3] = tv2;
+}
+
+extern "C" int j2p_session_objective(j2p_session *s, double out[4]) {
+    if (!s || !out) return fail(J2P_ERR_ARG, "null argument");
+    if (!s->logging || s->log_host_iter < 0) return fail(J2P_ERR_ARG, "no logged iteration (call j2p_session_set_logging(s, 1) before iterating)");
+    CK(cudaSetDevice(s->device));
+    CK(cudaStreamSynchronize(s->stream));
+    const int slot = (int)(s->log_host_iter & 1);
+    objective_terms(s, s->log_host[0], s->log_host[1], s->log_host + 2 + 3 * slot, out);
+    return J2P_OK;
+}
+
+// ---- the objective recorded on the device (libj2pobjective.so, objective/objective.cu) --------------
+// Loaded on first use from next to this library, like libj2pmixed.so.
+#include <dlfcn.h>
+namespace {
+struct ObjectiveApi {
+    int (*configure)(void) = nullptr;
+    int (*gradient)(const FrameDev *, float, int, int, int, int, const RecDev *, void *) = nullptr;
+    int (*project)(const FrameDev *, int, int, float, const RecDev *, void *, int *) = nullptr;
+    unsigned (*partials)(const FrameDev *, int) = nullptr;
+    char err[400] = "";
+};
+const ObjectiveApi &objective_api() {
+    static const ObjectiveApi api = [] {
+        ObjectiveApi a;
+        Dl_info info;
+        if (!dladdr((void *)&j2p_session_objective, &info) || !info.dli_fname) {
+            snprintf(a.err, sizeof a.err, "cannot locate libjpeg2png_b200.so to find libj2pobjective.so");
+            return a;
+        }
+        std::string path(info.dli_fname);
+        const size_t slash = path.rfind('/');
+        path = (slash == std::string::npos ? std::string(".") : path.substr(0, slash)) + "/../objective/libj2pobjective.so";
+        void *h = dlopen(path.c_str(), RTLD_NOW | RTLD_LOCAL);
+        if (!h) {
+            snprintf(a.err, sizeof a.err, "libj2pobjective.so (the recording kernels) cannot be loaded: %s", dlerror());
+            return a;
+        }
+        a.configure = (int (*)(void))dlsym(h, "j2p_objective_configure");
+        a.gradient = (decltype(a.gradient))dlsym(h, "j2p_objective_gradient");
+        a.project = (decltype(a.project))dlsym(h, "j2p_objective_project");
+        a.partials = (decltype(a.partials))dlsym(h, "j2p_objective_partials");
+        if (!a.configure || !a.gradient || !a.project || !a.partials) {
+            snprintf(a.err, sizeof a.err, "%s does not export the j2p_objective_* entry points", path.c_str());
+            a.configure = nullptr;
+            a.gradient = nullptr;
+        }
+        return a;
+    }();
+    return api;
+}
+std::once_flag g_objective_once[64];
+int g_objective_cfg[64];
+}  // namespace
+
+// what the recording kernels see: the session's descriptor with the device tables (a single frame runs
+// with batch addressing too), and row `iter` of the record
+static FrameDev record_view(const j2p_session *s) {
+    FrameDev V = s->F;
+    V.tables = s->dev_tables;
+    return V;
+}
+static RecDev record_args(const j2p_session *s, unsigned iter) {
+    RecDev R{};
+    R.hist = s->rec_hist;
+    R.pp = s->rec_pp;
+    R.iter = iter;
+    R.nframes = s->nframes;
+    R.pp_stride = s->rec_pp_stride;
+    for (int c = 0; c < 3; c++) R.pp_count[c] = s->rec_pp_count[c];
+    return R;
+}
+
+static int record_gradient(j2p_session *s, unsigned iter, float factor) {
+    const FrameDev V = record_view(s);
+    const RecDev R = record_args(s, iter);
+    int cx, bands, rows;
+    packed_gradient_geometry(V, &cx, &bands, &rows);                    // the unrecorded launch's bands
+    CK((cudaError_t)objective_api().gradient(&V, factor, cx, bands, rows, packed_gradient_gpm(V), &R, (void *)s->stream));
+    return J2P_OK;
+}
+
+// launch_project's planes and launches, each projection kernel replaced by its recording variant
+static int record_project(j2p_session *s, unsigned iter, float factor, int *nlaunch) {
+    const FrameDev V = record_view(s);
+    const RecDev R = record_args(s, iter);
+    *nlaunch = 0;
+    for (int c = 0; c < V.nc; c++) {
+        const PlaneDev &P = V.pl[c];
+        const bool p11 = P.sw == 1 && P.sh == 1, p22 = P.sw == 2 && P.sh == 2;
+        int count = 1;      // following planes of identical geometry ride in the same launch
+        while ((p11 || p22) && c + count < V.nc && V.pl[c + count].sw == P.sw && V.pl[c + count].sh == P.sh && V.pl[c + count].cw == P.cw &&
+               V.pl[c + count].ch == P.ch)
+            count++;
+        int n = 0;
+        CK((cudaError_t)objective_api().project(&V, c, count, factor, &R, (void *)s->stream, &n));
+        *nlaunch += n;
+        n = 0;
+        if (p11) CK(launch_project_tile(s->F, c, count, factor, s->stream, &n, true));
+        else if (p22) CK(launch_project_tile22(s->F, c, count, factor, s->stream, &n, true));
+        *nlaunch += n;
+        c += count - 1;
+    }
+    return J2P_OK;
+}
+
+extern "C" int j2p_session_record_objective(j2p_session *s, int enabled) {
+    if (!s) return fail(J2P_ERR_ARG, "null session");
+    if (!enabled) {
+        s->recording = false;
+        s->rec_armed = false;
+        return J2P_OK;
+    }
+    if (s->strip) return fail(J2P_ERR_ARG, "the objective cannot be recorded on a strip session");
+    if (s->logging) return fail(J2P_ERR_ARG, "the session logs the objective (j2p_session_set_logging); recording is the other way to get it");
+    const ObjectiveApi &api = objective_api();
+    if (!api.gradient) return fail(J2P_ERR_CUDA, "%s", api.err);
+    CK(cudaSetDevice(s->device));
+    std::call_once(g_objective_once[s->device & 63], [&] { g_objective_cfg[s->device & 63] = api.configure(); });
+    CK((cudaError_t)g_objective_cfg[s->device & 63]);
+    if (!s->rec_hist) {
+        unsigned stride = 1;
+        for (int c = 0; c < s->F.nc; c++) {
+            s->rec_pp_count[c] = api.partials(&s->F, c);
+            stride = std::max(stride, s->rec_pp_count[c]);
+        }
+        s->rec_pp_stride = stride;
+        CK(dev_alloc(s, &s->rec_hist, sizeof(double) * REC_FIELDS * s->desc.iterations * s->nframes));
+        CK(dev_alloc(s, &s->rec_pp, sizeof(double) * 3 * stride * s->nframes));
+    }
+    if (!s->dev_tables) {                // a single frame: its tables on the device as well (the kernels run with batch addressing)
+        CK(dev_alloc(s, &s->dev_tables, s->tables.size() * sizeof(float)));
+        s->tables_stale = true;
+    }
+    if (s->tables_stale) {               // pageable source: the copy has read it when the call returns
+        CK(cudaMemcpyAsync(s->dev_tables, s->tables.data(), s->tables.size() * sizeof(float), cudaMemcpyHostToDevice, s->stream));
+        s->tables_stale = false;
+    }
+    if (!s->recording) CK(cudaMemsetAsync(s->rec_hist, 0, sizeof(double) * REC_FIELDS * s->desc.iterations * s->nframes, s->stream));
+    s->recording = true;
+    s->rec_armed = s->next_iter == 0;
+    return J2P_OK;
+}
+
+extern "C" int j2p_session_objective_history(j2p_session *s, unsigned first, unsigned count, double *out) {
+    if (!s || (!out && count)) return fail(J2P_ERR_ARG, "null argument");
+    if (!s->recording) return fail(J2P_ERR_ARG, "the session does not record the objective (call j2p_session_record_objective(s, 1) before iterating)");
+    const unsigned done = s->rec_armed && !s->stale ? s->next_iter : 0;
+    if ((unsigned long long)first + count > done)
+        return fail(J2P_ERR_ARG, "iterations %u..%llu have not been recorded (%u recorded)", first, (unsigned long long)first + count - 1, done);
+    if (count == 0) return J2P_OK;
+    CK(cudaSetDevice(s->device));
+    CK(cudaStreamSynchronize(s->stream));
+    const size_t row = (size_t)s->nframes * REC_FIELDS;
+    std::vector<double> raw(row * count);
+    CK(cudaMemcpy(raw.data(), s->rec_hist + (size_t)first * row, raw.size() * sizeof(double), cudaMemcpyDeviceToHost));
+    for (unsigned f = 0; f < s->nframes; f++)
+        for (unsigned i = 0; i < count; i++) {
+            const double *r = raw.data() + (size_t)i * row + (size_t)f * REC_FIELDS;
+            objective_terms(s, r[0], r[1], r + 2, out + ((size_t)f * count + i) * 4);
+        }
     return J2P_OK;
 }
 
@@ -1771,6 +1968,7 @@ static int refuse_join(const j2p_session *s0, const j2p_session *s, unsigned k) 
     if (s->device != s0->device) return fail(J2P_ERR_ARG, "group session %u is on device %d, session 0 on %d", k, s->device, s0->device);
     if (s->strip) return fail(J2P_ERR_ARG, "group session %u is a strip session", k);
     if (s->logging) return fail(J2P_ERR_ARG, "group session %u logs the objective", k);
+    if (s->recording) return fail(J2P_ERR_ARG, "group session %u records the objective", k);
     if (b.nchannel != a.nchannel) return fail(J2P_ERR_ARG, "group session %u has %u planes, session 0 %u", k, b.nchannel, a.nchannel);
     for (unsigned c = 0; c < b.nchannel; c++) {
         if (!((b.w_samp[c] == 1 && b.h_samp[c] == 1) || (b.w_samp[c] == 2 && b.h_samp[c] == 2)))

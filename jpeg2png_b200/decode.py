@@ -21,6 +21,7 @@ torch.float32 the clamped value before truncation.  There is no CPU fallback.
 from __future__ import annotations
 
 import ctypes as C
+import math
 import numbers
 import os
 from concurrent.futures import ThreadPoolExecutor
@@ -368,11 +369,12 @@ def solved_planes(key, separate: bool, mode: str = 'RGB'):
     return 3, 3
 
 
-def frame_footprint(key, separate: bool, sample_bytes: int, mode: str = 'RGB') -> int:
+def frame_footprint(key, separate: bool, sample_bytes: int, mode: str = 'RGB', record_rows: int = 0) -> int:
     """Estimated device bytes one frame of `key` takes in its batch session(s) (DESIGN §4: x, xp, g,
     gp at frame size per plane; coefficients int16 and the conventional decode fp32 at plane size;
     the reduction state) plus its part of the output tensor, for the planes solved and the channels
-    written in `mode` (solved_planes)."""
+    written in `mode` (solved_planes).  record_rows: iterations the frame's sessions record
+    (return_objective), five fp64 sums each (DESIGN §7o), plus the projection's partials."""
     w, h, planes = key
     nsolved, nout = solved_planes(key, separate, mode)
     planes = planes[:nsolved]
@@ -387,6 +389,8 @@ def frame_footprint(key, separate: bool, sample_bytes: int, mode: str = 'RGB') -
         return n + (16 << 10)
 
     total = sum(session([p]) for p in planes) if separate else session(list(planes))
+    if record_rows:
+        total += 40 * record_rows + 3 * 8 * sum((pw // 8) * (ph // 8) for pw, ph, _, _ in planes)
     return total + w * h * nout * sample_bytes
 
 
@@ -551,8 +555,10 @@ class _Chunk:
     tensor either way."""
 
     def __init__(self, lib, device, items, flags, separate, dtype, layout, coefs=None, coef_stream=None, mode='RGB',
-                 orientations=None, grouped=False):
-        """grouped: create and upload only; the caller iterates the sessions in a group, then calls export()."""
+                 orientations=None, grouped=False, record=False):
+        """grouped: create and upload only; the caller iterates the sessions in a group, then calls export().
+        record: the sessions record the objective (j2p_session_record_objective); logs[j] is item j's
+        log after the solve (decode_jpeg's return_objective)."""
         iters, weights, pweights = flags
         self.lib, self.sessions, self.coefs = lib, [], coefs or {}
         first, n = items[0], len(items)
@@ -566,6 +572,8 @@ class _Chunk:
                 s = C.c_void_p()
                 self._check(lib.j2p_session_create_batch(C.byref(s), device, C.byref(desc), n))
                 self.sessions.append(s)
+                if record:
+                    self._check(lib.j2p_session_record_objective(s, 1))
             for s, (_, channels, it) in zip(self.sessions, work):
                 for f, parsed in enumerate(items):
                     for k, c in enumerate(channels):
@@ -580,6 +588,16 @@ class _Chunk:
                 if not grouped:
                     self._check(lib.j2p_session_iterate(s, 0, it))
             self.iterations = work[0][2]
+            self.logs = None
+            if record:
+                # one read per session after its solve; the key is the command line's CSV channel
+                self.logs = [{} for _ in range(n)]
+                for s, (_, channels, it) in zip(self.sessions, work):
+                    hist = np.zeros((n, it, 4), dtype=np.float64)
+                    self._check(lib.j2p_session_objective_history(s, 0, it, hist.ctypes.data_as(C.POINTER(C.c_double))))
+                    key = 3 if len(channels) == 3 else channels[0]
+                    for f in range(n):
+                        self.logs[f][key] = torch.from_numpy(hist[f].copy())
             self._export_args = (device, items, dtype, layout, nout, separate, orientations)
             if not grouped:
                 self.export()
@@ -686,7 +704,7 @@ def _front_end(data, device_ok, progressive=False, flags=0):
 
 def decode_jpeg(inputs, *, iterations=50, weight=0.3, pweight=0.001, separate=False,
                 dtype=torch.uint8, layout='CHW', device=None, max_frames=None, progressive_on_device=False,
-                mode='RGB', apply_exif_orientation=False):
+                mode='RGB', apply_exif_orientation=False, return_objective=False):
     """Decode JPEG files into RGB or gray tensors on a CUDA device, deblocked by the solver.
 
     inputs: bytes-like, a path (str / os.PathLike), or a list or tuple of them.  A single input
@@ -727,6 +745,15 @@ def decode_jpeg(inputs, *, iterations=50, weight=0.3, pweight=0.001, separate=Fa
     The samples are those of the unrotated decode, written to their rotated places by the export
     itself; mode, separate, dtype, layout, max_frames and progressive_on_device work as without it,
     and files of one geometry share a batch whatever their orientation.  Every tensor is contiguous.
+
+    return_objective: True or False (default).  With True the call returns (images, logs), or
+    (tensor, log) for a single input: each file's objective at every iteration, as the command line's
+    -c log has it.  A log is a dict keyed by the log's channel: {3: t} for a joint solve, {0: t0, 1: t1,
+    2: t2} with separate=True, {0: t} for a grayscale file and for mode='GRAY' with separate=True.
+    Each t is a CPU float64 tensor of shape (iterations, 4): objective, prob_dist, tv, tv2.  The
+    objective is recorded on the device (j2p_session_record_objective) and read once per batch after
+    its solve; the images are those of return_objective=False.  Batches are then solved one by one,
+    not grouped.  write_objective_csv writes the logs as the command line's CSV file.
     """
     flags = solver_flags(iterations, weight, pweight, separate)
     if not isinstance(mode, str) or mode not in MODES:
@@ -734,6 +761,8 @@ def decode_jpeg(inputs, *, iterations=50, weight=0.3, pweight=0.001, separate=Fa
     read_flags = 0 if mode == 'RGB' else READ_GRAY
     if apply_exif_orientation is not True and apply_exif_orientation is not False:
         raise ValueError(f'apply_exif_orientation must be True or False, not {apply_exif_orientation!r}')
+    if return_objective is not True and return_objective is not False:
+        raise ValueError(f'return_objective must be True or False, not {return_objective!r}')
     if dtype not in _SAMPLE:
         raise ValueError(f'dtype must be torch.uint8, torch.uint16 or torch.float32, not {dtype}')
     if layout not in _LAYOUT:
@@ -747,7 +776,7 @@ def decode_jpeg(inputs, *, iterations=50, weight=0.3, pweight=0.001, separate=Fa
     single = not isinstance(inputs, (list, tuple))
     read = [_read_input(x) for x in ([inputs] if single else inputs)]
     if not read:
-        return []
+        return ([], []) if return_objective else []
 
     # Without a device the host reader reads every input (its errors first), as the solver needs a
     # device anyway.  With one, the layout pass runs instead and only non-device-decodable files are
@@ -775,11 +804,21 @@ def decode_jpeg(inputs, *, iterations=50, weight=0.3, pweight=0.001, separate=Fa
     index = dev.index if dev.index is not None else torch.cuda.current_device()
     sample_bytes = _SAMPLE[dtype] // 8
     free = torch.cuda.mem_get_info(index)[0] if max_frames is None else 0
-    chunks = plan([p.key() for p in parsed],
-                  lambda k: chunk_frames(k, separate, sample_bytes, max_frames, free, mode))
+    # the rows a frame's sessions record (return_objective): per session, its iteration count
+    if return_objective:
+        def record_rows(k):
+            nsolved = solved_planes(k, separate, mode)[0]
+            return sum(flags[0][c] for c in range(nsolved)) if (separate or nsolved == 1) else flags[0][0]
+        chunks = plan([p.key() for p in parsed],
+                      lambda k: (min(int(max_frames), MAX_BATCH) if max_frames is not None else
+                                 max(1, min(MAX_BATCH, free // 4 // frame_footprint(k, separate, sample_bytes, mode, record_rows(k))))))
+    else:
+        chunks = plan([p.key() for p in parsed],
+                      lambda k: chunk_frames(k, separate, sample_bytes, max_frames, free, mode))
 
-    # packs of chunks iterated in one group; a pack of one chunk is solved as the chunk alone
-    if _group_chunks:
+    # packs of chunks iterated in one group; a pack of one chunk is solved as the chunk alone.  Groups
+    # refuse recording sessions: with return_objective every chunk is solved alone.
+    if _group_chunks and not return_objective:
         cap = (free if max_frames is None else torch.cuda.mem_get_info(index)[0]) // 4
         packs = pack(chunks, lambda k: group_class(k, separate, mode),
                      lambda k, n: n * frame_footprint(k, separate, sample_bytes, mode), cap)
@@ -787,6 +826,7 @@ def decode_jpeg(inputs, *, iterations=50, weight=0.3, pweight=0.001, separate=Fa
         packs = [[j] for j in range(len(chunks))]
 
     results = [None] * len(parsed)
+    logs = [None] * len(parsed)
     layout_id = _LAYOUT[layout]
     previous = []
     try:
@@ -824,7 +864,7 @@ def decode_jpeg(inputs, *, iterations=50, weight=0.3, pweight=0.001, separate=Fa
                         made.append(_Chunk(lib, index, [parsed[i] for i in idx], flags, separate, dtype, layout_id,
                                            chunk_coefs(idx), coef_stream, mode,
                                            None if orientations is None else [orientations[i] for i in idx],
-                                           grouped=len(p) > 1))
+                                           grouped=len(p) > 1, record=return_objective))
                     if len(p) > 1:
                         ss = [c.sessions[0] for c in made]
                         if lib.j2p_session_iterate_group((C.c_void_p * len(ss))(*ss), len(ss), 0, made[0].iterations) != 0:
@@ -838,10 +878,50 @@ def decode_jpeg(inputs, *, iterations=50, weight=0.3, pweight=0.001, separate=Fa
                 for j, c in zip(p, made):
                     for k, i in enumerate(chunks[j][1]):
                         results[i] = c.frame(k)
+                        if return_objective:
+                            logs[i] = c.logs[k]
                 for c in previous:              # this pack is queued: let the previous one finish
                     c.close()
                 previous = made
     finally:
         for c in previous:
             c.close()
+    if return_objective:
+        return (results[0], logs[0]) if single else (results, logs)
     return results[0] if single else results
+
+
+def _glibc_f(v: float) -> str:
+    """v as glibc's printf("%f") prints it, NaN and infinity included."""
+    if math.isnan(v):
+        return '-nan' if math.copysign(1.0, v) < 0 else 'nan'
+    if math.isinf(v):
+        return '-inf' if v < 0 else 'inf'
+    return '%f' % v
+
+
+def write_objective_csv(file, names, logs):
+    """Write the logs decode_jpeg(..., return_objective=True) returns as the command line's -c file:
+    the header "filename,channel,iteration,objective,prob_dist,tv,tv2", then one row per file,
+    channel and iteration, formatted "%s,%u,%u,%f,%f,%f,%f" (logger.c).  A file's rows are written
+    together, its channels in order and each channel's iterations in order.
+
+    file: a path or a text file object.  names: the filename column, one per log."""
+    names, logs = list(names), list(logs)
+    if len(names) != len(logs):
+        raise ValueError(f'{len(names)} names for {len(logs)} logs')
+    lines = ['filename,channel,iteration,objective,prob_dist,tv,tv2\n']
+    for name, log in zip(names, logs):
+        for channel in sorted(log):
+            t = log[channel]
+            rows = t.tolist() if hasattr(t, 'tolist') else list(t)
+            for i, row in enumerate(rows):
+                if len(row) != 4:
+                    raise ValueError(f'a log row holds objective, prob_dist, tv, tv2; got {len(row)} values')
+                lines.append(f'{name},{int(channel)},{i},' + ','.join(_glibc_f(float(v)) for v in row) + '\n')
+    text = ''.join(lines)
+    if hasattr(file, 'write'):
+        file.write(text)
+    else:
+        with open(file, 'w', newline='') as f:
+            f.write(text)

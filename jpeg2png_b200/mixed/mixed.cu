@@ -25,6 +25,8 @@ __global__ void J2P_GRAD_BOUNDS k_gradient_packed_grouped(const GroupFrame *__re
     const GroupGeo geo(e);
     const FrameDev &F = frames[e.d].F;
     const int band_rows = frames[e.d].band_rows;
+    constexpr bool REC = false;
+    const RecDev R{};
 #include "../csrc/gradient_packed_body.inc"
 }
 
@@ -45,6 +47,8 @@ __global__ void __launch_bounds__(PT_NT, J2P_TILE_MIN_CTAS - 1) k_project_tile_g
     __syncthreads();
     const GroupGeo geo(e);
     const int c0 = (int)e.c;                 // the plane; bx is the CTA column within it
+    constexpr bool REC = false;
+    const RecDev R{};
 #include "../csrc/project_tile_body.inc"
 }
 
