@@ -1,9 +1,12 @@
 /* jpeg_reader.c — JPEG file -> quantised DCT coefficients (see jpeg_reader.h).
  *
  * A from-scratch ITU T.81 entropy decoder that stops where libjpeg's jpeg_read_coefficients
- * stops: after Huffman decoding, before dequantisation.  Section references are to T.81.
+ * stops: after Huffman or arithmetic decoding, before dequantisation.  Section references are to
+ * T.81.  The QM decoder and the sequential arithmetic block step are ../arith/arith_core.h, shared
+ * with the device decoder of libj2parith.so; the progressive arithmetic steps are here.
  */
 #include "jpeg_reader.h"
+#include "../arith/arith_core.h"
 
 #include <stdarg.h>
 #include <stdio.h>
@@ -28,6 +31,7 @@ struct comp {
         unsigned pwb, phb;        /* MCU-padded block grid used while decoding */
         int16_t *blk;             /* [phb][pwb][64], natural order */
         int dc_pred;
+        int dc_ctx;               /* arithmetic coding: the DC conditioning category (F.1.4.4.1.2) */
         int td, ta;               /* tables of the current scan */
 };
 
@@ -41,6 +45,13 @@ struct dec {
         struct huff dc[4], ac[4];
         struct comp c[3];
         int ncomp, progressive;
+        int arith;                     /* SOF9/SOF10: arithmetic coding */
+        uint8_t dac_L[16], dac_U[16], dac_K[16];   /* DAC conditioning, T.81's defaults until a DAC sets them */
+        uint8_t dc_st[4][J2P_ARITH_DC_BINS], ac_st[4][J2P_ARITH_AC_BINS];   /* the statistics of the current segment */
+        uint8_t fixed_st;              /* the fixed-probability bin */
+        struct j2p_qm qm;
+        uint8_t *abuf;                 /* the current segment's unstuffed bytes */
+        size_t abuf_cap;
         unsigned flags;                /* J2P_READ_* */
         unsigned W, H, maxh, maxv, mcux, mcuy;
         unsigned restart_interval;
@@ -50,6 +61,7 @@ struct dec {
         struct j2p_jpeg_layout *lay;   /* the layout pass (j2p_read_jpeg_layout), NULL for a full read */
         unsigned scans_of[3];          /* layout pass: scans that name each component */
         struct j2p_jpeg_prog_layout *play;   /* the progressive layout pass (j2p_read_jpeg_prog_layout) */
+        struct j2p_jpeg_arith_layout *alay;  /* the arithmetic layout pass (j2p_read_jpeg_arith_layout) */
         int headers_only;              /* j2p_jpeg_keep_settings: stop at the first SOS */
         size_t data_cap, seg_cap, scan_cap;
 };
@@ -215,6 +227,92 @@ static void block_ac_refine(struct dec *d, struct comp *c, int16_t *b, int ss, i
         }
 }
 
+/* ---- arithmetic-coded blocks (jdarith.c's models: F.1.4.4 and G.1.3) ------------------------- */
+static int bad_arith(struct dec *d) { return fail(d, "corrupt jpeg: bad arithmetic code"); }
+
+static void arith_block(struct dec *d, struct comp *c, int16_t *b, int ss, int se, int ah, int al) {
+        const int td = c->td, ta = c->ta;
+        if (!d->progressive) {
+                if (j2p_arith_block_seq(&d->qm, d->dc_st[td], d->ac_st[ta], &c->dc_pred, &c->dc_ctx, d->dac_L[td], d->dac_U[td],
+                                        d->dac_K[ta], &d->fixed_st, b) != J2P_ARITH_OK) bad_arith(d);
+        } else if (ss == 0 && ah == 0) {                        /* G.1.3.1: DC first */
+                int diff;
+                if (j2p_arith_dc_diff(&d->qm, d->dc_st[td], &c->dc_ctx, d->dac_L[td], d->dac_U[td], &diff) != J2P_ARITH_OK) { bad_arith(d); return; }
+                c->dc_pred += diff;
+                b[0] = (int16_t)(int)((unsigned)c->dc_pred << al);
+        } else if (ss == 0) {                                   /* DC refine: one bit on the fixed bin */
+                if (j2p_qm_decode(&d->qm, &d->fixed_st)) b[0] |= (int16_t)(1 << al);
+        } else if (ah == 0) {                                   /* G.1.3.2: AC first */
+                if (j2p_arith_ac(&d->qm, d->ac_st[ta], d->dac_K[ta], &d->fixed_st, ss, se, al, b) != J2P_ARITH_OK) bad_arith(d);
+        } else {                                                /* G.1.3.3: AC refine */
+                const int p1 = 1 << al, m1 = (int)(~0u << al);
+                int kex = se;                                   /* the previous stages' EOB */
+                for (; kex > 0; kex--)
+                        if (b[ZZ[kex]]) break;
+                for (int k = ss; k <= se; k++) {
+                        uint8_t *st = d->ac_st[ta] + 3 * (k - 1);
+                        if (k > kex && j2p_qm_decode(&d->qm, st)) break;      /* EOB */
+                        for (;;) {
+                                int16_t *coef = &b[ZZ[k]];
+                                if (*coef) {                    /* a correction bit */
+                                        if (j2p_qm_decode(&d->qm, st + 2)) *coef = (int16_t)(*coef + (*coef < 0 ? m1 : p1));
+                                        break;
+                                }
+                                if (j2p_qm_decode(&d->qm, st + 1)) {          /* newly nonzero */
+                                        *coef = (int16_t)(j2p_qm_decode(&d->qm, &d->fixed_st) ? m1 : p1);
+                                        break;
+                                }
+                                st += 3;
+                                if (++k > se) { bad_arith(d); return; }
+                        }
+                }
+        }
+}
+
+/* the unstuffed bytes the entropy decoders read from *pp: up to the first FF not followed by 00,
+ * FF 00 -> FF; writes them to o, returns their count and leaves *pp at the FF */
+static size_t unstuff(const uint8_t **pp, const uint8_t *end, uint8_t *o) {
+        const uint8_t *p = *pp;
+        uint8_t *o0 = o;
+        while (p < end) {
+                const uint8_t *q = memchr(p, 0xFF, (size_t)(end - p));
+                const size_t run = (size_t)((q ? q : end) - p);
+                memcpy(o, p, run);
+                o += run;
+                p += run;
+                if (!q) break;
+                if (p + 1 < end && p[1] == 0x00) { *o++ = 0xFF; p += 2; }
+                else break;
+        }
+        *pp = p;
+        return (size_t)(o - o0);
+}
+
+static int grow(void **p, size_t *cap, size_t need, size_t elem) {
+        if (need <= *cap) return 0;
+        size_t n = *cap ? *cap : 4096 / elem + 1;
+        while (n < need) n *= 2;
+        void *q = realloc(*p, n * elem);
+        if (!q) return -1;
+        *p = q;
+        *cap = n;
+        return 0;
+}
+
+/* an arithmetic segment starts (the scan's first, or after RSTn): zeroed statistics and DC
+ * contexts, C = A = 0 and CT = -16 over the segment's bytes (F.1.4.4, G.1.3) */
+static int arith_segment(struct dec *d, struct comp **sc, int ns) {
+        memset(d->dc_st, 0, sizeof d->dc_st);
+        memset(d->ac_st, 0, sizeof d->ac_st);
+        d->fixed_st = J2P_ARITH_FIXED_STATE;
+        for (int i = 0; i < ns; i++) sc[i]->dc_ctx = 0;
+        if (grow((void **)&d->abuf, &d->abuf_cap, (size_t)(d->end - d->p) + 1, 1) != 0) return fail(d, "could not allocate memory for coefs");
+        const size_t n = unstuff(&d->p, d->end, d->abuf);
+        if (n > 0xffffffffu) return fail(d, "unsupported jpeg: an arithmetic segment of %zu bytes", n);
+        j2p_qm_start(&d->qm, d->abuf, (uint32_t)n);
+        return 0;
+}
+
 /* ---- one scan ------------------------------------------------------------------------------ */
 static int restart(struct dec *d, struct comp **sc, int ns, unsigned *eobrun, int expect) {
         /* byte-align, then RSTn (E.2.4) */
@@ -243,6 +341,7 @@ static int decode_scan(struct dec *d, struct comp **sc, int ns, int ss, int se, 
         d->nbits = 0;
         d->hit_marker = 0;
         for (int i = 0; i < ns; i++) sc[i]->dc_pred = 0;
+        if (d->arith && arith_segment(d, sc, ns) != 0) return -1;
         unsigned eobrun = 0, since_restart = 0;
         int rst = 0;
         const int interleaved = ns > 1;
@@ -253,6 +352,7 @@ static int decode_scan(struct dec *d, struct comp **sc, int ns, int ss, int se, 
                 for (unsigned mx = 0; mx < nmx; mx++) {
                         if (d->restart_interval && since_restart == d->restart_interval) {
                                 if (restart(d, sc, ns, &eobrun, rst++) != 0) return -1;
+                                if (d->arith && arith_segment(d, sc, ns) != 0) return -1;
                                 since_restart = 0;
                         }
                         for (int i = 0; i < ns; i++) {
@@ -263,7 +363,8 @@ static int decode_scan(struct dec *d, struct comp **sc, int ns, int ss, int se, 
                                                 const unsigned bx = interleaved ? mx * c->h + x : mx;
                                                 const unsigned by = interleaved ? my * c->v + y : my;
                                                 int16_t *b = c->blk + ((size_t)by * c->pwb + bx) * 64;
-                                                if (!d->progressive) block_sequential(d, c, b);
+                                                if (d->arith) arith_block(d, c, b, ss, se, ah, al);
+                                                else if (!d->progressive) block_sequential(d, c, b);
                                                 else if (ss == 0) { if (ah == 0) block_dc_first(d, c, b, al); else block_dc_refine(d, b, al); }
                                                 else if (ah == 0) block_ac_first(d, c, b, ss, se, al, &eobrun);
                                                 else block_ac_refine(d, c, b, ss, se, al, &eobrun);
@@ -277,16 +378,6 @@ static int decode_scan(struct dec *d, struct comp **sc, int ns, int ss, int se, 
 }
 
 /* ---- layout pass: one sequential scan cut into segments ------------------------------------ */
-static int grow(void **p, size_t *cap, size_t need, size_t elem) {
-        if (need <= *cap) return 0;
-        size_t n = *cap ? *cap : 4096 / elem + 1;
-        while (n < need) n *= 2;
-        void *q = realloc(*p, n * elem);
-        if (!q) return -1;
-        *p = q;
-        *cap = n;
-        return 0;
-}
 /* S: the scan's descriptor; the segments are appended to *seg (seg_n) and their bytes to *data
  * (data_len), which both layout passes own */
 static int layout_scan(struct dec *d, struct comp **sc, int ns, struct j2p_jpeg_scan *S, struct j2p_jpeg_segment **seg, unsigned *seg_n,
@@ -317,22 +408,9 @@ static int layout_scan(struct dec *d, struct comp **sc, int ns, struct j2p_jpeg_
                 if (grow((void **)data, &d->data_cap, *data_len + (size_t)(d->end - d->p), 1) != 0) return fail(d, "could not allocate memory for coefs");
                 struct j2p_jpeg_segment *g = &(*seg)[(*seg_n)++];
                 g->off = *data_len;
-                uint8_t *o = *data + *data_len;
-                const uint8_t *p = d->p;
-                while (p < d->end) {
-                        const uint8_t *q = memchr(p, 0xFF, (size_t)(d->end - p));
-                        const size_t run = (size_t)((q ? q : d->end) - p);
-                        memcpy(o, p, run);
-                        o += run;
-                        p += run;
-                        if (!q) break;
-                        if (p + 1 < d->end && p[1] == 0x00) { *o++ = 0xFF; p += 2; }
-                        else break;
-                }
-                g->len = (size_t)(o - (*data + *data_len));
+                g->len = unstuff(&d->p, d->end, *data + *data_len);
                 *data_len += g->len;
                 g->mcus = (unsigned)(d->restart_interval && k + 1 < nseg ? d->restart_interval : total - k * (d->restart_interval ? d->restart_interval : 0));
-                d->p = p;
         }
         skip_to_marker(d);
         return 0;
@@ -368,6 +446,18 @@ static int parse_dht(struct dec *d, const uint8_t *s, unsigned len) {
                 if (build_huff(d, h) != 0) return -1;
                 s += 17 + n;
                 len -= 17 + n;
+        }
+        return 0;
+}
+static int parse_dac(struct dec *d, const uint8_t *s, unsigned len) {     /* B.2.4.3, as libjpeg's get_dac */
+        if (len & 1) return fail(d, "corrupt jpeg: bad DAC length");
+        for (; len >= 2; s += 2, len -= 2) {
+                const unsigned index = s[0], val = s[1];
+                if (index >= 32) return fail(d, "corrupt jpeg: bad DAC table index %u", index);
+                if (index >= 16) { d->dac_K[index - 16] = (uint8_t)val; continue; }
+                if ((val & 15) > (val >> 4)) return fail(d, "corrupt jpeg: bad DAC value 0x%02x (L > U)", val);
+                d->dac_L[index] = (uint8_t)(val & 15);
+                d->dac_U[index] = (uint8_t)(val >> 4);
         }
         return 0;
 }
@@ -409,6 +499,15 @@ static int parse_sof(struct dec *d, const uint8_t *s, unsigned len) {
         return 0;
 }
 
+/* T.81's DAC defaults (L = 0, U = 1, Kx = 5), in force from SOI */
+static void dac_defaults(struct dec *d) {
+        for (int t = 0; t < 16; t++) {
+                d->dac_L[t] = 0;
+                d->dac_U[t] = 1;
+                d->dac_K[t] = 5;
+        }
+}
+
 /* The marker loop shared by j2p_read_jpeg_mem and j2p_read_jpeg_layout: reads the headers and
  * decodes every scan (full read) or cuts it into segments (layout pass).  Returns 1 when the layout
  * pass stopped early on a file that is not device-decodable. */
@@ -416,6 +515,7 @@ static int read_markers(struct dec *d, const uint8_t *buf, size_t len) {
         int have_sof = 0, done = 0;
         if (len < 4 || buf[0] != 0xFF || buf[1] != 0xD8) { fail(d, "not a jpeg file (no SOI marker)"); return 0; }
         d->p += 2;
+        dac_defaults(d);
         while (!done && !d->failed) {
                 /* find next marker */
                 while (d->p < d->end && *d->p != 0xFF) d->p++;
@@ -432,13 +532,16 @@ static int read_markers(struct dec *d, const uint8_t *buf, size_t len) {
                 d->p += seglen;
                 if (m == 0xDB) parse_dqt(d, s, sl);
                 else if (m == 0xC4) parse_dht(d, s, sl);
-                else if (m == 0xC0 || m == 0xC1 || m == 0xC2) {
+                else if (m == 0xCC) parse_dac(d, s, sl);
+                else if (m == 0xC0 || m == 0xC1 || m == 0xC2 || m == 0xC9 || m == 0xCA) {
                         if (have_sof) { fail(d, "unsupported jpeg: multiple frames"); break; }
-                        d->progressive = m == 0xC2;
-                        if (d->lay && d->progressive) return 1;
-                        if (d->play && !d->progressive) return 1;
+                        d->progressive = m == 0xC2 || m == 0xCA;
+                        d->arith = m == 0xC9 || m == 0xCA;
+                        if (d->lay && (d->progressive || d->arith)) return 1;
+                        if (d->play && (!d->progressive || d->arith)) return 1;
+                        if (d->alay && (d->progressive || !d->arith)) return 1;
                         if (parse_sof(d, s, sl) == 0) have_sof = 1;
-                } else if (m == 0xC3 || (m >= 0xC5 && m <= 0xC7) || (m >= 0xC9 && m <= 0xCB) || (m >= 0xCD && m <= 0xCF)) {
+                } else if (m == 0xC3 || (m >= 0xC5 && m <= 0xC7) || m == 0xCB || (m >= 0xCD && m <= 0xCF)) {
                         fail(d, "unsupported jpeg: SOF%u (arithmetic, lossless or hierarchical coding)", m - 0xC0);
                 } else if (m == 0xDD) {
                         if (sl < 2) fail(d, "corrupt jpeg: short DRI"); else d->restart_interval = be16(s);
@@ -461,7 +564,7 @@ static int read_markers(struct dec *d, const uint8_t *buf, size_t len) {
                         int ss = s[1 + 2 * ns], se = s[2 + 2 * ns], ah = s[3 + 2 * ns] >> 4, al = s[3 + 2 * ns] & 15;
                         if (!d->progressive) { ss = 0; se = 63; ah = al = 0; }
                         else if (ss > se || se > 63 || (ss == 0 && se != 0) || (ss > 0 && ns != 1) || al > 13) { fail(d, "corrupt jpeg: bad progressive scan parameters"); break; }
-                        for (int i = 0; i < ns; i++) {
+                        for (int i = 0; i < ns && !d->arith; i++) {
                                 if ((ss == 0 && !(d->progressive && ah) && !d->dc[sc[i]->td].present) ||
                                     ((!d->progressive || ss > 0) && !d->ac[sc[i]->ta].present)) { fail(d, "corrupt jpeg: scan uses an undefined huffman table"); break; }
                         }
@@ -484,6 +587,32 @@ static int read_markers(struct dec *d, const uint8_t *buf, size_t len) {
                                 S->ah = (unsigned)ah;
                                 S->al = (unsigned)al;
                                 layout_scan(d, sc, ns, &S->s, &l->seg, &l->nseg, &l->data, &l->data_len);
+                        } else if (d->alay) {
+                                for (int i = 0; i < ns; i++)
+                                        if (d->scans_of[sc[i] - d->c]++) return 1;      /* a component scanned twice */
+                                struct j2p_jpeg_arith_layout *l = d->alay;
+                                struct j2p_jpeg_scan S;
+                                layout_scan(d, sc, ns, &S, &l->seg, &l->nseg, &l->data, &l->data_len);
+                                struct j2p_jpeg_arith_scan *A = &l->scan[l->nscan++];
+                                A->ncomp = S.ncomp;
+                                for (int i = 0; i < 3; i++) {
+                                        A->comp[i] = S.comp[i];
+                                        A->bw[i] = S.bw[i];
+                                        A->bh[i] = S.bh[i];
+                                        A->dc_tbl[i] = A->ac_tbl[i] = A->dc_L[i] = A->dc_U[i] = A->ac_K[i] = 0;
+                                }
+                                for (int i = 0; i < ns; i++) {
+                                        A->dc_tbl[i] = (unsigned)sc[i]->td;
+                                        A->ac_tbl[i] = (unsigned)sc[i]->ta;
+                                        A->dc_L[i] = d->dac_L[sc[i]->td];
+                                        A->dc_U[i] = d->dac_U[sc[i]->td];
+                                        A->ac_K[i] = d->dac_K[sc[i]->ta];
+                                }
+                                A->mcux = S.mcux;
+                                A->mcuy = S.mcuy;
+                                A->restart_interval = S.restart_interval;
+                                A->seg0 = S.seg0;
+                                A->nseg = S.nseg;
                         } else {
                                 decode_scan(d, sc, ns, ss, se, ah, al);
                         }
@@ -545,6 +674,7 @@ int j2p_read_jpeg_mem_ex(const uint8_t *buf, size_t len, unsigned flags, struct 
                 }
         }
         for (int i = 0; i < 3; i++) free(d->c[i].blk);
+        free(d->abuf);
         const int rc = d->failed ? -1 : 0;
         if (rc != 0) for (int i = 0; i < 3; i++) { free(out->coefs[i].data); out->coefs[i].data = NULL; }
         free(d);
@@ -618,6 +748,47 @@ void j2p_free_jpeg_prog_layout(struct j2p_jpeg_prog_layout *l) {
         l->seg = NULL;
         l->data = NULL;
         l->nscan = 0;
+        l->nseg = 0;
+        l->data_len = 0;
+}
+
+int j2p_read_jpeg_arith_layout(const uint8_t *buf, size_t len, struct j2p_jpeg_arith_layout *out, char *err, size_t errlen) {
+        return j2p_read_jpeg_arith_layout_ex(buf, len, 0, out, err, errlen);
+}
+
+int j2p_read_jpeg_arith_layout_ex(const uint8_t *buf, size_t len, unsigned flags, struct j2p_jpeg_arith_layout *out, char *err,
+                                  size_t errlen) {
+        struct dec *d = calloc(1, sizeof *d);
+        if (!d) return -1;
+        d->p = buf; d->end = buf + len; d->err = err; d->errlen = errlen; d->flags = flags;
+        if (err && errlen) err[0] = 0;
+        memset(out, 0, sizeof *out);
+        d->alay = out;
+        const int stopped = read_markers(d, buf, len);
+        int decodable = !stopped && !d->failed;
+        for (int i = 0; i < d->ncomp && decodable; i++) decodable = d->scans_of[i] == 1;
+        if (decodable) {
+                check_planes(d, out->coefs);
+                out->w = d->W;
+                out->h = d->H;
+                out->ncomp = (unsigned)d->ncomp;
+                for (int i = 0; i < d->ncomp; i++) { out->comp_h[i] = (unsigned)d->c[i].h; out->comp_v[i] = (unsigned)d->c[i].v; }
+        }
+        const int rc = d->failed ? -1 : 0;
+        out->arith_decodable = rc == 0 && decodable;
+        if (!out->arith_decodable) {
+                j2p_free_jpeg_arith_layout(out);
+                out->nscan = 0;
+        }
+        free(d);
+        return rc;
+}
+
+void j2p_free_jpeg_arith_layout(struct j2p_jpeg_arith_layout *l) {
+        free(l->seg);
+        free(l->data);
+        l->seg = NULL;
+        l->data = NULL;
         l->nseg = 0;
         l->data_len = 0;
 }

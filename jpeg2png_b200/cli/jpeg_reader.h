@@ -11,8 +11,18 @@
  * (jpeg.c:41-45), component sizes that do not match the sampling factors (jpeg.c:59-64).
  *
  * Supported: baseline and extended sequential Huffman (SOF0, SOF1), progressive Huffman (SOF2),
- * 8-bit precision, restart intervals, interleaved and non-interleaved scans.  Not supported:
- * arithmetic coding, lossless, hierarchical, 12-bit.
+ * sequential and progressive arithmetic coding (SOF9, SOF10, with DAC conditioning), 8-bit
+ * precision, restart intervals, interleaved and non-interleaved scans.  Not supported: lossless,
+ * hierarchical, 12-bit (SOF3, SOF5-7, SOF11, SOF13-15: "unsupported jpeg: SOFn ...").
+ *
+ * Arithmetic coding follows libjpeg's jdarith.c (the QM decoder and sequential block step are
+ * ../arith/arith_core.h).  DAC segments are refused where libjpeg's get_dac refuses them: an odd
+ * length, a table index of 32 or more, L > U; any Kx byte is accepted.  One difference: libjpeg
+ * accepts arithmetic table selectors up to 15, this reader refuses selectors above 3 for every
+ * scan ("bad table selector").  Another: a segment's bytes end at the first FF not followed by 00,
+ * as for Huffman scans, where libjpeg's arithmetic decoder skips FF fill bytes and reads FF FF 00
+ * as one FF (encoders do not write that sequence inside entropy-coded data).  A magnitude category reaching 2^15 or a zero run or refinement past
+ * the band's end is "corrupt jpeg: bad arithmetic code" where libjpeg warns and stops decoding.
  */
 #ifndef J2P_JPEG_READER_H
 #define J2P_JPEG_READER_H
@@ -52,8 +62,8 @@ int j2p_read_jpeg_mem_ex(const uint8_t *buf, size_t len, unsigned flags, struct 
  *
  * device_decodable: the file is sequential Huffman (SOF0/SOF1) and each of its components is in
  * exactly one scan.  Only then are coefs (geometry and tables, data NULL), scans and segments
- * filled; for every other file the pass stops as soon as that is known (a progressive SOF, a
- * component's second scan) and returns 0 with device_decodable = 0: such files are for
+ * filled; for every other file the pass stops as soon as that is known (a progressive or
+ * arithmetic SOF, a component's second scan) and returns 0 with device_decodable = 0: such files are for
  * j2p_read_jpeg_mem.  A non-zero return means j2p_read_jpeg_mem rejects the file too (it may name an
  * earlier error, in the entropy-coded data). */
 struct j2p_jpeg_huff {
@@ -120,6 +130,41 @@ int j2p_read_jpeg_prog_layout(const uint8_t *buf, size_t len, struct j2p_jpeg_pr
 int j2p_read_jpeg_prog_layout_ex(const uint8_t *buf, size_t len, unsigned flags, struct j2p_jpeg_prog_layout *out, char *err,
                                  size_t errlen);
 void j2p_free_jpeg_prog_layout(struct j2p_jpeg_prog_layout *l);
+
+/* ---- arithmetic layout pass: a sequential arithmetic-coded file, cut as above ----
+ *
+ * j2p_read_jpeg_arith_layout runs the same marker loop and header checks and cuts every scan of a
+ * sequential arithmetic (SOF9) file into segments as j2p_read_jpeg_layout does.  Instead of Huffman
+ * tables each scan records, per component, its table selectors (components with equal selectors
+ * share statistics) and the conditioning in force at its SOS: L and U of its DC table, Kx of its AC
+ * table.  arith_decodable: the file is SOF9 and each of its components is in exactly one scan; every
+ * other file stops as soon as that is known and returns 0 with arith_decodable = 0.  A non-zero
+ * return means j2p_read_jpeg_mem rejects the file too.  The existing layout passes report SOF9 and
+ * SOF10 files as not device_decodable / progressive_decodable. */
+struct j2p_jpeg_arith_scan {
+        unsigned ncomp, comp[3], bw[3], bh[3];  /* as struct j2p_jpeg_scan */
+        unsigned mcux, mcuy, restart_interval;
+        unsigned dc_tbl[3], ac_tbl[3];          /* table selectors (0..3) */
+        unsigned dc_L[3], dc_U[3], ac_K[3];     /* DAC conditioning of those tables */
+        unsigned seg0, nseg;
+};
+struct j2p_jpeg_arith_layout {
+        unsigned w, h;
+        struct coef coefs[3];       /* as struct j2p_jpeg, but data NULL */
+        unsigned comp_h[3], comp_v[3];
+        int arith_decodable;
+        unsigned nscan;
+        struct j2p_jpeg_arith_scan scan[3];
+        unsigned nseg;
+        struct j2p_jpeg_segment *seg;    /* malloc'd */
+        uint8_t *data;                   /* malloc'd */
+        size_t data_len;
+        unsigned ncomp;                  /* set when arith_decodable */
+};
+int j2p_read_jpeg_arith_layout(const uint8_t *buf, size_t len, struct j2p_jpeg_arith_layout *out, char *err, size_t errlen);
+int j2p_read_jpeg_arith_layout_ex(const uint8_t *buf, size_t len, unsigned flags, struct j2p_jpeg_arith_layout *out, char *err,
+                                  size_t errlen);
+void j2p_free_jpeg_arith_layout(struct j2p_jpeg_arith_layout *l);
 
 /* ---- EXIF orientation ----
  * The Orientation tag (0x0112) of IFD0 in the first APP1 segment that starts with "Exif\0\0" before

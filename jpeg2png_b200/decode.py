@@ -3,7 +3,10 @@
 Every input's headers are read on the host with the JPEG reader of the command line
 (libj2pcodecs.so) before any device work: sequential files whose components are each in one scan
 go through its layout pass (j2p_read_jpeg_layout) and are Huffman-decoded on the device
-(libj2pentropy.so, DESIGN §7d); every other file is parsed by j2p_read_jpeg_mem.  Inputs of one geometry are solved
+(libj2pentropy.so, DESIGN §7d); arithmetic-coded sequential (SOF9) files of that shape go through
+j2p_read_jpeg_arith_layout and, per batch, are decoded on the device one restart segment per thread
+(libj2parith.so, DESIGN §7p) when that is expected to beat the host reader (arith_on_device); every other file, progressive arithmetic (SOF10)
+ones included, is parsed by j2p_read_jpeg_mem.  Inputs of one geometry are solved
 together in batch sessions (j2p_session_create_batch), with the conventional decode on the device as
 the command line does it, and the colour conversion writes straight into one freshly allocated tensor
 per chunk (j2p_session_export) on the caller's current stream.  The returned tensors of a chunk are
@@ -84,6 +87,27 @@ class ProgLayout(C.Structure):
                 ('data', C.POINTER(C.c_uint8)), ('data_len', C.c_size_t), ('ncomp', C.c_uint)]
 
 
+class ArithScan(C.Structure):
+    """struct j2p_jpeg_arith_scan — jpeg2png_b200/cli/jpeg_reader.h."""
+    _fields_ = [('ncomp', C.c_uint), ('comp', C.c_uint * 3), ('bw', C.c_uint * 3), ('bh', C.c_uint * 3),
+                ('mcux', C.c_uint), ('mcuy', C.c_uint), ('restart_interval', C.c_uint),
+                ('dc_tbl', C.c_uint * 3), ('ac_tbl', C.c_uint * 3), ('dc_L', C.c_uint * 3), ('dc_U', C.c_uint * 3),
+                ('ac_K', C.c_uint * 3), ('seg0', C.c_uint), ('nseg', C.c_uint)]
+
+
+class ArithLayout(C.Structure):
+    """struct j2p_jpeg_arith_layout — jpeg2png_b200/cli/jpeg_reader.h."""
+    _fields_ = [('w', C.c_uint), ('h', C.c_uint), ('coefs', abi.Coef * 3), ('comp_h', C.c_uint * 3),
+                ('comp_v', C.c_uint * 3), ('arith_decodable', C.c_int), ('nscan', C.c_uint), ('scan', ArithScan * 3),
+                ('nseg', C.c_uint), ('seg', C.POINTER(Segment)), ('data', C.POINTER(C.c_uint8)),
+                ('data_len', C.c_size_t), ('ncomp', C.c_uint)]
+
+
+class ArithStats(C.Structure):
+    """struct j2p_arith_stats — jpeg2png_b200/arith/arith.h."""
+    _fields_ = [('launches', C.c_uint), ('segments', C.c_uint)]
+
+
 class EntropyStats(C.Structure):
     """struct j2p_entropy_stats — jpeg2png_b200/entropy/entropy.h."""
     _fields_ = [('rounds', C.c_uint), ('round_trips', C.c_uint), ('launches', C.c_uint), ('subsequences', C.c_uint)]
@@ -99,6 +123,14 @@ PROGRESSIVE_LIB = os.path.join(abi._PKG_DIR, 'progressive', 'libj2pprogressive.s
 ENTROPY_LIB = os.path.join(abi._PKG_DIR, 'entropy', 'libj2pentropy.so')
 SUBSEQ_BITS = 1024                  # bits per subsequence of the device decoder (DESIGN §7d)
 ENT_FAILURES = {1: 'bad huffman code', 2: 'bad magnitude category', 3: 'coefficient index out of range'}
+ARITH_LIB = os.path.join(abi._PKG_DIR, 'arith', 'libj2parith.so')
+ARITH_FAILURES = {1: 'bad arithmetic code'}
+# The routing rule of arithmetic-coded files (DESIGN §7p, arith_on_device).  One device call decodes
+# every segment of a chunk at once, one thread each, so it lasts about as long as the serial walk of
+# the chunk's longest segment; the host reader pays for every byte of every file, on the threads of
+# decode_jpeg's pool.  Both rates measured on an H100 80GB HBM3 and its host (tools/arith_bench.py).
+ARITH_DEVICE_NS_PER_BYTE = 3800     # one device thread walking a segment
+ARITH_HOST_NS_PER_BYTE = 190        # j2p_read_jpeg_mem on one host thread
 
 class Keep(C.Structure):
     """struct j2p_jpeg_keep — jpeg2png_b200/cli/jpeg_reader.h."""
@@ -125,6 +157,10 @@ def _declare_codecs(lib):
     lib.j2p_free_jpeg_prog_layout.argtypes = [C.POINTER(ProgLayout)]
     lib.j2p_jpeg_exif_orientation.restype = C.c_int
     lib.j2p_jpeg_exif_orientation.argtypes = [C.c_char_p, C.c_size_t]
+    lib.j2p_read_jpeg_arith_layout_ex.restype = C.c_int
+    lib.j2p_read_jpeg_arith_layout_ex.argtypes = [C.c_char_p, C.c_size_t, C.c_uint, C.POINTER(ArithLayout), C.c_char_p, C.c_size_t]
+    lib.j2p_free_jpeg_arith_layout.restype = None
+    lib.j2p_free_jpeg_arith_layout.argtypes = [C.POINTER(ArithLayout)]
     lib.j2p_jpeg_keep_settings.restype = C.c_int
     lib.j2p_jpeg_keep_settings.argtypes = [C.c_char_p, C.c_size_t, C.POINTER(Keep), C.c_char_p, C.c_size_t]
 
@@ -151,6 +187,25 @@ def _declare_entropy(lib):
 def load_entropy() -> C.CDLL:
     """libj2pentropy.so (the device entropy decoder) from the package tree."""
     return abi.load_library(ENTROPY_LIB, 'entropy decoder', _declare_entropy)
+
+
+def _declare_arith(lib):
+    vp, lay = C.c_void_p, C.POINTER(C.POINTER(ArithLayout))
+    lib.j2p_arith_plan_size.restype = C.c_int
+    lib.j2p_arith_plan_size.argtypes = [lay, C.c_uint, C.POINTER(C.c_size_t), C.POINTER(C.c_size_t)]
+    lib.j2p_arith_pack.restype = C.c_int
+    lib.j2p_arith_pack.argtypes = [lay, C.c_uint, C.POINTER(vp), vp, C.c_size_t]
+    lib.j2p_arith_decode.restype = C.c_int
+    lib.j2p_arith_decode.argtypes = [vp, vp, vp, vp, vp, C.POINTER(ArithStats)]
+    lib.j2p_arith_decode_host.restype = C.c_int
+    lib.j2p_arith_decode_host.argtypes = [vp, vp, vp, C.POINTER(ArithStats)]
+    lib.j2p_arith_last_error.restype = C.c_char_p
+    lib.j2p_arith_last_error.argtypes = []
+
+
+def load_arith() -> C.CDLL:
+    """libj2parith.so (the device decoder of sequential arithmetic-coded files) from the package tree."""
+    return abi.load_library(ARITH_LIB, 'arithmetic decoder', _declare_arith)
 
 
 def _declare_progressive(lib):
@@ -224,6 +279,46 @@ class ProgFileLayout:
             pass
 
 
+class ArithFileLayout:
+    """A sequential arithmetic-coded file's layout (j2p_read_jpeg_arith_layout_ex with the J2P_READ_*
+    `flags`); frees the C buffers when collected.  longest_segment: the bytes of its longest segment
+    (0 when not arith_decodable)."""
+
+    def __init__(self, data: bytes, flags: int = 0):
+        lib = load_codecs()
+        self.lay = ArithLayout()
+        err = C.create_string_buffer(256)
+        if lib.j2p_read_jpeg_arith_layout_ex(data, len(data), flags, C.byref(self.lay), err, 256) != 0:
+            raise ValueError(err.value.decode(errors='replace'))
+        self.arith_decodable = bool(self.lay.arith_decodable)
+        self.w, self.h = int(self.lay.w), int(self.lay.h)
+        self.compressed = int(self.lay.data_len)
+        self.longest_segment = max((int(self.lay.seg[k].len) for k in range(self.lay.nseg)), default=0)
+        self.planes = [Plane(int(c.w), int(c.h), int(c.w_samp), int(c.h_samp), None,
+                             np.array(list(c.quant_table), np.uint16)) for c in self.lay.coefs[:self.lay.ncomp]]
+
+    def key(self):
+        return Parsed.key(self)
+
+    def __del__(self):
+        try:
+            load_codecs().j2p_free_jpeg_arith_layout(C.byref(self.lay))
+        except Exception:
+            pass
+
+
+def arith_on_device(layouts, workers: int) -> bool:
+    """Whether one device call on the ArithFileLayouts of a chunk is expected to beat the host reader
+    running on min(workers, len(layouts)) threads: the serial walk of the longest segment against
+    the host's share of all their bytes.  Files without restart intervals are one segment each, so a
+    chunk of them goes to the device only when it holds many more files than there are threads; a
+    file cut into many restart intervals goes there even alone."""
+    longest = max(lay.longest_segment for lay in layouts)
+    total = sum(lay.compressed for lay in layouts)
+    threads = max(1, min(int(workers), len(layouts)))
+    return longest * ARITH_DEVICE_NS_PER_BYTE < total * ARITH_HOST_NS_PER_BYTE / threads
+
+
 def _layout_ptrs(layouts):
     return (C.POINTER(Layout) * len(layouts))(*[C.pointer(x.lay) for x in layouts])
 
@@ -267,6 +362,26 @@ def progressive_plan(layouts, outs, subseq_bits=SUBSEQ_BITS, pinned=False):
     o = (C.c_void_p * len(outs))(*outs)
     if lib.j2p_progressive_pack(ptrs, len(layouts), subseq_bits, o, addr, plan_bytes.value) != 0:
         raise RuntimeError(lib.j2p_progressive_last_error().decode())
+    return buf, addr, plan_bytes.value, work_bytes.value
+
+
+def arith_plan(layouts, outs, subseq_bits=None, pinned=False):
+    """entropy_plan for ArithFileLayouts and libj2parith.so (subseq_bits: unused, the decoder works
+    per segment)."""
+    lib = load_arith()
+    ptrs = (C.POINTER(ArithLayout) * len(layouts))(*[C.pointer(x.lay) for x in layouts])
+    plan_bytes, work_bytes = C.c_size_t(), C.c_size_t()
+    if lib.j2p_arith_plan_size(ptrs, len(layouts), C.byref(plan_bytes), C.byref(work_bytes)) != 0:
+        raise RuntimeError(lib.j2p_arith_last_error().decode())
+    if pinned:
+        buf = torch.empty(plan_bytes.value, dtype=torch.uint8, pin_memory=True)
+        addr = buf.data_ptr()
+    else:
+        buf = np.zeros(plan_bytes.value + 16, np.uint8)
+        addr = (buf.ctypes.data + 15) & ~15
+    o = (C.c_void_p * len(outs))(*outs)
+    if lib.j2p_arith_pack(ptrs, len(layouts), o, addr, plan_bytes.value) != 0:
+        raise RuntimeError(lib.j2p_arith_last_error().decode())
     return buf, addr, plan_bytes.value, work_bytes.value
 
 
@@ -544,6 +659,13 @@ class _ProgCoefs(_DeviceCoefs):
                      ProgressiveStats())
 
 
+class _ArithCoefs(_DeviceCoefs):
+    """_DeviceCoefs for sequential arithmetic-coded files (ArithFileLayout), decoded by libj2parith.so."""
+
+    def __init__(self, device, layouts, stream, subseq_bits=None):
+        self._decode(device, layouts, stream, subseq_bits, arith_plan, load_arith(), 'arith', ArithStats())
+
+
 class _Chunk:
     """The batch session(s) of one chunk: created, uploaded, iterated and exported by the
     constructor; close() waits for them and returns their blocks to the device cache.
@@ -666,10 +788,11 @@ def _where(i, path):
 
 
 def _front_end(data, device_ok, progressive=False, flags=0):
-    """The host part of one input: a FileLayout for the device decoder, a ProgFileLayout for the
-    progressive device decoder (progressive=True), a Parsed from the host reader, or the ValueError
-    (always the host reader's message) or RuntimeError to raise.  flags: J2P_READ_*, for every
-    reader."""
+    """The host part of one input: a FileLayout for the device decoder, an ArithFileLayout for the
+    arithmetic device decoder (a SOF9 file whose components are each in one scan; decode_jpeg sends
+    a chunk's ArithFileLayouts back to the host reader when arith_on_device says so), a ProgFileLayout for the progressive device decoder (progressive=True), a Parsed from the host
+    reader, or the ValueError (always the host reader's message) or RuntimeError to raise.  flags:
+    J2P_READ_*, for every reader."""
     if not device_ok or _host_front_end:
         try:
             return parse_jpeg(data, flags)
@@ -685,6 +808,16 @@ def _front_end(data, device_ok, progressive=False, flags=0):
         return RuntimeError('the layout pass rejected a file the host reader accepts')
     if lay.device_decodable:
         return lay
+    try:
+        ari = ArithFileLayout(data, flags)
+    except ValueError:
+        try:
+            parse_jpeg(data, flags)
+        except ValueError as e:
+            return e
+        return RuntimeError('the arithmetic layout pass rejected a file the host reader accepts')
+    if ari.arith_decodable:
+        return ari
     if progressive:
         try:
             prog = ProgFileLayout(data, flags)
@@ -731,7 +864,11 @@ def decode_jpeg(inputs, *, iterations=50, weight=0.3, pweight=0.001, separate=Fa
     be used there without synchronising.
 
     Sequential (baseline or extended) files whose components are each coded in one scan are
-    Huffman-decoded on the device: only their compressed bytes are uploaded.  progressive_on_device:
+    Huffman-decoded on the device: only their compressed bytes are uploaded.  Arithmetic-coded files
+    (SOF9, SOF10, as `jpegtran -arithmetic` writes them) give the pixels of their Huffman originals:
+    SOF9 files of that shape are decoded on the device (libj2parith.so, DESIGN §7p) when one device
+    call on the batch's arithmetic files is expected to beat the host reader (arith_on_device: their
+    longest restart segment against all their bytes), the others on the host.  progressive_on_device:
     progressive files are Huffman-decoded on the device too (libj2pprogressive.so, DESIGN §7g);
     by default they are parsed on the host, as is every other file.  Raises ValueError for bad arguments and
     unreadable files, with the host reader's message: header errors before any device work, errors
@@ -816,6 +953,31 @@ def decode_jpeg(inputs, *, iterations=50, weight=0.3, pweight=0.001, separate=Fa
         chunks = plan([p.key() for p in parsed],
                       lambda k: chunk_frames(k, separate, sample_bytes, max_frames, free, mode))
 
+    # A chunk's arithmetic files are one device call, as long as the walk of their longest segment:
+    # where the host reader is expected to be faster (arith_on_device) they are parsed there instead.
+    # Their headers were read by the layout pass; errors in their entropy-coded data come here, before
+    # any device work.
+    to_host = []
+    for _, idx in chunks:
+        ari = [i for i in idx if isinstance(parsed[i], ArithFileLayout)]
+        if ari and not arith_on_device([parsed[i] for i in ari], workers):
+            to_host.extend(ari)
+    if to_host:
+        def host_parse(i):
+            try:
+                return parse_jpeg(read[i][0], read_flags)
+            except ValueError as e:
+                return e
+        if min(workers, len(to_host)) > 1:
+            with ThreadPoolExecutor(min(workers, len(to_host))) as pool:
+                reparsed = list(pool.map(host_parse, to_host))
+        else:
+            reparsed = [host_parse(i) for i in to_host]
+        for i, p in zip(to_host, reparsed):
+            if isinstance(p, ValueError):
+                raise ValueError(f'{_where(i, read[i][1])}: {p}')
+            parsed[i] = p
+
     # packs of chunks iterated in one group; a pack of one chunk is solved as the chunk alone.  Groups
     # refuse recording sessions: with return_objective every chunk is solved alone.
     if _group_chunks and not return_objective:
@@ -837,7 +999,8 @@ def decode_jpeg(inputs, *, iterations=50, weight=0.3, pweight=0.001, separate=Fa
 
             def chunk_coefs(idx):
                 coefs = {}
-                for kind, decoder in ((FileLayout, _DeviceCoefs), (ProgFileLayout, _ProgCoefs)):
+                for kind, decoder, failures in ((FileLayout, _DeviceCoefs, ENT_FAILURES), (ProgFileLayout, _ProgCoefs, ENT_FAILURES),
+                                                (ArithFileLayout, _ArithCoefs, ARITH_FAILURES)):
                     on_dev = [j for j, i in enumerate(idx) if isinstance(parsed[i], kind)]
                     if not on_dev:
                         continue
@@ -851,7 +1014,7 @@ def decode_jpeg(inputs, *, iterations=50, weight=0.3, pweight=0.001, separate=Fa
                             except ValueError as e:
                                 raise ValueError(f'{where}: {e}') from None
                             raise RuntimeError(f'{where}: the device entropy decoder failed '
-                                               f'({ENT_FAILURES.get(int(dc.status[k]), int(dc.status[k]))}) on a file '
+                                               f'({failures.get(int(dc.status[k]), int(dc.status[k]))}) on a file '
                                                'the host reader accepts (a decoder bug)')
                         coefs[j] = (dc, k)
                 return coefs
