@@ -309,6 +309,24 @@ int j2p_session_export_gray(j2p_session *s, unsigned frame0, unsigned nframes,
 int j2p_session_export_oriented(j2p_session *const *sessions, unsigned nsessions, unsigned channels,
                                 unsigned frame0, unsigned nframes, const unsigned char *orientation,
                                 const struct j2p_image_out *o, void *dst, void *stream);
+/* Four-component JPEGs (Adobe CMYK and YCCK files): the frames of `nframes` files from file frame0 on,
+ * one launch on `stream` ordered with the sessions as the exports above.  The four planes of a file
+ * come from `sessions` in channel order; session k holds q_k planes of every file, q_k = its nchannel
+ * times its frames over the file count N, and the q_k add up to 4 (N: the sessions' planes over 4).
+ * So four nchannel == 1 sessions of N frames, one of 4N frames (file f's plane c is its frame
+ * 4f + c), or for YCCK an nchannel == 3 session of N frames followed by a nchannel == 1 one.
+ * kind J2P_FOUR_CMYK: channel c = the inverse of plane c's gray sample (the gray export's sample g,
+ * 255 - g at 8 bits, 65535 - g at 16, 255.f - g at 32).  J2P_FOUR_YCCK: channels 0-2 the RGB
+ * samples of planes 0-2, channel 3 the inverse of plane 3's gray sample.  channels 4 writes these;
+ * channels 3 (sample 8 only) writes Pillow's CMYK -> RGB of the 8-bit samples: nk = 255 - K,
+ * t = x * nk + 128, each of R, G, B = clip(nk - ((t + (t >> 8)) >> 8), 0, 255).
+ * orientation: NULL writes every frame upright as j2p_session_export does; otherwise per-file EXIF
+ * orientations in device memory, as j2p_session_export_oriented.  Returns J2P_ERR_ARG for what the
+ * other exports refuse and for a kind, channel count or session set that is none of the above. */
+enum { J2P_FOUR_CMYK = 1, J2P_FOUR_YCCK = 2 };
+int j2p_session_export_four(j2p_session *const *sessions, unsigned nsessions, unsigned kind, unsigned channels,
+                            unsigned frame0, unsigned nframes, const unsigned char *orientation,
+                            const struct j2p_image_out *o, void *dst, void *stream);
 
 /* Iterations [first, first + count) of every frame of every session of `sessions`, in one launch chain:
  * each kernel of an iteration is launched once for all n sessions, whatever their frame sizes, on the

@@ -167,6 +167,8 @@ def declare_product(lib: C.CDLL) -> C.CDLL:
     lib.j2p_session_export_gray.argtypes = [vp, C.c_uint, C.c_uint, C.POINTER(ImageOut), vp, vp]
     lib.j2p_session_export_oriented.restype = C.c_int
     lib.j2p_session_export_oriented.argtypes = [C.POINTER(vp), C.c_uint, C.c_uint, C.c_uint, C.c_uint, vp, C.POINTER(ImageOut), vp, vp]
+    lib.j2p_session_export_four.restype = C.c_int
+    lib.j2p_session_export_four.argtypes = [C.POINTER(vp), C.c_uint, C.c_uint, C.c_uint, C.c_uint, C.c_uint, vp, C.POINTER(ImageOut), vp, vp]
     lib.j2p_session_iterate_group.restype = C.c_int
     lib.j2p_session_iterate_group.argtypes = [C.POINTER(vp), C.c_uint, C.c_uint, C.c_uint]
     lib.j2p_session_create_strip.restype = C.c_int
@@ -250,7 +252,7 @@ HEADER_SYMBOLS = [
     'j2p_session_launches', 'j2p_version', 'j2p_host_prefault', 'j2p_set_thread_device', 'j2p_thread_device', 'j2p_session_download_scanlines',
     'j2p_session_create_batch', 'j2p_session_frames', 'j2p_session_download_frame_scanlines',
     'j2p_session_export', 'j2p_session_export_separate', 'j2p_session_upload_device',
-    'j2p_session_export_gray', 'j2p_session_export_oriented', 'j2p_session_iterate_group',
+    'j2p_session_export_gray', 'j2p_session_export_oriented', 'j2p_session_export_four', 'j2p_session_iterate_group',
     'j2p_session_record_objective', 'j2p_session_objective_history',
 ]
 

@@ -43,8 +43,10 @@ struct dec {
         uint16_t qt[4][64];       /* natural order */
         int qt_present[4];
         struct huff dc[4], ac[4];
-        struct comp c[3];
+        struct comp c[4];
         int ncomp, progressive;
+        int adobe_transform;           /* the last Adobe APP14 segment's transform before the first SOS, -1 without one */
+        int seen_sos;
         int arith;                     /* SOF9/SOF10: arithmetic coding */
         uint8_t dac_L[16], dac_U[16], dac_K[16];   /* DAC conditioning, T.81's defaults until a DAC sets them */
         uint8_t dc_st[4][J2P_ARITH_DC_BINS], ac_st[4][J2P_ARITH_AC_BINS];   /* the statistics of the current segment */
@@ -59,7 +61,8 @@ struct dec {
         size_t errlen;
         int failed;
         struct j2p_jpeg_layout *lay;   /* the layout pass (j2p_read_jpeg_layout), NULL for a full read */
-        unsigned scans_of[3];          /* layout pass: scans that name each component */
+        struct j2p_jpeg_layout4 *lay4; /* the four-plane layout pass (j2p_read_jpeg_layout4) */
+        unsigned scans_of[4];          /* layout pass: scans that name each component */
         struct j2p_jpeg_prog_layout *play;   /* the progressive layout pass (j2p_read_jpeg_prog_layout) */
         struct j2p_jpeg_arith_layout *alay;  /* the arithmetic layout pass (j2p_read_jpeg_arith_layout) */
         int headers_only;              /* j2p_jpeg_keep_settings: stop at the first SOS */
@@ -380,7 +383,7 @@ static int decode_scan(struct dec *d, struct comp **sc, int ns, int ss, int se, 
 /* ---- layout pass: one sequential scan cut into segments ------------------------------------ */
 /* S: the scan's descriptor; the segments are appended to *seg (seg_n) and their bytes to *data
  * (data_len), which both layout passes own */
-static int layout_scan(struct dec *d, struct comp **sc, int ns, struct j2p_jpeg_scan *S, struct j2p_jpeg_segment **seg, unsigned *seg_n,
+static int layout_scan(struct dec *d, struct comp **sc, int ns, struct j2p_jpeg_scan4 *S, struct j2p_jpeg_segment **seg, unsigned *seg_n,
                        uint8_t **data, size_t *data_len) {
         const int interleaved = ns > 1;
         S->ncomp = (unsigned)ns;
@@ -414,6 +417,23 @@ static int layout_scan(struct dec *d, struct comp **sc, int ns, struct j2p_jpeg_
         }
         skip_to_marker(d);
         return 0;
+}
+
+/* a scan of at most three components as the three-component layouts store it */
+static void narrow_scan(const struct j2p_jpeg_scan4 *S4, struct j2p_jpeg_scan *S) {
+        S->ncomp = S4->ncomp;
+        for (int i = 0; i < 3; i++) {
+                S->comp[i] = S4->comp[i];
+                S->bw[i] = S4->bw[i];
+                S->bh[i] = S4->bh[i];
+                S->dc[i] = S4->dc[i];
+                S->ac[i] = S4->ac[i];
+        }
+        S->mcux = S4->mcux;
+        S->mcuy = S4->mcuy;
+        S->restart_interval = S4->restart_interval;
+        S->seg0 = S4->seg0;
+        S->nseg = S4->nseg;
 }
 
 /* ---- marker segments ----------------------------------------------------------------------- */
@@ -467,7 +487,9 @@ static int parse_sof(struct dec *d, const uint8_t *s, unsigned len) {
         d->H = be16(s + 1);
         d->W = be16(s + 3);
         d->ncomp = s[5];
-        if (d->flags & J2P_READ_GRAY) {
+        if (d->flags & J2P_READ_CMYK) {
+                if (d->ncomp != 1 && d->ncomp != 3 && d->ncomp != 4) return fail(d, "only 1, 3 and 4 component jpegs are supported");
+        } else if (d->flags & J2P_READ_GRAY) {
                 if (d->ncomp != 1 && d->ncomp != 3) return fail(d, "only 1 and 3 component jpegs are supported");
         } else if (d->ncomp != 3) return fail(d, "only 3 component jpegs are supported");    /* jpeg.c:34 */
         if (d->W == 0 || d->H == 0) return fail(d, "unsupported jpeg: empty image or DNL-defined height");
@@ -492,7 +514,7 @@ static int parse_sof(struct dec *d, const uint8_t *s, unsigned len) {
                 c->hb = (ch + 7) / 8;
                 c->pwb = d->mcux * c->h;
                 c->phb = d->mcuy * c->v;
-                if (d->lay || d->play || d->headers_only) continue;                                     /* the layout passes store no blocks */
+                if (d->lay || d->lay4 || d->play || d->headers_only) continue;                                     /* the layout passes store no blocks */
                 c->blk = calloc((size_t)c->pwb * c->phb * 64, sizeof(int16_t));
                 if (!c->blk) return fail(d, "could not allocate memory for coefs");                /* jpeg.c:69 */
         }
@@ -516,6 +538,7 @@ static int read_markers(struct dec *d, const uint8_t *buf, size_t len) {
         if (len < 4 || buf[0] != 0xFF || buf[1] != 0xD8) { fail(d, "not a jpeg file (no SOI marker)"); return 0; }
         d->p += 2;
         dac_defaults(d);
+        d->adobe_transform = -1;
         while (!done && !d->failed) {
                 /* find next marker */
                 while (d->p < d->end && *d->p != 0xFF) d->p++;
@@ -537,21 +560,26 @@ static int read_markers(struct dec *d, const uint8_t *buf, size_t len) {
                         if (have_sof) { fail(d, "unsupported jpeg: multiple frames"); break; }
                         d->progressive = m == 0xC2 || m == 0xCA;
                         d->arith = m == 0xC9 || m == 0xCA;
-                        if (d->lay && (d->progressive || d->arith)) return 1;
+                        if ((d->lay || d->lay4) && (d->progressive || d->arith)) return 1;
                         if (d->play && (!d->progressive || d->arith)) return 1;
                         if (d->alay && (d->progressive || !d->arith)) return 1;
+                        if ((d->lay || d->play || d->alay) && (d->flags & J2P_READ_CMYK) && sl >= 6 && s[5] == 4) return 1;   /* four components: host reader */
                         if (parse_sof(d, s, sl) == 0) have_sof = 1;
                 } else if (m == 0xC3 || (m >= 0xC5 && m <= 0xC7) || m == 0xCB || (m >= 0xCD && m <= 0xCF)) {
                         fail(d, "unsupported jpeg: SOF%u (arithmetic, lossless or hierarchical coding)", m - 0xC0);
+                } else if (m == 0xEE) {
+                        /* Adobe APP14 (libjpeg's examine_app14): 12 data bytes or more, "Adobe", transform at byte 11 */
+                        if (!d->seen_sos && sl >= 12 && memcmp(s, "Adobe", 5) == 0) d->adobe_transform = s[11];
                 } else if (m == 0xDD) {
                         if (sl < 2) fail(d, "corrupt jpeg: short DRI"); else d->restart_interval = be16(s);
                 } else if (m == 0xDA) {
                         if (!have_sof) { fail(d, "corrupt jpeg: scan before frame header"); break; }
                         if (d->headers_only) break;
+                        d->seen_sos = 1;
                         if (sl < 1) { fail(d, "corrupt jpeg: short SOS"); break; }
                         const int ns = s[0];
-                        if (ns < 1 || ns > 3 || sl < 1 + 2u * ns + 3) { fail(d, "corrupt jpeg: bad SOS"); break; }
-                        struct comp *sc[3];
+                        if (ns < 1 || ns > (d->ncomp == 4 ? 4 : 3) || sl < 1 + 2u * ns + 3) { fail(d, "corrupt jpeg: bad SOS"); break; }
+                        struct comp *sc[4];
                         for (int i = 0; i < ns; i++) {
                                 sc[i] = NULL;
                                 for (int k = 0; k < d->ncomp; k++) if (d->c[k].id == s[1 + 2 * i]) sc[i] = &d->c[k];
@@ -561,6 +589,11 @@ static int read_markers(struct dec *d, const uint8_t *buf, size_t len) {
                                 if (sc[i]->td > 3 || sc[i]->ta > 3) fail(d, "corrupt jpeg: bad table selector");
                         }
                         if (d->failed) break;
+                        if (d->ncomp == 4 && ns > 1) {          /* libjpeg's D_MAX_BLOCKS_IN_MCU, for the files this reader took from it */
+                                int bpm = 0;
+                                for (int i = 0; i < ns; i++) bpm += sc[i]->h * sc[i]->v;
+                                if (bpm > 10) { fail(d, "unsupported jpeg: %d blocks per MCU (at most 10)", bpm); break; }
+                        }
                         int ss = s[1 + 2 * ns], se = s[2 + 2 * ns], ah = s[3 + 2 * ns] >> 4, al = s[3 + 2 * ns] & 15;
                         if (!d->progressive) { ss = 0; se = 63; ah = al = 0; }
                         else if (ss > se || se > 63 || (ss == 0 && se != 0) || (ss > 0 && ns != 1) || al > 13) { fail(d, "corrupt jpeg: bad progressive scan parameters"); break; }
@@ -569,10 +602,18 @@ static int read_markers(struct dec *d, const uint8_t *buf, size_t len) {
                                     ((!d->progressive || ss > 0) && !d->ac[sc[i]->ta].present)) { fail(d, "corrupt jpeg: scan uses an undefined huffman table"); break; }
                         }
                         if (d->failed) break;
+                        struct j2p_jpeg_scan4 S4;
+                        memset(&S4, 0, sizeof S4);
                         if (d->lay) {
                                 for (int i = 0; i < ns; i++)
                                         if (d->scans_of[sc[i] - d->c]++) return 1;      /* a component scanned twice */
                                 struct j2p_jpeg_layout *l = d->lay;
+                                layout_scan(d, sc, ns, &S4, &l->seg, &l->nseg, &l->data, &l->data_len);
+                                narrow_scan(&S4, &l->scan[l->nscan++]);
+                        } else if (d->lay4) {
+                                for (int i = 0; i < ns; i++)
+                                        if (d->scans_of[sc[i] - d->c]++) return 1;      /* a component scanned twice */
+                                struct j2p_jpeg_layout4 *l = d->lay4;
                                 layout_scan(d, sc, ns, &l->scan[l->nscan++], &l->seg, &l->nseg, &l->data, &l->data_len);
                         } else if (d->play) {
                                 struct j2p_jpeg_prog_layout *l = d->play;
@@ -586,13 +627,15 @@ static int read_markers(struct dec *d, const uint8_t *buf, size_t len) {
                                 S->se = (unsigned)se;
                                 S->ah = (unsigned)ah;
                                 S->al = (unsigned)al;
-                                layout_scan(d, sc, ns, &S->s, &l->seg, &l->nseg, &l->data, &l->data_len);
+                                layout_scan(d, sc, ns, &S4, &l->seg, &l->nseg, &l->data, &l->data_len);
+                                narrow_scan(&S4, &S->s);
                         } else if (d->alay) {
                                 for (int i = 0; i < ns; i++)
                                         if (d->scans_of[sc[i] - d->c]++) return 1;      /* a component scanned twice */
                                 struct j2p_jpeg_arith_layout *l = d->alay;
                                 struct j2p_jpeg_scan S;
-                                layout_scan(d, sc, ns, &S, &l->seg, &l->nseg, &l->data, &l->data_len);
+                                layout_scan(d, sc, ns, &S4, &l->seg, &l->nseg, &l->data, &l->data_len);
+                                narrow_scan(&S4, &S);
                                 struct j2p_jpeg_arith_scan *A = &l->scan[l->nscan++];
                                 A->ncomp = S.ncomp;
                                 for (int i = 0; i < 3; i++) {
@@ -652,33 +695,51 @@ int j2p_read_jpeg_mem(const uint8_t *buf, size_t len, struct j2p_jpeg *out, char
         return rc;
 }
 
-int j2p_read_jpeg_mem_ex(const uint8_t *buf, size_t len, unsigned flags, struct j2p_jpeg *out, char *err, size_t errlen) {
+/* the full read behind j2p_read_jpeg_mem_ex and j2p_read_jpeg4_mem: coefs has room for ncomp_max
+ * planes (3, or 4 with J2P_READ_CMYK); *ncomp is the frame's count once its header is read (also on
+ * failure), *colour the J2P_JPEG_* kind of a four-component frame */
+static int read_full(const uint8_t *buf, size_t len, unsigned flags, unsigned *w, unsigned *h, struct coef *coefs, unsigned *ncomp,
+                     unsigned *colour, char *err, size_t errlen) {
         struct dec *d = calloc(1, sizeof *d);
         if (!d) return -1;
         d->p = buf; d->end = buf + len; d->err = err; d->errlen = errlen; d->flags = flags;
         if (err && errlen) err[0] = 0;
-        memset(out, 0, sizeof *out);
         read_markers(d, buf, len);
-        if (!d->failed) check_planes(d, out->coefs);
+        *ncomp = (unsigned)d->ncomp;
+        const int planes_failed = d->failed;        /* before the planes: ncomp may be any count, nothing is allocated */
+        if (!d->failed) check_planes(d, coefs);
         if (!d->failed) {
-                out->w = d->W;
-                out->h = d->H;
-                out->ncomp = (unsigned)d->ncomp;
+                *w = d->W;
+                *h = d->H;
+                if (colour && d->ncomp == 4) *colour = d->adobe_transform <= 0 ? J2P_JPEG_CMYK : J2P_JPEG_YCCK;   /* libjpeg's default_decompress_parms */
                 for (int i = 0; i < d->ncomp; i++) {
                         struct comp *c = &d->c[i];
-                        struct coef *o = &out->coefs[i];
+                        struct coef *o = &coefs[i];
                         o->data = malloc((size_t)o->w * o->h * sizeof(int16_t));
                         if (!o->data) { fail(d, "could not allocate memory for coefs"); break; }
                         for (unsigned by = 0; by < c->hb; by++)
                                 memcpy(o->data + (size_t)by * c->wb * 64, c->blk + (size_t)by * c->pwb * 64, (size_t)c->wb * 64 * sizeof(int16_t));
                 }
         }
-        for (int i = 0; i < 3; i++) free(d->c[i].blk);
+        for (int i = 0; i < 4; i++) free(d->c[i].blk);
         free(d->abuf);
         const int rc = d->failed ? -1 : 0;
-        if (rc != 0) for (int i = 0; i < 3; i++) { free(out->coefs[i].data); out->coefs[i].data = NULL; }
+        if (rc != 0 && !planes_failed) for (int i = 0; i < d->ncomp; i++) { free(coefs[i].data); coefs[i].data = NULL; }
         free(d);
         return rc;
+}
+
+int j2p_read_jpeg_mem_ex(const uint8_t *buf, size_t len, unsigned flags, struct j2p_jpeg *out, char *err, size_t errlen) {
+        memset(out, 0, sizeof *out);
+        unsigned ncomp;
+        const int rc = read_full(buf, len, flags & ~(unsigned)J2P_READ_CMYK, &out->w, &out->h, out->coefs, &ncomp, NULL, err, errlen);
+        if (rc == 0) out->ncomp = ncomp;
+        return rc;
+}
+
+int j2p_read_jpeg4_mem(const uint8_t *buf, size_t len, unsigned flags, struct j2p_jpeg4 *out, char *err, size_t errlen) {
+        memset(out, 0, sizeof *out);
+        return read_full(buf, len, flags | J2P_READ_CMYK, &out->w, &out->h, out->coefs, &out->ncomp, &out->colour, err, errlen);
 }
 
 int j2p_read_jpeg_layout(const uint8_t *buf, size_t len, struct j2p_jpeg_layout *out, char *err, size_t errlen) {
@@ -785,6 +846,43 @@ int j2p_read_jpeg_arith_layout_ex(const uint8_t *buf, size_t len, unsigned flags
 }
 
 void j2p_free_jpeg_arith_layout(struct j2p_jpeg_arith_layout *l) {
+        free(l->seg);
+        free(l->data);
+        l->seg = NULL;
+        l->data = NULL;
+        l->nseg = 0;
+        l->data_len = 0;
+}
+
+int j2p_read_jpeg_layout4(const uint8_t *buf, size_t len, unsigned flags, struct j2p_jpeg_layout4 *out, char *err, size_t errlen) {
+        struct dec *d = calloc(1, sizeof *d);
+        if (!d) return -1;
+        d->p = buf; d->end = buf + len; d->err = err; d->errlen = errlen; d->flags = flags | J2P_READ_CMYK;
+        if (err && errlen) err[0] = 0;
+        memset(out, 0, sizeof *out);
+        d->lay4 = out;
+        const int stopped = read_markers(d, buf, len);
+        int decodable = !stopped && !d->failed;
+        for (int i = 0; i < d->ncomp && decodable; i++) decodable = d->scans_of[i] == 1;
+        if (decodable) {
+                check_planes(d, out->coefs);
+                out->w = d->W;
+                out->h = d->H;
+                out->ncomp = (unsigned)d->ncomp;
+                if (d->ncomp == 4) out->colour = d->adobe_transform <= 0 ? J2P_JPEG_CMYK : J2P_JPEG_YCCK;
+                for (int i = 0; i < d->ncomp; i++) { out->comp_h[i] = (unsigned)d->c[i].h; out->comp_v[i] = (unsigned)d->c[i].v; }
+        }
+        const int rc = d->failed ? -1 : 0;
+        out->device_decodable = rc == 0 && decodable;
+        if (!out->device_decodable) {
+                j2p_free_jpeg_layout4(out);
+                out->nscan = 0;
+        }
+        free(d);
+        return rc;
+}
+
+void j2p_free_jpeg_layout4(struct j2p_jpeg_layout4 *l) {
         free(l->seg);
         free(l->data);
         l->seg = NULL;

@@ -47,8 +47,28 @@ int j2p_read_jpeg_mem(const uint8_t *buf, size_t len, struct j2p_jpeg *out, char
  * every other count with "only 1 and 3 component jpegs are supported".  A gray file's plane is
  * coefs[0] with w_samp = h_samp = 1 (whatever sampling factor its SOF gives it) and its scans are
  * non-interleaved over the plane's real block grid; coefs[1..2] stay empty. */
-enum { J2P_READ_GRAY = 1u };
+enum { J2P_READ_GRAY = 1u, J2P_READ_CMYK = 2u };
 int j2p_read_jpeg_mem_ex(const uint8_t *buf, size_t len, unsigned flags, struct j2p_jpeg *out, char *err, size_t errlen);
+
+/* ---- four-component files (Adobe CMYK and YCCK) ----
+ * J2P_READ_CMYK: accept one-, three- and four-component files, and refuse every other count with
+ * "only 1, 3 and 4 component jpegs are supported".  struct j2p_jpeg has room for three planes, so
+ * j2p_read_jpeg_mem_ex ignores the flag; j2p_read_jpeg4_mem always applies it.  A four-component
+ * file's planes keep the sampling factors of its SOF, as a colour file's do.
+ * colour (four components only, else 0): libjpeg's choice, from the Adobe APP14 segment (12 data
+ * bytes or more starting with "Adobe"; the last one before the first SOS counts; its transform is
+ * byte 11): J2P_JPEG_CMYK without such a segment or with transform 0, J2P_JPEG_YCCK with any other
+ * transform.  The three-plane layout passes report four-component files as not decodable when given
+ * the flag, and refuse them with the count message without it; j2p_read_jpeg_layout4 takes them. */
+enum { J2P_JPEG_CMYK = 1u, J2P_JPEG_YCCK = 2u };
+struct j2p_jpeg4 {
+        unsigned w, h;
+        struct coef coefs[4];       /* as struct j2p_jpeg; coefs[ncomp..3] empty */
+        unsigned ncomp;             /* 1, 3 or 4; on failure the frame header's count once it was read, else 0 */
+        unsigned colour;            /* J2P_JPEG_CMYK or J2P_JPEG_YCCK for four components, else 0 */
+};
+int j2p_read_jpeg4_mem(const uint8_t *buf, size_t len, unsigned flags, struct j2p_jpeg4 *out, char *err, size_t errlen);
+
 
 /* ---- layout pass: the headers and the entropy-coded data of a file, without Huffman decoding ----
  * (the _ex variant takes the J2P_READ_* flags of j2p_read_jpeg_mem_ex)
@@ -99,6 +119,34 @@ struct j2p_jpeg_layout {
 int j2p_read_jpeg_layout(const uint8_t *buf, size_t len, struct j2p_jpeg_layout *out, char *err, size_t errlen);
 int j2p_read_jpeg_layout_ex(const uint8_t *buf, size_t len, unsigned flags, struct j2p_jpeg_layout *out, char *err, size_t errlen);
 void j2p_free_jpeg_layout(struct j2p_jpeg_layout *l);
+
+/* The layout pass for four-component files (J2P_READ_CMYK always on): as j2p_read_jpeg_layout_ex,
+ * with room for four planes and scans of up to four components, and the colour kind.
+ * device_decodable: sequential Huffman, each component in exactly one scan (what
+ * libj2pentropy.so's j2p_entropy_pack4 takes).  The three-plane layout passes keep stopping at a
+ * four-component frame header.  A four-component file whose interleaved scan has more than 10
+ * blocks per MCU is refused by every entry point, as libjpeg refuses it. */
+struct j2p_jpeg_scan4 {
+        unsigned ncomp, comp[4], bw[4], bh[4];  /* as struct j2p_jpeg_scan */
+        unsigned mcux, mcuy, restart_interval;
+        struct j2p_jpeg_huff dc[4], ac[4];
+        unsigned seg0, nseg;
+};
+struct j2p_jpeg_layout4 {
+        unsigned w, h;
+        struct coef coefs[4];
+        unsigned comp_h[4], comp_v[4];
+        int device_decodable;
+        unsigned nscan;
+        struct j2p_jpeg_scan4 scan[4];
+        unsigned nseg;
+        struct j2p_jpeg_segment *seg;    /* malloc'd */
+        uint8_t *data;                   /* malloc'd */
+        size_t data_len;
+        unsigned ncomp, colour;          /* set when device_decodable; colour as struct j2p_jpeg4 */
+};
+int j2p_read_jpeg_layout4(const uint8_t *buf, size_t len, unsigned flags, struct j2p_jpeg_layout4 *out, char *err, size_t errlen);
+void j2p_free_jpeg_layout4(struct j2p_jpeg_layout4 *l);
 
 /* ---- progressive layout pass: every scan of a progressive file, cut as above ----
  *

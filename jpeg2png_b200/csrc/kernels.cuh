@@ -148,12 +148,17 @@ inline FrameDev rows_view(const FrameDev &F, int c0, int count, int brow, int fr
 // the R (= G = B) sample of that luma with zero chroma.
 // With `oriented` set (HWC / CHW only) a CTA covers a tile of the image instead of a row segment,
 // and each frame is written flipped or rotated by its EXIF orientation (orient[frame], 1..8).
+// With `four` set (HWC / CHW only) the frame has four planes (a four-component JPEG, DESIGN §7q):
+// EP_FOUR_CMYK, each plane's gray sample inverted; EP_FOUR_YCCK, planes 0-2 as RGB and plane 3's gray
+// sample inverted.  nc == 4 writes those samples, nc == 3 (8-bit only) Pillow's CMYK -> RGB of them.
 enum EpilogueMode { EP_SCANLINES = 0, EP_HWC = 1, EP_CHW = 2 };
+enum EpilogueFour { EP_FOUR_NONE = 0, EP_FOUR_CMYK = 1, EP_FOUR_YCCK = 2 };
 struct EpilogueArgs {
-    const float *plane[3];               // frame 0's Y, Cb, Cr (current iterates); Y alone when nc == 1
-    int nc;                              // samples per pixel: 3 (RGB) or 1 (gray)
-    unsigned long long frame_stride[3];  // elements from one frame's plane to the next frame's
-    int ld[3];                           // row stride of each plane, elements
+    const float *plane[4];               // frame 0's Y, Cb, Cr (current iterates); Y alone when nc == 1; four planes with `four`
+    int nc;                              // samples per pixel: 3 (RGB) or 1 (gray); 4 or 3 with `four`
+    unsigned long long frame_stride[4];  // elements from one frame's plane to the next frame's
+    int ld[4];                           // row stride of each plane, elements
+    int four;                            // EpilogueFour
     int w, h;                            // visible image, at most every plane's frame
     int row0;                            // first image row of this launch (launch_scanlines)
     int mode;                            // EpilogueMode

@@ -14,6 +14,8 @@
 // and adding +0 to a double that is not -0 leaves it unchanged).  The branch is uniform per launch.
 // With a.oriented (HWC / CHW) the same samples are written flipped or rotated per frame by its EXIF
 // orientation (DESIGN §7l): a CTA converts a 32 x 32 tile and writes it where the orientation puts it.
+// With a.four (HWC / CHW) the frame is a four-component JPEG's four planes (four_samples, DESIGN §7q):
+// four inverted CMYK samples per pixel, or three from Pillow's CMYK -> RGB of them.
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -24,9 +26,9 @@ namespace j2p {
 
 constexpr int EP_NT = 256;
 constexpr int EP_TILE = 32;                                 // oriented mode: tiles of EP_TILE x EP_TILE pixels
-constexpr int EP_TILE_ROW = EP_TILE * 12 + 4;               // largest staged output row (HWC float), + a pad word
-constexpr int EP_STAGE = 3 * EP_TILE * (EP_TILE * 4 + 4);   // largest staged tile (CHW float), rows padded by a word
-static_assert(EP_STAGE >= EP_TILE * EP_TILE_ROW && EP_STAGE >= EP_NT * 12, "the staging buffer holds every mode");
+constexpr int EP_TILE_ROW = EP_TILE * 16 + 4;               // largest staged output row (HWC float, four channels), + a pad word
+constexpr int EP_STAGE = 4 * EP_TILE * (EP_TILE * 4 + 4);   // largest staged tile (CHW float, four channels), rows padded by a word
+static_assert(EP_STAGE >= EP_TILE * EP_TILE_ROW && EP_STAGE >= EP_NT * 16, "the staging buffer holds every mode");
 
 // png.c:15-17 + :44-46: the double expression is narrowed to float by the call to clamp() and
 // compared with the double bounds 0. and 255.
@@ -74,6 +76,32 @@ __device__ __forceinline__ void pixel_samples(const EpilogueArgs &a, int frame, 
         s[k] = a.sample == 32 ? __float_as_uint(v[k]) : __float2uint_rz(__fmul_rn(v[k], bitfactor));    // png.c:44-46 truncation
 }
 
+// The samples of pixel (px, row) of a four-plane frame (a.four, DESIGN §7q).  A plane's gray sample
+// g is what the gray export writes for it; its inversion is 255 - g (8 bit), 65535 - g (16 bit) or
+// 255.f - g (float), Pillow's "CMYK;I" reading of Adobe files.  CMYK: every channel inverted.
+// YCCK: channels 0-2 the RGB samples of planes 0-2, channel 3 plane 3 inverted.  With a.nc == 3
+// (8 bit) the four 8-bit samples go through Pillow's CMYK -> RGB: nk = 255 - K, t = x * nk + 128,
+// each channel clip(nk - ((t + (t >> 8)) >> 8), 0, 255).
+__device__ __forceinline__ void four_samples(const EpilogueArgs &a, int frame, int row, int px, uint32_t s[4]) {
+    const int c0 = a.four == EP_FOUR_YCCK ? 3 : 0;
+    if (c0 == 3) pixel_samples(a, frame, row, px, false, s);
+#pragma unroll 1
+    for (int c = c0; c < 4; c++) {
+        const float *P = a.plane[c] + (size_t)frame * a.frame_stride[c] + (size_t)row * a.ld[c];
+        const float g = clamp_sample((double)__fadd_rn(P[px], 128.f));                                // the gray sample
+        s[c] = a.sample == 32 ? __float_as_uint(__fsub_rn(255.f, g))
+             : (a.sample == 8 ? 255u : 65535u) - __float2uint_rz(__fmul_rn(g, a.sample == 8 ? 1.0f : 256.0f));
+    }
+    if (a.nc == 3) {
+        const int nk = 255 - (int)s[3];
+#pragma unroll
+        for (int k = 0; k < 3; k++) {
+            const int t = (int)s[k] * nk + 128;
+            s[k] = (uint32_t)min(max(nk - ((t + (t >> 8)) >> 8), 0), 255);
+        }
+    }
+}
+
 __device__ __forceinline__ void stage_sample(uint8_t *p, uint32_t s, int es) {
     if (es == 1) *p = (uint8_t)s;
     else if (es == 2) *reinterpret_cast<uint16_t *>(p) = (uint16_t)s;
@@ -92,7 +120,7 @@ __device__ __forceinline__ void oriented_tile(const EpilogueArgs &a, uint8_t *sm
     const int tw = min(EP_TILE, a.w - tx0), th = min(EP_TILE, a.h - ty0);
     const int es = a.sample >> 3;
     const bool gray = a.nc == 1, chw = a.mode == EP_CHW;
-    const int nc = gray ? 1 : 3;
+    const int nc = a.nc;
     int k = a.orient ? a.orient[frame] : 1;
     if (k < 1 || k > 8) k = 1;
     const bool tr = k >= 5;
@@ -104,13 +132,14 @@ __device__ __forceinline__ void oriented_tile(const EpilogueArgs &a, uint8_t *sm
     const int plane_stage = EP_TILE * row_bytes;                            // CHW: one channel's staged tile
     if (lane < tw) {
         for (int ly = warp; ly < th; ly += EP_NT / 32) {
-            uint32_t s[3];
-            pixel_samples(a, frame, ty0 + ly, tx0 + lane, gray, s);
+            uint32_t s[4];
+            if (a.four) four_samples(a, frame, ty0 + ly, tx0 + lane, s);
+            else pixel_samples(a, frame, ty0 + ly, tx0 + lane, gray, s);
             const int sx = tr ? ly : lane, sy = tr ? lane : ly;
             const int ox = fx ? ow - 1 - sx : sx, oy = fy ? oh - 1 - sy : sy;
             uint8_t *e = sm + oy * row_bytes + ox * px_bytes;
 #pragma unroll
-            for (int c = 0; c < 3; c++) {
+            for (int c = 0; c < 4; c++) {
                 if (c >= nc) break;
                 stage_sample(chw ? e + c * plane_stage : e + c * es, s[c], es);
             }
@@ -145,12 +174,13 @@ __global__ void __launch_bounds__(EP_NT) k_scanlines(const EpilogueArgs a) {
     const int row = a.row0 + (int)blockIdx.y, frame = blockIdx.z, x0 = blockIdx.x * EP_NT, tid = threadIdx.x;
     const int es = a.sample >> 3, npx = min(EP_NT, a.w - x0);           // bytes per sample, pixels of this CTA
     const bool gray = a.nc == 1;
-    const int nc = gray ? 1 : 3;                                        // samples per pixel
+    const int nc = a.nc;                                                // samples per pixel
     if (tid < npx) {
-        uint32_t v[3];
-        pixel_samples(a, frame, row, x0 + tid, gray, v);
+        uint32_t v[4];
+        if (a.four) four_samples(a, frame, row, x0 + tid, v);
+        else pixel_samples(a, frame, row, x0 + tid, gray, v);
 #pragma unroll
-        for (int k = 0; k < 3; k++) {
+        for (int k = 0; k < 4; k++) {
             if (k >= nc) break;
             uint32_t s = v[k];
             if (a.mode == EP_SCANLINES && es == 2) s = ((s >> 8) & 0xffu) | ((s & 0xffu) << 8);                // png.c:58-60 big-endian

@@ -1066,24 +1066,35 @@ extern "C" int j2p_session_download_frame_scanlines(j2p_session *s, unsigned fra
 // nout: samples per pixel, 3 (RGB) or 1 (gray: plane 0 of the one session ss[0] alone).  oriented:
 // the tiled mode of the epilogue, each frame flipped or rotated by orient[frame - frame0] (device
 // memory; NULL = every frame 1).
+// four (EpilogueFour): the four-plane mode, whose files have q[k] planes in session k (frame0 and
+// nframes count files; j2p_session_export_four checked the q[k]).
 static int export_impl(j2p_session *const *ss, int nsess, int nout, unsigned frame0, unsigned nframes, const struct j2p_image_out *o,
-                       void *dst, void *stream, bool oriented = false, const unsigned char *orient = nullptr) {
+                       void *dst, void *stream, bool oriented = false, const unsigned char *orient = nullptr, int four = EP_FOUR_NONE,
+                       const unsigned *q = nullptr) {
     if (!o || !dst) return fail(J2P_ERR_ARG, "null argument");
     j2p_session *s0 = ss[0];
+    const unsigned nfiles = four ? s0->nframes * (unsigned)s0->F.nc / q[0] : s0->nframes;
     if (nframes == 0) return fail(J2P_ERR_ARG, "nframes must be at least 1");
-    if (frame0 >= s0->nframes || nframes > s0->nframes - frame0)
-        return fail(J2P_ERR_ARG, "frames %u..%u out of range (%u frames)", frame0, frame0 + nframes, s0->nframes);
+    if (frame0 >= nfiles || nframes > nfiles - frame0)
+        return fail(J2P_ERR_ARG, "frames %u..%u out of range (%u frames)", frame0, frame0 + nframes, nfiles);
     if (o->sample != 8 && o->sample != 16 && o->sample != 32) return fail(J2P_ERR_ARG, "sample must be 8, 16 or 32 (got %u)", o->sample);
     if (o->layout != J2P_LAYOUT_HWC && o->layout != J2P_LAYOUT_CHW) return fail(J2P_ERR_ARG, "unknown layout %u", o->layout);
     if (o->w == 0 || o->h == 0) return fail(J2P_ERR_ARG, "image %ux%u is empty", o->w, o->h);
     EpilogueArgs a{};
     a.nc = nout;
-    for (int c = 0; c < nout; c++) {
-        j2p_session *s = ss[nsess == 1 ? 0 : c];
+    a.four = four;
+    for (int c = 0, k = 0, j = 0; c < (four ? 4 : nout); c++) {
+        j2p_session *s = ss[four ? k : (nsess == 1 ? 0 : c)];
         const int W = s->F.W, H = s->F.Hg;
         if (o->w > (unsigned)W || o->h > (unsigned)H) return fail(J2P_ERR_ARG, "image %ux%u does not fit the %dx%d frame of plane %d", o->w, o->h, W, H, c);
-        a.plane[c] = plane_x(s, nsess == 1 ? frame0 * (unsigned)s->F.nc + (unsigned)c : frame0);
-        a.frame_stride[c] = s->F.frame_stride;
+        if (four) {         // file f's plane c is plane f * q[k] + j of session k
+            a.plane[c] = plane_x(s, frame0 * q[k] + (unsigned)j);
+            a.frame_stride[c] = (unsigned long long)(q[k] / (unsigned)s->F.nc) * s->F.frame_stride;
+            if (++j == (int)q[k]) { k++; j = 0; }
+        } else {
+            a.plane[c] = plane_x(s, nsess == 1 ? frame0 * (unsigned)s->F.nc + (unsigned)c : frame0);
+            a.frame_stride[c] = s->F.frame_stride;
+        }
         a.ld[c] = W;
     }
     const size_t image_bytes = (size_t)o->w * o->h * (size_t)nout * (o->sample / 8);
@@ -1184,6 +1195,42 @@ extern "C" int j2p_session_export_oriented(j2p_session *const *sessions, unsigne
         return fail(J2P_ERR_ARG, "a gray oriented export needs a whole-frame session with one or three planes (has %d)", s->F.nc);
     }
     return export_impl(sessions, (int)nsessions, (int)channels, frame0, nframes, o, dst, stream, true, orientation);
+}
+
+extern "C" int j2p_session_export_four(j2p_session *const *sessions, unsigned nsessions, unsigned kind, unsigned channels,
+                                       unsigned frame0, unsigned nframes, const unsigned char *orientation,
+                                       const struct j2p_image_out *o, void *dst, void *stream) {
+    if (!sessions || !o) return fail(J2P_ERR_ARG, "null argument");
+    if (kind != J2P_FOUR_CMYK && kind != J2P_FOUR_YCCK) return fail(J2P_ERR_ARG, "unknown four-component kind %u", kind);
+    if (channels != 4 && channels != 3) return fail(J2P_ERR_ARG, "a four-component export writes 4 or 3 channels (got %u)", channels);
+    if (channels == 3 && o->sample != 8) return fail(J2P_ERR_ARG, "the CMYK -> RGB conversion is defined for 8-bit samples only (got %u)", o->sample);
+    if (nsessions < 1 || nsessions > 4) return fail(J2P_ERR_ARG, "a four-component export takes 1 to 4 sessions (got %u)", nsessions);
+    unsigned long long planes = 0;
+    for (unsigned k = 0; k < nsessions; k++) {
+        j2p_session *s = sessions[k];
+        if (!s) return fail(J2P_ERR_ARG, "null session");
+        if ((s->F.nc != 1 && s->F.nc != 3) || s->strip)
+            return fail(J2P_ERR_ARG, "a four-component export needs whole-frame sessions with one or three planes (session %u has %d)", k, s->F.nc);
+        if (s->device != sessions[0]->device)
+            return fail(J2P_ERR_ARG, "the sessions live on different devices (%d, %d)", sessions[0]->device, s->device);
+        planes += (unsigned long long)s->nframes * (unsigned)s->F.nc;
+    }
+    unsigned q[4] = {0, 0, 0, 0}, sum = 0;
+    const unsigned long long nfiles = planes / 4;
+    for (unsigned k = 0; k < nsessions; k++) {
+        const unsigned long long p = (unsigned long long)sessions[k]->nframes * (unsigned)sessions[k]->F.nc;
+        if (planes % 4 || p % nfiles || p / nfiles > 4 || (p / nfiles) % (unsigned)sessions[k]->F.nc)
+            return fail(J2P_ERR_ARG, "the sessions do not hold whole planes of %llu files (session %u: %llu planes)", nfiles, k, p);
+        q[k] = (unsigned)(p / nfiles);
+        sum += q[k];
+    }
+    if (sum != 4) return fail(J2P_ERR_ARG, "the sessions hold %u planes per file, not 4", sum);
+    if (sessions[0]->F.nc == 3 && kind != J2P_FOUR_YCCK)
+        return fail(J2P_ERR_ARG, "a three-plane session holds the Y, Cb and Cr of a YCCK file");
+    for (unsigned k = 1; k < nsessions; k++)
+        if (sessions[k]->F.nc != 1) return fail(J2P_ERR_ARG, "only the first session may hold three planes");
+    return export_impl(sessions, (int)nsessions, (int)channels, frame0, nframes, o, dst, stream, orientation != nullptr, orientation,
+                       kind == J2P_FOUR_CMYK ? EP_FOUR_CMYK : EP_FOUR_YCCK, q);
 }
 
 extern "C" int j2p_session_sync(j2p_session *s) {

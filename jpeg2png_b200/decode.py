@@ -16,6 +16,9 @@ like the luma of colour files in mode='GRAY', exported as one channel (j2p_sessi
 With apply_exif_orientation=True each file's EXIF Orientation tag is read on the host
 (j2p_jpeg_exif_orientation) and a chunk that holds a file with an orientation other than 1 is exported
 in one call that flips or rotates every frame as it writes it (j2p_session_export_oriented, DESIGN §7l).
+With mode='RGB' or 'UNCHANGED', a file the front end refuses is offered to the four-component passes:
+j2p_read_jpeg_layout4 for the device decoder (four_on_device) or j2p_read_jpeg4_mem on the host; their
+chunks are exported by j2p_session_export_four (DESIGN §7q).
 
 The samples are those of the PNG the command line writes for the same file and flags:
 torch.uint8 the 8-bit PNG samples, torch.uint16 the 16-bit (-1) samples in native byte order,
@@ -42,11 +45,18 @@ _SAMPLE = {torch.uint8: 8, torch.uint16: 16, torch.float32: 32}
 _LAYOUT = {'HWC': abi.LAYOUT_HWC, 'CHW': abi.LAYOUT_CHW}
 MODES = ('RGB', 'UNCHANGED', 'GRAY')
 READ_GRAY = 1                       # J2P_READ_GRAY (jpeg_reader.h)
+READ_CMYK = 2                       # J2P_READ_CMYK
+CMYK, YCCK = 1, 2                   # J2P_JPEG_CMYK / J2P_JPEG_YCCK, and J2P_FOUR_CMYK / J2P_FOUR_YCCK of the export
 
 
 class Jpeg(C.Structure):
     """struct j2p_jpeg — jpeg2png_b200/cli/jpeg_reader.h."""
     _fields_ = [('w', C.c_uint), ('h', C.c_uint), ('coefs', abi.Coef * 3), ('ncomp', C.c_uint)]
+
+
+class Jpeg4(C.Structure):
+    """struct j2p_jpeg4 — jpeg2png_b200/cli/jpeg_reader.h."""
+    _fields_ = [('w', C.c_uint), ('h', C.c_uint), ('coefs', abi.Coef * 4), ('ncomp', C.c_uint), ('colour', C.c_uint)]
 
 
 class Huff(C.Structure):
@@ -72,6 +82,21 @@ class Layout(C.Structure):
                 ('comp_v', C.c_uint * 3), ('device_decodable', C.c_int), ('nscan', C.c_uint), ('scan', Scan * 3),
                 ('nseg', C.c_uint), ('seg', C.POINTER(Segment)), ('data', C.POINTER(C.c_uint8)),
                 ('data_len', C.c_size_t), ('ncomp', C.c_uint)]
+
+
+class Scan4(C.Structure):
+    """struct j2p_jpeg_scan4 — jpeg2png_b200/cli/jpeg_reader.h."""
+    _fields_ = [('ncomp', C.c_uint), ('comp', C.c_uint * 4), ('bw', C.c_uint * 4), ('bh', C.c_uint * 4),
+                ('mcux', C.c_uint), ('mcuy', C.c_uint), ('restart_interval', C.c_uint),
+                ('dc', Huff * 4), ('ac', Huff * 4), ('seg0', C.c_uint), ('nseg', C.c_uint)]
+
+
+class Layout4(C.Structure):
+    """struct j2p_jpeg_layout4 — jpeg2png_b200/cli/jpeg_reader.h."""
+    _fields_ = [('w', C.c_uint), ('h', C.c_uint), ('coefs', abi.Coef * 4), ('comp_h', C.c_uint * 4),
+                ('comp_v', C.c_uint * 4), ('device_decodable', C.c_int), ('nscan', C.c_uint), ('scan', Scan4 * 4),
+                ('nseg', C.c_uint), ('seg', C.POINTER(Segment)), ('data', C.POINTER(C.c_uint8)),
+                ('data_len', C.c_size_t), ('ncomp', C.c_uint), ('colour', C.c_uint)]
 
 
 class ProgScan(C.Structure):
@@ -162,6 +187,12 @@ def _declare_codecs(lib):
     lib.j2p_free_jpeg_arith_layout.restype = None
     lib.j2p_free_jpeg_arith_layout.argtypes = [C.POINTER(ArithLayout)]
     lib.j2p_jpeg_keep_settings.restype = C.c_int
+    lib.j2p_read_jpeg_layout4.restype = C.c_int
+    lib.j2p_read_jpeg_layout4.argtypes = [C.c_char_p, C.c_size_t, C.c_uint, C.POINTER(Layout4), C.c_char_p, C.c_size_t]
+    lib.j2p_free_jpeg_layout4.restype = None
+    lib.j2p_free_jpeg_layout4.argtypes = [C.POINTER(Layout4)]
+    lib.j2p_read_jpeg4_mem.restype = C.c_int
+    lib.j2p_read_jpeg4_mem.argtypes = [C.c_char_p, C.c_size_t, C.c_uint, C.POINTER(Jpeg4), C.c_char_p, C.c_size_t]
     lib.j2p_jpeg_keep_settings.argtypes = [C.c_char_p, C.c_size_t, C.POINTER(Keep), C.c_char_p, C.c_size_t]
 
 
@@ -176,6 +207,11 @@ def _declare_entropy(lib):
     lib.j2p_entropy_plan_size.argtypes = [lay, C.c_uint, C.c_uint, C.POINTER(C.c_size_t), C.POINTER(C.c_size_t)]
     lib.j2p_entropy_pack.restype = C.c_int
     lib.j2p_entropy_pack.argtypes = [lay, C.c_uint, C.c_uint, C.POINTER(vp), vp, C.c_size_t]
+    lay4 = C.POINTER(C.POINTER(Layout4))
+    lib.j2p_entropy_plan_size4.restype = C.c_int
+    lib.j2p_entropy_plan_size4.argtypes = [lay4, C.c_uint, C.c_uint, C.POINTER(C.c_size_t), C.POINTER(C.c_size_t)]
+    lib.j2p_entropy_pack4.restype = C.c_int
+    lib.j2p_entropy_pack4.argtypes = [lay4, C.c_uint, C.c_uint, C.POINTER(vp), vp, C.c_size_t]
     lib.j2p_entropy_decode.restype = C.c_int
     lib.j2p_entropy_decode.argtypes = [vp, vp, vp, vp, vp, C.POINTER(EntropyStats)]
     lib.j2p_entropy_decode_host.restype = C.c_int
@@ -249,6 +285,34 @@ class FileLayout:
     def __del__(self):
         try:
             load_codecs().j2p_free_jpeg_layout(C.byref(self.lay))
+        except Exception:
+            pass
+
+
+class FileLayout4:
+    """A four-component file's layout (j2p_read_jpeg_layout4 with the J2P_READ_* `flags`); frees the C
+    buffers when collected.  device_decodable: sequential Huffman, each component in one scan."""
+    planes_per_file = 4
+
+    def __init__(self, data: bytes, flags: int = 0):
+        lib = load_codecs()
+        self.lay = Layout4()
+        err = C.create_string_buffer(256)
+        if lib.j2p_read_jpeg_layout4(data, len(data), flags, C.byref(self.lay), err, 256) != 0:
+            raise ValueError(err.value.decode(errors='replace'))
+        self.device_decodable = bool(self.lay.device_decodable)
+        self.w, self.h = int(self.lay.w), int(self.lay.h)
+        self.colour = int(self.lay.colour)
+        self.compressed = int(self.lay.data_len)
+        self.planes = [Plane(int(c.w), int(c.h), int(c.w_samp), int(c.h_samp), None,
+                             np.array(list(c.quant_table), np.uint16)) for c in self.lay.coefs[:self.lay.ncomp]]
+
+    def key(self):
+        return Parsed.key(self)
+
+    def __del__(self):
+        try:
+            load_codecs().j2p_free_jpeg_layout4(C.byref(self.lay))
         except Exception:
             pass
 
@@ -346,6 +410,25 @@ def entropy_plan(layouts, outs, subseq_bits=SUBSEQ_BITS, pinned=False):
     return buf, addr, plan_bytes.value, work_bytes.value
 
 
+def entropy_plan4(layouts, outs, subseq_bits=SUBSEQ_BITS, pinned=False):
+    """entropy_plan for FileLayout4s (j2p_entropy_pack4); outs[4 * i + c]: file i's plane c."""
+    lib = load_entropy()
+    ptrs = (C.POINTER(Layout4) * len(layouts))(*[C.pointer(x.lay) for x in layouts])
+    plan_bytes, work_bytes = C.c_size_t(), C.c_size_t()
+    if lib.j2p_entropy_plan_size4(ptrs, len(layouts), subseq_bits, C.byref(plan_bytes), C.byref(work_bytes)) != 0:
+        raise RuntimeError(lib.j2p_entropy_last_error().decode())
+    if pinned:
+        buf = torch.empty(plan_bytes.value, dtype=torch.uint8, pin_memory=True)
+        addr = buf.data_ptr()
+    else:
+        buf = np.zeros(plan_bytes.value + 16, np.uint8)
+        addr = (buf.ctypes.data + 15) & ~15
+    o = (C.c_void_p * len(outs))(*outs)
+    if lib.j2p_entropy_pack4(ptrs, len(layouts), subseq_bits, o, addr, plan_bytes.value) != 0:
+        raise RuntimeError(lib.j2p_entropy_last_error().decode())
+    return buf, addr, plan_bytes.value, work_bytes.value
+
+
 def progressive_plan(layouts, outs, subseq_bits=SUBSEQ_BITS, pinned=False):
     """entropy_plan for ProgFileLayouts and libj2pprogressive.so."""
     lib = load_progressive()
@@ -397,14 +480,18 @@ class Plane:
 
 @dataclass
 class Parsed:
-    """One parsed JPEG: the visible size and its coefficient planes (three, or one for a gray file)."""
+    """One parsed JPEG: the visible size and its coefficient planes (three, one for a gray file,
+    four for a CMYK or YCCK file, whose kind is `colour`)."""
     w: int
     h: int
     planes: list
+    colour: int = 0             # CMYK or YCCK for four planes
 
     def key(self):
-        """Inputs with equal keys are solved in one batch session."""
-        return (self.w, self.h, tuple((p.w, p.h, p.w_samp, p.h_samp) for p in self.planes))
+        """Inputs with equal keys are solved in one batch session; a four-component file's key also
+        holds its kind."""
+        k = (self.w, self.h, tuple((p.w, p.h, p.w_samp, p.h_samp) for p in self.planes))
+        return k + (self.colour,) if len(self.planes) == 4 else k
 
 
 def parse_jpeg(data: bytes, flags: int = 0) -> Parsed:
@@ -422,6 +509,26 @@ def parse_jpeg(data: bytes, flags: int = 0) -> Parsed:
         abi.free_ptr(c.data)
         planes.append(Plane(int(c.w), int(c.h), int(c.w_samp), int(c.h_samp), d, np.array(list(c.quant_table), np.uint16)))
     return Parsed(int(j.w), int(j.h), planes)
+
+
+def parse_jpeg4(data: bytes, flags: int = 0) -> Parsed:
+    """Parse JPEG bytes with j2p_read_jpeg4_mem, which takes four-component files (J2P_READ_CMYK is
+    always on); a four-component Parsed has its colour kind.  The ValueError carries the reader's
+    message and, as .ncomp, the frame header's component count (0 when it was not read)."""
+    lib = load_codecs()
+    j = Jpeg4()
+    err = C.create_string_buffer(256)
+    if lib.j2p_read_jpeg4_mem(data, len(data), flags, C.byref(j), err, 256) != 0:
+        e = ValueError(err.value.decode(errors='replace'))
+        e.ncomp = int(j.ncomp)
+        raise e
+    planes = []
+    for c in j.coefs[:j.ncomp]:
+        n = c.w * c.h
+        d = np.ctypeslib.as_array(c.data, shape=(n,)).copy() if n else np.zeros(0, np.int16)
+        abi.free_ptr(c.data)
+        planes.append(Plane(int(c.w), int(c.h), int(c.w_samp), int(c.h_samp), d, np.array(list(c.quant_table), np.uint16)))
+    return Parsed(int(j.w), int(j.h), planes, int(j.colour))
 
 
 def exif_orientation(data: bytes) -> int:
@@ -475,10 +582,13 @@ def solver_flags(iterations, weight, pweight, separate):
 def solved_planes(key, separate: bool, mode: str = 'RGB'):
     """(planes solved, output channels) of a frame of `key` in `mode`: a gray file's one plane and
     one channel; for a colour file all three planes and three channels, or one channel in mode
-    'GRAY', from the luma alone when separate."""
+    'GRAY', from the luma alone when separate; for a four-component file all four planes, and four
+    channels, or three in mode 'RGB'."""
     planes = key[2]
     if len(planes) == 1:
         return 1, 1
+    if len(planes) == 4:
+        return 4, (3 if mode == 'RGB' else 4)
     if mode == 'GRAY':
         return (1 if separate else 3), 1
     return 3, 3
@@ -490,7 +600,7 @@ def frame_footprint(key, separate: bool, sample_bytes: int, mode: str = 'RGB', r
     the reduction state) plus its part of the output tensor, for the planes solved and the channels
     written in `mode` (solved_planes).  record_rows: iterations the frame's sessions record
     (return_objective), five fp64 sums each (DESIGN §7o), plus the projection's partials."""
-    w, h, planes = key
+    w, h, planes = key[:3]
     nsolved, nout = solved_planes(key, separate, mode)
     planes = planes[:nsolved]
 
@@ -503,19 +613,33 @@ def frame_footprint(key, separate: bool, sample_bytes: int, mode: str = 'RGB', r
             n += (pw * ph + 127) // 128 * 128 * 2 + (pw * ph + 63) // 64 * 64 * 4
         return n + (16 << 10)
 
-    total = sum(session([p]) for p in planes) if separate else session(list(planes))
+    if len(planes) == 4:        # CMYK: every plane alone; YCCK: Y, Cb, Cr as a colour file, K alone
+        total = (sum(session([p]) for p in planes) if separate or key[3] == CMYK else
+                 session(list(planes[:3])) + session([planes[3]]))
+    else:
+        total = sum(session([p]) for p in planes) if separate else session(list(planes))
     if record_rows:
         total += 40 * record_rows + 3 * 8 * sum((pw // 8) * (ph // 8) for pw, ph, _, _ in planes)
     return total + w * h * nout * sample_bytes
 
 
+def max_files(key) -> int:
+    """Files per chunk of `key` its sessions can hold: MAX_BATCH, or MAX_BATCH // 4 for a CMYK key
+    whose four planes share one grid, solved in one batch session of four frames per file."""
+    planes = key[2]
+    if len(planes) == 4 and key[3] == CMYK and len(set(planes)) == 1:
+        return MAX_BATCH // 4
+    return MAX_BATCH
+
+
 def chunk_frames(key, separate: bool, sample_bytes: int, max_frames, free_bytes: int, mode: str = 'RGB') -> int:
     """Frames per batch of `key`: max_frames, or as many as keep the estimated footprint of two
-    chunks in flight (one solving while the next is uploaded) under half of `free_bytes`."""
+    chunks in flight (one solving while the next is uploaded) under half of `free_bytes`; never more
+    than max_files(key)."""
     if max_frames is not None:
-        return min(int(max_frames), MAX_BATCH)
+        return min(int(max_frames), max_files(key))
     per = frame_footprint(key, separate, sample_bytes, mode)
-    return max(1, min(MAX_BATCH, free_bytes // 4 // per))
+    return max(1, min(max_files(key), free_bytes // 4 // per))
 
 
 def plan(keys, frames_for_key):
@@ -548,10 +672,11 @@ def group_class(key, separate: bool, mode: str = 'RGB'):
     """The class of a chunk of `key` for grouping, or None when it is solved on its own: chunks of one
     class may share a group (the join rules of j2p_session_iterate_group: one session per chunk, equal
     plane count and sampling factors, every plane 1x1 or 2x2), and only frames of at most
-    GROUP_MAX_PIXELS pixels are grouped.  Separate-mode colour chunks (a session per plane) are not."""
-    w, h, planes = key
+    GROUP_MAX_PIXELS pixels are grouped.  Separate-mode colour chunks (a session per plane) and
+    four-component chunks are not."""
+    w, h, planes = key[:3]
     nsolved, _ = solved_planes(key, separate, mode)
-    if separate and len(planes) > 1:
+    if (separate and len(planes) > 1) or len(planes) == 4:
         return None
     solved = planes[:nsolved]
     if any((ws, hs) not in ((1, 1), (2, 2)) for _, _, ws, hs in solved):
@@ -616,13 +741,15 @@ class _DeviceCoefs:
     the decoder runs there, and the constructor waits for the decode only.  status[i]: J2P_ENT_OK
     or the failure kind of file i."""
 
+    per = 3                     # planes per file in ptrs
+
     def __init__(self, device, layouts, stream, subseq_bits=SUBSEQ_BITS):
         self._decode(device, layouts, stream, subseq_bits, entropy_plan, load_entropy(), 'entropy', EntropyStats())
 
     def _decode(self, device, layouts, stream, subseq_bits, make_plan, lib, name, stats):
         dev = torch.device('cuda', device)
-        # three planes per file, the ones a gray file does not have empty
-        sizes = [lay.planes[c].w * lay.planes[c].h if c < len(lay.planes) else 0 for lay in layouts for c in range(3)]
+        # `per` planes per file, the ones a gray file does not have empty
+        sizes = [lay.planes[c].w * lay.planes[c].h if c < len(lay.planes) else 0 for lay in layouts for c in range(self.per)]
         offs = np.concatenate([[0], np.cumsum(sizes, dtype=np.int64)])
         with torch.cuda.stream(stream):
             self.coefs = torch.empty(max(int(offs[-1]), 1), dtype=torch.int16, device=dev)
@@ -642,13 +769,23 @@ class _DeviceCoefs:
         self.plan = self.work = self.plan_dev = None
 
     def plane(self, i, c):
-        return self.ptrs[3 * i + c]
+        return self.ptrs[self.per * i + c]
 
     def plane_tensor(self, i, c):
         """A view of file i's plane c in the coefficient tensor (int16, blocks * 64)."""
-        start = (self.ptrs[3 * i + c] - self.coefs.data_ptr()) // 2
-        end = (self.ptrs[3 * i + c + 1] - self.coefs.data_ptr()) // 2 if 3 * i + c + 1 < len(self.ptrs) else self.coefs.numel()
+        k = self.per * i + c
+        start = (self.ptrs[k] - self.coefs.data_ptr()) // 2
+        end = (self.ptrs[k + 1] - self.coefs.data_ptr()) // 2 if k + 1 < len(self.ptrs) else self.coefs.numel()
         return self.coefs[start:end]
+
+
+class _DeviceCoefs4(_DeviceCoefs):
+    """_DeviceCoefs for four-component files (FileLayout4), four planes per file, decoded by
+    libj2pentropy.so through j2p_entropy_pack4."""
+    per = 4
+
+    def __init__(self, device, layouts, stream, subseq_bits=SUBSEQ_BITS):
+        self._decode(device, layouts, stream, subseq_bits, entropy_plan4, load_entropy(), 'entropy', EntropyStats())
 
 
 class _ProgCoefs(_DeviceCoefs):
@@ -685,14 +822,28 @@ class _Chunk:
         self.lib, self.sessions, self.coefs = lib, [], coefs or {}
         first, n = items[0], len(items)
         nsolved, nout = solved_planes(first.key(), separate, mode)
-        if nsolved == 1 or separate:
-            work = [(_frame_desc(first, [c], weights[c], pweights, iters[c]), [c], iters[c]) for c in range(nsolved)]
+        # work: (descriptor, the planes a session holds of every file, iterations); a session has
+        # n * len(planes) / nchannel frames, file f's plane planes[k] in its plane f * len(planes) + k
+        self.four = first.colour if nsolved == 4 else 0
+        if self.four == CMYK:           # each plane alone with the luma's flags (DESIGN §7q)
+            pw = (pweights[0],) * 4
+            if len({(p.w, p.h, p.w_samp, p.h_samp) for p in first.planes}) == 1:
+                work = [(_frame_desc(first, [0], weights[0], pw, iters[0]), [0, 1, 2, 3], iters[0])]
+            else:
+                work = [(_frame_desc(first, [c], weights[0], pw, iters[0]), [c], iters[0]) for c in range(4)]
         else:
-            work = [(_frame_desc(first, [0, 1, 2], weights[0], pweights, iters[0]), [0, 1, 2], iters[0])]
+            pw = tuple(pweights) + (pweights[0],)
+            ncolour = 3 if self.four else nsolved
+            if ncolour == 1 or separate:
+                work = [(_frame_desc(first, [c], weights[c], pw, iters[c]), [c], iters[c]) for c in range(ncolour)]
+            else:
+                work = [(_frame_desc(first, [0, 1, 2], weights[0], pw, iters[0]), [0, 1, 2], iters[0])]
+            if self.four:               # YCCK: K alone with the luma's flags
+                work.append((_frame_desc(first, [3], weights[0], pw, iters[0]), [3], iters[0]))
         try:
-            for desc, _, _ in work:
+            for desc, channels, _ in work:
                 s = C.c_void_p()
-                self._check(lib.j2p_session_create_batch(C.byref(s), device, C.byref(desc), n))
+                self._check(lib.j2p_session_create_batch(C.byref(s), device, C.byref(desc), n * len(channels) // desc.nchannel))
                 self.sessions.append(s)
                 if record:
                     self._check(lib.j2p_session_record_objective(s, 1))
@@ -746,7 +897,15 @@ class _Chunk:
             # name it cudaStreamLegacy (1) instead
             stream = C.c_void_p(torch.cuda.current_stream(device).cuda_stream or 1)
             dst = C.c_void_p(self.out.data_ptr())
-            if self.shapes is not None:
+            if self.four:
+                orient = None
+                if self.shapes is not None:
+                    self.orient = torch.tensor(orientations, dtype=torch.uint8).to(cuda)
+                    orient = C.c_void_p(self.orient.data_ptr())
+                ss = self.sessions
+                self._check(lib.j2p_session_export_four((C.c_void_p * len(ss))(*ss), len(ss), self.four, nout, 0, n, orient,
+                                                        C.byref(o), dst, stream))
+            elif self.shapes is not None:
                 # uploaded on the current stream, which the export runs on
                 self.orient = torch.tensor(orientations, dtype=torch.uint8).to(cuda)
                 ss = self.sessions[:1] if nout == 1 else self.sessions
@@ -835,6 +994,53 @@ def _front_end(data, device_ok, progressive=False, flags=0):
         return e
 
 
+# Four-component files on the device decoder (DESIGN §7q): a decoder state at a subsequence boundary
+# is (bit, block within the MCU).  When every component of an interleaved scan uses the same Huffman
+# tables (Pillow's and libjpeg's CMYK files), a guessed state finds the bit alignment but not the
+# block's place in the MCU, so each sync round corrects one more subsequence of a segment: such a
+# file goes to the device only when its longest segment is at most FOUR_SYNC_SUBSEQ subsequences.
+# Measured on an H100 (tools/cmyk_bench.py, 64 1080p Pillow CMYK files): segments of 80 subsequences
+# (one restart interval per MCU row) decode in 2.9 ms per image on the device against 10.9 on the
+# host, one segment of about 8000 in 44.7 against 12.1; the limit lies between the two.
+FOUR_SYNC_SUBSEQ = 512
+
+
+def four_on_device(lay) -> bool:
+    """Whether a device-decodable FileLayout4 goes to the device decoder (see FOUR_SYNC_SUBSEQ)."""
+    same_tables = False
+    for k in range(lay.lay.nscan):
+        sc = lay.lay.scan[k]
+        tabs = {(bytes(sc.dc[s]), bytes(sc.ac[s])) for s in range(sc.ncomp)}
+        same_tables |= sc.ncomp > 1 and len(tabs) == 1
+    if not same_tables:
+        return True
+    longest = max((int(lay.lay.seg[k].len) for k in range(lay.lay.nseg)), default=0)
+    return -(-longest * 8 // SUBSEQ_BITS) <= FOUR_SYNC_SUBSEQ
+
+
+def _front_end_four(data, device_ok, progressive=False, flags=0):
+    """_front_end, and for a file it refuses, the four-component reader (parse_jpeg4): a four-component
+    file's Parsed, or the four-component reader's error for a four-component file; every other file's
+    result is _front_end's.  With a device, a four-component sequential Huffman file whose components
+    are each in one scan is a FileLayout4 for the device decoder when four_on_device says so; other
+    four-component files are parsed on the host (DESIGN §7q)."""
+    p = _front_end(data, device_ok, progressive, flags)
+    if not isinstance(p, ValueError):
+        return p
+    if device_ok and not _host_front_end:
+        try:
+            lay = FileLayout4(data, flags)
+        except ValueError:
+            lay = None          # the four-component reader below gives the message
+        if lay is not None and lay.device_decodable and len(lay.planes) == 4 and four_on_device(lay):
+            return lay
+    try:
+        q = parse_jpeg4(data, flags)
+    except ValueError as e:
+        return e if e.ncomp == 4 else p
+    return q if len(q.planes) == 4 else p
+
+
 def decode_jpeg(inputs, *, iterations=50, weight=0.3, pweight=0.001, separate=False,
                 dtype=torch.uint8, layout='CHW', device=None, max_frames=None, progressive_on_device=False,
                 mode='RGB', apply_exif_orientation=False, return_objective=False):
@@ -847,12 +1053,27 @@ def decode_jpeg(inputs, *, iterations=50, weight=0.3, pweight=0.001, separate=Fa
     PNG samples) or torch.float32 (the clamped samples before truncation).
 
     mode: 'RGB' (c = 3; a grayscale file is refused with the reader's "only 3 component jpegs are
-    supported"), 'UNCHANGED' (c = 1 for a grayscale file, 3 for a colour file) or 'GRAY' (c = 1
-    for every file).  A one-channel sample is the RGB sample of its luma with zero chroma, so a gray
+    supported"), 'UNCHANGED' (c = 1 for a grayscale file, 3 for a colour file, 4 for a CMYK or YCCK
+    file) or 'GRAY' (c = 1 for every file; four-component files are refused with the reader's "only 1
+    and 3 component jpegs are supported").  A one-channel sample is the RGB sample of its luma with zero chroma, so a gray
     tensor t gives the RGB image as t.expand(3, -1, -1) (CHW).  A grayscale file is solved as the
     luma of separate mode, with the first of three iterations, weights and pweights, so its result
     does not depend on `separate`.  For a colour file, mode='GRAY' gives the luma of the joint solve,
     or with separate=True the luma solve alone: its chroma planes are neither uploaded nor solved.
+
+    Four-component files (Adobe CMYK and YCCK, DESIGN §7q): the kind is libjpeg's, from the last
+    Adobe APP14 segment before the first SOS (none or transform 0: CMYK, any other transform: YCCK).
+    mode='UNCHANGED' gives Pillow's CMYK samples, which are inverted: channel c of a CMYK file is
+    255 - g (uint8), 65535 - g (uint16) or 255.0 - g (float32), with g the gray sample of plane c,
+    each plane solved alone as a grayscale file is, whatever `separate` is.  A YCCK file's channels
+    0-2 are the RGB samples of its Y, Cb, Cr solved as a colour file's planes (`separate` applies),
+    and channel 3 is its K plane inverted, solved alone.  mode='RGB' with torch.uint8 gives Pillow's
+    Image.convert('RGB') of the uint8 samples; with uint16 or float32 it raises ValueError (use
+    mode='UNCHANGED').  Sequential ones whose components are each in one scan are Huffman-decoded
+    on the device (j2p_read_jpeg_layout4, libj2pentropy.so), except files whose components all share
+    one Huffman table and whose longest segment is over FOUR_SYNC_SUBSEQ subsequences
+    (four_on_device); progressive and arithmetic ones go to the host reader whatever
+    progressive_on_device.  return_objective=True refuses them.
 
     iterations, weight, pweight, separate: the command line's -i, -w, -p and -s.  Scalars as there:
     a scalar weight sets luma only; three weights or three iteration counts need separate=True.
@@ -920,20 +1141,27 @@ def decode_jpeg(inputs, *, iterations=50, weight=0.3, pweight=0.001, separate=Fa
     # parsed on the host.  Either runs without the GIL (ctypes), many files in parallel.
     device_ok = torch.cuda.is_available()
     workers = min(len(read), os.cpu_count() or 1, 16)
+    front_end = _front_end if mode == 'GRAY' else _front_end_four
     if workers > 1:
         with ThreadPoolExecutor(workers) as pool:
-            parsed = list(pool.map(lambda d: _front_end(d, device_ok, progressive_on_device, read_flags),
+            parsed = list(pool.map(lambda d: front_end(d, device_ok, progressive_on_device, read_flags),
                                    [data for data, _ in read]))
             orientations = (list(pool.map(exif_orientation, [data for data, _ in read]))
                             if apply_exif_orientation else None)
     else:
-        parsed = [_front_end(data, device_ok, progressive_on_device, read_flags) for data, _ in read]
+        parsed = [front_end(data, device_ok, progressive_on_device, read_flags) for data, _ in read]
         orientations = [exif_orientation(data) for data, _ in read] if apply_exif_orientation else None
     for i, (p, (_, path)) in enumerate(zip(parsed, read)):
         if isinstance(p, ValueError):
             raise ValueError(f'{_where(i, path)}: {p}')
         if isinstance(p, RuntimeError):
             raise RuntimeError(f'{_where(i, path)}: {p} (a decoder bug)')
+        if isinstance(p, (Parsed, FileLayout4)) and len(p.planes) == 4:
+            if mode == 'RGB' and dtype != torch.uint8:
+                raise ValueError(f"{_where(i, path)}: a four-component (CMYK or YCCK) file has an RGB conversion for "
+                                 f"torch.uint8 only; use mode='UNCHANGED' for its four channels as {dtype}")
+            if return_objective:
+                raise ValueError(f'{_where(i, path)}: return_objective is not available for four-component (CMYK or YCCK) files')
 
     lib = abi.load_product()
     if not device_ok or lib.j2p_device_count() <= 0:
@@ -999,7 +1227,8 @@ def decode_jpeg(inputs, *, iterations=50, weight=0.3, pweight=0.001, separate=Fa
 
             def chunk_coefs(idx):
                 coefs = {}
-                for kind, decoder, failures in ((FileLayout, _DeviceCoefs, ENT_FAILURES), (ProgFileLayout, _ProgCoefs, ENT_FAILURES),
+                for kind, decoder, failures in ((FileLayout, _DeviceCoefs, ENT_FAILURES), (FileLayout4, _DeviceCoefs4, ENT_FAILURES),
+                                                (ProgFileLayout, _ProgCoefs, ENT_FAILURES),
                                                 (ArithFileLayout, _ArithCoefs, ARITH_FAILURES)):
                     on_dev = [j for j, i in enumerate(idx) if isinstance(parsed[i], kind)]
                     if not on_dev:
@@ -1010,7 +1239,7 @@ def decode_jpeg(inputs, *, iterations=50, weight=0.3, pweight=0.001, separate=Fa
                             i = idx[j]
                             where = _where(i, read[i][1])
                             try:
-                                parse_jpeg(read[i][0], read_flags)
+                                (parse_jpeg4 if kind is FileLayout4 else parse_jpeg)(read[i][0], read_flags)
                             except ValueError as e:
                                 raise ValueError(f'{where}: {e}') from None
                             raise RuntimeError(f'{where}: the device entropy decoder failed '

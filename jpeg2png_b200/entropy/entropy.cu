@@ -13,19 +13,24 @@ static const uint32_t kMagic = 0x4a32454eu;     // "J2EN"
 
 // ---- plan --------------------------------------------------------------------------------------
 struct Counts {
-    uint32_t nscan = 0, nseg = 0, nsub = 0;
+    uint32_t nscan = 0, nseg = 0, nsub = 0, nslot = 3;
     uint64_t nblocks = 0, data = 0;
 };
 
-static int count(const struct j2p_jpeg_layout *const *L, unsigned n, unsigned S, Counts *c) {
+// Layout: struct j2p_jpeg_layout (planes of three-component and gray files, out[3 * i + c]) or
+// struct j2p_jpeg_layout4 (four-component files, out[4 * i + c]); NP: its planes per file
+template <class Layout>
+static int count(const Layout *const *L, unsigned n, unsigned S, Counts *c) {
     if (S < 32 || S % 32) return fail("subseq_bits must be a positive multiple of 32 (got %u)", S);
     for (unsigned i = 0; i < n; i++) {
-        const struct j2p_jpeg_layout *l = L[i];
+        const Layout *l = L[i];
         if (!l || !l->device_decodable) return fail("layout %u is not device-decodable", i);
         for (unsigned k = 0; k < l->nscan; k++) {
-            const struct j2p_jpeg_scan *sc = &l->scan[k];
+            const auto *sc = &l->scan[k];
             unsigned bpm = 0;
             for (unsigned s = 0; s < sc->ncomp; s++) bpm += sc->bw[s] * sc->bh[s];
+            if (bpm > J2P_ENT_MAX_BPM) return fail("layout %u: %u blocks per MCU", i, bpm);
+            if (sc->ncomp > 3) c->nslot = 4;
             c->nblocks += (uint64_t)sc->mcux * sc->mcuy * bpm;
         }
         c->nscan += l->nscan;
@@ -46,7 +51,8 @@ static void offsets(unsigned n, const Counts &c, struct j2p_ent_header *h) {
     h->nfiles = n;
     h->nscan = c.nscan;
     h->nseg = c.nseg;
-    h->ntab = 6 * c.nscan;
+    h->ntab = 2 * J2P_ENT_PLANES * c.nscan;
+    h->nslot = c.nslot;
     h->nsub = c.nsub;
     h->nblocks = c.nblocks;
     size_t o = align16(sizeof *h);
@@ -59,14 +65,14 @@ static void offsets(unsigned n, const Counts &c, struct j2p_ent_header *h) {
     h->total = o;
 }
 
-// work area: exit states x2, start states, cnt, cnt_x, fcnt, dcs[3], dcs_x[3], diff, flag
+// work area: exit states x2, start states, cnt, cnt_x, fcnt, dcs[nslot], dcs_x[nslot], diff, flag
 static size_t work_layout(const struct j2p_ent_header *h, uint8_t *w, struct j2p_ent_view *v) {
     const size_t ns = h->nsub;
     size_t o = 0;
     auto take = [&](size_t bytes) { uint8_t *p = w ? w + o : nullptr; o = align16(o + bytes); return p; };
     uint8_t *e0 = take(ns * 8), *e1 = take(ns * 8), *st = take(ns * 8);
     uint8_t *cnt = take(ns * 4), *cnt_x = take(ns * 4), *fcnt = take(ns * 4);
-    uint8_t *dcs = take(ns * 12), *dcs_x = take(ns * 12);
+    uint8_t *dcs = take(ns * 4 * h->nslot), *dcs_x = take(ns * 4 * h->nslot);
     uint8_t *diff = take(h->nblocks * 4), *flag = take(4);
     if (v) {
         v->exit_st[0] = (uint64_t *)e0;
@@ -98,14 +104,15 @@ static int view_of(const void *plan_host, const void *plan, void *work, uint32_t
     v->data = b + h->off_data;
     v->nsub = h->nsub;
     v->subseq_bits = h->subseq_bits;
+    v->nslot = h->nslot;
     v->status = status;
     work_layout(h, (uint8_t *)work, v);
     *hp = h;
     return 0;
 }
 
-extern "C" int j2p_entropy_plan_size(const struct j2p_jpeg_layout *const *layouts, unsigned n, unsigned subseq_bits,
-                                     size_t *plan_bytes, size_t *work_bytes) {
+template <class Layout>
+static int plan_size(const Layout *const *layouts, unsigned n, unsigned subseq_bits, size_t *plan_bytes, size_t *work_bytes) {
     Counts c;
     if (count(layouts, n, subseq_bits, &c) != 0) return -1;
     struct j2p_ent_header h;
@@ -116,8 +123,8 @@ extern "C" int j2p_entropy_plan_size(const struct j2p_jpeg_layout *const *layout
     return 0;
 }
 
-extern "C" int j2p_entropy_pack(const struct j2p_jpeg_layout *const *L, unsigned n, unsigned S, int16_t *const *out, void *dst,
-                                size_t plan_bytes) {
+template <class Layout, int NP>
+static int pack(const Layout *const *L, unsigned n, unsigned S, int16_t *const *out, void *dst, size_t plan_bytes) {
     Counts c;
     if (count(L, n, S, &c) != 0) return -1;
     if (!dst || (!out && n)) return fail("null argument");
@@ -136,15 +143,16 @@ extern "C" int j2p_entropy_pack(const struct j2p_jpeg_layout *const *L, unsigned
     uint32_t iscan = 0, iseg = 0, isub = 0, diff_base = 0;
     uint64_t doff = 0;
     for (unsigned i = 0; i < n; i++) {
-        const struct j2p_jpeg_layout *l = L[i];
+        const Layout *l = L[i];
         j2p_ent_file *f = &files[i];
-        for (int p = 0; p < 3; p++) {
+        memset(f, 0, sizeof *f);
+        for (int p = 0; p < NP; p++) {
             f->wb[p] = l->coefs[p].w / 8;
             f->hb[p] = l->coefs[p].h / 8;
-            f->out[p] = f->wb[p] ? out[3 * i + p] : nullptr;     // a gray file's planes 1 and 2 are empty
+            f->out[p] = f->wb[p] ? out[NP * i + p] : nullptr;    // a gray file's planes 1 and 2 are empty
         }
         for (unsigned k = 0; k < l->nscan; k++, iscan++) {
-            const struct j2p_jpeg_scan *ls = &l->scan[k];
+            const auto *ls = &l->scan[k];
             j2p_ent_scan *sc = &scans[iscan];
             memset(sc, 0, sizeof *sc);
             sc->file = i;
@@ -155,8 +163,8 @@ extern "C" int j2p_entropy_pack(const struct j2p_jpeg_layout *const *L, unsigned
                 sc->comp[s] = ls->comp[s];
                 sc->bw[s] = ls->bw[s];
                 sc->bh[s] = ls->bh[s];
-                sc->dctab[s] = 6 * iscan + 2 * s;
-                sc->actab[s] = 6 * iscan + 2 * s + 1;
+                sc->dctab[s] = 2 * J2P_ENT_PLANES * iscan + 2 * s;
+                sc->actab[s] = 2 * J2P_ENT_PLANES * iscan + 2 * s + 1;
                 j2p_ent_build_table(&ls->dc[s], &tabs[sc->dctab[s]]);
                 j2p_ent_build_table(&ls->ac[s], &tabs[sc->actab[s]]);
                 for (unsigned y = 0; y < ls->bh[s]; y++)
@@ -166,7 +174,8 @@ extern "C" int j2p_entropy_pack(const struct j2p_jpeg_layout *const *L, unsigned
                         sc->dy[bpm] = (uint8_t)y;
                     }
             }
-            for (unsigned s = ls->ncomp; s < 3; s++) memset(&tabs[6 * iscan + 2 * s], 0, 2 * sizeof(j2p_ent_table));   // unused slots
+            for (unsigned s = ls->ncomp; s < J2P_ENT_PLANES; s++)
+                memset(&tabs[2 * J2P_ENT_PLANES * iscan + 2 * s], 0, 2 * sizeof(j2p_ent_table));   // unused slots
             sc->bpm = bpm;
             sc->diff_base = diff_base;
             diff_base += ls->mcux * ls->mcuy * bpm;
@@ -191,6 +200,26 @@ extern "C" int j2p_entropy_pack(const struct j2p_jpeg_layout *const *L, unsigned
         }
     }
     return 0;
+}
+
+extern "C" int j2p_entropy_plan_size(const struct j2p_jpeg_layout *const *layouts, unsigned n, unsigned subseq_bits,
+                                     size_t *plan_bytes, size_t *work_bytes) {
+    return plan_size(layouts, n, subseq_bits, plan_bytes, work_bytes);
+}
+
+extern "C" int j2p_entropy_pack(const struct j2p_jpeg_layout *const *L, unsigned n, unsigned S, int16_t *const *out, void *dst,
+                                size_t plan_bytes) {
+    return pack<struct j2p_jpeg_layout, 3>(L, n, S, out, dst, plan_bytes);
+}
+
+extern "C" int j2p_entropy_plan_size4(const struct j2p_jpeg_layout4 *const *layouts, unsigned n, unsigned subseq_bits,
+                                      size_t *plan_bytes, size_t *work_bytes) {
+    return plan_size(layouts, n, subseq_bits, plan_bytes, work_bytes);
+}
+
+extern "C" int j2p_entropy_pack4(const struct j2p_jpeg_layout4 *const *L, unsigned n, unsigned S, int16_t *const *out, void *dst,
+                                 size_t plan_bytes) {
+    return pack<struct j2p_jpeg_layout4, 4>(L, n, S, out, dst, plan_bytes);
 }
 
 // ---- host driver -------------------------------------------------------------------------------
@@ -222,7 +251,7 @@ extern "C" int j2p_entropy_decode_host(const void *plan, void *work, uint32_t *s
         const uint32_t file = v.scans[v.segs[v.sub_seg[j]].scan].file;
         if (rc != J2P_ENT_OK && status[file] == 0) status[file] = (uint32_t)rc;
     }
-    scan_host(v.dcs, v.dcs_x, h->nsub, 3);
+    scan_host(v.dcs, v.dcs_x, h->nsub, (int)h->nslot);
     for (uint32_t j = 0; j < h->nsub; j++) j2p_ent_dc_one(&v, j);
     if (stats) {
         stats->rounds = rounds;
@@ -342,7 +371,7 @@ extern "C" int j2p_entropy_decode(const void *plan_host, const void *plan_dev, v
         CK(cudaGetLastError());
         k_ent_final<<<grid, kThreads, 0, st>>>(v);
         CK(cudaGetLastError());
-        k_ent_scan<<<1, kScanThreads, 0, st>>>(v.dcs, v.dcs_x, h->nsub, 3);
+        k_ent_scan<<<1, kScanThreads, 0, st>>>(v.dcs, v.dcs_x, h->nsub, (int)h->nslot);
         CK(cudaGetLastError());
         k_ent_dc<<<grid, kThreads, 0, st>>>(v);
         CK(cudaGetLastError());

@@ -26,6 +26,7 @@ extern "C" {
 enum { J2P_ENT_OK = 0, J2P_ENT_BAD_CODE = 1, J2P_ENT_BAD_MAGNITUDE = 2, J2P_ENT_BAD_INDEX = 3 };
 
 struct j2p_jpeg_layout;
+struct j2p_jpeg_layout4;
 
 struct j2p_entropy_stats {
         unsigned rounds;        /* sync rounds launched */
@@ -43,6 +44,13 @@ int j2p_entropy_plan_size(const struct j2p_jpeg_layout *const *layouts, unsigned
  * (J2P_READ_GRAY, w = h = 0) are never written and their out entries are not read. */
 int j2p_entropy_pack(const struct j2p_jpeg_layout *const *layouts, unsigned n, unsigned subseq_bits, int16_t *const *out,
                      void *dst, size_t plan_bytes);
+/* The same for four-component files (struct j2p_jpeg_layout4 of j2p_read_jpeg_layout4, device
+ * decodable): out[4 * i + c] is where plane c of file i goes.  One- and three-component layouts of
+ * j2p_read_jpeg_layout4 are taken too, their empty planes' out entries not read. */
+int j2p_entropy_plan_size4(const struct j2p_jpeg_layout4 *const *layouts, unsigned n, unsigned subseq_bits, size_t *plan_bytes,
+                           size_t *work_bytes);
+int j2p_entropy_pack4(const struct j2p_jpeg_layout4 *const *layouts, unsigned n, unsigned subseq_bits, int16_t *const *out,
+                      void *dst, size_t plan_bytes);
 /* Decodes on `stream` (a cudaStream_t; NULL: the legacy default stream).  plan_host: the packed
  * plan; plan_dev: its copy in device memory (uploaded on `stream` or before it); work_dev:
  * work_bytes of device memory; status_dev: uint32 per file.  Returns when the last kernel is

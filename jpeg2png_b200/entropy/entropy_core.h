@@ -29,7 +29,9 @@
 #include "../common/codec_host.h"       /* J2P_HD */
 #include "entropy.h"
 
-#define J2P_ENT_MAX_BPM 48      /* blocks per MCU: three components of up to 4x4 (the reader allows 4) */
+#define J2P_ENT_MAX_BPM 48      /* blocks per MCU: three components of up to 4x4 (the reader allows 4); a
+                                   four-component file's interleaved scan has at most 10 (jpeg_reader.h) */
+#define J2P_ENT_PLANES 4        /* planes per file: three (colour), one (gray) or four (CMYK, YCCK) used */
 
 /* one Huffman table: T.81 F.2.2.3 as jpeg_reader.c's build_huff, plus a 9-bit first level */
 struct j2p_ent_table {
@@ -38,12 +40,12 @@ struct j2p_ent_table {
         uint8_t vals[256];
 };
 struct j2p_ent_file {
-        int16_t *out[3];        /* int16 [hb][wb][64] per plane, natural order */
-        uint32_t wb[3], hb[3];  /* real block grids */
+        int16_t *out[J2P_ENT_PLANES];       /* int16 [hb][wb][64] per plane, natural order */
+        uint32_t wb[J2P_ENT_PLANES], hb[J2P_ENT_PLANES];   /* real block grids */
 };
 struct j2p_ent_scan {
         uint32_t file, ncomp, bpm, mcux;
-        uint32_t comp[3], bw[3], bh[3], dctab[3], actab[3];
+        uint32_t comp[J2P_ENT_PLANES], bw[J2P_ENT_PLANES], bh[J2P_ENT_PLANES], dctab[J2P_ENT_PLANES], actab[J2P_ENT_PLANES];
         uint32_t diff_base;     /* the scan's first block in the DC-difference array */
         uint8_t slot[J2P_ENT_MAX_BPM], dx[J2P_ENT_MAX_BPM], dy[J2P_ENT_MAX_BPM];   /* block r of an MCU */
 };
@@ -54,7 +56,8 @@ struct j2p_ent_seg {
         uint32_t sub0, nsub;    /* its subsequences */
 };
 struct j2p_ent_header {
-        uint32_t magic, nfiles, nscan, nseg, ntab, nsub, subseq_bits, pad;
+        uint32_t magic, nfiles, nscan, nseg, ntab, nsub, subseq_bits;
+        uint32_t nslot;         /* scan slots with DC sums: 3, or 4 when a scan has four components */
         uint64_t nblocks;       /* DC differences (all blocks of all scans, padding included) */
         uint64_t off_files, off_scans, off_segs, off_subs, off_tabs, off_data, total;
 };
@@ -67,13 +70,13 @@ struct j2p_ent_view {
         const uint32_t *sub_seg;    /* subsequence -> segment */
         const struct j2p_ent_table *tabs;
         const uint8_t *data;
-        uint32_t nsub, subseq_bits;
+        uint32_t nsub, subseq_bits, nslot;
         /* work */
         uint64_t *exit_st[2];       /* exit state per subsequence, by round parity */
         uint64_t *start_st;         /* the start state of its last decode */
         uint32_t *cnt, *cnt_x;      /* blocks owned (sync), exclusive scan */
         uint32_t *fcnt;             /* blocks decoded by the final pass */
-        uint32_t *dcs, *dcs_x;      /* [3][nsub] DC sums per scan slot, exclusive scan */
+        uint32_t *dcs, *dcs_x;      /* [nslot][nsub] DC sums per scan slot, exclusive scan */
         int32_t *diff;              /* DC difference per block */
         uint32_t *changed;
         uint32_t *status;           /* per file */
@@ -273,7 +276,7 @@ J2P_HD int j2p_ent_final_one(const struct j2p_ent_view *v, uint32_t j) {
         const uint64_t start = v->start_st[j];
         uint32_t gi = g->block0 + (v->cnt_x[j] - v->cnt_x[g->sub0]);
         const uint32_t limit = g->block0 + g->nblocks;
-        uint32_t sum[3] = {0, 0, 0}, n = 0;
+        uint32_t sum[4] = {0, 0, 0, 0}, n = 0;
         int rc = J2P_ENT_OK;
         struct j2p_ent_bits b;
         j2p_ent_seek(&b, v->data + g->data_off, g->nbytes, (uint32_t)(start >> 8));
@@ -289,9 +292,14 @@ J2P_HD int j2p_ent_final_one(const struct j2p_ent_view *v, uint32_t j) {
                 sum[0] += s == 0 ? (uint32_t)diff : 0;     /* no dynamic index: keeps the sums in registers */
                 sum[1] += s == 1 ? (uint32_t)diff : 0;
                 sum[2] += s == 2 ? (uint32_t)diff : 0;
+                sum[3] += s == 3 ? (uint32_t)diff : 0;
         }
         v->fcnt[j] = n;
-        for (int s = 0; s < 3; s++) v->dcs[(size_t)s * v->nsub + j] = sum[s];
+#ifdef __CUDA_ARCH__
+#pragma unroll
+#endif
+        for (int s = 0; s < 4; s++)
+                if ((uint32_t)s < v->nslot) v->dcs[(size_t)s * v->nsub + j] = sum[s];
         return rc;
 }
 
@@ -301,8 +309,8 @@ J2P_HD void j2p_ent_dc_one(const struct j2p_ent_view *v, uint32_t j) {
         const struct j2p_ent_seg *g = j2p_ent_range(v, j, &i, &end);
         const struct j2p_ent_scan *sc = &v->scans[g->scan];
         const struct j2p_ent_file *f = &v->files[sc->file];
-        uint32_t pred[3];
-        for (int s = 0; s < 3; s++) pred[s] = v->dcs_x[(size_t)s * v->nsub + j] - v->dcs_x[(size_t)s * v->nsub + g->sub0];
+        uint32_t pred[4] = {0, 0, 0, 0};
+        for (uint32_t s = 0; s < v->nslot; s++) pred[s] = v->dcs_x[(size_t)s * v->nsub + j] - v->dcs_x[(size_t)s * v->nsub + g->sub0];
         const uint32_t gi0 = g->block0 + (v->cnt_x[j] - v->cnt_x[g->sub0]), n = v->fcnt[j];
         for (uint32_t gi = gi0; gi < gi0 + n; gi++) {
                 const uint32_t m = gi / sc->bpm, r = gi - m * sc->bpm, s = sc->slot[r], c = sc->comp[s];
