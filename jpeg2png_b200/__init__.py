@@ -1,7 +1,7 @@
 """jpeg2png_b200: the jpeg2png solver on H100.  `decode_jpeg` (jpeg2png_b200.decode) turns JPEG files
 into CUDA tensors (RGB, or one channel for grayscale files and `mode='GRAY'`), `encode_png`
-(jpeg2png_b200.encode, RGB or gray) and `encode_jpeg` (jpeg2png_b200.jpeg_encode, RGB)
-turn such tensors into PNG or JPEG files on the device (`encode_jpeg(..., optimize=True)` with
+(jpeg2png_b200.encode, RGB or gray) and `encode_jpeg` (jpeg2png_b200.jpeg_encode, RGB or gray,
+and with `cmyk=True` four-channel CMYK tensors as Pillow's Adobe CMYK files) turn such tensors into PNG or JPEG files on the device (`encode_jpeg(..., optimize=True)` with
 per-image optimized Huffman tables, as Pillow's `optimize=True`, and `encode_jpeg(...,
 progressive=True)` with Pillow's progressive files, and `encode_jpeg(..., qtables=)` with given
 quantisation tables, per image if need be); `keep_settings` reads a JPEG file's tables and

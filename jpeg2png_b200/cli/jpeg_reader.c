@@ -956,11 +956,11 @@ int j2p_jpeg_exif_orientation(const void *data, size_t len) {
 int j2p_jpeg_keep_settings(const void *data, size_t len, struct j2p_jpeg_keep *out, char *err, size_t errlen) {
         struct dec *d = calloc(1, sizeof *d);
         if (!d) return -1;
-        d->p = data; d->end = d->p + len; d->err = err; d->errlen = errlen; d->flags = J2P_READ_GRAY; d->headers_only = 1;
+        d->p = data; d->end = d->p + len; d->err = err; d->errlen = errlen; d->flags = J2P_READ_GRAY | J2P_READ_CMYK; d->headers_only = 1;
         if (err && errlen) err[0] = 0;
         memset(out, 0, sizeof *out);
         read_markers(d, data, len);
-        struct coef coefs[3];
+        struct coef coefs[4];                   /* J2P_READ_CMYK: up to four planes */
         memset(coefs, 0, sizeof coefs);
         if (!d->failed) check_planes(d, coefs);
         if (!d->failed) {

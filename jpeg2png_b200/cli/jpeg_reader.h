@@ -228,13 +228,14 @@ int j2p_jpeg_exif_orientation(const void *data, size_t len);
  * for table t: Pillow's Image.quantization) and its frame's components and sampling factors (what
  * Pillow's get_sampling reads).  The headers up to the first SOS go through the reader's own marker
  * loop and segment parsers, and the frame through its table and geometry checks, with
- * J2P_READ_GRAY: a file the reader refuses in its headers is refused with the reader's message, and
- * nothing after the first SOS is read.  Returns 0, or -1 with the message in err. */
+ * J2P_READ_GRAY and J2P_READ_CMYK: a file the reader refuses in its headers is refused with the
+ * reader's message, and nothing after the first SOS is read.  Returns 0, or -1 with the message in
+ * err. */
 struct j2p_jpeg_keep {
         uint16_t qt[4][64];
         unsigned present;
-        unsigned ncomp;             /* 1 or 3 */
-        unsigned comp_h[3], comp_v[3];
+        unsigned ncomp;             /* 1, 3 or 4 (Adobe CMYK or YCCK) */
+        unsigned comp_h[4], comp_v[4];
 };
 int j2p_jpeg_keep_settings(const void *data, size_t len, struct j2p_jpeg_keep *out, char *err, size_t errlen);
 

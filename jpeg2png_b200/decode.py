@@ -159,8 +159,8 @@ ARITH_HOST_NS_PER_BYTE = 190        # j2p_read_jpeg_mem on one host thread
 
 class Keep(C.Structure):
     """struct j2p_jpeg_keep — jpeg2png_b200/cli/jpeg_reader.h."""
-    _fields_ = [('qt', (C.c_uint16 * 64) * 4), ('present', C.c_uint), ('ncomp', C.c_uint), ('comp_h', C.c_uint * 3),
-                ('comp_v', C.c_uint * 3)]
+    _fields_ = [('qt', (C.c_uint16 * 64) * 4), ('present', C.c_uint), ('ncomp', C.c_uint), ('comp_h', C.c_uint * 4),
+                ('comp_v', C.c_uint * 4)]
 
 
 def _declare_codecs(lib):

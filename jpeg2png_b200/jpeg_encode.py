@@ -10,7 +10,8 @@ per image from its own symbol counts.  With `progressive=True` the encoder is li
 libjpeg's ten-scan progression, each scan with tables built from its own symbol counts.
 `restart_marker_blocks` and `restart_marker_rows` add restart intervals to any of the three files,
 as Pillow's keywords of the same names do (DESIGN §7i).  One-channel tensors are written as
-Pillow's one-component ('L') files by the same three libraries, one call per kind (DESIGN §7k).
+Pillow's one-component ('L') files by the same three libraries, one call per kind (DESIGN §7k), and
+with `cmyk=True` four-channel tensors as Pillow's Adobe CMYK files (DESIGN §7r).
 `qtables` writes given quantisation tables, per image if need be, as Pillow's keyword of the same
 name does, and `keep_settings` reads a file's tables and sampling as Pillow's quality='keep' does
 (DESIGN §7n).
@@ -55,7 +56,7 @@ class Qtables(C.Structure):
 class Params(C.Structure):
     """struct j2p_jpegenc_params — jpeg2png_b200/jpegenc/jpegenc.h."""
     _fields_ = [('quality', C.c_int), ('sampling', C.c_int), ('restart_marker_blocks', C.c_int), ('restart_marker_rows', C.c_int),
-                ('components', C.c_int), ('qtables', C.POINTER(Qtables)), ('nqtables', C.c_uint)]
+                ('components', C.c_int), ('qtables', C.POINTER(Qtables)), ('nqtables', C.c_uint), ('cmyk', C.c_int)]
 
 
 class Stats(C.Structure):
@@ -127,17 +128,26 @@ def check_subsampling(subsampling):
         raise ValueError(f"subsampling must be '4:4:4', '4:2:2' or '4:2:0', not {subsampling!r}")
 
 
-def params(quality, subsampling, restart_marker_blocks=0, restart_marker_rows=0, components=3) -> Params:
+def check_cmyk(cmyk):
+    if not isinstance(cmyk, bool):
+        raise ValueError(f'cmyk must be True or False, not {cmyk!r}')
+
+
+def params(quality, subsampling, restart_marker_blocks=0, restart_marker_rows=0, components=3, cmyk=False) -> Params:
     """Checked call parameters: quality an integer in 1..100, subsampling '4:4:4', '4:2:2' or '4:2:0',
     the restart keywords integers in 0..65535, components 3 (RGB images, YCbCr files) or 1 (gray
-    images, one-component files)."""
+    images, one-component files); cmyk=True (with components 3, the default): CMYK images, Adobe
+    CMYK files."""
     check_quality(quality)
     check_subsampling(subsampling)
     blocks = _check_restart('restart_marker_blocks', restart_marker_blocks)
     rows = _check_restart('restart_marker_rows', restart_marker_rows)
     if components not in (1, 3) or isinstance(components, bool):
         raise ValueError(f'components must be 3 or 1, not {components!r}')
-    return Params(int(quality), SAMPLINGS[subsampling], blocks, rows, int(components))
+    check_cmyk(cmyk)
+    if cmyk and components != 3:
+        raise ValueError('cmyk=True writes four-component files: it does not combine with gray (components=1)')
+    return Params(int(quality), SAMPLINGS[subsampling], blocks, rows, 0 if cmyk else int(components), cmyk=int(cmyk))
 
 
 def _check_size(shape, h, w):
@@ -153,7 +163,8 @@ CODEC_PROG = B.Codec('jpegprog', lambda: load_jpegprog(), Image, _check_size)
 def codec(p: Params, optimize=False, progressive=False, sets=None) -> B.Codec:
     """libj2pjpegenc.so, or libj2pjpegopt.so when optimize, or libj2pjpegprog.so when progressive
     (whatever optimize), for the shared driver, with the call parameters p: it takes one-channel
-    images when p is gray (p.components == 1), three-channel ones otherwise.  sets: None (the IJG
+    images when p is gray (p.components == 1), four-channel ones when p is CMYK (p.cmyk), and
+    three-channel ones otherwise.  sets: None (the IJG
     tables of p.quality), or each image's final tables in call order (lists of 64 integers in
     natural order, or None for the IJG tables of p.quality); the distinct ones become the call's
     sets, each stored once."""
@@ -174,7 +185,8 @@ def codec(p: Params, optimize=False, progressive=False, sets=None) -> B.Codec:
         def place(d):
             for x, k in zip(d, index):
                 x.qtables = k
-    return dataclasses.replace(c, params=(C.byref(p),), channels=(1,) if p.components == 1 else c.channels, place=place)
+    channels = (4,) if p.cmyk else (1,) if p.components == 1 else c.channels
+    return dataclasses.replace(c, params=(C.byref(p),), channels=channels, place=place)
 
 
 # ---- quantisation tables ---------------------------------------------------------------------------
@@ -262,7 +274,7 @@ def _subsamplings(subsampling, n):
 def _calls(quality, subsampling, optimize, progressive, restart_marker_blocks, restart_marker_rows, qtables, n, channels):
     """calls(items) for the shared driver: one library call per (channel count, subsampling) kind of
     the n images, each with the distinct tables of its images as its sets; channels(x): x's channel
-    count."""
+    count, 3 (RGB), 1 (gray) or 4 (CMYK)."""
     check_quality(quality, allow_none=True)
     subs = _subsamplings(subsampling, n)
     sets = per_image(qtables, quality, n)
@@ -274,13 +286,15 @@ def _calls(quality, subsampling, optimize, progressive, restart_marker_blocks, r
         kinds = {}
         for i, x in enumerate(items):
             kinds.setdefault((channels(x), subs[i]), []).append(i)
-        return [(codec(params(q, s, blocks, rows, c), optimize, progressive, [sets[i] for i in idx]), idx) for (c, s), idx in kinds.items()]
+        return [(codec(params(q, s, blocks, rows, 1 if c == 1 else 3, c == 4), optimize, progressive, [sets[i] for i in idx]), idx)
+                for (c, s), idx in kinds.items()]
     return calls
 
 
-def _codecs(quality, subsampling, optimize, progressive, restart_marker_blocks, restart_marker_rows):
-    """The codec of each channel count encode_jpeg takes: {3: RGB, 1: gray}."""
-    return {c: codec(params(quality, subsampling, restart_marker_blocks, restart_marker_rows, c), optimize, progressive) for c in (3, 1)}
+def _codecs(quality, subsampling, optimize, progressive, restart_marker_blocks, restart_marker_rows, cmyk=False):
+    """The codec of each channel count encode_jpeg takes: {3: RGB, 1: gray}, and 4: CMYK when cmyk."""
+    return {c: codec(params(quality, subsampling, restart_marker_blocks, restart_marker_rows, 1 if c == 1 else 3, c == 4), optimize, progressive)
+            for c in ((3, 1, 4) if cmyk else (3, 1))}
 
 
 def check_optimize(optimize):
@@ -315,22 +329,26 @@ def _work_bytes(descs, p):
 
 
 def encode_host(images, quality=None, subsampling='4:2:0', layout='HWC', optimize=False, progressive=False, restart_marker_blocks=0,
-                restart_marker_rows=0, gray=False, qtables=None):
+                restart_marker_rows=0, gray=False, qtables=None, cmyk=False):
     """The serial host driver (j2p_jpegenc_encode_host, or j2p_jpegopt_encode_host when optimize,
     or j2p_jpegprog_encode_host when progressive) on numpy uint8 arrays: a list of JPEG files as
     bytes, the same bytes the device writes.  The arrays are RGB, or with gray=True all gray,
-    (h, w, 1) or (1, h, w), written as one-component files.  quality, subsampling and qtables as
-    encode_jpeg takes them (per-image lists included: one call per subsampling)."""
+    (h, w, 1) or (1, h, w), written as one-component files, or with cmyk=True all CMYK, (h, w, 4)
+    or (4, h, w), written as Adobe CMYK files.  quality, subsampling and qtables as encode_jpeg
+    takes them (per-image lists included: one call per subsampling)."""
     B.check_layout(layout)
     if not isinstance(gray, bool):
         raise ValueError(f'gray must be True or False, not {gray!r}')
+    check_cmyk(cmyk)
+    if gray and cmyk:
+        raise ValueError('gray=True and cmyk=True are different kinds of file; give one')
     check_optimize(optimize)
     check_progressive(progressive)
     for x in images:
         if x.dtype != np.uint8:
             raise ValueError(f'samples are uint8, not {x.dtype}')
     calls = _calls(quality, subsampling, optimize, progressive, restart_marker_blocks, restart_marker_rows, qtables, len(images),
-                   lambda x: 1 if gray else 3)
+                   lambda x: 1 if gray else 4 if cmyk else 3)
     out = [None] * len(images)
     for c, idx in calls(images):
         for i, f in zip(idx, B.encode_host(c, [images[i] for i in idx], layout)):
@@ -339,8 +357,8 @@ def encode_host(images, quality=None, subsampling='4:2:0', layout='HWC', optimiz
 
 
 def encode_jpeg(images, *, quality=None, subsampling='4:2:0', layout='CHW', optimize=False, progressive=False, restart_marker_blocks=0,
-                restart_marker_rows=0, qtables=None):
-    """Encode RGB or gray CUDA tensors as baseline or progressive JPEG files on the device.
+                restart_marker_rows=0, qtables=None, cmyk=False):
+    """Encode RGB, gray or CMYK CUDA tensors as baseline or progressive JPEG files on the device.
 
     images: one tensor or a list or tuple of them, torch.uint8, shaped (3, h, w) for layout='CHW'
     or (h, w, 3) for 'HWC', with any strides, 1..65535 pixels high and wide.  quality: an integer
@@ -372,6 +390,18 @@ def encode_jpeg(images, *, quality=None, subsampling='4:2:0', layout='CHW', opti
     subsampling='4:4:4' here.
     Gray and RGB images mix in one list; each kind is one library call.
 
+    cmyk: with True, a tensor with four channels, (4, h, w) or (h, w, 4) (what
+    decode_jpeg(mode='UNCHANGED') returns for a CMYK file), is written as an Adobe CMYK file:
+    Pillow's file of the 'CMYK' image, with every keyword applied.  The samples are stored inverted,
+    as Pillow stores them, so Pillow and decode_jpeg read the tensor's values back.  As in Pillow,
+    subsampling applies to the first component (C) alone and makes M, Y and K half-resolution
+    planes: the default '4:2:0' halves M, Y and K in both directions.  Pillow saving a 'CMYK' image
+    without a subsampling keyword samples every component 1 x 1: that file is subsampling='4:4:4'
+    here.  Without qtables all four components use table 0; with n tables component c uses table
+    min(c, n - 1), so a fourth table is written and used by K.  Gray, RGB and CMYK images mix in
+    one list, one library call per kind.  cmyk is explicit because a four-channel tensor is more
+    often RGBA, which this would write as a wrong file; without it four-channel tensors are refused.
+
     optimize: False writes the Annex K Huffman tables; True builds each image's tables from its own
     symbol counts, on the device, as libjpeg does for `optimize=True`: the same coefficients, files
     typically 6-9% smaller, at the cost of two more kernels per call.
@@ -396,16 +426,18 @@ def encode_jpeg(images, *, quality=None, subsampling='4:2:0', layout='CHW', opti
     written on that stream needs no synchronisation.  Images of any mix of sizes go into one call;
     a list is split into several only when the work area would not fit in a quarter of the free
     device memory.  Raises ValueError for a wrong dtype, shape, layout, quality, subsampling,
-    optimize or progressive (not a bool), restart keyword or size, and for a tensor that is not on
+    optimize, progressive or cmyk (not a bool), restart keyword or size, and for a tensor that is not on
     a CUDA device, and RuntimeError when no CUDA device is usable.
     """
     B.check_layout(layout)
     check_optimize(optimize)
     check_progressive(progressive)
+    check_cmyk(cmyk)
     n = len(images) if isinstance(images, (list, tuple)) else 1
+    channels = (3, 1, 4) if cmyk else (3, 1)
     calls = _calls(quality, subsampling, optimize, progressive, restart_marker_blocks, restart_marker_rows, qtables, n,
-                   lambda x: x.shape[B.axes(x.shape, layout, (3, 1))[4]])
-    codecs = _codecs(75, '4:2:0', optimize, progressive, restart_marker_blocks, restart_marker_rows)      # the checks of the images
+                   lambda x: x.shape[B.axes(x.shape, layout, channels)[4]])
+    codecs = _codecs(75, '4:2:0', optimize, progressive, restart_marker_blocks, restart_marker_rows, cmyk)      # the checks of the images
     return B.encode_tensors('encode_jpeg', codecs, images, layout, (torch.uint8,), calls)
 
 
@@ -416,7 +448,10 @@ def keep_settings(inputs):
     the file defines before its first scan (Pillow's Image.quantization) and its sampling as
     Pillow's get_sampling reads it, '4:4:4', '4:2:2' or '4:2:0' for those colour layouts and, for
     any other (a gray file, 4:4:0, ...), libjpeg's default that Pillow then writes: '4:2:0' for
-    colour, 1 x 1 ('4:4:4' here) for gray.  For a list, the same keys holding lists, which
+    colour, 1 x 1 ('4:4:4' here) for gray.  A four-component file (Adobe CMYK or YCCK) is always
+    '4:4:4': Pillow's get_sampling gives -1 for it, which Pillow writes as 1 x 1 for a CMYK image;
+    so encode_jpeg(decode_jpeg(files, mode='UNCHANGED'), cmyk=True, **keep_settings(files)) is
+    Pillow's quality='keep' re-save of CMYK files.  For a list, the same keys holding lists, which
     encode_jpeg takes per image.  The headers are read by the project's JPEG reader
     (j2p_jpeg_keep_settings): a file it refuses raises ValueError with its message."""
     from . import decode as D
@@ -431,7 +466,7 @@ def keep_settings(inputs):
             raise ValueError(f'{D._where(i, path)}: {err.value.decode(errors="replace")}')
         out['qtables'].append({t: list(k.qt[t]) for t in range(4) if k.present >> t & 1})
         hv = tuple(v for c in range(k.ncomp) for v in (k.comp_h[c], k.comp_v[c]))
-        out['subsampling'].append({(1, 1, 1, 1, 1, 1): '4:4:4', (2, 1, 1, 1, 1, 1): '4:2:2', (2, 2, 1, 1, 1, 1): '4:2:0'}.get(
-            hv, '4:2:0' if k.ncomp == 3 else '4:4:4'))
+        out['subsampling'].append('4:4:4' if k.ncomp == 4 else {(1, 1, 1, 1, 1, 1): '4:4:4', (2, 1, 1, 1, 1, 1): '4:2:2',
+                                                                (2, 2, 1, 1, 1, 1): '4:2:0'}.get(hv, '4:2:0' if k.ncomp == 3 else '4:4:4'))
     return {key: v[0] for key, v in out.items()} if single else out
 

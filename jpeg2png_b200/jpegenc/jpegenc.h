@@ -59,6 +59,23 @@
  * qtables is the IJG tables of params->quality, one set that every image uses (the images' qtables
  * fields are not read); a zero-initialised params keeps that meaning.  The header's length is per
  * set, 623 bytes for the quality tables of a colour file, at most 884 with three 16-bit tables.
+ *
+ * CMYK images (params->cmyk == 1, components 0): each image is four 8-bit channels, C M Y K at
+ * data, data + chan_stride, data + 2 chan_stride, data + 3 chan_stride.  The file is the one
+ * libjpeg writes for a four-component JCS_CMYK image as Pillow drives it for a 'CMYK' image: SOI;
+ * APP14 "Adobe" version 100, flags 0 and 0, transform 0 (FF EE 00 0E 'Adobe' 00 64 00 00 00 00 00)
+ * and no APP0; the DQTs; SOF0 (SOF1 with a 16-bit table) with components 'C' 'M' 'Y' 'K' (67, 77,
+ * 89, 75), C sampled 1x1, 2x1 or 2x2 and M, Y, K 1x1, as Pillow applies subsampling to component 0
+ * alone; DHT DC0 and AC0 only, which every component codes with; SOS of one interleaved scan of
+ * the four.  The samples are coded inverted (Pillow's raw mode CMYK;I): 255 - t for a tensor
+ * sample t, so a decoder that undoes the Adobe inversion, as Pillow and decode_jpeg do, reads t
+ * back.  M, Y and K are downsampled like chroma, from the inverted samples, with no colour
+ * conversion; an MCU is hs x vs blocks of C and one each of M, Y and K.  The quality tables give
+ * table 0 to all four components and one DQT, a 341-byte header; n given tables give component c
+ * table min(c, n - 1) (one: 0 0 0 0; two: 0 1 1 1; three: 0 1 2 2; four: 0 1 2 3, the fourth
+ * table written and used by K) and one DQT each.  The longest header, four 16-bit DQTs, is 804
+ * bytes.  A block costs at most the luma bound, 1658 bits.  Any other cmyk value is refused, and
+ * so is cmyk = 1 with a components value other than 0.
  */
 #ifndef J2P_JPEGENC_H
 #define J2P_JPEGENC_H
@@ -75,7 +92,7 @@ extern "C" {
 enum j2p_jpegenc_sampling { J2P_JPEGENC_444 = 0, J2P_JPEGENC_422 = 1, J2P_JPEGENC_420 = 2 };
 
 struct j2p_jpegenc_image {
-        const void *data;               /* first sample (R of the top-left pixel, or its gray value), uint8 */
+        const void *data;               /* first sample (R, gray or C of the top-left pixel), uint8 */
         uint32_t width, height;         /* 1 .. 65535 */
         int64_t row_stride, col_stride, chan_stride;      /* in samples */
         uint32_t qtables;               /* the image's set of params->qtables; not read when that is NULL */
@@ -96,6 +113,7 @@ struct j2p_jpegenc_params {
         int components;                 /* 0 or 3: RGB images, YCbCr files; 1: gray images, one-component files */
         const struct j2p_jpegenc_qtables *qtables;        /* nqtables sets, or NULL: the IJG tables of quality */
         unsigned nqtables;
+        int cmyk;                       /* 0: as components says; 1: CMYK images, Adobe CMYK files (components 0) */
 };
 
 struct j2p_jpegenc_stats {
@@ -106,7 +124,7 @@ struct j2p_jpegenc_stats {
 /* Work area for the n images: work_bytes in all, the files at out_offset in it.  Refuses null
  * pointers, n == 0, a width or height of 0 or above 65535 (SOF's 16-bit fields), a quality outside
  * 1 .. 100, an unknown sampling, a restart field outside 0 .. 65535, components other than 0, 1
- * or 3, and given tables with nqtables == 0, a set with ntables outside 1 .. 4 or an entry of 0 or
+ * or 3, cmyk other than 0 or 1 or with components not 0, and given tables with nqtables == 0, a set with ntables outside 1 .. 4 or an entry of 0 or
  * above 8191, or an image whose set is not below nqtables.  Returns 0, or -1 (j2p_jpegenc_last_error). */
 int j2p_jpegenc_plan(const struct j2p_jpegenc_image *images, unsigned n, const struct j2p_jpegenc_params *params, size_t *work_bytes,
                      size_t *out_offset);

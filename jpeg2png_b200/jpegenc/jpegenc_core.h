@@ -21,6 +21,11 @@
 // A gray call (j2p_je_tables.nc == 1) is the same steps for one component: libjpeg's null gray
 // conversion (the pixel minus 128), luma sampling 1 x 1 whatever the SOF declares, one block per
 // MCU, so the MCU grid is the block grid, no dummies, and the DC predicted along the raster.
+//
+// A CMYK call (nc == 4) is the colour steps for four components with no conversion: a component's
+// full-resolution sample is 255 minus the tensor's (the Adobe inversion Pillow writes), M, Y and K
+// are downsampled as chroma is, from those inverted samples, and every component codes with the
+// luma Huffman tables (j2p_je_htab).
 #ifndef J2P_JPEGENC_CORE_H
 #define J2P_JPEGENC_CORE_H
 
@@ -38,12 +43,18 @@ static_assert(J2P_JE_WORDS_PER_BLOCK * 32 >= J2P_JPEGENC_BLOCK_BITS && (J2P_JE_W
 static_assert(J2P_JE_WORDS_PER_BLOCK * 32 % 8 == 0, "the padding of a stream's last byte fits its words");
 #define J2P_JE_TILE 256u                // blocks per tile of the size and emit kernels (never across images)
 #define J2P_JE_CHUNK 8192u              // entropy bytes per chunk of the stuffing kernels
-// A header template is SOI, APP0, one DQT per used quantisation table (67 bytes 8-bit, 131
-// 16-bit), SOF0 or SOF1, the DHTs and SOS; its length is its set's.  The quality tables give 2 + 18
-// + 2 x 67 + 19 + 2 x 33 + 2 x 183 + 14 = 623 bytes for a colour file, 2 + 18 + 67 + 13 + 33 + 183 +
-// 10 = 328 for a gray one.  The longest is a colour file's with three 16-bit tables:
-#define J2P_JE_PRE_MAX (2u + 18u + 3u * 133u + 19u)       // SOI .. the SOF's end, three 16-bit DQTs
-#define J2P_JE_HEAD_MAX (J2P_JE_PRE_MAX + 2u * 33u + 2u * 183u + 14u)
+// A header template is SOI, APP0 (APP14 for CMYK), one DQT per used quantisation table (67 bytes
+// 8-bit, 131 16-bit), SOF0 or SOF1, the DHTs and SOS; its length is its set's.  The quality tables
+// give 2 + 18 + 2 x 67 + 19 + 2 x 33 + 2 x 183 + 14 = 623 bytes for a colour file, 2 + 18 + 67 + 13
+// + 33 + 183 + 10 = 328 for a gray one and 2 + 16 + 67 + 22 + 33 + 183 + 16 = 341 for a CMYK one.
+// SOI .. the SOF's end is longest in a colour file with three 16-bit DQTs, and in a CMYK file with
+// four; the whole header is longest in the colour file, whose two DHT pairs outweigh CMYK's fourth
+// DQT:
+#define J2P_JE_PRE_MAX (2u + 18u + 3u * 133u + 19u)       // colour: 438
+#define J2P_JE_PRE_MAX_CMYK (2u + 16u + 4u * 133u + 22u)  // CMYK: 572
+#define J2P_JE_HEAD_MAX (J2P_JE_PRE_MAX + 2u * 33u + 2u * 183u + 14u)                 // 884
+#define J2P_JE_HEAD_MAX_CMYK (J2P_JE_PRE_MAX_CMYK + 33u + 183u + 16u)                 // 804
+static_assert(J2P_JE_HEAD_MAX_CMYK <= J2P_JE_HEAD_MAX, "a CMYK header fits the template's room");
 
 // per image of a call, or per bit stream (host plan, read by the kernels).  A stream is an image's
 // scan, or one restart interval of it; it carries its image's fields, and blk0, nblk, the tiles,
@@ -81,18 +92,28 @@ struct j2p_je_huff {
 // fields, the derived Huffman codes and the geometry, are the call's and the same in every set, so
 // the steps that read only them take set 0.
 struct j2p_je_tables {
-        uint16_t recip[3][64], corr[3][64];             // per component: Y, Cb, Cr
-        uint8_t shift[3][64];           // total right shift of the product
+        uint16_t recip[4][64], corr[4][64];             // per component: Y, Cb, Cr, or C, M, Y, K
+        uint8_t shift[4][64];           // total right shift of the product
         struct j2p_je_huff huff;        // the Annex K tables
         uint8_t zz[64];                 // zig-zag position of each natural index
-        uint32_t hs, vs;                // luma sampling factors (chroma 1 x 1); 1 x 1 for gray
-        uint32_t nc;                    // components: 3, or 1 for gray
+        uint32_t hs, vs;                // component 0's sampling factors (the others 1 x 1); 1 x 1 for gray
+        uint32_t nc;                    // the call's kind: 3 colour, 1 gray, 4 CMYK
         uint32_t head_len, sof_at;      // the header template's length and the offset of its SOF
         uint8_t head[J2P_JE_HEAD_MAX];
 };
 
-// blocks per MCU: the luma blocks and two chroma blocks, or a gray file's one block
+// blocks per MCU: component 0's blocks and one of each other component, or a gray file's one block
 J2P_HD uint32_t j2p_je_bpm(const struct j2p_je_tables *t) { return t->hs * t->vs + t->nc - 1; }
+
+// the Huffman tables component comp codes with: 0 DC0 / AC0, 1 DC1 / AC1 (a colour file's chroma);
+// every component of a CMYK file codes with DC0 / AC0
+J2P_HD uint32_t j2p_je_htab(const struct j2p_je_tables *t, uint32_t comp) { return t->nc == 4 ? 0u : comp; }
+
+// the identifier of component comp in the SOF and SOS: 1, 2, 3, or 'C', 'M', 'Y', 'K' in a CMYK file
+J2P_HD uint32_t j2p_je_comp_id(const struct j2p_je_tables *t, uint32_t comp) {
+        if (t->nc != 4) return comp + 1;
+        return comp == 0 ? 'C' : comp == 1 ? 'M' : comp == 2 ? 'Y' : 'K';
+}
 
 // the end of the template's SOF (10 + 3 bytes per component) and the length of the SOS that ends it
 J2P_HD uint32_t j2p_je_sof_end(const struct j2p_je_tables *t) { return t->sof_at + 10 + 3 * t->nc; }
@@ -148,13 +169,6 @@ J2P_HD uint64_t j2p_je_prev(const struct j2p_je_tables *t, uint64_t b) {
 }
 
 // ---- samples --------------------------------------------------------------------------------------
-J2P_HD void j2p_je_rgb(const struct j2p_je_img *im, uint32_t y, uint32_t x, int *r, int *g, int *b) {
-        const uint8_t *p = im->src + (int64_t)y * im->s_row + (int64_t)x * im->s_col;
-        *r = p[0];
-        *g = p[im->s_chan];
-        *b = p[2 * im->s_chan];
-}
-
 J2P_HD int j2p_je_y(int r, int g, int b) { return (19595 * r + 38470 * g + 7471 * b + 32768) >> 16; }
 J2P_HD int j2p_je_cb(int r, int g, int b) { return (-11059 * r - 21709 * g + 32768 * b + (128 << 16) + 32767) >> 16; }
 J2P_HD int j2p_je_cr(int r, int g, int b) { return (32768 * r - 27439 * g - 5329 * b + (128 << 16) + 32767) >> 16; }
@@ -163,33 +177,40 @@ J2P_HD int j2p_je_conv(int comp, int r, int g, int b) {
         return comp == 0 ? j2p_je_y(r, g, b) : comp == 1 ? j2p_je_cb(r, g, b) : j2p_je_cr(r, g, b);
 }
 
+// The sampling steps take the call's kind as K: 4 CMYK, 3 colour or gray (t->nc tells which), 0 read
+// from t.  The kernels branch once per block on the kind and run K = 4 or 3, so the colour samples
+// are not compiled around the CMYK ones.
+template <uint32_t K>
+J2P_HD bool j2p_je_is_cmyk(const struct j2p_je_tables *t) { return K == 4 || (K == 0 && t->nc == 4); }
+
+// component comp's full-resolution sample at pixel (y, x) of the image: the colour conversion of the
+// RGB pixel, or the inverted CMYK sample (Pillow's raw mode CMYK;I)
+template <uint32_t K>
+J2P_HD int j2p_je_full(const struct j2p_je_img *im, const struct j2p_je_tables *t, uint32_t comp, uint32_t y, uint32_t x) {
+        const uint8_t *p = im->src + (int64_t)y * im->s_row + (int64_t)x * im->s_col;
+        if (j2p_je_is_cmyk<K>(t)) return 255 - p[(int64_t)comp * im->s_chan];
+        return j2p_je_conv((int)comp, p[0], p[im->s_chan], p[2 * im->s_chan]);
+}
+
 // Sample (y, x) of a component, in its block grid, minus 128.
+template <uint32_t K = 0>
 J2P_HD int j2p_je_sample(const struct j2p_je_img *im, const struct j2p_je_tables *t, uint32_t comp, uint32_t y, uint32_t x) {
-        int r, g, b;
         const uint32_t W = im->w - 1, H = im->h - 1;
-        if (t->nc == 1)                                 // gray: the pixel itself
+        if (K != 4 && t->nc == 1)                       // gray: the pixel itself
                 return im->src[(int64_t)(y < H ? y : H) * im->s_row + (int64_t)(x < W ? x : W) * im->s_col] - 128;
-        if (comp == 0 || t->hs == 1) {                  // full size
-                j2p_je_rgb(im, y < H ? y : H, x < W ? x : W, &r, &g, &b);
-                return j2p_je_conv((int)comp, r, g, b) - 128;
-        }
+        if (comp == 0 || t->hs == 1)                    // full size
+                return j2p_je_full<K>(im, t, comp, y < H ? y : H, x < W ? x : W) - 128;
         const uint32_t x0 = 2 * x < W ? 2 * x : W, x1 = 2 * x + 1 < W ? 2 * x + 1 : W;
         if (t->vs == 1) {                               // 2x1, bias 0, 1, 0, 1 along the row
                 const uint32_t yy = y < H ? y : H;
-                j2p_je_rgb(im, yy, x0, &r, &g, &b);
-                int s = j2p_je_conv((int)comp, r, g, b);
-                j2p_je_rgb(im, yy, x1, &r, &g, &b);
-                s += j2p_je_conv((int)comp, r, g, b);
+                const int s = j2p_je_full<K>(im, t, comp, yy, x0) + j2p_je_full<K>(im, t, comp, yy, x1);
                 return ((s + (int)(x & 1)) >> 1) - 128;
         }
         const uint32_t ylast = (im->h + 1) / 2 - 1;     // the last computed row; below it repeats
         const uint32_t yc = y < ylast ? y : ylast;
         const uint32_t y0 = 2 * yc, y1 = 2 * yc + 1 < H ? 2 * yc + 1 : H;
-        int s = 0;
-        j2p_je_rgb(im, y0, x0, &r, &g, &b); s += j2p_je_conv((int)comp, r, g, b);
-        j2p_je_rgb(im, y0, x1, &r, &g, &b); s += j2p_je_conv((int)comp, r, g, b);
-        j2p_je_rgb(im, y1, x0, &r, &g, &b); s += j2p_je_conv((int)comp, r, g, b);
-        j2p_je_rgb(im, y1, x1, &r, &g, &b); s += j2p_je_conv((int)comp, r, g, b);
+        const int s = j2p_je_full<K>(im, t, comp, y0, x0) + j2p_je_full<K>(im, t, comp, y0, x1) + j2p_je_full<K>(im, t, comp, y1, x0) +
+                      j2p_je_full<K>(im, t, comp, y1, x1);
         return ((s + 1 + (int)(x & 1)) >> 2) - 128;     // bias 1, 2, 1, 2 along the row
 }
 
@@ -233,11 +254,12 @@ J2P_HD void j2p_je_fdct_1d(int *d) {
 }
 
 // Row y of a block: its 8 samples through pass 1.
+template <uint32_t K = 0>
 J2P_HD void j2p_je_block_row(const struct j2p_je_img *im, const struct j2p_je_tables *t, const struct j2p_je_where *w, int y, int *d) {
 #ifdef __CUDA_ARCH__
 #pragma unroll
 #endif
-        for (int x = 0; x < 8; x++) d[x] = j2p_je_sample(im, t, w->comp, w->srow * 8 + y, w->scol * 8 + x);
+        for (int x = 0; x < 8; x++) d[x] = j2p_je_sample<K>(im, t, w->comp, w->srow * 8 + y, w->scol * 8 + x);
         j2p_je_fdct_1d<1>(d);
 }
 
@@ -256,9 +278,10 @@ J2P_HD int j2p_je_nbits(int v) {
         return (int)n;
 }
 
-// Walks the symbols of a block (zig-zag coefficients c, DC prediction pred): sym(table, symbol)
-// for each Huffman-coded symbol (table 0 DC0, 1 AC0, 2 DC1, 3 AC1; the DC category, run << 4 |
-// size, ZRL 0xF0 or EOB 0x00) and extra(bits, n) for each run of extra bits, in order.
+// Walks the symbols of a block (zig-zag coefficients c, DC prediction pred) coded with the tables
+// comp (j2p_je_htab: 0 DC0 / AC0, else DC1 / AC1): sym(table, symbol) for each Huffman-coded symbol
+// (table 0 DC0, 1 AC0, 2 DC1, 3 AC1; the DC category, run << 4 | size, ZRL 0xF0 or EOB 0x00) and
+// extra(bits, n) for each run of extra bits, in order.
 #ifdef __CUDACC__
 #pragma nv_exec_check_disable           // sym / extra are host lambdas in the host driver, device ones in the kernels
 #endif

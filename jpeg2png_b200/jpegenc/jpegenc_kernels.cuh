@@ -79,7 +79,8 @@ __device__ __forceinline__ void blocks_body(const struct j2p_je_img *__restrict_
         if (lane == 0) sets[grp] = im.set;
         wh = j2p_je_locate(&im, t, g - im.blk0);
         int d[8];
-        j2p_je_block_row(&im, t, &wh, (int)lane, d);
+        if (t->nc == 4) j2p_je_block_row<4>(&im, t, &wh, (int)lane, d);
+        else j2p_je_block_row<3>(&im, t, &wh, (int)lane, d);
 #pragma unroll
         for (int x = 0; x < 8; x++) rows[grp][lane * 9 + x] = d[x];
     }
@@ -119,7 +120,7 @@ __device__ __forceinline__ void sizes_body(const StreamMap<PER> &sm, const struc
     const uint64_t b = (uint64_t)(tile - im->tile0) * J2P_JE_TILE + threadIdx.x;
     const uint64_t blk0 = im->blk0;
     uint32_t bits = 0;
-    if (b < im->nblk) bits = j2p_je_block_bits(coef + (blk0 + b) * 64, pred_of(t, coef, blk0, b), h, comp_of(t, b));
+    if (b < im->nblk) bits = j2p_je_block_bits(coef + (blk0 + b) * 64, pred_of(t, coef, blk0, b), h, htab_of(t, b));
     uint32_t excl, total;
     Scan(tmp).ExclusiveSum(bits, excl, total);
     if (b < im->nblk) intra[blk0 + b] = excl;
@@ -151,7 +152,7 @@ __device__ __forceinline__ void emit_body(const struct j2p_je_img *__restrict__ 
     if (b >= im->nblk) return;
     const uint64_t blk0 = im->blk0;
     uint32_t *rw = raw + im->raw_off;
-    j2p_je_emit(coef + (blk0 + b) * 64, pred_of(t, coef, blk0, b), huff, comp_of(t, b), toff[tile] + intra[blk0 + b],
+    j2p_je_emit(coef + (blk0 + b) * 64, pred_of(t, coef, blk0, b), huff, htab_of(t, b), toff[tile] + intra[blk0 + b],
                 [&](uint64_t k, uint32_t v) { atomicOr(rw + k, v); });
 }
 

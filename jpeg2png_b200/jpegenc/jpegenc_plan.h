@@ -64,20 +64,33 @@ static void quality_set(int quality, struct j2p_jpegenc_qtables *q) {
         }
 }
 
-// the sets of quantisation tables of a call, and set k of them
+// the call's kind: whether it is gray (one-component files) or CMYK, and its components
+static bool is_gray(const struct j2p_jpegenc_params *p) { return p->components == 1; }
+static bool is_cmyk(const struct j2p_jpegenc_params *p) { return p->cmyk == 1; }
+static uint32_t nc_of(const struct j2p_jpegenc_params *p) { return is_cmyk(p) ? 4u : is_gray(p) ? 1u : 3u; }
+
+// the sets of quantisation tables of a call, and set k of them.  A CMYK file's quality tables are
+// table 0 alone: libjpeg gives all four components table 0, so table 1 is neither written nor used.
 static uint32_t nsets_of(const struct j2p_jpegenc_params *p) { return p->qtables ? p->nqtables : 1u; }
 
 static void set_of(const struct j2p_jpegenc_params *p, uint32_t k, struct j2p_jpegenc_qtables *q) {
     if (p->qtables) *q = p->qtables[k];
     else quality_set(p->quality, q);
+    if (!p->qtables && is_cmyk(p)) q->ntables = 1;
 }
 
-// the table component c (0 Y, 1 Cb, 2 Cr) quantises with, as Pillow maps n tables onto them: one
-// for all; two, Y 0 and Cb, Cr 1; three or four, Y 0, Cb 1, Cr 2
-static uint32_t table_of(uint32_t n, uint32_t c) { return n == 1 || c == 0 ? 0u : n == 2 ? 1u : c; }
+// the table component c of a file of nc components quantises with, as Pillow maps n tables onto
+// them: colour (0 Y, 1 Cb, 2 Cr), one for all, two Y 0 and Cb, Cr 1, three or four Y 0, Cb 1, Cr 2;
+// CMYK, min(c, n - 1)
+static uint32_t table_of(uint32_t nc, uint32_t n, uint32_t c) {
+    if (nc == 4) return c < n - 1 ? c : n - 1;
+    return n == 1 || c == 0 ? 0u : n == 2 ? 1u : c;
+}
 
 // the tables a file of nc components writes (a DQT each, in this order): 0 .. dqts - 1
-static uint32_t dqts_of(const struct j2p_jpegenc_qtables *q, uint32_t nc) { return nc == 1 ? 1u : q->ntables < 3 ? q->ntables : 3u; }
+static uint32_t dqts_of(const struct j2p_jpegenc_qtables *q, uint32_t nc) {
+    return nc == 1 ? 1u : nc == 4 ? q->ntables : q->ntables < 3 ? q->ntables : 3u;
+}
 
 // whether table tb needs a 16-bit DQT
 static bool wide_table(const struct j2p_jpegenc_qtables *q, uint32_t tb) {
@@ -135,19 +148,16 @@ static uint8_t *put_dht(uint8_t *o, int index, const uint8_t *bits, const uint8_
     return o + 16 + n;
 }
 
-// whether a call is gray (one-component files)
-static bool is_gray(const struct j2p_jpegenc_params *p) { return p->components == 1; }
-
 // the luma sampling factors the SOF declares
 static uint32_t sof_hs(const struct j2p_jpegenc_params *p) { return p->sampling == J2P_JPEGENC_444 ? 1 : 2; }
 static uint32_t sof_vs(const struct j2p_jpegenc_params *p) { return p->sampling == J2P_JPEGENC_420 ? 2 : 1; }
 
-// the length of set k's header template: SOI, APP0, its DQTs, SOF, DHTs, SOS
+// the length of set k's header template: SOI, APP0 (CMYK: APP14), its DQTs, SOF, DHTs, SOS
 static uint32_t head_len_of(const struct j2p_jpegenc_params *p, uint32_t k) {
     struct j2p_jpegenc_qtables q;
     set_of(p, k, &q);
-    const uint32_t nc = is_gray(p) ? 1 : 3;
-    uint32_t n = 2 + 18 + (10 + 3 * nc) + (nc == 1 ? 33 + 183 : 2 * 33 + 2 * 183) + (8 + 2 * nc);
+    const uint32_t nc = nc_of(p);
+    uint32_t n = 2 + (nc == 4 ? 16 : 18) + (10 + 3 * nc) + (nc == 3 ? 2 * 33 + 2 * 183 : 33 + 183) + (8 + 2 * nc);
     for (uint32_t tb = 0; tb < dqts_of(&q, nc); tb++) n += wide_table(&q, tb) ? 133 : 69;
     return n;
 }
@@ -158,11 +168,11 @@ static void make_tables(const struct j2p_jpegenc_params *p, uint32_t set, struct
     const bool gray = is_gray(p);
     t->hs = gray ? 1 : sof_hs(p);       // a gray component is sampled 1 x 1 whatever the SOF says
     t->vs = gray ? 1 : sof_vs(p);
-    t->nc = gray ? 1 : 3;
+    t->nc = nc_of(p);
     struct j2p_jpegenc_qtables q;
     set_of(p, set, &q);
-    for (uint32_t c = 0; c < 3; c++) {
-        const uint16_t *tb = q.table[table_of(q.ntables, c)];
+    for (uint32_t c = 0; c < t->nc; c++) {
+        const uint16_t *tb = q.table[table_of(t->nc, q.ntables, c)];
         for (int i = 0; i < 64; i++) reciprocal((uint32_t)tb[i] << 3, &t->recip[c][i], &t->corr[c][i], &t->shift[c][i]);
     }
     for (int k = 0; k < 64; k++) t->zz[kNatural[k]] = (uint8_t)k;
@@ -174,8 +184,10 @@ static void make_tables(const struct j2p_jpegenc_params *p, uint32_t set, struct
     uint8_t *o = t->head;
     o = put16(o, 0xffd8);
     static const uint8_t app0[18] = {0xff, 0xe0, 0, 16, 'J', 'F', 'I', 'F', 0, 1, 1, 0, 0, 1, 0, 1, 0, 0};
-    memcpy(o, app0, 18);
-    o += 18;
+    static const uint8_t app14[16] = {0xff, 0xee, 0, 14, 'A', 'd', 'o', 'b', 'e', 0, 100, 0, 0, 0, 0, 0};   // transform 0: CMYK
+    const bool cmyk = t->nc == 4;
+    memcpy(o, cmyk ? app14 : app0, cmyk ? 16 : 18);
+    o += cmyk ? 16 : 18;
     bool sof1 = false;                  // libjpeg's frame is not baseline with a 16-bit table
     for (uint32_t tbl = 0; tbl < dqts_of(&q, t->nc); tbl++) {
         const bool wide = wide_table(&q, tbl);
@@ -196,19 +208,21 @@ static void make_tables(const struct j2p_jpegenc_params *p, uint32_t set, struct
     o = put16(o, 0);
     o = put16(o, 0);
     *o++ = (uint8_t)t->nc;
-    const uint8_t comps[9] = {1, (uint8_t)(sof_hs(p) << 4 | sof_vs(p)), 0, 2, 0x11, (uint8_t)table_of(q.ntables, 1), 3, 0x11,
-                              (uint8_t)table_of(q.ntables, 2)};
-    memcpy(o, comps, 3 * t->nc);
-    o += 3 * t->nc;
+    for (uint32_t c = 0; c < t->nc; c++) {
+        *o++ = (uint8_t)j2p_je_comp_id(t, c);
+        *o++ = (uint8_t)(c ? 0x11 : sof_hs(p) << 4 | sof_vs(p));
+        *o++ = (uint8_t)table_of(t->nc, q.ntables, c);
+    }
     o = put_dht(o, 0x00, kDcBits[0], kDcVals);
     o = put_dht(o, 0x10, kAcBits[0], kAcVals[0]);
-    if (!gray) {
+    if (t->nc == 3) {
         o = put_dht(o, 0x01, kDcBits[1], kDcVals);
         o = put_dht(o, 0x11, kAcBits[1], kAcVals[1]);
     }
     static const uint8_t sos[14] = {0xff, 0xda, 0, 12, 3, 1, 0x00, 2, 0x11, 3, 0x11, 0, 63, 0};
     static const uint8_t sos_gray[10] = {0xff, 0xda, 0, 8, 1, 1, 0x00, 0, 63, 0};
-    memcpy(o, gray ? sos_gray : sos, j2p_je_sos_len(t));
+    static const uint8_t sos_cmyk[16] = {0xff, 0xda, 0, 14, 4, 'C', 0x00, 'M', 0x00, 'Y', 0x00, 'K', 0x00, 0, 63, 0};
+    memcpy(o, gray ? sos_gray : cmyk ? sos_cmyk : sos, j2p_je_sos_len(t));
     t->head_len = (uint32_t)(o - t->head) + j2p_je_sos_len(t);
 }
 
@@ -311,6 +325,8 @@ static int check_call(const struct j2p_jpegenc_image *im, unsigned n, const stru
         return fail("restart_marker_rows must be 0 .. 65535 (got %d)", p->restart_marker_rows);
     if (p->components != 0 && p->components != 1 && p->components != 3)
         return fail("components must be 0 or 3 (colour) or 1 (gray) (got %d)", p->components);
+    if (p->cmyk != 0 && p->cmyk != 1) return fail("cmyk must be 0 or 1 (got %d)", p->cmyk);
+    if (p->cmyk && p->components != 0) return fail("cmyk = 1 needs components 0 (got %d)", p->components);
     if (p->qtables && p->nqtables == 0) return fail("qtables given with nqtables 0");
     for (unsigned k = 0; p->qtables && k < p->nqtables; k++) {
         const struct j2p_jpegenc_qtables *q = &p->qtables[k];
@@ -335,7 +351,7 @@ static int check_call(const struct j2p_jpegenc_image *im, unsigned n, const stru
 // A gray image's MCU is one block, so its MCU grid is its block grid.
 static void image_desc(const struct j2p_jpegenc_image *x, uint32_t i, const struct j2p_jpegenc_params *p, uint64_t blk0, struct j2p_je_img *g) {
     const bool gray = is_gray(p);
-    const uint32_t hs = gray ? 1 : sof_hs(p), vs = gray ? 1 : sof_vs(p), bpm = gray ? 1 : hs * vs + 2;
+    const uint32_t hs = gray ? 1 : sof_hs(p), vs = gray ? 1 : sof_vs(p), bpm = gray ? 1 : hs * vs + nc_of(p) - 1;
     memset(g, 0, sizeof *g);
     g->src = (const uint8_t *)x->data;
     g->s_row = x->row_stride;
@@ -472,6 +488,9 @@ J2P_HD uint32_t comp_of(const struct j2p_je_tables *t, uint64_t b) {
     return k < nl ? 0 : 1 + (k - nl);
 }
 
+// the Huffman tables block b codes with (j2p_je_htab)
+J2P_HD uint32_t htab_of(const struct j2p_je_tables *t, uint64_t b) { return j2p_je_htab(t, comp_of(t, b)); }
+
 // column x of a block whose rows are through pass 1 (rows[y * stride + x]): pass 2, quantise with
 // the tables of t (the image's set), and store in zig-zag order; a dummy keeps only its DC
 J2P_HD void finish_column(const struct j2p_je_tables *t, const struct j2p_je_where *w, const int *rows, int stride, int x, int16_t *coef) {
@@ -551,7 +570,7 @@ static int encode_host_steps(const struct j2p_jpegenc_image *images, unsigned n,
             uint32_t sum = 0;
             for (uint64_t b = (uint64_t)k * J2P_JE_TILE; b < im->nblk && b < (uint64_t)(k + 1) * J2P_JE_TILE; b++) {
                 intra[im->blk0 + b] = sum;
-                sum += j2p_je_block_bits(coef + (im->blk0 + b) * 64, pred_of(t, coef, im->blk0, b), c.huff(im->img), comp_of(t, b));
+                sum += j2p_je_block_bits(coef + (im->blk0 + b) * 64, pred_of(t, coef, im->blk0, b), c.huff(im->img), htab_of(t, b));
             }
             tsum[im->tile0 + k] = sum;
             toff[im->tile0 + k] = bits;
@@ -566,7 +585,7 @@ static int encode_host_steps(const struct j2p_jpegenc_image *images, unsigned n,
         const struct j2p_je_img *im = &strs[s];
         for (uint64_t b = 0; b < im->nblk; b++) {
             const uint64_t pos = toff[im->tile0 + b / J2P_JE_TILE] + intra[im->blk0 + b];
-            j2p_je_emit(coef + (im->blk0 + b) * 64, pred_of(t, coef, im->blk0, b), c.huff(im->img), comp_of(t, b), pos,
+            j2p_je_emit(coef + (im->blk0 + b) * 64, pred_of(t, coef, im->blk0, b), c.huff(im->img), htab_of(t, b), pos,
                         [&](uint64_t k, uint32_t v) { raw[im->raw_off + k] |= v; });
         }
     }

@@ -61,7 +61,7 @@ extern "C" int j2p_jpegopt_encode_host(const struct j2p_jpegenc_image *images, u
             const struct j2p_je_img *st = &strs[s];
             uint64_t *h = hist + (size_t)st->img * 4 * J2P_JE_SYMBOLS;
             for (uint64_t b = 0; b < st->nblk; b++)
-                j2p_je_symbols(coef + (st->blk0 + b) * 64, pred_of(t, coef, st->blk0, b), comp_of(t, b),
+                j2p_je_symbols(coef + (st->blk0 + b) * 64, pred_of(t, coef, st->blk0, b), htab_of(t, b),
                                [&](int tb, int v) { h[tb * J2P_JE_SYMBOLS + v]++; }, [](uint32_t, int) {});
         }
         for (unsigned i = 0; i < n; i++) {                              // tables
@@ -111,7 +111,7 @@ __global__ void __launch_bounds__(kTileThreads) k_jo_hist(const struct j2p_je_im
     const uint64_t b = (uint64_t)(tile - im->tile0) * J2P_JE_TILE + threadIdx.x;
     const uint64_t blk0 = im->blk0;
     if (b < im->nblk)
-        j2p_je_symbols(coef + (blk0 + b) * 64, pred_of(t, coef, blk0, b), comp_of(t, b),
+        j2p_je_symbols(coef + (blk0 + b) * 64, pred_of(t, coef, blk0, b), htab_of(t, b),
                        [&](int tb, int s) { atomicAdd(&cnt[tb * J2P_JE_SYMBOLS + s], 1u); }, [](uint32_t, int) {});
     __syncthreads();
     unsigned long long *h = hist + (size_t)i * 4 * J2P_JE_SYMBOLS;
@@ -120,8 +120,8 @@ __global__ void __launch_bounds__(kTileThreads) k_jo_hist(const struct j2p_je_im
 }
 
 // per image, a warp per table: code lengths, symbols and codes; then the image's header (from its
-// set's template) and its length.  A gray image's warps 2 and 3 have no table (its chroma counts are
-// all 0).
+// set's template) and its length.  A gray or CMYK image's warps 2 and 3 have no table (its chroma
+// counts are all 0).
 __global__ void __launch_bounds__(kTableThreads) k_jo_tables(const struct j2p_je_img *__restrict__ imgs, const struct j2p_je_tables *__restrict__ t,
                                                             const uint64_t *__restrict__ hist, struct j2p_je_huff *__restrict__ huffs,
                                                             uint8_t *__restrict__ heads, uint32_t *__restrict__ hlens) {

@@ -24,6 +24,10 @@
  * Gray calls (components == 1, jpegenc.h): each image counts and builds two tables, DC0 and AC0,
  * and its header is jpegenc.h's gray header with its own DHT 0x00 and 0x10.  The work-area bound
  * is the same J2P_JPEGOPT_BLOCK_BITS per block, and a call still runs the nine kernels once.
+ *
+ * CMYK calls (cmyk == 1, jpegenc.h): each image counts the symbols of all four components into two
+ * tables, DC0 and AC0, and its header is jpegenc.h's CMYK header with its own DHT 0x00 and 0x10.
+ * The bound and the nine kernels are the same.
  */
 #ifndef J2P_JPEGOPT_H
 #define J2P_JPEGOPT_H

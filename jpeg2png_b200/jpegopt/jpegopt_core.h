@@ -4,7 +4,8 @@
 //
 //   counts     per image and table, the symbols j2p_je_symbols walks (dummy blocks included): table
 //              0 counts the luma DC categories, 1 the luma AC symbols, 2 and 3 those of Cb and Cr
-//              together (a gray image has tables 0 and 1 only, and its header DHTs 0x00 and 0x10);
+//              together (a gray image has tables 0 and 1 only, and its header DHTs 0x00 and 0x10;
+//              so has a CMYK image, whose four components all count into them);
 //              a pseudo-symbol 256 with count 1 keeps any real code from being all 1-bits;
 //   lengths    T.81 Annex K.2: merge the two least counts until one node is left, lengthening both
 //              chains through others[].  V1 is the highest-numbered symbol among those of least
@@ -183,8 +184,8 @@ J2P_HD void j2p_jo_table(const uint64_t *counts, struct j2p_jo_scratch *s, struc
         if (L.lane == 0) j2p_je_derive(d->bits[tb], d->vals[tb], h->code[tb], h->size[tb]);
 }
 
-// the tables of an image of the call: DC0, AC0, DC1, AC1, or a gray image's DC0 and AC0
-J2P_HD uint32_t j2p_jo_ntables(const struct j2p_je_tables *t) { return t->nc == 1 ? 2 : 4; }
+// the tables of an image of the call: DC0, AC0, DC1, AC1, or a gray or CMYK image's DC0 and AC0
+J2P_HD uint32_t j2p_jo_ntables(const struct j2p_je_tables *t) { return t->nc == 3 ? 4 : 2; }
 
 J2P_HD uint32_t j2p_jo_head_len(const struct j2p_je_tables *t, const struct j2p_jo_dht *d) {
         uint32_t n = j2p_je_sof_end(t) + j2p_je_sos_len(t);

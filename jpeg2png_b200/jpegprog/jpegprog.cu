@@ -38,14 +38,13 @@ static StreamPlan prog_streams(const struct j2p_je_img *imgs, unsigned n, const 
                                struct j2p_je_img *strs, struct j2p_jp_scanplan *scs, uint64_t *nsblk) {
     StreamPlan sp;
     uint64_t sblk = 0;
-    const bool g = j2p_jp_gray(t);
-    const uint32_t per = j2p_jp_nscans(g);
+    const uint32_t nc = t->nc, per = j2p_jp_nscans(nc);
     for (unsigned i = 0; i < n; i++) {
         const struct j2p_je_img *im = &imgs[i];
         uint32_t last_ri = 0;                                   // the interval of the last DRI written
         for (uint32_t k = 0; k < per; k++) {
-            const bool ac = j2p_jp_is_ac(g, k);
-            const uint32_t comp = j2p_jp_scan_of(g, k).comp, wpb = j2p_jp_bound_words(g, k);
+            const bool ac = j2p_jp_is_ac(nc, k);
+            const uint32_t comp = j2p_jp_scan_of(nc, k).comp, wpb = j2p_jp_bound_words(nc, k);
             // an MCU of an AC scan is one block of the component's own grid; of a DC scan, an MCU of the image
             const uint32_t per_row = ac ? j2p_jp_grid_w(im, t, comp) : im->mcux, upm = ac ? 1 : j2p_je_bpm(t);
             const uint64_t mcus = ac ? (uint64_t)per_row * j2p_jp_grid_h(im, t, comp) : (uint64_t)im->mcux * im->mcuy;
@@ -79,7 +78,7 @@ static int prog_plan(const struct j2p_jpegenc_image *im, unsigned n, const struc
     uint64_t sblk;
     const StreamPlan sp = prog_streams(imgs.data(), n, p, &t, nullptr, nullptr, &sblk);
     if (sp.check(nblk) != 0) return -1;
-    const size_t nsc = (size_t)n * j2p_jp_nscans(j2p_jp_gray(&t));
+    const size_t nsc = (size_t)n * j2p_jp_nscans(t.nc), ntab = (size_t)n * j2p_jp_ntables(t.nc);
     size_t o = 0;
     P->off_imgs = o;  o = align16(o + n * sizeof(struct j2p_je_img));
     P->off_tab = o;   o = align16(o + nsets_of(p) * sizeof(struct j2p_je_tables));
@@ -108,10 +107,10 @@ static int prog_plan(const struct j2p_jpegenc_image *im, unsigned n, const struc
     P->off_ffc = o;   o = align16(o + sp.chunks * sizeof(uint32_t));
     P->off_ffpre = o; o = align16(o + (sp.chunks + 1) * sizeof(uint64_t));
     P->off_offs = o;  o = align16(o + (n + 1) * sizeof(uint64_t));
-    P->off_huff = o;  o = align16(o + (size_t)n * J2P_JP_TABLES * sizeof(struct j2p_jp_huff));
+    P->off_huff = o;  o = align16(o + ntab * sizeof(struct j2p_jp_huff));
     P->off_head = o;  o = align16(o + nsc * J2P_JP_HEAD);
     P->off_hlen = o;  o = align16(o + nsc * sizeof(uint32_t));
-    P->off_hist = o;  o = align16(o + (size_t)n * J2P_JP_TABLES * 256 * sizeof(uint64_t));
+    P->off_hist = o;  o = align16(o + ntab * 256 * sizeof(uint64_t));
     P->off_raw = o;   o = align16(o + sp.words * sizeof(uint32_t));
     P->off_out = o;   o = align16(o + sp.out);
     P->total = o;
@@ -135,24 +134,23 @@ struct Ctx {
     const int16_t *coef;
     const uint8_t *summ;
     const uint32_t *state;
-    bool plain;                         // no restart intervals: stream s is scan s % 10 of image s / 10 (6 for gray)
-    bool gray;                          // the call's images are gray: the six-scan script
+    bool plain;                         // no restart intervals: stream s is scan s % 10 of image s / 10 (6 gray, 18 CMYK)
+    uint32_t nc;                        // the call's kind: 3 colour, 1 gray (the six-scan script), 4 CMYK (18 scans)
 };
 
 // the scan and the image of stream s: arithmetic without restart intervals, the descriptor with them
-J2P_HD uint32_t scan_of(const Ctx &x, uint32_t s) {
-    return x.plain ? (x.gray ? s % J2P_JP_SCANS_GRAY : s % J2P_JP_SCANS) : x.strs[s].scan;
-}
-J2P_HD uint32_t image_of(const Ctx &x, uint32_t s) {
-    return x.plain ? (x.gray ? s / J2P_JP_SCANS_GRAY : s / J2P_JP_SCANS) : x.strs[s].img;
-}
+J2P_HD uint32_t scan_of(const Ctx &x, uint32_t s) { return x.plain ? s % j2p_jp_nscans(x.nc) : x.strs[s].scan; }
+J2P_HD uint32_t image_of(const Ctx &x, uint32_t s) { return x.plain ? s / j2p_jp_nscans(x.nc) : x.strs[s].img; }
+
+// the first of image i's Huffman table slots (tables and symbol counts), j2p_jp_ntables a image
+J2P_HD size_t slot0(const Ctx &x, uint32_t i) { return (size_t)i * j2p_jp_ntables(x.nc); }
 
 // the first block of stream s in its scan's order (the MCU grid's stored order for a DC scan, the
 // component's raster order for an AC scan): a multiple of an MCU, so a DC prediction restarts there
 J2P_HD uint64_t stream_first(const Ctx &x, uint32_t s) {
     if (x.plain) return 0;
     const struct j2p_je_img *st = &x.strs[s];
-    return (uint64_t)st->part * st->ri * (j2p_jp_is_ac(x.gray, st->scan) ? 1u : j2p_je_bpm(x.t));
+    return (uint64_t)st->part * st->ri * (j2p_jp_is_ac(x.nc, st->scan) ? 1u : j2p_je_bpm(x.t));
 }
 
 // the coefficients of block j of an AC scan over component comp of image im
@@ -168,18 +166,18 @@ template <class Out>
 J2P_HD void code_block(const Ctx &x, uint32_t s, uint64_t j, Out &o) {
     const uint32_t k = scan_of(x, s);
     const struct j2p_je_img *st = &x.strs[s], *im = &x.imgs[image_of(x, s)];
-    const struct j2p_jp_scan sc = j2p_jp_scan_of(x.gray, k);
+    const struct j2p_jp_scan sc = j2p_jp_scan_of(x.nc, k);
     const uint64_t f = stream_first(x, s);
     const bool last = j + 1 == st->nblk;
-    if (j2p_jp_is_ac(x.gray, k))
+    if (j2p_jp_is_ac(x.nc, k))
         j2p_jp_code(sc, ac_coef(x, im, sc.comp, f + j), 0, sc.comp, x.state[st->blk0 + j], j, last, o);
     else
-        j2p_jp_code(sc, x.coef + (im->blk0 + f + j) * 64, pred_of(x.t, x.coef, im->blk0 + f, j), comp_of(x.t, j), 0, j, last, o);
+        j2p_jp_code(sc, x.coef + (im->blk0 + f + j) * 64, pred_of(x.t, x.coef, im->blk0 + f, j), htab_of(x.t, j), 0, j, last, o);
 }
 
 // the summary of block j of AC stream s
 J2P_HD uint32_t summary_of(const Ctx &x, uint32_t s, uint64_t j) {
-    const struct j2p_jp_scan sc = j2p_jp_scan_of(x.gray, scan_of(x, s));
+    const struct j2p_jp_scan sc = j2p_jp_scan_of(x.nc, scan_of(x, s));
     return j2p_jp_summary(sc, ac_coef(x, &x.imgs[image_of(x, s)], sc.comp, stream_first(x, s) + j));
 }
 
@@ -214,7 +212,7 @@ struct EmitBits {
     // the correction bits of the run's blocks that have any, in order
     J2P_HD void deferred(uint64_t first, uint32_t run, uint32_t) {
         const struct j2p_je_img *st = &x.strs[s], *im = &x.imgs[image_of(x, s)];
-        const struct j2p_jp_scan sc = j2p_jp_scan_of(x.gray, scan_of(x, s));
+        const struct j2p_jp_scan sc = j2p_jp_scan_of(x.nc, scan_of(x, s));
         const uint64_t f = stream_first(x, s);
         for (uint64_t q = first; q < first + run; q++)
             if (x.summ[st->blk0 + q] & 63u) j2p_jp_tail(sc, ac_coef(x, im, sc.comp, f + q), *this);
@@ -250,13 +248,12 @@ extern "C" int j2p_jpegprog_encode_host(const struct j2p_jpegenc_image *images, 
     struct j2p_jp_huff *huffs = (struct j2p_jp_huff *)(w + P.off_huff);
     uint8_t *heads = w + P.off_head, *out = w + P.off_out;
     memset(w + P.off_hist, 0, P.off_raw - P.off_hist + P.words * sizeof(uint32_t));
-    const bool g = j2p_jp_gray(t);
-    const uint32_t per = j2p_jp_nscans(g);
-    const Ctx x = {imgs, strs, t, coef, summ, state, P.plain, g};
+    const uint32_t nc = t->nc, per = j2p_jp_nscans(nc);
+    const Ctx x = {imgs, strs, t, coef, summ, state, P.plain, nc};
     for (unsigned i = 0; i < n; i++) host_blocks(&imgs[i], t + imgs[i].set, coef);      // blocks
     for (uint32_t s = 0; s < P.ns; s++) {                               // summaries, runs
         const struct j2p_je_img *st = &strs[s];
-        if (!j2p_jp_is_ac(g, st->scan)) continue;
+        if (!j2p_jp_is_ac(nc, st->scan)) continue;
         for (uint64_t j = 0; j < st->nblk; j++) summ[st->blk0 + j] = (uint8_t)summary_of(x, s, j);
         for (uint64_t j = 0; j < st->nblk; j++)
             if (j == 0 || (summ[st->blk0 + j - 1] & J2P_JP_RESET))
@@ -264,7 +261,7 @@ extern "C" int j2p_jpegprog_encode_host(const struct j2p_jpegenc_image *images, 
                             [&](uint64_t q, uint32_t v) { state[st->blk0 + q] = v; });
     }
     for (uint32_t s = 0; s < P.ns; s++) {                               // hist
-        uint64_t *h = hist + ((size_t)strs[s].img * J2P_JP_TABLES + j2p_jp_slot(g, strs[s].scan)) * 256;
+        uint64_t *h = hist + (slot0(x, strs[s].img) + j2p_jp_slot(nc, strs[s].scan)) * 256;
         const auto count = [h](int tb, int v) { h[tb * 256 + v]++; };
         CountSymbols<decltype(count)> o = {count};
         for (uint64_t j = 0; j < strs[s].nblk; j++) code_block(x, s, j, o);
@@ -272,8 +269,8 @@ extern "C" int j2p_jpegprog_encode_host(const struct j2p_jpegenc_image *images, 
     for (unsigned i = 0; i < n; i++) {                                  // tables, scan headers
         struct j2p_jo_scratch scr;
         struct j2p_jp_dht d;
-        for (uint32_t tb = 0; tb < j2p_jp_ntables(g); tb++)
-            j2p_jp_table(hist + ((size_t)i * J2P_JP_TABLES + tb) * 256, &scr, &d, &huffs[(size_t)i * J2P_JP_TABLES + tb], tb, j2p_jo_serial());
+        for (uint32_t tb = 0; tb < j2p_jp_ntables(nc); tb++)
+            j2p_jp_table(hist + (slot0(x, i) + tb) * 256, &scr, &d, &huffs[slot0(x, i) + tb], tb, j2p_jo_serial());
         const struct j2p_je_tables *ts = t + imgs[i].set;
         for (uint32_t k = 0; k < per; k++) {
             const size_t q = (size_t)i * per + k;
@@ -283,7 +280,7 @@ extern "C" int j2p_jpegprog_encode_host(const struct j2p_jpegenc_image *images, 
     }
     for (uint32_t s = 0; s < P.ns; s++) {                               // sizes, emit, padding
         struct j2p_je_img *st = &strs[s];
-        const struct j2p_jp_huff *h = huffs + (size_t)st->img * J2P_JP_TABLES + j2p_jp_slot(g, st->scan);
+        const struct j2p_jp_huff *h = huffs + slot0(x, st->img) + j2p_jp_slot(nc, st->scan);
         uint64_t pos = 0;
         for (uint64_t j = 0; j < st->nblk; j++) {
             CountBits c = {h, 0};
@@ -320,13 +317,13 @@ extern "C" int j2p_jpegprog_encode_host(const struct j2p_jpegenc_image *images, 
 }
 
 // ---- device ------------------------------------------------------------------------------------
-static const int kTableThreads = 32 * J2P_JP_TABLES;    // one warp per table of an image
+static const int kTableThreads = 32 * J2P_JP_TABLES;    // one warp per table of a colour image
 
-// the derived tables of stream s (two for a colour scan 0, one for an AC scan or a gray scan 0, none
-// for the DC refine) into shared memory, by every thread of the CTA
+// the derived tables of stream s (two for a colour scan 0, one for an AC scan or a gray or CMYK
+// scan 0, none for the DC refine) into shared memory, by every thread of the CTA
 __device__ __forceinline__ const struct j2p_jp_huff *stage(struct j2p_jp_huff *sh, const struct j2p_jp_huff *huffs, const Ctx &x, uint32_t s) {
-    const uint32_t k = scan_of(x, s), nt = j2p_jp_ntab(x.gray, k);
-    const uint4 *src = (const uint4 *)(huffs + (size_t)image_of(x, s) * J2P_JP_TABLES + j2p_jp_slot(x.gray, k));
+    const uint32_t k = scan_of(x, s), nt = j2p_jp_ntab(x.nc, k);
+    const uint4 *src = (const uint4 *)(huffs + slot0(x, image_of(x, s)) + j2p_jp_slot(x.nc, k));
     uint4 *dst = (uint4 *)sh;
     for (uint32_t q = threadIdx.x; q < nt * sizeof(struct j2p_jp_huff) / 16; q += blockDim.x) dst[q] = src[q];
     __syncthreads();
@@ -340,30 +337,36 @@ __device__ __forceinline__ uint32_t tile_block(const struct j2p_je_img *strs, ui
     return s;
 }
 
-// x with the call's kind as the constant G.  k_jp_hist and k_jp_emit branch once on the kind, which
-// is uniform over the launch, and run their body with as_kind<true> or as_kind<false>, so each
-// kind's body is compiled for it alone; k_jp_blocks does the same with its summaries.
-template <bool G>
+// x with the call's kind as the constant NC.  k_jp_hist branches once on the kind, which is uniform
+// over the launch, and runs its body with as_kind<3>, <1> or <4>, so each kind's body is compiled
+// for it alone; k_jp_emit does so for colour and runs gray and CMYK calls through one body with the
+// kind as a runtime value (a third body would take it past 64 registers); k_jp_blocks does the same
+// with its summaries.
+template <uint32_t NC>
 __device__ __forceinline__ Ctx as_kind(Ctx x) {
-    x.gray = G;
+    x.nc = NC;
     return x;
 }
 
-// each real block's summary in each AC scan of its component (a lane per scan), G: gray
-template <bool G>
+// each real block's summary in each AC scan of its component (a lane per scan).  A component's AC
+// scans are the gray script's in a gray or a CMYK call, the colour script's otherwise: SC, 1 or 3,
+// is that script, and nc the call's kind, which places the scan among the image's.
+template <uint32_t SC>
 __device__ __forceinline__ void summaries(const struct j2p_je_img *__restrict__ imgs, uint32_t n, const struct j2p_je_tables *__restrict__ t,
                                           uint64_t nblk, const int16_t *__restrict__ coef, const struct j2p_je_img *__restrict__ strs,
-                                          const struct j2p_jp_scanplan *__restrict__ scs, bool plain, uint8_t *__restrict__ summ) {
+                                          const struct j2p_jp_scanplan *__restrict__ scs, bool plain, uint8_t *__restrict__ summ, uint32_t nc) {
     const uint64_t g = ((uint64_t)blockIdx.x * kBlockThreads + threadIdx.x) >> 3;
     if (g >= nblk) return;
     const uint32_t i = find_image(imgs, n, g, 0);
     const struct j2p_je_img *im = &imgs[i];
     const struct j2p_je_where wh = j2p_je_locate(im, t, g - im->blk0);
-    const int k = j2p_jp_comp_scan(G, wh.comp, threadIdx.x & 7);
-    if (wh.dummy || k < 0) return;
+    const uint32_t lane = threadIdx.x & 7;
+    const int ks = j2p_jp_comp_scan(SC, SC == 1 ? 0 : wh.comp, lane);          // the scan in script SC
+    if (wh.dummy || ks < 0) return;
+    const int k = SC == 1 && nc == 4 ? j2p_jp_comp_scan(4, wh.comp, lane) : ks;  // the scan of the image
     const uint64_t j = (uint64_t)wh.row * j2p_jp_grid_w(im, t, wh.comp) + wh.col;
-    const size_t q = (size_t)i * j2p_jp_nscans(G) + k;
-    summ[strs[plain ? q : scs[q].s0].blk0 + j] = (uint8_t)j2p_jp_summary(j2p_jp_scan_of(G, (uint32_t)k), coef + g * 64);
+    const size_t q = (size_t)i * j2p_jp_nscans(nc) + k;
+    summ[strs[plain ? q : scs[q].s0].blk0 + j] = (uint8_t)j2p_jp_summary(j2p_jp_scan_of(SC, (uint32_t)ks), coef + g * 64);
 }
 
 // kBlockThreads threads, 8 per block: the shared blocks body, then the summaries.  Six CTAs per SM
@@ -372,23 +375,24 @@ __global__ void __launch_bounds__(kBlockThreads, 6) k_jp_blocks(const struct j2p
                                                             const struct j2p_je_tables *__restrict__ t, uint64_t nblk,
                                                             int16_t *__restrict__ coef, const struct j2p_je_img *__restrict__ strs,
                                                             const struct j2p_jp_scanplan *__restrict__ scs, bool plain,
-                                                            uint8_t *__restrict__ summ, bool gray) {
+                                                            uint8_t *__restrict__ summ, uint32_t nc) {
     blocks_body(imgs, n, t, nblk, coef);
     __syncthreads();
-    if (gray) summaries<true>(imgs, n, t, nblk, coef, strs, scs, plain, summ);
-    else summaries<false>(imgs, n, t, nblk, coef, strs, scs, plain, summ);
+    if (nc == 3) summaries<3>(imgs, n, t, nblk, coef, strs, scs, plain, summ, nc);
+    else summaries<1>(imgs, n, t, nblk, coef, strs, scs, plain, summ, nc);
 }
 
-// The stream-arithmetic kernels take the call's kind as a flag and run the body with PER = its
-// scans per image, J2P_JP_SCANS or J2P_JP_SCANS_GRAY: two instantiations in one kernel.
-template <uint32_t PER>
+// The stream-arithmetic kernels take the call's kind and run the body with NC = it, and so PER =
+// its scans per image, J2P_JP_SCANS, J2P_JP_SCANS_GRAY or J2P_JP_SCANS_CMYK: three instantiations
+// in one kernel.
+template <uint32_t NC>
 __device__ __forceinline__ void runs_body(const struct j2p_je_img *__restrict__ strs, uint32_t ns, bool plain, const uint8_t *__restrict__ summ,
                                           uint32_t *__restrict__ state) {
-    const StreamMap<PER> sm = {strs, ns, plain};
+    const StreamMap<j2p_jp_nscans(NC)> sm = {strs, ns, plain};
     uint64_t j;
     const uint32_t s = tile_block(sm.strs, sm.ns, &j);
     const struct j2p_je_img *st = &sm.strs[s];
-    if (!j2p_jp_is_ac(PER == J2P_JP_SCANS_GRAY, sm.scan(s)) || j >= st->nblk) return;
+    if (!j2p_jp_is_ac(NC, sm.scan(s)) || j >= st->nblk) return;
     const uint8_t *m = summ + st->blk0;
     if (j && !(m[j - 1] & J2P_JP_RESET)) return;
     uint32_t *out = state + st->blk0;
@@ -398,16 +402,17 @@ __device__ __forceinline__ void runs_body(const struct j2p_je_img *__restrict__ 
 // per block of an AC stream that starts a segment: the walk to the segment's end (a RESET block or
 // the stream's end, which a restart marker follows)
 __global__ void __launch_bounds__(kTileThreads) k_jp_runs(const struct j2p_je_img *__restrict__ strs, uint32_t ns, bool plain, const uint8_t *__restrict__ summ,
-                                                         uint32_t *__restrict__ state, bool gray) {
-    if (gray) runs_body<J2P_JP_SCANS_GRAY>(strs, ns, plain, summ, state);
-    else runs_body<J2P_JP_SCANS>(strs, ns, plain, summ, state);
+                                                         uint32_t *__restrict__ state, uint32_t nc) {
+    if (nc == 1) runs_body<1>(strs, ns, plain, summ, state);
+    else if (nc == 4) runs_body<4>(strs, ns, plain, summ, state);
+    else runs_body<3>(strs, ns, plain, summ, state);
 }
 
 // per tile: the symbols of its blocks counted in shared memory, then added to the image's counts
 __device__ __forceinline__ void hist_body(const Ctx &x, uint32_t ns, unsigned long long *__restrict__ hist, uint32_t *cnt) {
     uint64_t j;
     const uint32_t s = tile_block(x.strs, ns, &j), k = scan_of(x, s);
-    if (!j2p_jp_ntab(x.gray, k)) return;                // the DC refine has no symbols
+    if (!j2p_jp_ntab(x.nc, k)) return;                  // the DC refine has no symbols
     for (uint32_t q = threadIdx.x; q < 2 * 256; q += kTileThreads) cnt[q] = 0;
     __syncthreads();
     if (j < x.strs[s].nblk) {
@@ -416,31 +421,34 @@ __device__ __forceinline__ void hist_body(const Ctx &x, uint32_t ns, unsigned lo
         code_block(x, s, j, o);
     }
     __syncthreads();
-    unsigned long long *h = hist + ((size_t)image_of(x, s) * J2P_JP_TABLES + j2p_jp_slot(x.gray, k)) * 256;
+    unsigned long long *h = hist + (slot0(x, image_of(x, s)) + j2p_jp_slot(x.nc, k)) * 256;
     for (uint32_t q = threadIdx.x; q < 2 * 256; q += kTileThreads)
         if (cnt[q]) atomicAdd(h + q, (unsigned long long)cnt[q]);
 }
 
 __global__ void __launch_bounds__(kTileThreads) k_jp_hist(const Ctx x, uint32_t ns, unsigned long long *__restrict__ hist) {
     __shared__ uint32_t cnt[2 * 256];
-    if (x.gray) hist_body(as_kind<true>(x), ns, hist, cnt);
-    else hist_body(as_kind<false>(x), ns, hist, cnt);
+    if (x.nc == 1) hist_body(as_kind<1>(x), ns, hist, cnt);
+    else if (x.nc == 4) hist_body(as_kind<4>(x), ns, hist, cnt);
+    else hist_body(as_kind<3>(x), ns, hist, cnt);
 }
 
 // per image, a warp per table: code lengths, symbols and codes; then its scans' headers, from its
-// set's template.  A gray image's warps past its five tables have none to build.
+// set's template.  A gray image's warps past its five tables have none to build; a CMYK image's
+// seventeen take two rounds of the ten warps.
 __global__ void __launch_bounds__(kTableThreads) k_jp_tables(const struct j2p_je_img *__restrict__ imgs, const struct j2p_je_tables *__restrict__ t,
                                                             const struct j2p_jp_scanplan *__restrict__ scs, const uint64_t *__restrict__ hist,
                                                             struct j2p_jp_huff *__restrict__ huffs, uint8_t *__restrict__ heads,
                                                             uint32_t *__restrict__ hlens) {
-    __shared__ struct j2p_jo_scratch scr[J2P_JP_TABLES];
+    __shared__ struct j2p_jo_scratch scr[kTableThreads / 32];
     __shared__ struct j2p_jp_dht d;
-    const uint32_t i = blockIdx.x, tb = threadIdx.x >> 5;
-    const bool gray = j2p_jp_gray(t);
-    const uint32_t per = j2p_jp_nscans(gray);
+    const uint32_t i = blockIdx.x, w = threadIdx.x >> 5, nc = t->nc;
+    const uint32_t per = j2p_jp_nscans(nc), ntab = j2p_jp_ntables(nc);
     const WarpLanes L = {threadIdx.x & 31, 32};
-    const size_t tab = (size_t)i * J2P_JP_TABLES + tb;
-    if (tb < j2p_jp_ntables(gray)) j2p_jp_table(hist + tab * 256, &scr[tb], &d, &huffs[tab], tb, L);
+    for (uint32_t tb = w; tb < ntab; tb += kTableThreads / 32) {
+        const size_t tab = (size_t)i * ntab + tb;
+        j2p_jp_table(hist + tab * 256, &scr[w], &d, &huffs[tab], tb, L);
+    }
     __syncthreads();
     const struct j2p_je_tables *ts = t + imgs[i].set;
     for (uint32_t k = 0; k < per; k++) {
@@ -494,8 +502,8 @@ __global__ void __launch_bounds__(kTileThreads) k_jp_emit(const Ctx x, uint32_t 
                                                          const uint32_t *__restrict__ intra, const uint64_t *__restrict__ toff,
                                                          uint32_t *__restrict__ raw) {
     __shared__ __align__(16) struct j2p_jp_huff sh[2];
-    if (x.gray) emit_kind_body(as_kind<true>(x), ns, huffs, intra, toff, raw, sh);
-    else emit_kind_body(as_kind<false>(x), ns, huffs, intra, toff, raw, sh);
+    if (x.nc == 3) emit_kind_body(as_kind<3>(x), ns, huffs, intra, toff, raw, sh);
+    else emit_kind_body(x, ns, huffs, intra, toff, raw, sh);
 }
 
 __global__ void __launch_bounds__(kChunkThreads) k_jp_ffcount(const struct j2p_je_img *__restrict__ strs, uint32_t ns,
@@ -513,8 +521,9 @@ __device__ __forceinline__ void prog_offsets_body(struct j2p_je_img *__restrict_
 
 __global__ void __launch_bounds__(kScanThreads) k_jp_offsets(struct j2p_je_img *__restrict__ strs, uint32_t ns, bool plain, uint32_t n,
                                                             const uint32_t *__restrict__ ffc, uint32_t nchunks, const uint32_t *__restrict__ hlens,
-                                                            uint64_t *__restrict__ ffpre, uint64_t *__restrict__ offsets, bool gray) {
-    if (gray) prog_offsets_body<J2P_JP_SCANS_GRAY>(strs, ns, plain, n, ffc, nchunks, hlens, ffpre, offsets);
+                                                            uint64_t *__restrict__ ffpre, uint64_t *__restrict__ offsets, uint32_t nc) {
+    if (nc == 1) prog_offsets_body<J2P_JP_SCANS_GRAY>(strs, ns, plain, n, ffc, nchunks, hlens, ffpre, offsets);
+    else if (nc == 4) prog_offsets_body<J2P_JP_SCANS_CMYK>(strs, ns, plain, n, ffc, nchunks, hlens, ffpre, offsets);
     else prog_offsets_body<J2P_JP_SCANS>(strs, ns, plain, n, ffc, nchunks, hlens, ffpre, offsets);
 }
 
@@ -529,8 +538,9 @@ __device__ __forceinline__ void prog_stuff_body(const struct j2p_je_img *__restr
 
 __global__ void __launch_bounds__(kChunkThreads) k_jp_stuff(const struct j2p_je_img *__restrict__ strs, uint32_t ns, bool plain, const uint8_t *__restrict__ heads,
                                                            const uint32_t *__restrict__ hlens, const uint32_t *__restrict__ raw,
-                                                           const uint64_t *__restrict__ ffpre, uint8_t *__restrict__ out, bool gray) {
-    if (gray) prog_stuff_body<J2P_JP_SCANS_GRAY>(strs, ns, plain, heads, hlens, raw, ffpre, out);
+                                                           const uint64_t *__restrict__ ffpre, uint8_t *__restrict__ out, uint32_t nc) {
+    if (nc == 1) prog_stuff_body<J2P_JP_SCANS_GRAY>(strs, ns, plain, heads, hlens, raw, ffpre, out);
+    else if (nc == 4) prog_stuff_body<J2P_JP_SCANS_CMYK>(strs, ns, plain, heads, hlens, raw, ffpre, out);
     else prog_stuff_body<J2P_JP_SCANS>(strs, ns, plain, heads, hlens, raw, ffpre, out);
 }
 
@@ -550,15 +560,15 @@ extern "C" int j2p_jpegprog_encode(const struct j2p_jpegenc_image *images, unsig
         int16_t *coef = (int16_t *)(w + P.off_coef);
         uint8_t *summ = w + P.off_summ, *heads = w + P.off_head;
         struct j2p_jp_huff *huffs = (struct j2p_jp_huff *)(w + P.off_huff);
-        const bool gray = is_gray(params);
-        const Ctx x = {imgs, strs, t, coef, summ, state, P.plain, gray};
+        const uint32_t nc = nc_of(params);
+        const Ctx x = {imgs, strs, t, coef, summ, state, P.plain, nc};
         // the symbol counts and the entropy words, which follow them
         const cudaError_t em = cudaMemsetAsync(hist, 0, P.off_raw - P.off_hist + P.words * sizeof(uint32_t), st);
         if (em != cudaSuccess) return fail("clearing the symbol counts and entropy words: %s", cudaGetErrorString(em));
         const uint64_t bgrid = (P.nblk * 8 + kBlockThreads - 1) / kBlockThreads;
-        k_jp_blocks<<<(unsigned)bgrid, kBlockThreads, 0, st>>>(imgs, n, t, P.nblk, coef, strs, scs, P.plain, summ, gray);
+        k_jp_blocks<<<(unsigned)bgrid, kBlockThreads, 0, st>>>(imgs, n, t, P.nblk, coef, strs, scs, P.plain, summ, nc);
         counted();
-        k_jp_runs<<<P.ntiles, kTileThreads, 0, st>>>(strs, P.ns, P.plain, summ, state, gray);
+        k_jp_runs<<<P.ntiles, kTileThreads, 0, st>>>(strs, P.ns, P.plain, summ, state, nc);
         counted();
         k_jp_hist<<<P.ntiles, kTileThreads, 0, st>>>(x, P.ns, (unsigned long long *)hist);
         counted();
@@ -572,9 +582,9 @@ extern "C" int j2p_jpegprog_encode(const struct j2p_jpegenc_image *images, unsig
         counted();
         k_jp_ffcount<<<P.nchunks, kChunkThreads, 0, st>>>(strs, P.ns, raw, ffc);
         counted();
-        k_jp_offsets<<<1, kScanThreads, 0, st>>>(strs, P.ns, P.plain, n, ffc, P.nchunks, hlens, ffpre, offs, gray);
+        k_jp_offsets<<<1, kScanThreads, 0, st>>>(strs, P.ns, P.plain, n, ffc, P.nchunks, hlens, ffpre, offs, nc);
         counted();
-        k_jp_stuff<<<P.nchunks, kChunkThreads, 0, st>>>(strs, P.ns, P.plain, heads, hlens, raw, ffpre, w + P.off_out, gray);
+        k_jp_stuff<<<P.nchunks, kChunkThreads, 0, st>>>(strs, P.ns, P.plain, heads, hlens, raw, ffpre, w + P.off_out, nc);
         counted();
         return 0;
     };

@@ -35,6 +35,16 @@
  * raster order.  Per-scan bounds: 27, 160, 1538, 1101, 1 and 1101 bits a block, all within
  * J2P_JPEGPROG_BLOCK_BITS.  Every scan has the same restart interval, so a file has one DRI.  A call
  * still runs the J2P_JPEGPROG_LAUNCHES kernels once each.
+ *
+ * CMYK calls (cmyk == 1, jpegenc.h): the APP14 header and DQTs of jpegenc.h's CMYK file, SOF2 with
+ * the four components, then libjpeg's generic script for four components, eighteen scans: DC first
+ * of all four interleaved (0 0 0 1); C, M, Y, K each 1 5 0 2, then each 6 63 0 2, then each 1 63 2
+ * 1; DC refine of all four (0 0 1 0); C, M, Y, K each 1 63 1 0.  Seventeen tables per image (the
+ * DC refine has none), each written as DHT 0x00 (scan 0) or 0x10.  An AC scan walks its component's
+ * own block grid and counts its blocks per row for restart_marker_rows, so the interval, and a DRI,
+ * can change between scans.  Per-scan bounds are the gray script's, per component.  The per-image
+ * tables and symbol counts are sized by the call's kind (5, 10 or 17 slots), and a call still runs
+ * the J2P_JPEGPROG_LAUNCHES kernels once each.
  */
 #ifndef J2P_JPEGPROG_H
 #define J2P_JPEGPROG_H

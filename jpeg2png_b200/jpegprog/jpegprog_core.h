@@ -26,8 +26,21 @@
 //   5     Y           1..63   1  0   4: 0x10
 //
 // Every gray scan is non-interleaved over the component's block grid, which is also its MCU grid,
-// so the stored order is the raster and every scan has the same restart interval.  The kind is
-// the call's: the kernels take it as a launch-uniform flag (`g` below).
+// so the stored order is the raster and every scan has the same restart interval.
+//
+// and, for a CMYK call (nc == 4), as jpeg_simple_progression scripts any other colour space, its
+// generic script for four components:
+//
+//   scan   components  Ss..Se  Ah Al  tables (slot: DHT index)
+//   0      C M Y K     0..0    0  1   0: 0x00                          DC first, interleaved
+//   1..4   C, M, Y, K  1..5    0  2   1..4: 0x10
+//   5..8   C, M, Y, K  6..63   0  2   5..8: 0x10
+//   9..12  C, M, Y, K  1..63   2  1   9..12: 0x10                      AC refine
+//   13     C M Y K     0..0    1  0   none                             DC refine, interleaved
+//   14..17 C, M, Y, K  1..63   1  0   13..16: 0x10
+//
+// Every CMYK table is DC0 or AC0 in the file (each scan's DHT replaces the last).  The kind is the
+// call's, its component count nc: the kernels take it as a launch-uniform value.
 //
 // The coding is T.81 Annex G as libjpeg's progressive Huffman encoder applies it:
 //
@@ -61,10 +74,16 @@
 
 #define J2P_JP_SCANS 10u                // scans, and so bit streams, per colour image
 #define J2P_JP_SCANS_GRAY 6u            // per gray image
-#define J2P_JP_TABLES 10u               // Huffman table slots per image (a gray image uses 5)
+#define J2P_JP_SCANS_CMYK 18u           // per CMYK image
+#define J2P_JP_TABLES 10u               // Huffman table slots per colour image
 #define J2P_JP_TABLES_GRAY 5u
-#define J2P_JP_HEAD 1024u               // room for a scan's header: SOI .. SOF2, two DHTs, DRI, SOS
+#define J2P_JP_TABLES_CMYK 17u
+#define J2P_JP_TABLES_MAX J2P_JP_TABLES_CMYK
+#define J2P_JP_ALL 4u                   // j2p_jp_scan.comp of an interleaved scan: every component
+#define J2P_JP_HEAD 1024u               // room for a scan's header: SOI .. SOF2, its DHTs, DRI, SOS
+// scan 0's header is the longest: colour, three 16-bit DQTs and two DHTs; CMYK, four 16-bit DQTs and one
 static_assert(J2P_JP_HEAD >= J2P_JE_PRE_MAX + 2 * (21 + 256) + J2P_JE_DRI + 14 && J2P_JP_HEAD % 16 == 0, "a scan's header fits");
+static_assert(J2P_JP_HEAD >= J2P_JE_PRE_MAX_CMYK + (21 + 256) + J2P_JE_DRI + 16, "a CMYK scan's header fits");
 #define J2P_JP_MAX_RUN 0x7fffu          // the longest EOB run
 #define J2P_JP_MAX_BE 937u              // correction bits an EOB run may buffer before it is emitted
 #define J2P_JP_RESET 0x80u              // summary: the block emits the incoming state and sets its own
@@ -92,18 +111,41 @@ static_assert(J2P_JP_AC_FIRST_BITS(5u) == 5u * 32u && 32u % 8u == 0u, "a bound i
 // The gray script's per-scan bounds: DC first 27, AC first over 1..5 160 and over 6..63 1538, AC
 // refine over 1..63 1101, DC refine 1 bit a block.
 static_assert(J2P_JP_AC_FIRST_BITS(58u) == 1538u && J2P_JP_AC_FIRST_BITS(58u) < J2P_JPEGPROG_BLOCK_BITS, "the gray scans are within the bound");
+// The CMYK script's scans are the gray script's, per component: the same per-scan bounds.
 
 struct j2p_jp_scan {
-        uint32_t comp;                  // 0 Y, 1 Cb, 2 Cr; 3 all three, interleaved
+        uint32_t comp;                  // 0 Y, 1 Cb, 2 Cr (C, M, Y, K: 0 .. 3); J2P_JP_ALL: all, interleaved
         uint32_t ss, se, ah, al;
 };
 
-// the scans and the table slots of an image of the call (g: gray)
-J2P_HD uint32_t j2p_jp_nscans(bool g) { return g ? J2P_JP_SCANS_GRAY : J2P_JP_SCANS; }
-J2P_HD uint32_t j2p_jp_ntables(bool g) { return g ? J2P_JP_TABLES_GRAY : J2P_JP_TABLES; }
+// the scans and the table slots of an image of a call of nc components
+constexpr J2P_HD uint32_t j2p_jp_nscans(uint32_t nc) { return nc == 1 ? J2P_JP_SCANS_GRAY : nc == 4 ? J2P_JP_SCANS_CMYK : J2P_JP_SCANS; }
+J2P_HD uint32_t j2p_jp_ntables(uint32_t nc) { return nc == 1 ? J2P_JP_TABLES_GRAY : nc == 4 ? J2P_JP_TABLES_CMYK : J2P_JP_TABLES; }
 
-J2P_HD struct j2p_jp_scan j2p_jp_scan_of(bool g, uint32_t k) {
-        if (g) {
+J2P_HD struct j2p_jp_scan j2p_jp_scan_of(uint32_t nc, uint32_t k) {
+        if (nc == 4) {
+                switch (k) {
+                case 0: return {J2P_JP_ALL, 0, 0, 0, 1};
+                case 1: return {0, 1, 5, 0, 2};
+                case 2: return {1, 1, 5, 0, 2};
+                case 3: return {2, 1, 5, 0, 2};
+                case 4: return {3, 1, 5, 0, 2};
+                case 5: return {0, 6, 63, 0, 2};
+                case 6: return {1, 6, 63, 0, 2};
+                case 7: return {2, 6, 63, 0, 2};
+                case 8: return {3, 6, 63, 0, 2};
+                case 9: return {0, 1, 63, 2, 1};
+                case 10: return {1, 1, 63, 2, 1};
+                case 11: return {2, 1, 63, 2, 1};
+                case 12: return {3, 1, 63, 2, 1};
+                case 13: return {J2P_JP_ALL, 0, 0, 1, 0};
+                case 14: return {0, 1, 63, 1, 0};
+                case 15: return {1, 1, 63, 1, 0};
+                case 16: return {2, 1, 63, 1, 0};
+                default: return {3, 1, 63, 1, 0};
+                }
+        }
+        if (nc == 1) {
                 switch (k) {
                 case 0: return {0, 0, 0, 0, 1};
                 case 1: return {0, 1, 5, 0, 2};
@@ -114,41 +156,45 @@ J2P_HD struct j2p_jp_scan j2p_jp_scan_of(bool g, uint32_t k) {
                 }
         }
         switch (k) {
-        case 0: return {3, 0, 0, 0, 1};
+        case 0: return {J2P_JP_ALL, 0, 0, 0, 1};
         case 1: return {0, 1, 5, 0, 2};
         case 2: return {2, 1, 63, 0, 1};
         case 3: return {1, 1, 63, 0, 1};
         case 4: return {0, 6, 63, 0, 2};
         case 5: return {0, 1, 63, 2, 1};
-        case 6: return {3, 0, 0, 1, 0};
+        case 6: return {J2P_JP_ALL, 0, 0, 1, 0};
         case 7: return {2, 1, 63, 1, 0};
         case 8: return {1, 1, 63, 1, 0};
         default: return {0, 1, 63, 1, 0};
         }
 }
 
-// the DC refine scan: 6, or a gray image's 4
-J2P_HD bool j2p_jp_is_ac(bool g, uint32_t k) { return k != 0 && k != (g ? 4u : 6u); }
+// the DC refine scan: 6, a gray image's 4, a CMYK image's 13
+J2P_HD bool j2p_jp_is_ac(uint32_t nc, uint32_t k) { return k != 0 && k != (nc == 1 ? 4u : nc == 4 ? 13u : 6u); }
 
-// the table slot of scan k's first table (scan 0: luma 0, chroma 1); the DC refine has none (its
-// slot is the next scan's, and it counts no symbols there)
-J2P_HD uint32_t j2p_jp_slot(bool g, uint32_t k) { return g ? (k < 4 ? k : 4) : k == 0 ? 0 : k < 6 ? k + 1 : k; }
+// the table slot of scan k's first table (colour scan 0: luma 0, chroma 1); the DC refine has none
+// (its slot is the next scan's, and it counts no symbols there)
+J2P_HD uint32_t j2p_jp_slot(uint32_t nc, uint32_t k) {
+        if (nc == 4) return k < 14 ? k : k - 1;
+        return nc == 1 ? (k < 4 ? k : 4) : k == 0 ? 0 : k < 6 ? k + 1 : k;
+}
 
 // the tables scan k codes with: two for a colour DC first scan, none for the DC refine, else one
-J2P_HD uint32_t j2p_jp_ntab(bool g, uint32_t k) { return j2p_jp_is_ac(g, k) ? 1 : k ? 0 : g ? 1 : 2; }
+J2P_HD uint32_t j2p_jp_ntab(uint32_t nc, uint32_t k) { return j2p_jp_is_ac(nc, k) ? 1 : k ? 0 : nc == 3 ? 2 : 1; }
 
 // the worst case of a block of scan k, in bits and in 32-bit words
-J2P_HD uint32_t j2p_jp_bound_bits(bool g, uint32_t k) {
-        const struct j2p_jp_scan s = j2p_jp_scan_of(g, k);
-        if (!j2p_jp_is_ac(g, k)) return s.ah ? J2P_JP_DC_REFINE_BITS : J2P_JP_DC_FIRST_BITS;
+J2P_HD uint32_t j2p_jp_bound_bits(uint32_t nc, uint32_t k) {
+        const struct j2p_jp_scan s = j2p_jp_scan_of(nc, k);
+        if (!j2p_jp_is_ac(nc, k)) return s.ah ? J2P_JP_DC_REFINE_BITS : J2P_JP_DC_FIRST_BITS;
         return s.ah ? J2P_JP_AC_REFINE_BITS(s.se - s.ss + 1) : J2P_JP_AC_FIRST_BITS(s.se - s.ss + 1);
 }
 
-J2P_HD uint32_t j2p_jp_bound_words(bool g, uint32_t k) { return (j2p_jp_bound_bits(g, k) + 31) / 32; }
+J2P_HD uint32_t j2p_jp_bound_words(uint32_t nc, uint32_t k) { return (j2p_jp_bound_bits(nc, k) + 31) / 32; }
 
 // the AC scans of component comp, q = 0, 1, ...; -1 past the last
-J2P_HD int j2p_jp_comp_scan(bool g, uint32_t comp, uint32_t q) {
-        if (g) return q == 0 ? 1 : q == 1 ? 2 : q == 2 ? 3 : q == 3 ? 5 : -1;
+J2P_HD int j2p_jp_comp_scan(uint32_t nc, uint32_t comp, uint32_t q) {
+        if (nc == 4) return q < 3 ? (int)(1 + 4 * q + comp) : q == 3 ? (int)(14 + comp) : -1;
+        if (nc == 1) return q == 0 ? 1 : q == 1 ? 2 : q == 2 ? 3 : q == 3 ? 5 : -1;
         if (comp == 0) return q == 0 ? 1 : q == 1 ? 4 : q == 2 ? 5 : q == 3 ? 9 : -1;
         if (comp == 1) return q == 0 ? 3 : q == 1 ? 8 : -1;
         return q == 0 ? 2 : q == 1 ? 7 : -1;
@@ -346,11 +392,11 @@ J2P_HD void j2p_jp_code(const struct j2p_jp_scan &s, const int16_t *c, int pred,
 }
 
 // ---- headers --------------------------------------------------------------------------------------
-// the DHT contents of an image's ten tables
+// the DHT contents of an image's tables (ten, five for gray, seventeen for CMYK)
 struct j2p_jp_dht {
-        uint8_t bits[J2P_JP_TABLES][16];
-        uint8_t vals[J2P_JP_TABLES][256];
-        uint32_t nvals[J2P_JP_TABLES];
+        uint8_t bits[J2P_JP_TABLES_MAX][16];
+        uint8_t vals[J2P_JP_TABLES_MAX][256];
+        uint32_t nvals[J2P_JP_TABLES_MAX];
 };
 
 // derived codes of one table
@@ -375,16 +421,16 @@ J2P_HD void j2p_jp_table(const uint64_t *counts, struct j2p_jo_scratch *s, struc
 
 J2P_HD uint32_t j2p_jp_dht_len(const struct j2p_jp_dht *d, uint32_t tb) { return 21 + d->nvals[tb]; }
 
-J2P_HD uint32_t j2p_jp_sos_len(bool g, uint32_t k) { return j2p_jp_scan_of(g, k).comp == 3 ? 14 : 10; }
-
-J2P_HD bool j2p_jp_gray(const struct j2p_je_tables *t) { return t->nc == 1; }
+// the components of scan k's SOS, and its length
+J2P_HD uint32_t j2p_jp_sos_ns(uint32_t nc, uint32_t k) { return j2p_jp_scan_of(nc, k).comp == J2P_JP_ALL ? nc : 1; }
+J2P_HD uint32_t j2p_jp_sos_len(uint32_t nc, uint32_t k) { return 8 + 2 * j2p_jp_sos_ns(nc, k); }
 
 // the header of scan k of an image whose set is t: SOI .. SOF2 (its set's DQTs) before scan 0, the
 // DHTs of its tables, its SOS (without DRI)
 J2P_HD uint32_t j2p_jp_head_len(const struct j2p_je_tables *t, const struct j2p_jp_dht *d, uint32_t k) {
-        const bool g = j2p_jp_gray(t);
-        if (k == 0) return j2p_je_sof_end(t) + j2p_jp_dht_len(d, 0) + (g ? 0 : j2p_jp_dht_len(d, 1)) + j2p_jp_sos_len(g, 0);
-        return (j2p_jp_is_ac(g, k) ? j2p_jp_dht_len(d, j2p_jp_slot(g, k)) : 0) + j2p_jp_sos_len(g, k);
+        const uint32_t nc = t->nc;
+        if (k == 0) return j2p_je_sof_end(t) + j2p_jp_dht_len(d, 0) + (nc == 3 ? j2p_jp_dht_len(d, 1) : 0) + j2p_jp_sos_len(nc, 0);
+        return (j2p_jp_is_ac(nc, k) ? j2p_jp_dht_len(d, j2p_jp_slot(nc, k)) : 0) + j2p_jp_sos_len(nc, k);
 }
 
 J2P_HD uint8_t j2p_jp_dht_byte(const struct j2p_jp_dht *d, uint32_t tb, uint32_t index, uint32_t k) {
@@ -398,40 +444,40 @@ J2P_HD uint8_t j2p_jp_dht_byte(const struct j2p_jp_dht *d, uint32_t tb, uint32_t
 
 // SOS: the components with their table selectors (td << 4 | ta, 0 where the scan uses none), Ss,
 // Se, Ah << 4 | Al
-J2P_HD uint8_t j2p_jp_sos_byte(bool g, uint32_t k, uint32_t b) {
-        const struct j2p_jp_scan s = j2p_jp_scan_of(g, k);
-        const uint32_t ns = s.comp == 3 ? 3 : 1, len = 6 + 2 * ns;
+J2P_HD uint8_t j2p_jp_sos_byte(const struct j2p_je_tables *t, uint32_t k, uint32_t b) {
+        const struct j2p_jp_scan s = j2p_jp_scan_of(t->nc, k);
+        const uint32_t ns = j2p_jp_sos_ns(t->nc, k), len = 6 + 2 * ns;
         if (b < 2) return b ? 0xda : 0xff;
         if (b < 4) return (uint8_t)(b == 2 ? 0 : len);
         if (b == 4) return (uint8_t)ns;
         if (b < 5 + 2 * ns) {
-                const uint32_t q = (b - 5) / 2, comp = s.comp == 3 ? q : s.comp;
-                if ((b - 5) % 2 == 0) return (uint8_t)(comp + 1);
-                if (s.ss == 0) return (uint8_t)(s.ah == 0 && comp ? 0x10 : 0);
-                return (uint8_t)(comp ? 0x01 : 0);
+                const uint32_t q = (b - 5) / 2, comp = s.comp == J2P_JP_ALL ? q : s.comp, h = j2p_je_htab(t, comp);
+                if ((b - 5) % 2 == 0) return (uint8_t)j2p_je_comp_id(t, comp);
+                if (s.ss == 0) return (uint8_t)(s.ah == 0 && h ? 0x10 : 0);
+                return (uint8_t)(h ? 0x01 : 0);
         }
         b -= 5 + 2 * ns;
         return (uint8_t)(b == 0 ? s.ss : b == 1 ? s.se : s.ah << 4 | s.al);
 }
 
 J2P_HD uint8_t j2p_jp_head_byte(const struct j2p_je_tables *t, const struct j2p_je_img *im, const struct j2p_jp_dht *d, uint32_t k, uint32_t b) {
-        const bool g = j2p_jp_gray(t);
+        const uint32_t nc = t->nc;
         if (k == 0) {
                 const uint32_t pre = j2p_je_sof_end(t);
                 if (b < pre) return b == t->sof_at + 1 ? 0xc2 : j2p_je_head_byte(t, im, b);
                 b -= pre;
-                for (uint32_t tb = 0; tb < j2p_jp_ntab(g, 0); tb++) {
+                for (uint32_t tb = 0; tb < j2p_jp_ntab(nc, 0); tb++) {
                         if (b < j2p_jp_dht_len(d, tb)) return j2p_jp_dht_byte(d, tb, tb, b);
                         b -= j2p_jp_dht_len(d, tb);
                 }
-                return j2p_jp_sos_byte(g, 0, b);
+                return j2p_jp_sos_byte(t, 0, b);
         }
-        if (j2p_jp_is_ac(g, k)) {
-                const uint32_t tb = j2p_jp_slot(g, k);
-                if (b < j2p_jp_dht_len(d, tb)) return j2p_jp_dht_byte(d, tb, j2p_jp_scan_of(g, k).comp ? 0x11 : 0x10, b);
+        if (j2p_jp_is_ac(nc, k)) {
+                const uint32_t tb = j2p_jp_slot(nc, k);
+                if (b < j2p_jp_dht_len(d, tb)) return j2p_jp_dht_byte(d, tb, j2p_je_htab(t, j2p_jp_scan_of(nc, k).comp) ? 0x11 : 0x10, b);
                 b -= j2p_jp_dht_len(d, tb);
         }
-        return j2p_jp_sos_byte(g, k, b);
+        return j2p_jp_sos_byte(t, k, b);
 }
 
 // scan k's header with DRI for dri (0: none) before its SOS
@@ -441,7 +487,7 @@ J2P_HD uint32_t j2p_jp_scan_head_len(const struct j2p_je_tables *t, const struct
 
 J2P_HD uint8_t j2p_jp_scan_head_byte(const struct j2p_je_tables *t, const struct j2p_je_img *im, const struct j2p_jp_dht *d, uint32_t k,
                                      uint32_t dri, uint32_t b) {
-        return j2p_je_dri_head(dri, j2p_jp_head_len(t, d, k), j2p_jp_sos_len(j2p_jp_gray(t), k), b,
+        return j2p_je_dri_head(dri, j2p_jp_head_len(t, d, k), j2p_jp_sos_len(t->nc, k), b,
                                [&](uint32_t b1) { return j2p_jp_head_byte(t, im, d, k, b1); });
 }
 

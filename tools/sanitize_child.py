@@ -1,6 +1,7 @@
 """Small solves through the C ABI for compute-sanitizer (tools/run_sanitizers.sh): every kernel family once
 — joint 4:4:4, joint 4:2:0 with a frame larger than the luma grid, one-plane (-s) solves, odd sampling —
-and four-component files through decode_jpeg (device entropy decoding and the four-plane export)."""
+and four-component files through decode_jpeg (device entropy decoding and the four-plane export), and
+CMYK encoding through the three JPEG encoders."""
 import os
 import sys
 
@@ -38,3 +39,16 @@ for mode, dtype in (('UNCHANGED', torch.uint8), ('UNCHANGED', torch.float32), ('
         ts = decode_jpeg(files, mode=mode, dtype=dtype, iterations=2, apply_exif_orientation=orient)
         torch.cuda.synchronize()
         print('ok four-component', mode, dtype, 'oriented' if orient else 'plain', [tuple(t.shape) for t in ts])
+
+# CMYK encoding (DESIGN §7r): libj2pjpegenc.so, libj2pjpegopt.so and libj2pjpegprog.so on four-channel
+# tensors, with and without restart intervals, strided and in two samplings
+from jpeg2png_b200 import encode_jpeg  # noqa: E402
+from tests import cmyk_jpeg_cases as K  # noqa: E402
+
+xs = [torch.from_numpy(K.cmyk(kind, h, w, 3)).cuda() for kind, h, w in (('cartoon', 37, 53), ('noise', 16, 24), ('flat128', 1, 1))]
+xs.append(xs[0].permute(2, 0, 1).contiguous().permute(1, 2, 0)[::2, 1:])
+for mode in K.MODES.values():
+    for s, kw in (('4:2:0', {}), ('4:4:4', {'restart_marker_rows': 1})):
+        fs = encode_jpeg(xs, layout='HWC', subsampling=s, cmyk=True, **mode, **kw)
+        torch.cuda.synchronize()
+        print('ok cmyk encode', mode, s, kw, [len(f) for f in fs])
